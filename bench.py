@@ -2,6 +2,7 @@
 """bench.py -- transitions/sec through PPO ``Algorithm.update()`` (v1: ``learn()``), obs=17.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--config c2|c5] [--scaling weak|strong]
+                    [--dump-outputs DIR]
 
 Workload (BASELINE.json configs[1], SURVEY.md 8d): synthetic HalfCheetah-shaped rollout of
 4096 envs x 128 steps per GPU (N = 524,288 transitions, obs 17, act 6), actor/critic MLP[64,64]
@@ -28,6 +29,10 @@ checks itself: ``multi_gpu_check`` = {replicas_equal, loss_rel_err (N ranks vs 1
 ``--config c5`` = BASELINE configs[4] (8192 envs x 256 steps, minibatch N/8); the default run reports it as the extra
 key ``config4`` (strong-scaled over the N GPUs).  The timed arms use the DEFAULT public API (reference-exact
 ``np.random.permutation`` minibatch order); the opt-in device-generated order is reported as ``*_device_order``.
+``--dump-outputs DIR``: after the timed steps, rank 0 writes what the last timed ``update`` step computed -- the flat actor
+and critic parameters, the per-minibatch loss table and the batch's v_s / returns / advantages / logp_old -- as
+``DIR/<name>.npy`` (float32 / float64, ~10 MB at the default config).  Inputs are seeded, so two builds run with the same
+arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -58,11 +63,12 @@ def load_peaks() -> tuple[dict, str]:
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return json.load(open(p)), "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    # NVIDIA H100 SXM data sheet (700 W card): HBM3 bandwidth, dense BF16 tensor-core rate -- not measured figures
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "H100 SXM data sheet"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -210,7 +216,7 @@ def run_reference_arm(args) -> None:
         return
     cfg = CONFIGS[args.config]
     E = int(os.environ.get("TS_BENCH_CPU_ENVS", "1024"))      # 1/4 of configs[1]: 8 minibatches of 16384 per pass
-    res = cpu_reference_run(E, cfg["T"], max(3, args.steps), max(1, min(args.warmup, 1)))
+    res = cpu_reference_run(E, cfg["T"], max(1, args.steps), max(1, min(args.warmup, 1)))
     line = {
         "impl": "reference", "metric": METRIC, "value": res["value"], "unit": "transitions/s", "n_gpus": args.gpus,
         "steps": args.steps, "warmup": args.warmup, "ms_per_step": res["ms_per_step"], "higher_is_better": True,
@@ -250,6 +256,8 @@ def main() -> None:
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed as DIR/<name>.npy (rank 0)")
     ap.add_argument("--config", default="c2", choices=sorted(CONFIGS))
     ap.add_argument("--scaling", default="weak", choices=["weak", "strong"])
     ap.add_argument("--envs", type=int, default=0, help="override the config's env count (diagnostics)")
@@ -334,11 +342,13 @@ def main() -> None:
 
     with policy_within_training_step(algo.policy), policy_within_training_step(algo_dv.policy):
         dev_batch, dev_idx = algo._sample(buf, 0)
+        last_batch = {}
 
         def device_step(a=algo):
             with a._minibatch_order_job(buf, REPEAT):       # what update() does first: the minibatch-order draws start in the background
                 b = a._preprocess_batch(dev_batch, buf, dev_idx)
                 a._update_with_batch(b, BS, REPEAT)
+            last_batch[a] = b
 
         def e2e_step(a=algo):
             a.update(buffer=buf, batch_size=BS, repeat=REPEAT)
@@ -363,6 +373,8 @@ def main() -> None:
         _cabi.reset_launch_count()
         ms_dev = timed(device_step, K)
         launches = _cabi.launch_count()
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, algo, last_batch[algo])
         for _ in range(W):
             e2e_step()
         ms_e2e = timed(e2e_step, K)
@@ -565,7 +577,7 @@ def main() -> None:
         "config4": config4,
         "ingest": ingest,
         "roofline": {"kernel": "ppo_tc_kernel<EPOCH> (persistent: every optimiser step of one pass = minibatch fwd/bwd + "
-                               "gradient fold + clip + Adam; tcgen05 bf16x3 = fp32-faithful)", "bound": "tensor",
+                               "gradient fold + clip + Adam; wgmma bf16x3 = fp32-faithful)", "bound": "tensor",
                      "achieved": grad_tflops, "peak": peaks["bf16_tflops"], "unit": "TFLOP/s",
                      "frac": grad_tflops / peaks["bf16_tflops"], "traffic": traffic, "peak_source": peak_src,
                      "algorithmic_flops_per_launch": grad_flops, "launch_ms": epoch_ms, "rows_per_launch": N,
@@ -597,6 +609,17 @@ def main() -> None:
     print(json.dumps(line))
     if world > 1:
         dist.destroy_process_group()
+
+
+def dump_outputs(out_dir: str, algo, batch) -> None:
+    """The arrays a caller of the timed step receives or reads back after it (see the module docstring)."""
+    import torch
+    arrays = {"params": algo._flat.flat, "loss_table": algo.last_loss_table, "v_s": batch.v_s, "returns": batch.returns,
+              "adv": batch.adv, "logp_old": batch.logp_old}
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        a = a.detach().cpu().numpy() if isinstance(a, torch.Tensor) else np.asarray(a)
+        np.save(os.path.join(out_dir, f"{name}.npy"), a.astype(np.float64 if a.dtype == np.float64 else np.float32))
 
 
 def offpolicy_extras(dev) -> dict:

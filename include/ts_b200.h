@@ -1,5 +1,5 @@
 /*
- * ts_b200.h -- C ABI of the B200-native policy-update hot path for Tianshou-style RL.
+ * ts_b200.h -- C ABI of the GPU-native (H100, sm_90a) policy-update hot path for Tianshou-style RL.
  *
  * The reference (thu-ml/tianshou 2.0.1) has NO FFI: its hot path is Python + numba @njit +
  * stock torch ops.  This header declares the entry points a maintainer binds (ctypes / cffi,
@@ -10,7 +10,7 @@
  * Pointers are DEVICE pointers unless a parameter is documented as "host".  "u8" flags are
  * numpy/torch bool storage (one byte, 0/1).
  *
- * Each declaration cites the reference code it replaces (path:line under /root/reference).
+ * Each declaration cites the reference code it replaces (path:line in thu-ml/tianshou 2.0.1).
  */
 #ifndef TS_B200_H_
 #define TS_B200_H_
@@ -398,7 +398,7 @@ int ts_narrow_i64_i32(const int64_t* src, int64_t n, int32_t* dst, ts_stream_t s
  * (9) Layered networks of the off-policy algorithms (SURVEY.md 8(f) ranks 2-3): every nn.Linear / nn.Conv2d
  * forward and autograd backward inside SAC._update_with_batch (modelfree/sac.py:304-336),
  * _minimize_critic_squared_loss (modelfree/ddpg.py:267-285), DQN._update_with_batch (modelfree/dqn.py:382-404)
- * and DQNet (env/atari/atari_network.py:60-122) is ONE call of ts_net_gemm (tcgen05, fp32-faithful bf16x3):
+ * and DQNet (env/atari/atari_network.py:60-122) is ONE call of ts_net_gemm (wgmma, fp32-faithful bf16x3):
  *
  *     C[M,N] (+)= act'(act_grad_src) * act( A[M,K] * B[N,K]^T + bias[N] )
  *
@@ -496,10 +496,10 @@ int ts_polyak_update(float* target, const float* source, int64_t n, double tau, 
 
 #ifdef TS_B200_DIAGNOSTICS
 /* Diagnostics build only (libts_b200_diag.so, `python -m tianshou_b200.csrc.build --diag`): not part of the product library. */
-/* Hardware self-test of the tcgen05 / TMEM building blocks (csrc/umma.cuh), one CTA:
- * D[M,N] = a[M,K] * b[N,K]^T with dtype 0 = 3xTF32 (kind::tf32) or 1 = 3-way bf16 split (kind::f16),
- * M in {64,128}; a_mn / b_mn place the operand MN-major instead of K-major in shared memory; swap
- * exchanges LBO/SBO (diagnostic).  d receives the RAW accumulator: 128 TMEM lanes x N columns. */
+/* Hardware self-test of the wgmma building blocks (csrc/wgmma.cuh), one CTA:
+ * D[M,N] = a[M,K] * b[N,K]^T with dtype 1 = 3-way bf16 split (the only one; other values are rejected),
+ * M in {64,128}, N <= 128, K <= 128 (multiples of 16); a_mn / b_mn place the operand MN-major instead of K-major in
+ * shared memory; swap exchanges LBO/SBO (diagnostic).  d receives D row-major [M][N]. */
 int ts_umma_selftest(const float* a, const float* b, float* d, int32_t M, int32_t N, int32_t K,
                      int32_t dtype, int32_t a_mn, int32_t b_mn, int32_t swap, ts_stream_t stream);
 

@@ -156,7 +156,7 @@ def test_cabi_library_exports_every_declared_symbol():
         assert hasattr(lib, n), f"{n} declared in include/ts_b200.h but not exported"
     bound = set(_cabi.SIGNATURES) | set(_cabi.OTHER_SYMBOLS)
     assert set(names) == bound, set(names) ^ bound
-    # diagnostics (phase timeline, tcgen05 self-test) live in a separate build and are NOT in the product library
+    # diagnostics (phase timeline, wgmma self-test) live in a separate build and are NOT in the product library
     diag = header_functions(diagnostics=True)
     assert set(diag) == set(_cabi.DIAG_SIGNATURES) and len(diag) == 2
     for n in diag:

@@ -1,4 +1,4 @@
-"""Layer-wise actor-critic path (algorithm/layered.py: every Linear forward / backward = one tcgen05 GEMM launch, loss rows
+"""Layer-wise actor-critic path (algorithm/layered.py: every Linear forward / backward = one wgmma GEMM launch, loss rows
 in between) -- the path networks OUTSIDE the fused 17-64-64 kernels' envelope take.  Checked (a) on the reference's own
 goldens by forcing the path onto shapes the fused kernels also cover (discrete shared-trunk ReLU net ppo_ref_C1*, MuJoCo
 tanh net ppo_ref_A/B), and (b) on shapes only this path accepts (obs 376, MLP[256,256] -- Humanoid / BASELINE configs[3]

@@ -1,5 +1,5 @@
 """Layered-network kernels (csrc/net_gemm.cu, csrc/net_ops.cu) against plain torch references on the same inputs:
-the tcgen05 bf16x3 GEMM in its three operand arrangements (forward / input gradient / weight gradient), im2col /
+the wgmma bf16x3 GEMM in its three operand arrangements (forward / input gradient / weight gradient), im2col /
 col2im / flatten permutes, and a full ``FusedStack`` forward + backward vs torch autograd (fp32, tolerance stated)."""
 import numpy as np
 import pytest

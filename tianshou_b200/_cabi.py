@@ -136,7 +136,7 @@ DIAG_LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "libts_
 
 
 def use_diagnostics_library() -> C.CDLL:
-    """Make the process-wide library the DIAGNOSTICS build (phase timeline, tcgen05 self-test); tools/ only."""
+    """Make the process-wide library the DIAGNOSTICS build (phase timeline, wgmma self-test); tools/ only."""
     global _lib
     if not os.path.exists(DIAG_LIB_PATH):
         raise ExtensionMissingError(f"{DIAG_LIB_PATH} not found: build it with `python -m tianshou_b200.csrc.build --diag`")
@@ -165,7 +165,7 @@ def load_library(path: str | None = None) -> C.CDLL:
     if not os.path.exists(p):
         raise ExtensionMissingError(
             f"{p} not found: build it with `python -m tianshou_b200.csrc.build` "
-            "(nvcc, sm_100a).  tianshou_b200 has no CPU fallback."
+            "(nvcc, sm_90a).  tianshou_b200 has no CPU fallback."
         )
     lib = C.CDLL(p)
     for name, argtypes in SIGNATURES.items():

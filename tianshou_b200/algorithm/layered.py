@@ -1,9 +1,9 @@
 """Actor-critic networks OUTSIDE the fused 17-64-64 kernels' shape envelope, layer by layer on the tensor cores.
 
-``describe_actor_critic`` (flat_params.py) accepts exactly the shapes the persistent tcgen05 / SIMT update kernels were
+``describe_actor_critic`` (flat_params.py) accepts exactly the shapes the persistent tensor-core / SIMT update kernels were
 written for (two-layer 64-wide trunks, obs <= 64).  Everything else that is still a Linear / ReLU | Tanh actor-critic --
 wider or deeper trunks, large observations (Humanoid: 376), the reference's shared-trunk discrete PPO net at other widths
--- runs here: every Linear forward / input gradient / weight gradient is one ``ts_net_gemm`` launch (tcgen05,
+-- runs here: every Linear forward / input gradient / weight gradient is one ``ts_net_gemm`` launch (wgmma,
 fp32-faithful), the PPO / A2C loss between them is ``ts_ppo_rows``, the optimiser ``ts_adam_step`` (global-norm clip + Adam).
 Same public behaviour as the fused path (ppo.py:146-224, a2c.py:115-153); single GPU.
 

@@ -10,7 +10,7 @@ Per ``update(buffer, sample_size)``:
          one D2H of the loss scalar (+ the TD errors for the priority update, as in the reference).
   GPU  : frame-stack index chains (``ts_stack_prev_indices``) -> the first convolution's im2col reads the uint8 frames
          of the buffer's device mirror directly (no stacked observation is ever materialised) -> conv / linear layers
-         as tcgen05 GEMMs (``ts_net_gemm``) for the online and the lagged network -> ``ts_dqn_target`` ->
+         as wgmma GEMMs (``ts_net_gemm``) for the online and the lagged network -> ``ts_dqn_target`` ->
          ``ts_nstep_return`` -> ``ts_dqn_loss`` -> backward GEMMs + col2im -> Adam; target copy = one device memcpy.
 """
 from __future__ import annotations

@@ -10,7 +10,7 @@ Per ``update(buffer, sample_size)``:
   GPU  : row gathers from the buffer's device mirror (or one upload of the sampled rows), target actor + lagged critics
          forward -> ``ts_sac_target`` -> ``ts_nstep_return``; per critic forward / loss / backward (``ts_net_gemm``) + Adam;
          actor forward, critics' input-gradient GEMMs, tanh-Gaussian head backward, actor backward + Adam; Polyak axpy.
-Every Linear layer's forward / input gradient / weight gradient is one tcgen05 GEMM launch (csrc/net_gemm.cu).
+Every Linear layer's forward / input gradient / weight gradient is one wgmma GEMM launch (csrc/net_gemm.cu).
 """
 from __future__ import annotations
 

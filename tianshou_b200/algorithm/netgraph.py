@@ -3,7 +3,7 @@
 A ``FusedStack`` is the kernel-side view of a torch module stack made of ``nn.Linear`` / ``nn.Conv2d`` /
 ``nn.ReLU`` / ``nn.Flatten`` (the reference's ``MLP`` / ``Net`` / ``ContinuousCritic`` / ``DQNet``,
 utils/net/common.py:76-369, utils/net/continuous.py:96-238, env/atari/atari_network.py:60-122): every layer's
-forward, input gradient and weight gradient is ONE ``ts_net_gemm`` launch (tcgen05, fp32-faithful), convolutions
+forward, input gradient and weight gradient is ONE ``ts_net_gemm`` launch (wgmma, fp32-faithful), convolutions
 run as implicit GEMM over im2col rows.  Parameters live in a ``FlatGroup`` (one flat fp32 buffer per optimiser,
 ``nn.Parameter``s are views of it) so Adam and the Polyak update are single kernels and ``state_dict()`` keeps
 working.  There is no autograd graph and no eager-PyTorch path: unsupported layers raise ``UnsupportedModelError``.

@@ -1,4 +1,4 @@
-"""Build libts_b200.so in-tree with nvcc for sm_100a (no torch extension machinery: the library is
+"""Build libts_b200.so in-tree with nvcc for sm_90a (H100; no torch extension machinery: the library is
 a plain C-ABI shared object loaded with ctypes, see tianshou_b200/_cabi.py)."""
 from __future__ import annotations
 
@@ -10,13 +10,14 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 SOURCES = ["capi.cu", "gae.cu", "nstep.cu", "index.cu", "segtree.cu", "mlp.cu", "mlp_tc.cu", "peer.cu", "hostperm.cu", "net_gemm.cu", "net_ops.cu", "ppo_rows.cu",
            "hostperm_simd.cpp"]      # .cpp = host-only, compiled by g++
-DIAG_SOURCES = ["umma_selftest.cu"]       # diagnostics library only (-DTS_B200_DIAGNOSTICS: phase timeline + tcgen05 self-test)
+DIAG_SOURCES = ["umma_selftest.cu"]       # diagnostics library only (-DTS_B200_DIAGNOSTICS: phase timeline + wgmma self-test)
 LIB = os.path.join(os.path.dirname(HERE), "libts_b200.so")
 DIAG_LIB = os.path.join(os.path.dirname(HERE), "libts_b200_diag.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 CXX = os.environ.get("CXX", "g++")
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    *ARCH,
     "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
     "-Xptxas", "-v",
 ]
@@ -31,7 +32,7 @@ def _newer(target: str, deps: list[str]) -> bool:
 
 def build(force: bool = False, verbose: bool = False, diag: bool = False) -> str:
     """Product library (default) or, with ``diag``, the diagnostics build ``libts_b200_diag.so`` (same sources compiled with
-    -DTS_B200_DIAGNOSTICS plus the tcgen05 self-test; used by tools/tc_timeline.py and tools/umma_*probe.py only)."""
+    -DTS_B200_DIAGNOSTICS plus the wgmma self-test; used by tools/tc_timeline.py and tools/umma_probe.py only)."""
     hdrs = [os.path.join(HERE, "common.cuh"), os.path.join(HERE, "..", "..", "include", "ts_b200.h")]
     hdrs += [os.path.join(HERE, f) for f in os.listdir(HERE) if f.endswith((".cuh", ".h"))]
     srcs = [os.path.join(HERE, s) for s in SOURCES + (DIAG_SOURCES if diag else [])]
@@ -64,7 +65,7 @@ def build(force: bool = False, verbose: bool = False, diag: bool = False) -> str
     with ThreadPoolExecutor(max_workers=min(8, len(srcs))) as ex:
         objs = list(ex.map(compile_one, srcs))
     tmp = lib + ".tmp"      # link next to the target and rename: a reader never sees a half-written library
-    cmd = [NVCC, "-shared", "-o", tmp, *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-lcudart", "-lpthread"]
+    cmd = [NVCC, "-shared", "-o", tmp, *objs, *ARCH, "-lcudart", "-lpthread"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         sys.stderr.write(r.stdout + r.stderr)

@@ -29,7 +29,7 @@ int num_sms() {      // of the CURRENT device (the one the caller's stream and t
     const int dev = device_ordinal();
     if (sms[dev] == 0) {
         int n = 0;
-        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;  // B200
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;  // H100 SXM
         sms[dev] = n;
     }
     return sms[dev];

@@ -1,4 +1,4 @@
-// Shared helpers for the ts_b200 kernels (sm_100a only).
+// Shared helpers for the ts_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

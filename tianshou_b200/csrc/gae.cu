@@ -1,4 +1,4 @@
-// GAE as a single-pass segmented reverse scan (decoupled look-back), sm_100a.
+// GAE as a single-pass segmented reverse scan (decoupled look-back), sm_90a.
 //
 // Reference semantics: numba `_gae` (tianshou/algorithm/algorithm_base.py:1085-1140) plus the
 // value-mask / end-flag / return-scaling arithmetic of compute_episodic_return (:704-719) and

@@ -1,4 +1,4 @@
-// Replay-buffer index kernels (bit-exact int64) and row gathers, sm_100a.
+// Replay-buffer index kernels (bit-exact int64) and row gathers, sm_90a.
 //
 // Reference semantics (all under tianshou/data/buffer/):
 //   numba _next_index / _prev_index        manager.py:339-363 / :311-336
@@ -309,7 +309,7 @@ extern "C" int ts_sample_all_indices(const int64_t* offset, int64_t E, const int
     seg_start_kernel<<<1, 1024, 0, st>>>(lengths, E, seg_start, total_out);
     if (tsb::check_launch("ts_sample_all_indices/scan")) return 1;
     if (out_capacity == 0) return 0;
-    const unsigned grid = (unsigned)tsb::imin((int64_t)blocks_for(out_capacity, 256), 148 * 16);
+    const unsigned grid = (unsigned)tsb::imin((int64_t)blocks_for(out_capacity, 256), tsb::num_sms() * 16);
     sample_all_kernel<<<grid, 256, 0, st>>>(offset, E, last_index, lengths, insertion_idx, seg_start, out, out_capacity);
     return tsb::check_launch("ts_sample_all_indices");
 }
@@ -320,7 +320,7 @@ extern "C" int ts_buffer_end_flags(const uint8_t* done, const int64_t* offset,
     TS_REQUIRE(done && offset && last_index && lengths && end_flag_out && E > 0,
                "ts_buffer_end_flags: null pointer");
     cudaStream_t st = tsb::as_stream(stream);
-    end_flags_kernel<<<148 * 4, 256, 0, st>>>(done, offset, last_index, lengths, E, end_flag_out);
+    end_flags_kernel<<<tsb::num_sms() * 4, 256, 0, st>>>(done, offset, last_index, lengths, E, end_flag_out);
     if (tsb::check_launch("ts_buffer_end_flags/copy")) return 1;
     end_flags_mark_kernel<<<blocks_for(E, 256), 256, 0, st>>>(last_index, lengths, E, end_flag_out);
     return tsb::check_launch("ts_buffer_end_flags");
@@ -362,16 +362,16 @@ extern "C" int ts_gather_rows(const void* src, int64_t row_bytes, const int64_t*
     const bool a16 = ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15u) == 0;
     if (row_bytes % 16 == 0 && a16) {
         const int64_t rw = row_bytes / 16;
-        const unsigned grid = (unsigned)tsb::imin((int64_t)blocks_for(n * rw, 256), 148 * 32);
+        const unsigned grid = (unsigned)tsb::imin((int64_t)blocks_for(n * rw, 256), tsb::num_sms() * 32);
         gather_rows_kernel<uint4><<<grid, 256, 0, st>>>(static_cast<const uint4*>(src), rw, idx, n, static_cast<uint4*>(dst));
     } else if (row_bytes % 4 == 0) {
         const int64_t rw = row_bytes / 4;
-        const unsigned grid = (unsigned)tsb::imin((int64_t)blocks_for(n * rw, 256), 148 * 32);
+        const unsigned grid = (unsigned)tsb::imin((int64_t)blocks_for(n * rw, 256), tsb::num_sms() * 32);
         gather_rows_kernel<uint32_t><<<grid, 256, 0, st>>>(static_cast<const uint32_t*>(src), rw, idx, n, static_cast<uint32_t*>(dst));
     } else if (row_bytes == 1) {
         gather_bytes_kernel<<<blocks_for(n, 256), 256, 0, st>>>(static_cast<const uint8_t*>(src), idx, n, static_cast<uint8_t*>(dst));
     } else {
-        const unsigned grid = (unsigned)tsb::imin((int64_t)blocks_for(n * row_bytes, 256), 148 * 32);
+        const unsigned grid = (unsigned)tsb::imin((int64_t)blocks_for(n * row_bytes, 256), tsb::num_sms() * 32);
         gather_rows_kernel<uint8_t><<<grid, 256, 0, st>>>(static_cast<const uint8_t*>(src), row_bytes, idx, n, static_cast<uint8_t*>(dst));
     }
     return tsb::check_launch("ts_gather_rows");
@@ -385,14 +385,14 @@ extern "C" int ts_scatter_rows(const void* src, int64_t row_bytes, const int64_t
     const bool a16 = ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15u) == 0;
     if (row_bytes % 16 == 0 && a16) {
         const int64_t rw = row_bytes / 16;
-        const unsigned grid = (unsigned)tsb::imin((int64_t)blocks_for(n * rw, 256), 148 * 32);
+        const unsigned grid = (unsigned)tsb::imin((int64_t)blocks_for(n * rw, 256), tsb::num_sms() * 32);
         scatter_rows_kernel<uint4><<<grid, 256, 0, st>>>(static_cast<const uint4*>(src), rw, idx, n, static_cast<uint4*>(dst));
     } else if (row_bytes % 4 == 0 && (((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 3u) == 0)) {
         const int64_t rw = row_bytes / 4;
-        const unsigned grid = (unsigned)tsb::imin((int64_t)blocks_for(n * rw, 256), 148 * 32);
+        const unsigned grid = (unsigned)tsb::imin((int64_t)blocks_for(n * rw, 256), tsb::num_sms() * 32);
         scatter_rows_kernel<uint32_t><<<grid, 256, 0, st>>>(static_cast<const uint32_t*>(src), rw, idx, n, static_cast<uint32_t*>(dst));
     } else {
-        const unsigned grid = (unsigned)tsb::imin((int64_t)blocks_for(n * row_bytes, 256), 148 * 32);
+        const unsigned grid = (unsigned)tsb::imin((int64_t)blocks_for(n * row_bytes, 256), tsb::num_sms() * 32);
         scatter_rows_kernel<uint8_t><<<grid, 256, 0, st>>>(static_cast<const uint8_t*>(src), row_bytes, idx, n, static_cast<uint8_t*>(dst));
     }
     return tsb::check_launch("ts_scatter_rows");

@@ -1,4 +1,4 @@
-// Actor-critic MLP kernels for the PPO update, fp32 SIMT baseline path (sm_100a).
+// Actor-critic MLP kernels for the PPO update, fp32 SIMT baseline path (sm_90a).
 //
 // Network (examples/mujoco/mujoco_ppo.py:90-120): actor  obs -> 64 -> 64 -(tanh)-> mu[act] with a
 // state-independent log-sigma, critic obs -> 64 -> 64 -(tanh)-> 1; torch layouts ([out][in]).
@@ -955,7 +955,7 @@ extern "C" int ts_ppo_grad(const float* params, const ts_actor_critic_desc* desc
         *n_partials_out = (int32_t)tsb::imin(tiles_, tsb::num_sms());
     }
     TS_REQUIRE(!hp->advantage_normalization || adv_moments, "ts_ppo_grad: advantage_normalization needs adv_moments");
-    if (tsb::tc_supported(*desc) && !tsb::simt_forced())   // tcgen05 path (mlp_tc.cu); SIMT covers obs_dim > 32
+    if (tsb::tc_supported(*desc) && !tsb::simt_forced())   // tensor-core path (mlp_tc.cu); SIMT covers obs_dim > 32
         return tsb::launch_ppo_grad_tc(params, *desc, *hp, obs, act, adv, ret, logp_old, v_s, perm, lo, hi,
                                        global_rows, adv_moments, partials, tsb::as_stream(stream));
     const size_t smem = smem_bytes(*desc, 2);

@@ -1,48 +1,42 @@
-// Actor-critic MLP kernels on the 5th-generation tensor cores (tcgen05 + TMEM), sm_100a.
+// Actor-critic MLP kernels on the Hopper tensor cores (wgmma), sm_90a.
 //
 // Same contract as the SIMT kernels in mlp.cu (ts_ppo_grad / ts_critic_forward / ts_actor_logp);
 // reference code replaced: modelfree/ppo.py:157-161,179-211, modelfree/a2c.py:123-126,
 // algorithm_base.py:497.
 //
 // Numerics: every GEMM is an fp32-faithful product built from bf16 tensor-core MMAs with fp32
-// accumulation in TMEM: each operand element x is stored as three bf16 pieces b0 + b1 + b2 = x
-// (24 significant bits) and the six partial products of weight >= 2^-16 are accumulated
-// (umma::gemm_bf16x3).  A single-pass bf16/tf32 MMA would be 6x / 3x cheaper but is ~1e-3 off
+// accumulation: each operand element x is stored as three bf16 pieces b0 + b1 + b2 = x (24
+// significant bits) and the six partial products of weight >= 2^-16 are accumulated
+// (wg::gemm_bf16x3).  A single-pass bf16/tf32 MMA would be 6x / 3x cheaper but is ~1e-3 off
 // the reference's fp32 results, which breaks the 1e-5 parity bar on v_s / returns / advantages.
 //
-// Layout: one CTA = one tile of 128 transitions = the 128 TMEM lanes.  Every operand matrix
-// (activations X, H1, H2, gradients, weights) lives in shared memory in the blocked no-swizzle
-// layout of umma.cuh (8-row x 16-byte core matrices), ONE copy per matrix: the same bytes are
-// consumed K-major by the forward / input-gradient GEMMs and MN-major (reduction over the 128
-// rows) by the weight-gradient GEMMs.  Activations never leave the SM between forward and backward:
+// Layout: one CTA = one tile of 128 transitions, 512 threads = four warpgroups.  Every operand
+// matrix (activations X, H1, H2, gradients, weights) lives in shared memory in the blocked
+// no-swizzle layout of wgmma.cuh (8-row x 16-byte core matrices), ONE copy per matrix: the same
+// bytes are consumed K-major by the forward / input-gradient GEMMs and MN-major (reduction over
+// the 128 rows) by the weight-gradient GEMMs.  Activations never leave the SM between forward and backward:
 //   X -(W1)-> D1 -tanh-> H1 -(W2)-> D2 -tanh-> H2 -(W3)-> D3 -> loss -> dOut
 //   dW3 = H2^T dOut ; dZ2 = (dOut W3) (1-H2^2) [overwrites H2] ; dW2 = dZ2^T H1 ; db2 = dZ2^T 1 ;
 //   dH1 = dZ2 W2 ; dZ1 = dH1 (1-H1^2) [overwrites H1] ; dW1 = dZ1^T X ; db1 = dZ1^T 1
 // Bias gradients come out of the tensor core too (B operand = a 128 x 8 block of ones).
-// MMAs are issued by one thread, completion is signalled through an mbarrier (tcgen05.commit);
-// the 8 warps do the TMEM -> register epilogues (tanh, loss, splits) and the gradient REDs.
+// A 128 x 64 layer product is split over the warpgroups (warpgroup g: rows 64 (g & 1) .., columns
+// 32 (g >> 1) ..); its register accumulator feeds the thread's epilogue (tanh, loss, bf16x3 split)
+// directly, and h1 / h2 stay in the same registers for the backward pass.
 #include <cuda_bf16.h>
 #include <math.h>
 
 #include "common.cuh"
 #include "ppo_math.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace {
 
 constexpr int H = 64;
 constexpr int kRows = 128;
-constexpr int kThreads = 512;        // 16 warps: 4 per TMEM sub-partition, 16 accumulator columns per thread
-constexpr int kCols = 16;            // columns of a 64-wide layer owned by one thread in the epilogues
+constexpr int kThreads = 512;        // four warpgroups
+constexpr int kCols = 16;            // accumulator elements of a 128 x 64 layer held by one thread (64 x 32 per warpgroup)
 constexpr int kMaxAct = 16;
 constexpr int NO = 16;            // padded head width (N of the head GEMM, columns of dOut)
-
-// TMEM column map (fp32 accumulators)
-// dW2 / dW1 carry one extra 8-column block: the bias gradient (B operand extended by a block of ones)
-constexpr uint32_t cD1 = 0, cD2 = 64, cD3 = 128, cDH1 = 192, cDW2 = 256 /* 72 */, cDW3 = 328 /* 16 */, cDW1 = 344 /* <= 40 */;
-// TS-mode A operand (bf16x3 pieces of the CURRENT activation / gradient tile: H1, then H2, then dZ2), 3 x 32 packed columns
-constexpr uint32_t cT = 384, kTPart = 32;
-constexpr uint32_t kTmemCols = 512;
 
 // Optional phase timeline (DIAGNOSTICS build only, -DTS_B200_DIAGNOSTICS -> libts_b200_diag.so): when enabled, one CTA /
 // thread 0 stores %globaltimer at each phase boundary; read back with ts_tc_timeline().  Compiled out of the product library.
@@ -95,25 +89,21 @@ __device__ __forceinline__ void store_chunk8(uint8_t* sm0, const Mat& m, uint32_
     *reinterpret_cast<uint4*>(p + 2 * m.part) = make_uint4(w2[0], w2[1], w2[2], w2[3]);
 }
 
-// 16 consecutive columns [c0, c0 + 16) of row r: bf16x3 split once, stored to the shared-memory operand (consumed
-// MN-major by the weight-gradient GEMMs) AND to the thread's TMEM lane (A operand of the next TS-mode GEMM:
-// packed columns t_col + c0 / 2 of each piece).  t_lane_col = 0xffffffff: shared memory only.
-__device__ __forceinline__ void store_row16(uint8_t* sm0, const Mat& m, uint32_t r, uint32_t c0, const float* v,
-                                            uint32_t t_lane_col) {
-    uint32_t w0[8], w1[8], w2[8];
+// Layer tiles: warpgroup g = tid / 128 computes rows [64 (g & 1), + 64) x columns [32 (g >> 1), + 32) of a 128 x 64
+// product; element e of the thread's accumulator is (lay_row0() + wg::frag_row(e), lay_col0() + wg::frag_col(e)).
+__device__ __forceinline__ int lay_row0() { return 64 * ((threadIdx.x >> 7) & 1); }
+__device__ __forceinline__ int lay_col0() { return 32 * (threadIdx.x >> 8); }
+
+// the thread's 16 layer elements -> bf16x3 operand M (two consecutive columns per 32-bit store)
+__device__ __forceinline__ void store_frag(uint8_t* sm0, const Mat& m, const float (&v)[kCols]) {
 #pragma unroll
-    for (int j = 0; j < 8; ++j) split3_pair(v[2 * j], v[2 * j + 1], w0[j], w1[j], w2[j]);
-#pragma unroll
-    for (int hlf = 0; hlf < 2; ++hlf) {
-        uint8_t* p = sm0 + (m.base + moff(r, c0 + 8 * hlf, m.RS));
-        *reinterpret_cast<uint4*>(p) = make_uint4(w0[4 * hlf], w0[4 * hlf + 1], w0[4 * hlf + 2], w0[4 * hlf + 3]);
-        *reinterpret_cast<uint4*>(p + m.part) = make_uint4(w1[4 * hlf], w1[4 * hlf + 1], w1[4 * hlf + 2], w1[4 * hlf + 3]);
-        *reinterpret_cast<uint4*>(p + 2 * m.part) = make_uint4(w2[4 * hlf], w2[4 * hlf + 1], w2[4 * hlf + 2], w2[4 * hlf + 3]);
-    }
-    if (t_lane_col != 0xffffffffu) {
-        umma::tmem_st8(t_lane_col + (c0 >> 1), w0);
-        umma::tmem_st8(t_lane_col + (c0 >> 1) + kTPart, w1);
-        umma::tmem_st8(t_lane_col + (c0 >> 1) + 2 * kTPart, w2);
+    for (int e = 0; e < kCols; e += 2) {
+        uint32_t w0, w1, w2;
+        split3_pair(v[e], v[e + 1], w0, w1, w2);
+        uint8_t* p = sm0 + (m.base + moff((uint32_t)(lay_row0() + wg::frag_row(e)), (uint32_t)(lay_col0() + wg::frag_col(e)), m.RS));
+        *reinterpret_cast<uint32_t*>(p) = w0;
+        *reinterpret_cast<uint32_t*>(p + m.part) = w1;
+        *reinterpret_cast<uint32_t*>(p + 2 * m.part) = w2;
     }
 }
 
@@ -126,14 +116,17 @@ __device__ __forceinline__ float tanh_mufu(float x) {
     return fmaf(-2.0f, r, 1.0f);
 }
 
-// D[M x N] = A * B (operand usage K-major / MN-major per flag).  WARP-LEVEL: call from all lanes of
-// one warp; K = 16 * KSTEPS.
-template <int KSTEPS, bool FULL = true>
-__device__ __forceinline__ void gemm(uint32_t d_tmem, int M, int N, const Mat& A, int a_mn, const Mat& B, int b_mn) {
-    const uint32_t a_lbo = a_mn ? A.RS : 128u, a_sbo = a_mn ? 128u : A.RS, a_step = a_mn ? 2u * A.RS : 256u;
-    const uint32_t b_lbo = b_mn ? B.RS : 128u, b_sbo = b_mn ? 128u : B.RS, b_step = b_mn ? 2u * B.RS : 256u;
-    umma::gemm_bf16x3_warp<KSTEPS, 3, 3, FULL>(d_tmem, A.base, A.part, a_lbo, a_sbo, a_step, B.base, B.part, b_lbo, b_sbo, b_step,
-                                               umma::idesc_bf16(M, N, a_mn, b_mn));
+// D[64 x N] (the calling warpgroup's tile) = A * B with fp32-faithful bf16x3 MMAs, K = 16 * KSTEPS.  TA / TB = 1: the
+// operand is used MN-major.  a_mn0 / b_mn0: first M / N index of the tile within A / B.  Runs to completion.
+template <int N, int KSTEPS, int TA, int TB, bool FULL = true>
+__device__ __forceinline__ void wg_gemm(float (&d)[N / 2], const Mat& A, uint32_t a_mn0, const Mat& B, uint32_t b_mn0) {
+    const uint32_t a_lbo = TA ? A.RS : 128u, a_sbo = TA ? 128u : A.RS, a_step = TA ? 2u * A.RS : 256u;
+    const uint32_t b_lbo = TB ? B.RS : 128u, b_sbo = TB ? 128u : B.RS, b_step = TB ? 2u * B.RS : 256u;
+    wg::fence();
+    wg::gemm_bf16x3<N, KSTEPS, TA, TB, FULL>(d, A.base + (a_mn0 >> 3) * a_sbo, A.part, a_lbo, a_sbo, a_step,
+                                             B.base + (b_mn0 >> 3) * b_sbo, B.part, b_lbo, b_sbo, b_step, false);
+    wg::commit();
+    wg::wait<0>();
 }
 // weight-gradient GEMMs: three-product scheme unless TS_B200_WGRAD_FULL is defined at build time
 #ifdef TS_B200_WGRAD_FULL
@@ -141,20 +134,15 @@ constexpr bool kWgradFull = true;
 #else
 constexpr bool kWgradFull = false;
 #endif
-// TS mode: A = the bf16x3 pieces at TMEM columns cT (written by the preceding epilogue), M = 128, K = 64
-__device__ __forceinline__ void gemm_ts(uint32_t tmem, uint32_t d_col, int N, const Mat& B, int b_mn) {
-    const uint32_t b_lbo = b_mn ? B.RS : 128u, b_sbo = b_mn ? 128u : B.RS, b_step = b_mn ? 2u * B.RS : 256u;
-    umma::gemm_bf16x3_ts_warp<H / 16>(tmem + d_col, tmem + cT, kTPart, B.base, B.part, b_lbo, b_sbo, b_step,
-                                      umma::idesc_bf16(128, N, 0, b_mn));
-}
-// runtime K in {16, 32} (padded observation width)
-__device__ __forceinline__ void gemm_kx(uint32_t d_tmem, int M, int N, const Mat& A, int a_mn, const Mat& B, int b_mn, int K) {
-    if (K == 16) gemm<1>(d_tmem, M, N, A, a_mn, B, b_mn); else gemm<2>(d_tmem, M, N, A, a_mn, B, b_mn);
+// all threads: shared-memory operand writes become visible to the tensor core and to every thread
+__device__ __forceinline__ void publish() {
+    wg::fence_async_smem();
+    __syncthreads();
 }
 struct Smem {   // byte offsets from the dynamic shared memory base (all multiples of 128)
     int KXP;
     Mat X, H1, H2, DO, W1, W2, W3;
-    uint32_t w3f, b1, b2, b3, ls, dof, rowv, red, act;
+    uint32_t w3f, b1, b2, b3, ls, dof, d3, rowv, red, act;
     uint32_t wblk, wblk_bytes;   // the "weight block" W1 | W2 | W3 | w3f | b1 | b2 | b3 | ls: one contiguous range, the unit
                                  // of the pre-split weight image in global memory (one bulk copy per network)
     uint32_t total;
@@ -183,6 +171,7 @@ __host__ __device__ inline Smem make_smem(int obs_dim, uint32_t sbase) {
     s.ls = o;   o += kMaxAct * 4;
     s.wblk_bytes = o - s.wblk;             // multiple of 128
     s.dof = o;  o += kRows * kMaxAct * 4;  // dOut in fp32 [a][r] (rows on consecutive banks)
+    s.d3 = o;   o += kRows * NO * 4;       // head GEMM output (without bias) in fp32 [a][r]
     s.act = o;  o += kRows * kMaxAct * 4;  // actions of the tile
     s.rowv = o; o += 4 * kRows * 4;        // adv, ret, logp_old, v_s
     s.red = o;  o += 256 * 4;              // [0,12) per-warp sums, [64,80) 1/var, [80,96) log sigma + log sqrt(2 pi),
@@ -324,86 +313,32 @@ __global__ void weight_image_build_kernel(const float* __restrict__ params, cons
         img_scatter(d, S, 0u, i, params[i], wimg);
 }
 
-struct Pipe {   // MMA issue / completion handshake
-    uint64_t* bar;
-    uint32_t phase;
-    // all threads: make smem writes + tcgen05.ld's visible; then WARP 0 (all lanes, warp-uniform
-    // control flow) runs `f`, whose MMAs are issued by one elected lane, and commits.
-    template <class F>
-    __device__ __forceinline__ void issue(F&& f) {
-        umma::tmem_wait_st();
-        umma::fence_async_smem();
-        umma::fence_before_sync();
-        __syncthreads();
-        const int warp_u = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
-        if (warp_u == 0) {
-            umma::fence_after_sync();
-            f();
-            if (umma::elect_one()) umma::mma_commit(bar);
-            __syncwarp();
-        }
-    }
-    // all threads: the MMAs of the last issue() have completed (work that does not touch their operands or
-    // accumulators may run between issue() and wait())
-    __device__ __forceinline__ void wait() {
-        umma::mbar_wait(bar, phase);
-        phase ^= 1u;
-        umma::fence_after_sync();
-    }
-    template <class F>
-    __device__ __forceinline__ void run(F&& f) { issue(f); wait(); }
-};
-
-// Epilogue thread map: warp w -> TMEM sub-partition q = w & 3 (rows 32q + lane), column group
-// cq = w >> 2 -> columns [16 cq, 16 cq + 16) of a 64-wide accumulator.
-// TMEM -> h = tanh(x + bias) -> bf16x3 rows of OUT; h stays in registers for the backward pass
-__device__ __forceinline__ void epi_tanh(uint8_t* sm0, const Mat& OUT, uint32_t tmem, uint32_t col,
-                                         const float* __restrict__ bias, float (&h)[kCols]) {
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t r = 32u * (warp & 3) + lane, c0 = (uint32_t)kCols * (warp >> 2);
-    umma::tmem_ld16(tmem + ((32u * (warp & 3)) << 16) + col + c0, h);
+// h = tanh(acc + bias) -> bf16x3 operand OUT; h stays in registers for the backward pass
+__device__ __forceinline__ void epi_tanh(uint8_t* sm0, const Mat& OUT, const float (&acc)[kCols], const float* __restrict__ bias,
+                                         float (&h)[kCols]) {
 #pragma unroll
-    for (int j = 0; j < kCols; ++j) h[j] = tanh_mufu(h[j] + bias[c0 + j]);
-    store_row16(sm0, OUT, r, c0, h, tmem + ((32u * (warp & 3)) << 16) + cT);
+    for (int e = 0; e < kCols; ++e) h[e] = tanh_mufu(acc[e] + bias[lay_col0() + wg::frag_col(e)]);
+    store_frag(sm0, OUT, h);
 }
-// TMEM dH -> dZ = dH * (1 - h^2) written over ACT (h from registers)
-__device__ __forceinline__ void epi_dtanh(uint8_t* sm0, const Mat& ACT, uint32_t tmem, uint32_t col,
-                                          const float (&h)[kCols]) {
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t r = 32u * (warp & 3) + lane, c0 = (uint32_t)kCols * (warp >> 2);
-    float v[kCols];
-    umma::tmem_ld16(tmem + ((32u * (warp & 3)) << 16) + col + c0, v);
+// dZ2 = (dOut W3) * (1 - H2^2) for the thread's layer elements (K = out_dim is tiny: SIMT)
+__device__ __forceinline__ void head_input_grad(uint8_t* sm, const Smem& S, int out_dim, const float (&h)[kCols],
+                                                float (&acc)[kCols]) {
+    const int r0 = lay_row0() + wg::frag_row(0);        // rows r0 (elements 4 i, 4 i + 1) and r0 + 8 (4 i + 2, 4 i + 3)
+    const float* dof = reinterpret_cast<const float*>(sm + S.dof);
+    const float* w3f = reinterpret_cast<const float*>(sm + S.w3f) + lay_col0();
 #pragma unroll
-    for (int j = 0; j < kCols; ++j) v[j] = v[j] * fmaf(-h[j], h[j], 1.0f);
-    store_chunk8(sm0, ACT, r, c0, v);
-    store_chunk8(sm0, ACT, r, c0 + 8, v + 8);
-}
-// dZ2 = (dOut W3) * (1 - H2^2) (K = out_dim is tiny: SIMT).  Split in two so that the arithmetic overlaps the dW3 MMA
-// that is still reading H2: compute into registers, then (after the MMA completed) store over H2 and into TMEM.
-__device__ __forceinline__ void head_input_grad_compute(uint8_t* sm, const Smem& S, int out_dim, const float (&h)[kCols],
-                                                        float (&acc)[kCols]) {
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t r = 32u * (warp & 3) + lane, c0 = (uint32_t)kCols * (warp >> 2);
-    const float* dof = reinterpret_cast<const float*>(sm + S.dof) + r;
-    const float* w3f = reinterpret_cast<const float*>(sm + S.w3f);
-#pragma unroll
-    for (int j = 0; j < kCols; ++j) acc[j] = 0.0f;
+    for (int e = 0; e < kCols; ++e) acc[e] = 0.0f;
     for (int a = 0; a < out_dim; ++a) {
-        const float dv = dof[a * kRows];
+        const float d0 = dof[a * kRows + r0], d1 = dof[a * kRows + r0 + 8];
 #pragma unroll
-        for (int j = 0; j < kCols; j += 4) {
-            const float4 w = *reinterpret_cast<const float4*>(w3f + a * H + c0 + j);
-            acc[j] = fmaf(dv, w.x, acc[j]); acc[j + 1] = fmaf(dv, w.y, acc[j + 1]);
-            acc[j + 2] = fmaf(dv, w.z, acc[j + 2]); acc[j + 3] = fmaf(dv, w.w, acc[j + 3]);
+        for (int i = 0; i < kCols / 4; ++i) {
+            const float2 w = *reinterpret_cast<const float2*>(w3f + a * H + wg::frag_col(4 * i));
+            acc[4 * i] = fmaf(d0, w.x, acc[4 * i]); acc[4 * i + 1] = fmaf(d0, w.y, acc[4 * i + 1]);
+            acc[4 * i + 2] = fmaf(d1, w.x, acc[4 * i + 2]); acc[4 * i + 3] = fmaf(d1, w.y, acc[4 * i + 3]);
         }
     }
 #pragma unroll
-    for (int j = 0; j < kCols; ++j) acc[j] = acc[j] * fmaf(-h[j], h[j], 1.0f);
-}
-__device__ __forceinline__ void head_input_grad_store(uint8_t* sm0, const Smem& S, uint32_t tmem, const float (&acc)[kCols]) {
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t r = 32u * (warp & 3) + lane, c0 = (uint32_t)kCols * (warp >> 2);
-    store_row16(sm0, S.H2, r, c0, acc, tmem + ((32u * (warp & 3)) << 16) + cT);
+    for (int e = 0; e < kCols; ++e) acc[e] = acc[e] * fmaf(-h[e], h[e], 1.0f);
 }
 // write one row of dOut: fp32 side copy + bf16x3 operand (columns >= out_dim are zero)
 __device__ __forceinline__ void write_dout_row(uint8_t* sm, uint8_t* sm0, const Smem& S, uint32_t r, const float* dv) {
@@ -417,44 +352,36 @@ __device__ __forceinline__ void write_dout_row(uint8_t* sm, uint8_t* sm0, const 
 // The partial row is private to the CTA: the first tile of a CTA stores, later tiles read-modify-write.
 __device__ __forceinline__ void out_acc(float* p, float v, bool first) { *p = first ? v : *p + v; }
 
-// Weight-gradient accumulators (TMEM, M = 64: row o = 16 q + lane for lane < 16) -> the CTA's partial
-// gradient row.  A lane owns a ROW of an accumulator, so direct stores would touch one 32-byte sector
-// per value (measured: 4-8 us per net).  The tile is transposed through shared memory instead (the H2
-// operand is dead by then; padded leading dimensions keep both sides bank-conflict free) and
-// written out with consecutive threads on consecutive addresses.
+// Weight-gradient accumulators (M = 64: row o of the accumulator = output feature o) -> the CTA's partial gradient row.
+// A thread owns scattered elements of an accumulator, so they are transposed through shared memory (the H2 operand is
+// dead by then; padded leading dimensions keep the reads bank-conflict free) and written out with consecutive threads
+// on consecutive addresses.
 constexpr int kLdW2 = H + 1, kLdW1 = 33, kScrW2 = 0, kScrW1 = kScrW2 + H * kLdW2, kScrW3 = kScrW1 + H * kLdW1,
               kScrB1 = kScrW3 + NO * kLdW2, kScrB2 = kScrB1 + H, kScrEnd = kScrB2 + H;
 static_assert(kScrEnd * 4 <= 3 * kRows * H * 2, "gradient scratch must fit in the H2 operand");
-// PART 0: dW2, db2, dW3 (complete after the dW2 / dH1 stage: runs while the dW1 MMA is in flight); PART 1: dW1, db1.
+__device__ __forceinline__ float* grad_scratch(uint8_t* sm0, const Smem& S) { return reinterpret_cast<float*>(sm0 + S.H2.base); }
+
+// [dW1 | db1] = dZ1^T [X | 1] (one warpgroup, N = KXP + 8 columns) -> scratch
+template <int N>
+__device__ __forceinline__ void wgrad_w1(uint8_t* sm0, const Smem& S) {
+    float d[N / 2];
+    wg_gemm<N, kRows / 16, 1, 1, kWgradFull>(d, S.H1, 0u, S.X, 0u);
+    float* scr = grad_scratch(sm0, S);
+#pragma unroll
+    for (int e = 0; e < N / 2; ++e) {
+        const int o = wg::frag_row(e), c = wg::frag_col(e);
+        if (c < S.KXP) scr[kScrW1 + o * kLdW1 + c] = d[e];
+        else if (c == S.KXP) scr[kScrB1 + o] = d[e];          // the ones column
+    }
+}
+
+// PART 0: dW2, db2, dW3 (in scratch after the dW2 / dH1 stage: written out while the dW1 MMA runs); PART 1: dW1, db1.
 template <int PART>
-__device__ __forceinline__ void grad_out(uint8_t* sm0, const Smem& S, uint32_t tmem, const NetG& g, int obs_dim, int out_dim,
+__device__ __forceinline__ void grad_out(uint8_t* sm0, const Smem& S, const NetG& g, int obs_dim, int out_dim,
                                          float* __restrict__ grad, bool first) {
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int q = warp & 3, cq = warp >> 2;
-    float* scr = reinterpret_cast<float*>(sm0 + S.H2.base);       // H2 (dZ2) is dead after the dW2 / dH1 stage
-    const uint32_t t0 = tmem + ((32u * q) << 16);
-    const int o = 16 * q + lane;
-    float v[8];
+    const float* scr = grad_scratch(sm0, S);
     if (PART == 0) {
-#pragma unroll
-        for (int c0 = 0; c0 < H; c0 += 32) {                  // dW2 [o][i]
-            umma::tmem_ld8(t0 + cDW2 + c0 + 8 * cq, v);
-            if (lane < 16) {
-#pragma unroll
-                for (int j = 0; j < 8; ++j) scr[kScrW2 + o * kLdW2 + c0 + 8 * cq + j] = v[j];
-            }
-        }
-        if (cq < NO / 8) {                                     // dW3^T [k][a] -> [a][k]
-            umma::tmem_ld8(t0 + cDW3 + 8 * cq, v);
-            if (lane < 16) {
-#pragma unroll
-                for (int j = 0; j < 8; ++j) scr[kScrW3 + (8 * cq + j) * kLdW2 + o] = v[j];
-            }
-        } else if (cq == 2) {                                  // db2: the ones column of [dW2 | db2]
-            umma::tmem_ld8(t0 + cDW2 + (uint32_t)H, v);
-            if (lane < 16) scr[kScrB2 + o] = v[0];
-        }
-        __syncthreads();
 #pragma unroll
         for (int u = 0; u < H * H / kThreads; ++u) {
             const int e = tid + u * kThreads;
@@ -466,18 +393,6 @@ __device__ __forceinline__ void grad_out(uint8_t* sm0, const Smem& S, uint32_t t
         }
         if (tid < H) out_acc(grad + g.b2 + tid, scr[kScrB2 + tid], first);
     } else {
-        if (8 * cq < S.KXP) {                                  // dW1 [o][i]   (warp-uniform)
-            umma::tmem_ld8(t0 + cDW1 + 8 * cq, v);
-            if (lane < 16) {
-#pragma unroll
-                for (int j = 0; j < 8; ++j) scr[kScrW1 + o * kLdW1 + 8 * cq + j] = v[j];
-            }
-        }
-        if (cq == 3) {                                         // db1: the ones column of [dW1 | db1]
-            umma::tmem_ld8(t0 + cDW1 + (uint32_t)S.KXP, v);
-            if (lane < 16) scr[kScrB1 + o] = v[0];
-        }
-        __syncthreads();
         if (lane < obs_dim) {
 #pragma unroll
             for (int r = warp; r < H; r += kThreads / 32)
@@ -503,46 +418,75 @@ __device__ __forceinline__ float warp_transpose_sum32(float (&v)[32]) {
     return v[0];
 }
 
-// forward of one trunk: X -> H1 -> H2 -> head accumulator D3 (TMEM); h1 / h2 of the thread's
-// (row, 16 columns) stay in registers
-__device__ __forceinline__ void trunk_forward(uint8_t* sm, uint8_t* sm0, const Smem& S, uint32_t tmem, Pipe& pipe,
-                                              float (&h1)[kCols], float (&h2)[kCols]) {
-    pipe.run([&] { gemm_kx(tmem + cD1, 128, H, S.X, 0, S.W1, 0, S.KXP); });
-    epi_tanh(sm0, S.H1, tmem, cD1, reinterpret_cast<const float*>(sm + S.b1), h1);
-    pipe.run([&] { gemm_ts(tmem, cD2, H, S.W2, 0); });                                 // A = H1 from TMEM
-    epi_tanh(sm0, S.H2, tmem, cD2, reinterpret_cast<const float*>(sm + S.b2), h2);
-    pipe.run([&] { gemm_ts(tmem, cD3, NO, S.W3, 0); });                                // A = H2 from TMEM
+// forward of one trunk: X -> H1 -> H2 -> head D3 (fp32 [a][r] in shared memory, without bias); h1 / h2 of the thread's
+// layer elements stay in registers
+__device__ __forceinline__ void trunk_forward(uint8_t* sm, uint8_t* sm0, const Smem& S, float (&h1)[kCols], float (&h2)[kCols]) {
+    float acc[kCols];
+    publish();
+    if (S.KXP == 16) wg_gemm<2 * kCols, 1, 0, 0>(acc, S.X, lay_row0(), S.W1, lay_col0());
+    else wg_gemm<2 * kCols, 2, 0, 0>(acc, S.X, lay_row0(), S.W1, lay_col0());
+    epi_tanh(sm0, S.H1, acc, reinterpret_cast<const float*>(sm + S.b1), h1);
+    publish();
+    wg_gemm<2 * kCols, H / 16, 0, 0>(acc, S.H1, lay_row0(), S.W2, lay_col0());
+    epi_tanh(sm0, S.H2, acc, reinterpret_cast<const float*>(sm + S.b2), h2);
+    publish();
+    float d3[4];                                          // head: warpgroup g -> rows 64 (g & 1) .., columns 8 (g >> 1) ..
+    const int c0 = 8 * (threadIdx.x >> 8);
+    wg_gemm<8, H / 16, 0, 0>(d3, S.H2, lay_row0(), S.W3, c0);
+    float* out = reinterpret_cast<float*>(sm + S.d3);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) out[(c0 + wg::frag_col(e)) * kRows + lay_row0() + wg::frag_row(e)] = d3[e];
+    __syncthreads();
 }
 
 // backward of one trunk given dOut (S.DO / dof); writes all weight and bias gradients of the net.
 // `weights_dead()` is called (all threads) once nothing reads the network's weight block any more.
 template <class F>
-__device__ __forceinline__ void trunk_backward(uint8_t* sm, uint8_t* sm0, const Smem& S, uint32_t tmem, Pipe& pipe,
-                                               const NetG& g, int obs_dim, int out_dim, float* __restrict__ grad,
-                                               const float (&h1)[kCols], const float (&h2)[kCols], bool first,
-                                               F&& weights_dead) {
-    pipe.issue([&] { gemm<kRows / 16, kWgradFull>(tmem + cDW3, 64, NO, S.H2, 1, S.DO, 1); });    // dW3^T = H2^T dOut
+__device__ __forceinline__ void trunk_backward(uint8_t* sm, uint8_t* sm0, const Smem& S, const NetG& g, int obs_dim, int out_dim,
+                                               float* __restrict__ grad, const float (&h1)[kCols], const float (&h2)[kCols],
+                                               bool first, F&& weights_dead) {
+    const int wgi = threadIdx.x >> 7;
+    float* scr = grad_scratch(sm0, S);
+    publish();                                                 // dOut (fp32 and operand) complete
     float dz2[kCols];
-    head_input_grad_compute(sm, S, out_dim, h2, dz2);          // overlaps the MMA (reads dof / w3f / registers only)
-    pipe.wait();
+    head_input_grad(sm, S, out_dim, h2, dz2);
+    float dw3[NO / 2];
+    if (wgi == 3) wg_gemm<NO, kRows / 16, 1, 1, kWgradFull>(dw3, S.H2, 0u, S.DO, 0u);        // dW3^T = H2^T dOut
     tstamp(16);
-    head_input_grad_store(sm0, S, tmem, dz2);                  // H2 := dZ2 (the MMA no longer reads H2), T := dZ2
+    __syncthreads();                                           // H2 is no longer read
+    store_frag(sm0, S.H2, dz2);                                // H2 := dZ2
     tstamp(17);
-    pipe.run([&] {
-        gemm<kRows / 16, kWgradFull>(tmem + cDW2, 64, H + 8, S.H2, 1, S.H1, 1);                   // [dW2 | db2] = dZ2^T [H1 | 1]
-        gemm_ts(tmem, cDH1, H, S.W2, 1);                                              // dH1 = dZ2 W2, A = dZ2 from TMEM
-    });
+    publish();
+    float dw2[12], dh1[kCols];
+    if (wgi < 3) wg_gemm<24, kRows / 16, 1, 1, kWgradFull>(dw2, S.H2, 0u, S.H1, 24u * wgi);  // [dW2 | db2] = dZ2^T [H1 | 1]
+    wg_gemm<2 * kCols, H / 16, 0, 1>(dh1, S.H2, lay_row0(), S.W2, lay_col0());              // dH1 = dZ2 W2
+    __syncthreads();                                           // H2 (now scratch), H1 and the weight block are no longer read
     tstamp(18);
     weights_dead();
-    epi_dtanh(sm0, S.H1, tmem, cDH1, h1);                                             // H1 := dZ1
+    if (wgi < 3) {
+#pragma unroll
+        for (int e = 0; e < 12; ++e) {
+            const int o = wg::frag_row(e), c = 24 * wgi + wg::frag_col(e);
+            if (c < H) scr[kScrW2 + o * kLdW2 + c] = dw2[e];
+            else if (c == H) scr[kScrB2 + o] = dw2[e];        // the ones column
+        }
+    } else {
+#pragma unroll
+        for (int e = 0; e < NO / 2; ++e) scr[kScrW3 + wg::frag_col(e) * kLdW2 + wg::frag_row(e)] = dw3[e];   // dW3^T [k][a] -> [a][k]
+    }
+#pragma unroll
+    for (int e = 0; e < kCols; ++e) dh1[e] *= fmaf(-h1[e], h1[e], 1.0f);
+    store_frag(sm0, S.H1, dh1);                                // H1 := dZ1
     tstamp(19);
-    pipe.issue([&] {
-        gemm<kRows / 16, kWgradFull>(tmem + cDW1, 64, S.KXP + 8, S.H1, 1, S.X, 1);                // [dW1 | db1] = dZ1^T [X | 1]
-    });
-    grad_out<0>(sm0, S, tmem, g, obs_dim, out_dim, grad, first);     // dW2 / db2 / dW3 leave while the MMA runs
-    pipe.wait();
+    publish();
+    if (wgi == 0) {
+        if (S.KXP == 16) wgrad_w1<24>(sm0, S);
+        else wgrad_w1<40>(sm0, S);
+    }
+    grad_out<0>(sm0, S, g, obs_dim, out_dim, grad, first);    // dW2 / db2 / dW3 leave while warpgroup 0 runs the dW1 MMAs
+    __syncthreads();
     tstamp(20);
-    grad_out<1>(sm0, S, tmem, g, obs_dim, out_dim, grad, first);
+    grad_out<1>(sm0, S, g, obs_dim, out_dim, grad, first);
 }
 
 __device__ __forceinline__ float warp_sum(float v) {
@@ -655,8 +599,6 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_tc_kernel(
     const float* __restrict__ adv_moments, float* __restrict__ partials, const AdamArgs opt, uint8_t* wimg /* nullable */,
     const tsb::PeerArgs px) {
     extern __shared__ __align__(1024) uint8_t sm[];
-    __shared__ uint32_t s_tmem;
-    __shared__ __align__(8) uint64_t s_bar;
     __shared__ __align__(8) uint64_t s_wbar;
     __shared__ float s_coef, s_norm, s_step_size, s_bc2_sqrt;
     __shared__ int32_t s_row[kRows];
@@ -676,7 +618,7 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_tc_kernel(
         }
     };
     if ((int64_t)blockIdx.x < mb_tiles(0)) prefetch_rows(0, blockIdx.x);
-    const uint32_t sbase = umma::smem_u32(sm);
+    const uint32_t sbase = wg::smem_u32(sm);
     uint8_t* sm0 = sm - sbase;     // so that (sm0 + shared_address) is the generic pointer
     const Smem S = make_smem(d.obs_dim, sbase);
     const int A = d.act_dim;
@@ -685,8 +627,7 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_tc_kernel(
     const int64_t step0 = EPOCH ? *opt.step_count : 0;
     const unsigned int seq0 = (EPOCH && px.world > 1) ? *((volatile unsigned int*)px.hdr) : 0u;
 
-    if (warp == 0) umma::tmem_alloc(&s_tmem, kTmemCols);
-    if (tid == 0) { umma::mbar_init(&s_bar, 1); umma::mbar_init(&s_wbar, 1); umma::fence_mbar_init(); }
+    if (tid == 0) { wg::mbar_init(&s_wbar, 1); wg::fence_mbar_init(); }
     for (int e = tid; e < 2 * 3 * kRows; e += kThreads) {   // the ones chunks of X and H1 (bf16 1.0 = 0x3F80 in piece 0)
         const int r = e % kRows, pc = (e / kRows) % 3;
         const Mat& M = e < 3 * kRows ? S.X : S.H1;
@@ -694,11 +635,7 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_tc_kernel(
         const uint32_t w = pc == 0 ? 0x3F803F80u : 0u;
         *reinterpret_cast<uint4*>(sm0 + (M.base + pc * M.part + moff((uint32_t)r, c, M.RS))) = make_uint4(w, w, w, w);
     }
-    umma::fence_before_sync();
     __syncthreads();
-    umma::fence_after_sync();
-    const uint32_t tmem = s_tmem;
-    Pipe pipe{&s_bar, 0u};
     EpochCtl* ctl = wimg != nullptr ? reinterpret_cast<EpochCtl*>(wimg - kCtlBytes) : &g_ep_ctl;
     GridBarrier gbar{0u, &ctl->arrive};
     // Weight staging.  With a weight image: one bulk copy (TMA engine) per network, issued as early as the
@@ -707,14 +644,14 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_tc_kernel(
     bool critic_issued = false;
     auto issue_weights = [&](int net) {   // every earlier access to the weight block is ordered before this call
         if (wimg != nullptr && tid == 0) {
-            umma::fence_proxy_async_all();
-            umma::mbar_expect_tx(&s_wbar, S.wblk_bytes);
-            umma::bulk_g2s(sbase + S.wblk, wimg + (size_t)net * S.wblk_bytes, S.wblk_bytes, &s_wbar);
+            wg::fence_proxy_async_all();
+            wg::mbar_expect_tx(&s_wbar, S.wblk_bytes);
+            wg::bulk_g2s(sbase + S.wblk, wimg + (size_t)net * S.wblk_bytes, S.wblk_bytes, &s_wbar);
         }
     };
     auto wait_weights = [&](const NetG& g, int out_dim) {
         if (wimg == nullptr) { stage_weights(sm, sm0, S, params, g, d.obs_dim, out_dim); return; }
-        umma::mbar_wait(&s_wbar, wphase);
+        wg::mbar_wait(&s_wbar, wphase);
         wphase ^= 1u;
         if (g.ls >= 0 && tid < kMaxAct) {     // per-dimension constants of the diagonal Gaussian
             float* gs = reinterpret_cast<float*>(sm + S.red) + 64;
@@ -798,16 +735,15 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_tc_kernel(
             critic_issued = false;
             wait_weights(gc, 1);
             tstamp(2);
-            trunk_forward(sm, sm0, S, tmem, pipe, h1, h2);
+            trunk_forward(sm, sm0, S, h1, h2);
             tstamp(3);
             float vf_row = 0.0f;
             if (tid < kRows) {
-                float v16[16], dv[kMaxAct];
-                umma::tmem_ld16(tmem + ((32u * warp) << 16) + cD3, v16);
+                float dv[kMaxAct];
 #pragma unroll
                 for (int a = 0; a < kMaxAct; ++a) dv[a] = 0.0f;
                 if (tid < nrows) {
-                    const float value = v16[0] + reinterpret_cast<const float*>(sm + S.b3)[0];
+                    const float value = reinterpret_cast<const float*>(sm + S.d3)[tid] + reinterpret_cast<const float*>(sm + S.b3)[0];
                     ppo::critic_row(sc, value, rowv[kRows + tid], rowv[3 * kRows + tid], vf_row, dv[0]);
                 }
                 write_dout_row(sm, sm0, S, tid, dv);
@@ -815,7 +751,7 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_tc_kernel(
                 if (lane == 0) red[warp] = sdv;                    // db3 (critic), one slot per warp
             }
             tstamp(4);
-            trunk_backward(sm, sm0, S, tmem, pipe, gc, d.obs_dim, 1, grad, h1, h2, first, [&] { issue_weights(1); });
+            trunk_backward(sm, sm0, S, gc, d.obs_dim, 1, grad, h1, h2, first, [&] { issue_weights(1); });
             tstamp(5);
             __syncthreads();
             if (tid == 0) out_acc(grad + gc.b3, (red[0] + red[1]) + (red[2] + red[3]), first);
@@ -826,7 +762,7 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_tc_kernel(
             // ================= actor =================================================================
             wait_weights(ga, A);
             tstamp(6);
-            trunk_forward(sm, sm0, S, tmem, pipe, h1, h2);
+            trunk_forward(sm, sm0, S, h1, h2);
             tstamp(7);
             // Actor loss epilogue on all 16 warps: thread (row r = 32 q + lane, group cq) owns the actions a = cq + 4 u -- the
             // four groups' log-prob partials meet in shared memory, every thread then evaluates the row's surrogate and writes
@@ -845,7 +781,7 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_tc_kernel(
                     const int a = cq + 4 * u;
                     diff[u] = 0.0f; d2v[u] = 0.0f;
                     if (a < A) {     // warp-uniform
-                        const float mu = umma::tmem_ld1(tmem + ((32u * q) << 16) + cD3 + (uint32_t)a) + b3[a];
+                        const float mu = reinterpret_cast<const float*>(sm + S.d3)[a * kRows + r] + b3[a];
                         diff[u] = actt[a * kRows + r] - mu;
                         d2v[u] = diff[u] * diff[u] * inv_var[a];
                         lpp += fmaf(-0.5f, d2v[u], -logc[a]);      // log N(x; mu, sigma)
@@ -878,7 +814,7 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_tc_kernel(
                 }
             }
             tstamp(8);
-            trunk_backward(sm, sm0, S, tmem, pipe, ga, d.obs_dim, A, grad, h1, h2, first, [] {});
+            trunk_backward(sm, sm0, S, ga, d.obs_dim, A, grad, h1, h2, first, [] {});
             tstamp(9);
 
             // ================= loss sums + small gradients ===========================================
@@ -1017,7 +953,7 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_tc_kernel(
                 adam_elem(i, opt.grad_scratch[i], opt.params_w[i], opt.exp_avg[i], opt.exp_avg_sq[i]);
         }
         tstamp(26);
-        if (wimg != nullptr) umma::fence_proxy_async_all();      // image stores (generic proxy) before the peers' bulk copies
+        if (wimg != nullptr) wg::fence_proxy_async_all();      // image stores (generic proxy) before the peers' bulk copies
         tstamp(14);
         const bool more = m + 1 < n_mb;
         if (more) gbar.arrive();                                    // barrier 3 (updated parameters visible to every CTA) ...
@@ -1041,9 +977,6 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_tc_kernel(
         }
         tstamp(15);
     }
-    umma::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) umma::tmem_dealloc(tmem, kTmemCols);
     if (EPOCH && tid == 0) {
         if (blockIdx.x == 0) {
             *opt.step_count = step0 + n_mb;
@@ -1059,16 +992,11 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_tc_kernel(
 
 
 // ---- forward-only kernels (value pass / log-prob pass), persistent over 128-row tiles -----------
-// TS mode: the activations (X, H1) are the A operand IN TENSOR MEMORY -- the staging / epilogue threads split
-// them to bf16x3 and tcgen05.st them to their own TMEM lane (lane = row), so an MMA reads only the 2 KB weight
-// operand from shared memory and runs at its 32-cycle math floor instead of being paced by 6 KB of operand reads
-// (ncu, SS mode: tensor pipe busy 76 % of the pass).  Two tiles are in flight per CTA (slots 0 / 1: own
-// accumulator and operand columns): the MMAs of one slot run while the 16 warps do the other slot's epilogues, and
-// the next tiles' rows are loaded from global memory one stage ahead of their conversion.
-// TMEM columns of a slot: D (64: layer-1, then layer-2 accumulator) | T (96: X pieces, then H1 pieces).
+// Per tile: X (bf16x3) -> layer 1 -> tanh -> H1 (bf16x3) -> layer 2 -> tanh in registers -> head as SIMT dot products
+// over the thread's columns.  The next tile's rows are loaded from global memory while this tile's MMAs run.
 struct SmemF {
     int KXP;
-    Mat W1, W2;
+    Mat X, H1, W1, W2;
     uint32_t w3f, b1, b2, b3, ls, part;
     uint32_t total;
 };
@@ -1079,6 +1007,8 @@ __host__ __device__ inline SmemF make_smem_f(int obs_dim, uint32_t sbase) {
     auto mat = [&](Mat& m, int rows, int cols) {
         m.base = sbase + o; m.part = mat_bytes(rows, cols); m.RS = (uint32_t)(cols / 8) * 128u; o += 3u * m.part;
     };
+    mat(s.X, kRows, s.KXP);
+    mat(s.H1, kRows, H);
     mat(s.W1, H, s.KXP);
     mat(s.W2, H, H);
     s.w3f = o;  o += kMaxAct * H * 4;
@@ -1086,40 +1016,9 @@ __host__ __device__ inline SmemF make_smem_f(int obs_dim, uint32_t sbase) {
     s.b2 = o;   o += H * 4;
     s.b3 = o;   o += kMaxAct * 4;
     s.ls = o;   o += kMaxAct * 4;
-    s.part = o; o += 4 * kRows * kMaxAct * 4;   // head partial sums of the four column groups
+    s.part = o; o += 2 * kRows * kMaxAct * 4;   // head partial sums of the two column halves [half][a][row]
     s.total = o;
     return s;
-}
-constexpr uint32_t kSlotCols = 160, kSlotD = 0, kSlotT = 64;     // 2 slots -> 320 columns (512 allocated)
-
-// all threads: publish smem / TMEM operands, retire TMEM reads, then warp 0 issues `f` and commits to `bar` (no wait)
-template <class F>
-__device__ __forceinline__ void mma_issue(uint64_t* bar, F&& f) {
-    umma::tmem_wait_st();
-    umma::fence_async_smem();
-    umma::fence_before_sync();
-    __syncthreads();
-    const int warp_u = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
-    if (warp_u == 0) {
-        umma::fence_after_sync();
-        f();
-        if (umma::elect_one()) umma::mma_commit(bar);
-        __syncwarp();
-    }
-}
-__device__ __forceinline__ void mma_wait(uint64_t* bar, uint32_t& phase) {
-    umma::mbar_wait(bar, phase);
-    phase ^= 1u;
-    umma::fence_after_sync();
-}
-// 16 consecutive values of the calling thread's row -> bf16x3 -> 8 packed columns per piece of its TMEM lane
-__device__ __forceinline__ void store_row16_tmem(uint32_t t_lane, uint32_t col0, uint32_t part_cols, const float* v) {
-    uint32_t w0[8], w1[8], w2[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) split3_pair(v[2 * j], v[2 * j + 1], w0[j], w1[j], w2[j]);
-    umma::tmem_st8(t_lane + col0, w0);
-    umma::tmem_st8(t_lane + col0 + part_cols, w1);
-    umma::tmem_st8(t_lane + col0 + 2u * part_cols, w2);
 }
 
 // MODE 0: out0[r] = critic(in0[r]) and (if in1) out1[r] = critic(in1[r])      (a2c.py:123-126)
@@ -1129,22 +1028,13 @@ __global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(
     const float* __restrict__ params, const ts_actor_critic_desc d, const float* __restrict__ in0,
     float* __restrict__ out0, const float* __restrict__ in1, float* __restrict__ out1, int64_t n) {
     extern __shared__ __align__(1024) uint8_t sm[];
-    __shared__ uint32_t s_tmem;
-    __shared__ __align__(8) uint64_t s_bar[2][2];      // [slot][layer]
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int q = warp & 3, cq = warp >> 2;
-    const uint32_t sbase = umma::smem_u32(sm);
+    const int tid = threadIdx.x, lane = tid & 31;
+    const uint32_t sbase = wg::smem_u32(sm);
     uint8_t* sm0 = sm - sbase;
     const SmemF S = make_smem_f(d.obs_dim, sbase);
     const int out_dim = MODE == 0 ? 1 : d.act_dim;
     const NetG g = MODE == 0 ? NetG{d.c_w1, d.c_b1, d.c_w2, d.c_b2, d.c_w3, d.c_b3, -1}
                              : NetG{d.a_w1, d.a_b1, d.a_w2, d.a_b2, d.a_w3, d.a_b3, d.a_logstd};
-    if (warp == 0) umma::tmem_alloc(&s_tmem, 512);
-    if (tid == 0) {
-        umma::mbar_init(&s_bar[0][0], 1); umma::mbar_init(&s_bar[0][1], 1);
-        umma::mbar_init(&s_bar[1][0], 1); umma::mbar_init(&s_bar[1][1], 1);
-        umma::fence_mbar_init();
-    }
     // weights: W1, W2 as tensor-core B operands (shared memory); head weights / biases as fp32
     stage_chunks(sm0, S.W1, H, d.obs_dim, S.KXP, [&](int o) { return params + g.w1 + (int64_t)o * d.obs_dim; });
     stage_chunks(sm0, S.W2, H, H, H, [&](int o) { return params + g.w2 + (int64_t)o * H; });
@@ -1161,13 +1051,6 @@ __global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(
         // sigma_a = exp(logstd_a), once per CTA; the log-prob keeps torch's expression order (normal_logp_term)
         ls[tid] = (MODE == 1 && tid < out_dim) ? expf(__ldg(params + g.ls + tid)) : 1.0f;
     }
-    umma::fence_before_sync();
-    __syncthreads();
-    umma::fence_after_sync();
-    const uint32_t tmem = s_tmem;
-    const uint32_t t_lane = tmem + ((32u * q) << 16);       // this thread's TMEM lane group
-    uint32_t ph[2][2] = {{0u, 0u}, {0u, 0u}};
-    const uint32_t xcols = (uint32_t)S.KXP / 2u;            // packed columns of one X piece (8 or 16)
 
     const int64_t tiles_per = (n + kRows - 1) / kRows;
     const int64_t tiles = tiles_per * ((MODE == 0 && in1) ? 2 : 1);
@@ -1179,102 +1062,65 @@ __global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(
         nrows = (int)tsb::imin((int64_t)kRows, n - row0);
         src = (MODE == 0 && second) ? in1 : in0;
     };
-    // X staging: thread (q, cq, lane) owns row 32 q + lane, columns [16 cq, 16 cq + 16) (warps with 16 cq >= KXP idle)
-    const bool x_owner = 16 * cq < S.KXP;
-    auto x_load = [&](int64_t k, float (&xv)[16]) {
-        if (!x_owner) return;
+    auto x_load = [&](int64_t k, float (&xv)[8]) {     // one (row, 8-column chunk) per thread
         const float* src; int64_t row0; int nrows; bool second;
         tile_src(tile_of(k), src, row0, nrows, second);
-        const int r = 32 * q + lane;
-        const float* row = src + (row0 + r) * d.obs_dim;
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-            const int c = 16 * cq + j;
-            xv[j] = (r < nrows && c < d.obs_dim) ? __ldg(row + c) : 0.0f;
-        }
+        chunk_load(kRows, d.obs_dim, S.KXP, [&](int r) {
+            return r < nrows ? src + (row0 + r) * d.obs_dim : (const float*)nullptr;
+        }, xv);
     };
-    auto x_store = [&](int slot, const float (&xv)[16]) {
-        if (x_owner) store_row16_tmem(t_lane, kSlotCols * slot + kSlotT + 8u * cq, xcols, xv);
-    };
-    auto l1 = [&](int slot) {
-        mma_issue(&s_bar[slot][0], [&] {
-            const uint32_t dcol = tmem + kSlotCols * slot + kSlotD, acol = tmem + kSlotCols * slot + kSlotT;
-            const uint32_t idesc = umma::idesc_bf16(128, H, 0, 0);
-            if (S.KXP == 16) umma::gemm_bf16x3_ts_warp<1>(dcol, acol, xcols, S.W1.base, S.W1.part, 128u, S.W1.RS, 256u, idesc);
-            else umma::gemm_bf16x3_ts_warp<2>(dcol, acol, xcols, S.W1.base, S.W1.part, 128u, S.W1.RS, 256u, idesc);
-        });
-    };
-    auto epi1_l2 = [&](int slot) {     // h1 = tanh(D + b1) -> T (3 x 32 packed columns); issue layer 2 into D
-        mma_wait(&s_bar[slot][0], ph[slot][0]);
-        {
-            const uint32_t c0 = (uint32_t)kCols * cq;
-            float h[kCols];
-            umma::tmem_ld16(t_lane + kSlotCols * slot + kSlotD + c0, h);
-#pragma unroll
-            for (int j = 0; j < kCols; ++j) h[j] = tanh_mufu(h[j] + b1[c0 + j]);
-            store_row16_tmem(t_lane, kSlotCols * slot + kSlotT + 8u * cq, (uint32_t)H / 2u, h);
-        }
-        mma_issue(&s_bar[slot][1], [&] {
-            umma::gemm_bf16x3_ts_warp<H / 16>(tmem + kSlotCols * slot + kSlotD, tmem + kSlotCols * slot + kSlotT, (uint32_t)H / 2u,
-                                              S.W2.base, S.W2.part, 128u, S.W2.RS, 256u, umma::idesc_bf16(128, H, 0, 0));
-        });
-    };
-    auto epi2 = [&](int slot, int64_t k) {   // h2 = tanh(D + b2) in registers; head = h2 . W3^T (K = 64 split over the four column groups)
+    const int half = tid >> 8;                 // column half of the thread's layer elements
+    const int r0 = lay_row0() + wg::frag_row(0);    // its rows: r0 and r0 + 8
+
+    float xv[8];
+    if (my_n > 0) x_load(0, xv);
+    for (int64_t k = 0; k < my_n; ++k) {
         const float* src; int64_t row0; int nrows; bool second;
         tile_src(tile_of(k), src, row0, nrows, second);
-        mma_wait(&s_bar[slot][1], ph[slot][1]);
-        {
-            const uint32_t r = 32u * q + lane, c0 = (uint32_t)kCols * cq;
-            float v[kCols];
-            umma::tmem_ld16(t_lane + kSlotCols * slot + kSlotD + c0, v);
+        __syncthreads();                       // the previous tile's operand and `part` reads are complete
+        chunk_store(sm0, S.X, kRows, S.KXP, xv);
+        if (k + 1 < my_n) x_load(k + 1, xv);   // global loads fly under this tile's MMAs
+        publish();
+        float acc[kCols], h[kCols];
+        if (S.KXP == 16) wg_gemm<2 * kCols, 1, 0, 0>(acc, S.X, lay_row0(), S.W1, lay_col0());
+        else wg_gemm<2 * kCols, 2, 0, 0>(acc, S.X, lay_row0(), S.W1, lay_col0());
+        epi_tanh(sm0, S.H1, acc, b1, h);
+        publish();
+        wg_gemm<2 * kCols, H / 16, 0, 0>(acc, S.H1, lay_row0(), S.W2, lay_col0());
 #pragma unroll
-            for (int j = 0; j < kCols; ++j) v[j] = tanh_mufu(v[j] + b2[c0 + j]);
-            for (int a = 0; a < out_dim; ++a) {
-                float acc = 0.0f;
+        for (int e = 0; e < kCols; ++e) h[e] = tanh_mufu(acc[e] + b2[lay_col0() + wg::frag_col(e)]);
+        // head = h2 . W3^T: the thread's 8 columns, then the quad (same rows, the 32 columns of the half)
+        for (int a = 0; a < out_dim; ++a) {
+            float p0 = 0.0f, p1 = 0.0f;
 #pragma unroll
-                for (int j = 0; j < kCols; ++j) acc = fmaf(v[j], w3f[a * H + c0 + j], acc);
-                part[(cq * kMaxAct + a) * kRows + r] = acc;     // [column group][a][row]: rows on consecutive banks
+            for (int i = 0; i < kCols / 4; ++i) {
+                const float2 w = *reinterpret_cast<const float2*>(w3f + a * H + lay_col0() + wg::frag_col(4 * i));
+                p0 = fmaf(h[4 * i], w.x, p0); p0 = fmaf(h[4 * i + 1], w.y, p0);
+                p1 = fmaf(h[4 * i + 2], w.x, p1); p1 = fmaf(h[4 * i + 3], w.y, p1);
+            }
+            p0 += __shfl_xor_sync(0xffffffffu, p0, 1); p0 += __shfl_xor_sync(0xffffffffu, p0, 2);
+            p1 += __shfl_xor_sync(0xffffffffu, p1, 1); p1 += __shfl_xor_sync(0xffffffffu, p1, 2);
+            if ((lane & 3) == 0) {
+                part[(half * kMaxAct + a) * kRows + r0] = p0;
+                part[(half * kMaxAct + a) * kRows + r0 + 8] = p1;
             }
         }
-        umma::fence_before_sync();
         __syncthreads();
         if (tid < nrows) {
             const int r = tid;
             if (MODE == 0) {
-                (second ? out1 : out0)[row0 + r] = (part[r] + part[kMaxAct * kRows + r]) +
-                                                   (part[2 * kMaxAct * kRows + r] + part[3 * kMaxAct * kRows + r]) + b3[0];
+                (second ? out1 : out0)[row0 + r] = (part[r] + part[kMaxAct * kRows + r]) + b3[0];
             } else {
                 float lp = 0.0f;
                 for (int a = 0; a < out_dim; ++a) {
-                    const float* pa = part + a * kRows + r;
-                    const float mu = (pa[0] + pa[kMaxAct * kRows]) + (pa[2 * kMaxAct * kRows] + pa[3 * kMaxAct * kRows]) + b3[a];
+                    const float mu = (part[a * kRows + r] + part[(kMaxAct + a) * kRows + r]) + b3[a];
                     lp += ppo::normal_logp_term(__ldg(in1 + (row0 + r) * out_dim + a), mu, ls[a]);
                     if (out1) out1[(row0 + r) * out_dim + a] = mu;
                 }
                 out0[row0 + r] = lp;
             }
         }
-        __syncthreads();     // `part` is free again; every thread has read this slot's D (layer 1 of the next tile may overwrite it)
-    };
-
-    float xa[16], xb[16];
-    if (my_n > 0) { x_load(0, xa); x_store(0, xa); l1(0); }
-    if (my_n > 1) { x_load(1, xb); x_store(1, xb); l1(1); }
-    for (int64_t k = 0; k < my_n; k += 2) {
-        const bool hasB = k + 1 < my_n, nextA = k + 2 < my_n, nextB = k + 3 < my_n;
-        if (nextA) x_load(k + 2, xa);              // global loads fly under the epilogues below
-        epi1_l2(0);
-        if (nextB) x_load(k + 3, xb);
-        if (hasB) epi1_l2(1);                      // layer 2 of slot 0 runs on the tensor core meanwhile
-        epi2(0, k);
-        // slot 0 is completely retired (its T columns were last read by layer 2, its D by the epilogue above)
-        if (nextA) { x_store(0, xa); l1(0); }
-        if (hasB) epi2(1, k + 1);
-        if (nextB) { x_store(1, xb); l1(1); }
     }
-    umma::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) umma::tmem_dealloc(tmem, 512);
 }
 
 }  // namespace

@@ -1,6 +1,6 @@
-// Generic fp32-faithful GEMM on the 5th-generation tensor cores (tcgen05 + TMEM, sm_100a) for the layered
-// networks of the off-policy algorithms (SAC / DDPG critics MLP[256,256] on obs 376, DQN NatureCNN as implicit
-// GEMM over im2col rows):                       C[M,N] (+)= epilogue( A[M,K] * B[N,K]^T )
+// Generic fp32-faithful GEMM on the Hopper tensor cores (wgmma, sm_90a) for the layered networks of the off-policy
+// algorithms (SAC / DDPG critics MLP[256,256] on obs 376, DQN NatureCNN as implicit GEMM over im2col rows):
+//                       C[M,N] (+)= epilogue( A[M,K] * B[N,K]^T )
 //
 // Reference code replaced: every nn.Linear / nn.Conv2d forward and its autograd backward inside
 // SAC._update_with_batch (modelfree/sac.py:304-336), _minimize_critic_squared_loss (modelfree/ddpg.py:267-285),
@@ -10,12 +10,12 @@
 // MN-major (mn contiguous: a[k*ld + mn]), which covers forward (X W^T), input gradient (dY W) and weight
 // gradient (dY^T X) without materialising a transpose.  A CTA computes a 128 x 128 tile: the 256 threads stage
 // 128 x 64 operand chunks into shared memory as bf16x3 pieces (x = b0 + b1 + b2, 24 significant bits) in the
-// blocked no-swizzle layout of umma.cuh, two stages deep, and one elected lane issues the six partial-product
-// MMAs per K = 16 step (same scheme as mlp_tc.cu) into an fp32 TMEM accumulator; staging of chunk i + 1 overlaps
-// the MMAs of chunk i (completion through tcgen05.commit -> mbarrier).  Epilogue: TMEM -> registers -> bias ->
-// activation -> optional ReLU-derivative mask -> coalesced fp32 stores (or split-K partial).
+// blocked no-swizzle layout of wgmma.cuh, two stages deep, and each of the two warpgroups issues the six
+// partial-product wgmma.mma_async per K = 16 step for its 64 rows into an fp32 register accumulator (64 x 128);
+// staging of chunk i + 1 overlaps the MMAs of chunk i.  Epilogue: registers -> bias -> activation -> optional
+// ReLU-derivative mask -> fp32 stores (or split-K partial).
 #include "common.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace {
 
@@ -104,38 +104,6 @@ __device__ __forceinline__ void store_operand(uint8_t* sm0, uint32_t base, const
     }
 }
 
-// One elected lane: the six partial products of `ksteps` K = 16 steps of the chunk in stage `st`.
-__device__ __forceinline__ void issue_chunk(uint32_t d_tmem, uint32_t a_base, int a_mn, uint32_t b_base, int b_mn, int ksteps,
-                                            bool accumulate, uint32_t idesc) {
-    const uint32_t a_lbo = a_mn ? 2048u : 128u, a_sbo = a_mn ? 128u : 1024u, a_step = a_mn ? 4096u : 256u;
-    const uint32_t b_lbo = b_mn ? 2048u : 128u, b_sbo = b_mn ? 128u : 1024u, b_step = b_mn ? 4096u : 256u;
-    const uint32_t ahi = umma::desc_hi(a_sbo), bhi = umma::desc_hi(b_sbo);
-    uint32_t alo[3], blo[3];
-#pragma unroll
-    for (int p = 0; p < 3; ++p) {
-        alo[p] = umma::desc_lo(a_base + p * kPartBytes, a_lbo);
-        blo[p] = umma::desc_lo(b_base + p * kPartBytes, b_lbo);
-    }
-    if (umma::elect_one()) {
-        for (int k = 0; k < ksteps; ++k) {
-            uint64_t A[3], B[3];
-#pragma unroll
-            for (int p = 0; p < 3; ++p) {
-                A[p] = umma::desc_pack(alo[p] + k * (a_step >> 4), ahi);
-                B[p] = umma::desc_pack(blo[p] + k * (b_step >> 4), bhi);
-            }
-            const uint32_t acc0 = (accumulate || k > 0) ? 1u : 0u;
-            umma::mma_bf16(d_tmem, A[2], B[0], idesc, acc0);     // smallest terms first
-            umma::mma_bf16(d_tmem, A[0], B[2], idesc, 1u);
-            umma::mma_bf16(d_tmem, A[1], B[1], idesc, 1u);
-            umma::mma_bf16(d_tmem, A[1], B[0], idesc, 1u);
-            umma::mma_bf16(d_tmem, A[0], B[1], idesc, 1u);
-            umma::mma_bf16(d_tmem, A[0], B[0], idesc, 1u);
-        }
-    }
-    __syncwarp();
-}
-
 __device__ __forceinline__ float apply_act_grad(float x, float y, int kind) {
     return kind == TS_ACT_TANH ? x * fmaf(-y, y, 1.0f) : (y > 0.0f ? x : 0.0f);
 }
@@ -145,105 +113,76 @@ __device__ __forceinline__ float apply_act(float x, int act) {
     return x;
 }
 
+// TA / TB: operand A / B given MN-major (the wgmma transpose flags are immediates)
+template <int TA, int TB>
 __global__ void __launch_bounds__(kThreads, 1) net_gemm_kernel(const GemmParams P) {
     extern __shared__ __align__(1024) uint8_t sm[];
-    __shared__ uint32_t s_tmem;
-    __shared__ __align__(8) uint64_t s_empty[2];
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x, wgi = tid >> 7;
     const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
     const int kb = blockIdx.z * P.k_per_split;
     const int ke = P.splits > 1 ? (int)tsb::imin((int64_t)P.K, (int64_t)kb + P.k_per_split) : P.K;
-    const uint32_t sbase = umma::smem_u32(sm);
+    const uint32_t sbase = wg::smem_u32(sm);
     uint8_t* sm0 = sm - sbase;
-    if (warp == 0) umma::tmem_alloc(&s_tmem, BN);
-    if (tid == 0) { umma::mbar_init(&s_empty[0], 1); umma::mbar_init(&s_empty[1], 1); umma::fence_mbar_init(); }
-    umma::fence_before_sync();
-    __syncthreads();
-    umma::fence_after_sync();
-    const uint32_t tmem = s_tmem;
-    const int n_tile = (int)tsb::imin((int64_t)BN, (int64_t)(((P.N - n0) + 15) & ~15));   // UMMA N: multiple of 16
-    const uint32_t idesc = umma::idesc_bf16(BM, n_tile, P.a.mn_major, P.b.mn_major);
+    // descriptor strides (see wgmma.cuh); warpgroup wgi reads rows [64 wgi, 64 wgi + 64) of A = 8 core matrices along MN
+    constexpr uint32_t a_lbo = TA ? 2048u : 128u, a_sbo = TA ? 128u : 1024u, a_step = TA ? 4096u : 256u;
+    constexpr uint32_t b_lbo = TB ? 2048u : 128u, b_sbo = TB ? 128u : 1024u, b_step = TB ? 4096u : 256u;
+    const uint32_t a_rows = 8u * a_sbo * (uint32_t)wgi;
+    float acc[BN / 2];
+#pragma unroll
+    for (int j = 0; j < BN / 2; ++j) acc[j] = 0.0f;
     const int chunks = (ke - kb + BK - 1) / BK;
-    uint32_t phase[2] = {0u, 0u};
     for (int i = 0; i < chunks; ++i) {
         const int st = i & 1;
         const int k0 = kb + i * BK;
         Staged sa, sb;
         load_operand(sa, P.a, m0, k0, ke);
         load_operand(sb, P.b, n0, k0, ke);
-        if (i >= 2) { umma::mbar_wait(&s_empty[st], phase[st]); phase[st] ^= 1u; }    // MMAs of chunk i - 2 done with this stage
-        const uint32_t a_base = sbase + st * kStageBytes, b_base = a_base + kOperandBytes;
-        store_operand(sm0, a_base, sa, P.a.mn_major);
-        store_operand(sm0, b_base, sb, P.b.mn_major);
-        umma::fence_async_smem();
-        umma::fence_before_sync();
-        __syncthreads();
-        const int warp_u = __shfl_sync(0xffffffffu, warp, 0);
-        if (warp_u == 0) {
-            umma::fence_after_sync();
-            const int ksteps = ((int)tsb::imin((int64_t)BK, (int64_t)(ke - k0)) + 15) >> 4;
-            issue_chunk(tmem, a_base, P.a.mn_major, b_base, P.b.mn_major, ksteps, i > 0, idesc);
-            if (umma::elect_one()) umma::mma_commit(&s_empty[st]);
-            __syncwarp();
+        if (i >= 2) {            // both warpgroups' MMAs of chunk i - 2 are done with this stage
+            wg::wait<1>();
+            __syncthreads();
         }
+        const uint32_t a_base = sbase + st * kStageBytes, b_base = a_base + kOperandBytes;
+        store_operand(sm0, a_base, sa, TA);
+        store_operand(sm0, b_base, sb, TB);
+        wg::fence_async_smem();
+        __syncthreads();
+        // a tail chunk shorter than BK is zero-padded by load_operand: all BK / 16 steps run
+        wg::fence();
+        wg::gemm_bf16x3<BN, BK / 16, TA, TB>(acc, a_base + a_rows, kPartBytes, a_lbo, a_sbo, a_step, b_base, kPartBytes, b_lbo, b_sbo,
+                                              b_step, i > 0);
+        wg::commit();
     }
-    // drain: the last commit covers every earlier MMA of the issuing thread
-    if (chunks > 0) {
-        const int st = (chunks - 1) & 1;
-        if (chunks >= 2) { const int so = st ^ 1; umma::mbar_wait(&s_empty[so], phase[so]); }
-        umma::mbar_wait(&s_empty[st], phase[st]);
-    }
-    umma::fence_after_sync();
+    wg::wait<0>();
 
-    // ---- epilogue: warp w -> TMEM lanes 32 (w & 3) .. + 31 (row m), columns [64 (w >> 2), + 64) --------------
-    const int q = warp & 3, ch = warp >> 2;
-    const int m = m0 + 32 * q + lane;
+    // ---- epilogue: the thread's accumulator elements, two consecutive columns per store ------------------------
     float* cbase = P.c + (P.splits > 1 ? (int64_t)blockIdx.z * P.M * P.N : 0);
     const int64_t ldc = P.splits > 1 ? P.N : P.ldc;
     const bool plain = P.splits > 1;         // partials: raw accumulator, epilogue ops happen in the reduce kernel
-#pragma unroll 1
-    for (int c0 = 64 * ch; c0 < 64 * ch + 64; c0 += 16) {
-        if (c0 >= n_tile) break;             // warp-uniform
-        float v[16];
-        if (chunks > 0) umma::tmem_ld16(tmem + ((32u * q) << 16) + (uint32_t)c0, v);
-        else {
 #pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = 0.0f;
+    for (int e = 0; e < BN / 2; e += 2) {
+        const int m = m0 + 64 * wgi + wg::frag_row(e), n = n0 + wg::frag_col(e);
+        if (m >= P.M || n >= P.N) continue;
+        float* dst = cbase + (int64_t)m * ldc + n;
+        float v[2] = {acc[e], acc[e + 1]};
+        const bool pair = n + 1 < P.N;
+        if (!plain) {
+#pragma unroll
+            for (int j = 0; j < 2; ++j) {
+                if (j == 1 && !pair) break;
+                float x = v[j];
+                if (P.bias) x += __ldg(P.bias + n + j);
+                x = apply_act(x, P.act);
+                if (P.mask) x = apply_act_grad(x, __ldg(P.mask + (int64_t)m * P.ld_mask + n + j), P.mask_kind);
+                if (P.accumulate) x += dst[j];
+                v[j] = x;
+            }
         }
-        if (m < P.M) {
-            float* row = cbase + (int64_t)m * ldc + n0 + c0;
-            if (!plain) {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    const int n = n0 + c0 + j;
-                    if (n < P.N) {
-                        float x = v[j];
-                        if (P.bias) x += __ldg(P.bias + n);
-                        x = apply_act(x, P.act);
-                        if (P.mask) x = apply_act_grad(x, __ldg(P.mask + (int64_t)m * P.ld_mask + n), P.mask_kind);
-                        if (P.accumulate) x += row[j];
-                        v[j] = x;
-                    }
-                }
-            }
-            // a lane owns 16 consecutive columns of ITS row: four 16-byte stores when the run is whole and aligned (a scalar
-            // store per element makes every warp store touch 32 sectors -- ~8 us for a 128 x 128 tile, profiles/r2d_net_gemm_ncu.md)
-            if (n0 + c0 + 16 <= P.N && (reinterpret_cast<uintptr_t>(row) & 15u) == 0) {
-                float4* r4 = reinterpret_cast<float4*>(row);
-                r4[0] = make_float4(v[0], v[1], v[2], v[3]);
-                r4[1] = make_float4(v[4], v[5], v[6], v[7]);
-                r4[2] = make_float4(v[8], v[9], v[10], v[11]);
-                r4[3] = make_float4(v[12], v[13], v[14], v[15]);
-            } else {
-#pragma unroll
-                for (int j = 0; j < 16; ++j)
-                    if (n0 + c0 + j < P.N) row[j] = v[j];
-            }
+        if (pair && (reinterpret_cast<uintptr_t>(dst) & 7u) == 0) *reinterpret_cast<float2*>(dst) = make_float2(v[0], v[1]);
+        else {
+            dst[0] = v[0];
+            if (pair) dst[1] = v[1];
         }
     }
-    umma::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) umma::tmem_dealloc(tmem, BN);
 }
 
 // C (+)= epilogue( sum_z partial[z] ), fixed summation order (deterministic)
@@ -289,13 +228,13 @@ namespace tsb {
 
 size_t net_gemm_workspace_floats(int M, int N, int K, int* splits_out) {
     // split-K whenever the output tiles alone leave most SMs idle: weight gradients over im2col rows (K = tens of thousands),
-    // and every layer of a batch-256 MLP (4 output tiles, 4 .. 7 chunks: a lone CTA per tile walks them one round trip after
-    // the other -- 30 .. 57 us under ncu, profiles/r2d_net_gemm_ncu.md -- while 144 SMs idle)
+    // and every layer of a batch-256 MLP (4 output tiles, 4 .. 7 chunks: a lone CTA per tile would walk them one round trip
+    // after the other while the other SMs idle)
     const int tiles = ((M + BM - 1) / BM) * ((N + BN - 1) / BN);
     const int chunks = (K + BK - 1) / BK;
     int splits = 1;
     if (chunks >= 2 && tiles < 64) {
-        splits = (int)imin((int64_t)((148 + tiles - 1) / tiles), (int64_t)chunks);
+        splits = (int)imin((int64_t)((num_sms() + tiles - 1) / tiles), (int64_t)chunks);
         if (splits < 1) splits = 1;
     }
     if (splits_out) *splits_out = splits;
@@ -308,7 +247,10 @@ int net_gemm(const float* a, int64_t lda, int a_mn, const float* b, int64_t ldb,
     static bool configured[kMaxDevices] = {};
     const int dev = device_ordinal();
     if (!configured[dev]) {
-        TS_CUDA(cudaFuncSetAttribute(net_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
+        TS_CUDA(cudaFuncSetAttribute(net_gemm_kernel<0, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
+        TS_CUDA(cudaFuncSetAttribute(net_gemm_kernel<0, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
+        TS_CUDA(cudaFuncSetAttribute(net_gemm_kernel<1, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
+        TS_CUDA(cudaFuncSetAttribute(net_gemm_kernel<1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
         configured[dev] = true;
     }
     if (M <= 0 || N <= 0) return 0;
@@ -329,11 +271,14 @@ int net_gemm(const float* a, int64_t lda, int a_mn, const float* b, int64_t ldb,
         P.c = workspace;
     }
     const dim3 grid((M + BM - 1) / BM, (N + BN - 1) / BN, splits);
-    net_gemm_kernel<<<grid, kThreads, kSmemBytes, st>>>(P);
+    if (a_mn && b_mn) net_gemm_kernel<1, 1><<<grid, kThreads, kSmemBytes, st>>>(P);
+    else if (a_mn) net_gemm_kernel<1, 0><<<grid, kThreads, kSmemBytes, st>>>(P);
+    else if (b_mn) net_gemm_kernel<0, 1><<<grid, kThreads, kSmemBytes, st>>>(P);
+    else net_gemm_kernel<0, 0><<<grid, kThreads, kSmemBytes, st>>>(P);
     if (check_launch("ts_net_gemm")) return 1;
     if (splits > 1) {
         const int64_t total = (int64_t)M * N;
-        splitk_reduce_kernel<<<(unsigned)imin((total + 255) / 256, 148 * 8), 256, 0, st>>>(workspace, splits, c, ldc, M, N, bias, act,
+        splitk_reduce_kernel<<<(unsigned)imin((total + 255) / 256, num_sms() * 8), 256, 0, st>>>(workspace, splits, c, ldc, M, N, bias, act,
                                                                                            mask, ld_mask, mask_kind, accumulate);
         if (check_launch("ts_net_gemm/splitk")) return 1;
     }

@@ -1,4 +1,4 @@
-// n-step return: windowed gather-reduce over VectorReplayBuffer index rows, sm_100a.
+// n-step return: windowed gather-reduce over VectorReplayBuffer index rows, sm_90a.
 //
 // Reference: numba `_nstep_return` (tianshou/algorithm/algorithm_base.py:1160-1222):
 //   gammas = N; acc = 0

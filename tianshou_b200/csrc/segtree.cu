@@ -1,4 +1,4 @@
-// Sum tree for prioritized experience replay (f64 tree resident in HBM), sm_100a.
+// Sum tree for prioritized experience replay (f64 tree resident in HBM), sm_90a.
 //
 // Reference: tianshou/data/utils/segtree.py (numba `_setitem` :95-101, `_reduce` :104-116,
 // `_get_prefix_sum_idx` :119-134) and tianshou/data/buffer/prio.py (:46-47,:63-90,:104-106).

@@ -1,134 +1,67 @@
-// Hardware self-test of the tcgen05 building blocks in umma.cuh.  One CTA computes
+// Hardware self-test of the tensor-core building blocks in wgmma.cuh.  One CTA computes
 //     D[M x N] = A[M x K] * B[N x K]^T           (a, b given row-major in global memory)
-// with either the 3xTF32 split (kind::tf32, K = 8 per MMA) or the 3-way bf16 split (kind::f16,
-// K = 16 per MMA, 6 MMAs per step), M in {64, 128}, each operand placed in shared memory either
-// K-major or MN-major (blocked no-swizzle layout, see umma.cuh), and dumps the raw TMEM
-// accumulator (128 lanes x N columns) so that the lane mapping of M = 64 can be checked too.
+// with the 3-way bf16 split (6 wgmma per K = 16 step), M in {64, 128} (one warpgroup per 64 rows), each operand
+// placed in shared memory either K-major or MN-major (blocked no-swizzle layout, see wgmma.cuh), and writes D
+// row-major from the register accumulators.  B is padded with zero rows to N = 128.
 #include <cuda_bf16.h>
 
 #include "common.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace {
 
-constexpr int kThreads = 128;
+constexpr int kThreads = 256, kN = 128;
 
-__global__ void __launch_bounds__(kThreads, 1) umma_selftest_kernel(const float* __restrict__ a,
-                                                                   const float* __restrict__ b, float* __restrict__ d,
-                                                                   int M, int N, int K, int dtype, int a_mn, int b_mn,
-                                                                   int swap) {
+template <int TA, int TB>
+__global__ void __launch_bounds__(kThreads, 1) wgmma_selftest_kernel(const float* __restrict__ a, const float* __restrict__ b,
+                                                                    float* __restrict__ d, int M, int N, int K, int swap) {
     extern __shared__ __align__(128) uint8_t smem[];
-    __shared__ uint32_t s_tmem;
-    __shared__ __align__(8) uint64_t s_bar;
-    const int tid = threadIdx.x, warp = tid >> 5;
-    const int esz = dtype == 0 ? 4 : 2;            // bytes per element
-    const int cw = 16 / esz;                       // elements per 16-byte chunk
-    const int parts = dtype == 0 ? 2 : 3;          // hi/lo or b0/b1/b2
-    // operand X (logical [MN x K]) is stored as a matrix with rows = (major ? K : MN), cols = the other
-    auto place = [&](const float* src, int MN, int mn_major, uint8_t* base, uint32_t& RS, uint32_t& CS, uint32_t& bytes) {
-        const int rows = mn_major ? K : MN, cols = mn_major ? MN : K;
-        CS = 128; RS = (uint32_t)(cols / cw) * 128; bytes = (uint32_t)rows * cols * esz;
-        for (int e = tid; e < MN * K; e += kThreads) {
+    const int tid = threadIdx.x, wgi = tid >> 7;
+    // operand X (logical [MN x K], MN rows valid) is stored as a matrix with rows = (major ? K : MN), cols = the other
+    auto place = [&](const float* src, int MN, int MN_pad, int mn_major, uint8_t* base, uint32_t& RS, uint32_t& bytes) {
+        const int rows = mn_major ? K : MN_pad, cols = mn_major ? MN_pad : K;
+        RS = (uint32_t)(cols / 8) * 128; bytes = (uint32_t)rows * cols * 2;
+        for (int e = tid; e < MN_pad * K; e += kThreads) {
             const int mn = e / K, k = e % K;
             const int r = mn_major ? k : mn, c = mn_major ? mn : k;
-            const uint32_t off = (uint32_t)(r >> 3) * RS + (uint32_t)(c / cw) * CS + (uint32_t)(r & 7) * 16 + (uint32_t)(c % cw) * esz;
-            const float x = src[e];
-            if (dtype == 0) {
-                float hi, lo; umma::split_tf32(x, hi, lo);
-                *reinterpret_cast<float*>(base + off) = hi;
-                *reinterpret_cast<float*>(base + bytes + off) = lo;
-            } else {
-                const __nv_bfloat16 b0 = __float2bfloat16_rn(x);
-                const float r1 = x - __bfloat162float(b0);
-                const __nv_bfloat16 b1 = __float2bfloat16_rn(r1);
-                const float r2 = r1 - __bfloat162float(b1);
-                const __nv_bfloat16 b2 = __float2bfloat16_rn(r2);
-                *reinterpret_cast<__nv_bfloat16*>(base + off) = b0;
-                *reinterpret_cast<__nv_bfloat16*>(base + bytes + off) = b1;
-                *reinterpret_cast<__nv_bfloat16*>(base + 2 * bytes + off) = b2;
-            }
+            const uint32_t off = (uint32_t)(r >> 3) * RS + (uint32_t)(c / 8) * 128 + (uint32_t)(r & 7) * 16 + (uint32_t)(c % 8) * 2;
+            const float x = mn < MN ? src[mn * K + k] : 0.0f;
+            const __nv_bfloat16 b0 = __float2bfloat16_rn(x);
+            const float r1 = x - __bfloat162float(b0);
+            const __nv_bfloat16 b1 = __float2bfloat16_rn(r1);
+            const __nv_bfloat16 b2 = __float2bfloat16_rn(r1 - __bfloat162float(b1));
+            *reinterpret_cast<__nv_bfloat16*>(base + off) = b0;
+            *reinterpret_cast<__nv_bfloat16*>(base + bytes + off) = b1;
+            *reinterpret_cast<__nv_bfloat16*>(base + 2 * bytes + off) = b2;
         }
     };
-    uint32_t aRS, aCS, aB, bRS, bCS, bB;
+    uint32_t aRS, aB, bRS, bB;
     uint8_t* a_base = smem;
-    const bool a_ts = (a_mn == 2);        // A operand in tensor memory (TS mode): bf16, M = 128, K-major
-    if (a_ts) a_mn = 0;
-    place(a, M, a_mn, a_base, aRS, aCS, aB);
-    uint8_t* b_base = a_base + (size_t)parts * aB;
-    place(b, N, b_mn, b_base, bRS, bCS, bB);
-    if (warp == 0) umma::tmem_alloc(&s_tmem, 512);
-    if (tid == 0) { umma::mbar_init(&s_bar, 1); umma::fence_mbar_init(); }
-    umma::fence_async_smem();
-    umma::fence_before_sync();
+    place(a, M, M, TA, a_base, aRS, aB);
+    uint8_t* b_base = a_base + 3 * (size_t)aB;
+    place(b, N, kN, TB, b_base, bRS, bB);
+    wg::fence_async_smem();
     __syncthreads();
-    umma::fence_after_sync();
-    const uint32_t tmem = s_tmem;
-    constexpr uint32_t kACol = 256;        // A pieces: columns 256 + p * 64 + (k / 2)
-    if (a_ts) {                            // thread = lane = row of A: split to bf16x3 and tcgen05.st 8 packed columns per K step
-        for (int k0 = 0; k0 < K; k0 += 16) {
-            uint32_t w[3][8];
-            for (int j = 0; j < 8; ++j) {
-                uint32_t pk[3] = {0u, 0u, 0u};
-                for (int h = 0; h < 2; ++h) {
-                    const float x = a[tid * K + k0 + 2 * j + h];
-                    const __nv_bfloat16 b0 = __float2bfloat16_rn(x);
-                    const float r1 = x - __bfloat162float(b0);
-                    const __nv_bfloat16 b1 = __float2bfloat16_rn(r1);
-                    const __nv_bfloat16 b2 = __float2bfloat16_rn(r1 - __bfloat162float(b1));
-                    pk[0] |= (uint32_t)__bfloat16_as_ushort(b0) << (16 * h);
-                    pk[1] |= (uint32_t)__bfloat16_as_ushort(b1) << (16 * h);
-                    pk[2] |= (uint32_t)__bfloat16_as_ushort(b2) << (16 * h);
-                }
-                w[0][j] = pk[0]; w[1][j] = pk[1]; w[2][j] = pk[2];
-            }
-            for (int p = 0; p < 3; ++p)
-                umma::tmem_st8(tmem + ((uint32_t)(32 * warp) << 16) + kACol + 64u * p + (uint32_t)(k0 / 2), w[p]);
-        }
-        umma::tmem_wait_st();
-        umma::fence_before_sync();
-        __syncthreads();
-        umma::fence_after_sync();
-        if (warp == 0) {
-            uint32_t blbo = bCS, bsbo = bRS, bstep = 2 * bCS;
-            if (b_mn) { bsbo = bCS; blbo = bRS; bstep = 2 * bRS; }
-            const uint32_t B0 = umma::smem_u32(b_base);
-            const uint32_t idesc = umma::idesc_bf16(M, N, 0, b_mn);
-            if (K == 16) umma::gemm_bf16x3_ts_warp<1>(tmem, tmem + kACol, 64u, B0, bB, blbo, bsbo, bstep, idesc);
-            else if (K == 32) umma::gemm_bf16x3_ts_warp<2>(tmem, tmem + kACol, 64u, B0, bB, blbo, bsbo, bstep, idesc);
-            else umma::gemm_bf16x3_ts_warp<4>(tmem, tmem + kACol, 64u, B0, bB, blbo, bsbo, bstep, idesc);
-            if (umma::elect_one()) umma::mma_commit(&s_bar);
-            __syncwarp();
-        }
-    } else if (tid == 0) {
-        const int kper = dtype == 0 ? 8 : 16;
-        auto strides = [&](int mn_major, uint32_t RS, uint32_t CS, uint32_t& lbo, uint32_t& sbo, uint32_t& step) {
-            if (!mn_major) { lbo = CS; sbo = RS; step = 2 * CS; }        // K-major: 2 chunks of 16 B per MMA
-            else { sbo = CS; lbo = RS; step = (uint32_t)(kper / 8) * RS; }  // MN-major: kper/8 row groups per MMA
-            if (swap) { const uint32_t t = lbo; lbo = sbo; sbo = t; }
-        };
-        uint32_t albo, asbo, astep, blbo, bsbo, bstep;
-        strides(a_mn, aRS, aCS, albo, asbo, astep);
-        strides(b_mn, bRS, bCS, blbo, bsbo, bstep);
-        const uint32_t A0 = umma::smem_u32(a_base), B0 = umma::smem_u32(b_base);
-        if (dtype == 0) {
-            const uint32_t idesc = umma::idesc_tf32(M, N, a_mn, b_mn);
-            umma::gemm_3xtf32(tmem, A0, A0 + aB, albo, asbo, astep, B0, B0 + bB, blbo, bsbo, bstep, idesc, K / 8, false);
-        } else {
-            const uint32_t idesc = umma::idesc_bf16(M, N, a_mn, b_mn);
-            umma::gemm_bf16x3(tmem, A0, aB, albo, asbo, astep, B0, bB, blbo, bsbo, bstep, idesc, K / 16, false);
-        }
-        umma::mma_commit(&s_bar);
+    if (64 * wgi >= M) return;                  // warpgroup-uniform
+    auto strides = [&](int mn_major, uint32_t RS, uint32_t& lbo, uint32_t& sbo, uint32_t& step) {
+        if (!mn_major) { lbo = 128; sbo = RS; step = 256; }       // K-major: 2 chunks of 16 B per MMA
+        else { lbo = RS; sbo = 128; step = 2 * RS; }               // MN-major: 2 row groups per MMA
+        if (swap) { const uint32_t t = lbo; lbo = sbo; sbo = t; }
+    };
+    uint32_t albo, asbo, astep, blbo, bsbo, bstep;
+    strides(TA, aRS, albo, asbo, astep);
+    strides(TB, bRS, blbo, bsbo, bstep);
+    const uint32_t A0 = wg::smem_u32(a_base) + 8u * (TA ? 128u : aRS) * (uint32_t)wgi, B0 = wg::smem_u32(b_base);
+    float acc[kN / 2];
+    wg::fence();
+    for (int k = 0; k < K / 16; ++k)
+        wg::gemm_bf16x3<kN, 1, TA, TB>(acc, A0 + k * astep, aB, albo, asbo, astep, B0 + k * bstep, bB, blbo, bsbo, bstep, k > 0);
+    wg::commit();
+    wg::wait<0>();
+    for (int e = 0; e < kN / 2; ++e) {
+        const int m = 64 * wgi + wg::frag_row(e), n = wg::frag_col(e);
+        if (n < N) d[m * N + n] = acc[e];
     }
-    umma::mbar_wait(&s_bar, 0);
-    umma::fence_after_sync();
-    for (int c0 = 0; c0 < N; c0 += 8) {          // raw dump: lane = 32*warp + laneid
-        float v[8];
-        umma::tmem_ld8(tmem + ((uint32_t)(32 * warp) << 16) + c0, v);
-        for (int j = 0; j < 8; ++j) d[tid * N + c0 + j] = v[j];
-    }
-    umma::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) umma::tmem_dealloc(tmem, 512);
 }
 
 }  // namespace
@@ -136,13 +69,14 @@ __global__ void __launch_bounds__(kThreads, 1) umma_selftest_kernel(const float*
 extern "C" int ts_umma_selftest(const float* a, const float* b, float* d, int32_t M, int32_t N, int32_t K,
                                 int32_t dtype, int32_t a_mn, int32_t b_mn, int32_t swap, ts_stream_t stream) {
     TS_REQUIRE(a && b && d, "ts_umma_selftest: null pointer");
+    TS_REQUIRE(dtype == 1, "ts_umma_selftest: only the bf16x3 split (dtype 1) exists on this architecture");
     TS_REQUIRE(M == 64 || M == 128, "ts_umma_selftest: M must be 64 or 128");
-    const int kper = dtype == 0 ? 8 : 16;
-    TS_REQUIRE(N % 8 == 0 && N >= 8 && N <= 128 && K % kper == 0 && K >= kper && K <= 128, "ts_umma_selftest: bad N/K");
-    TS_REQUIRE(M == 64 || N % 16 == 0, "ts_umma_selftest: M=128 needs N % 16 == 0");
-    TS_REQUIRE(a_mn != 2 || (dtype == 1 && M == 128 && (K == 16 || K == 32 || K == 64)), "ts_umma_selftest: TS mode is bf16, M=128, K in {16,32,64}");
-    const size_t smem = (size_t)(dtype == 0 ? 8 : 6) * (size_t)(M * K + N * K);
-    TS_CUDA(cudaFuncSetAttribute(umma_selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    umma_selftest_kernel<<<1, kThreads, smem, tsb::as_stream(stream)>>>(a, b, d, M, N, K, dtype, a_mn, b_mn, swap);
+    TS_REQUIRE(N % 8 == 0 && N >= 8 && N <= kN && K % 16 == 0 && K >= 16 && K <= 128, "ts_umma_selftest: bad N/K");
+    TS_REQUIRE((a_mn == 0 || a_mn == 1) && (b_mn == 0 || b_mn == 1), "ts_umma_selftest: operands are K-major (0) or MN-major (1)");
+    const size_t smem = (size_t)6 * (size_t)(M * K + kN * K);
+    auto kern = a_mn ? (b_mn ? wgmma_selftest_kernel<1, 1> : wgmma_selftest_kernel<1, 0>)
+                     : (b_mn ? wgmma_selftest_kernel<0, 1> : wgmma_selftest_kernel<0, 0>);
+    TS_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kern<<<1, kThreads, smem, tsb::as_stream(stream)>>>(a, b, d, M, N, K, swap);
     return tsb::check_launch("ts_umma_selftest");
 }

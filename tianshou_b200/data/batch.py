@@ -762,7 +762,7 @@ class NumpyGlobalPermutationJob:
         nw = (n_workers or int(os.environ.get("TS_B200_PERM_WORKERS", "0") or 0)
               or max(1, min(repeat, 8 if self._n >= (1 << 20) else (2 if local_world >= 4 else 4), cores // local_world - 2)))
         # (>= 4 local ranks: two appliers per rank still finish every row ahead of the GPU and leave the host threads that feed the
-        # GPUs more room -- weak scaling at N = 4: 15.0 ms per update against 15.8 with four, profiles/r2_ab_n4.txt)
+        # GPUs more room)
         h = C.c_void_p()
         try:
             call("ts_host_perm_job_start", self._key.ctypes.data_as(C.c_void_p), int(self._st[2]), self._n, repeat,

@@ -6,7 +6,7 @@ Contract mirrored from the reference:
   ReplayBufferManager     tianshou/data/buffer/manager.py:13-310  (+ numba kernels :311-363)
   VectorReplayBuffer      tianshou/data/buffer/vecbuf.py:14-37
 
-Design differences (B200-first, same observable behaviour):
+Design differences (GPU-first, same observable behaviour):
   * ONE implementation for E >= 1 sub-buffers: all per-sub-buffer bookkeeping (size, insertion
     index, episode return/length/start) lives in numpy arrays of length E, so ``add`` for
     thousands of envs is a handful of vectorised numpy ops instead of a Python loop over child

@@ -1,6 +1,6 @@
 """CONTEXT ONLY (never the target, never on the product path): the same PPO ``update()`` written the way the reference writes
 it -- stock PyTorch modules, autograd, ``clip_grad_norm_``, ``torch.optim.Adam``, one minibatch at a time (ppo.py:164-224,
-a2c.py:115-153) -- but with every tensor on the B200 and the chunked 256-row no-grad passes replaced by full-batch forwards.
+a2c.py:115-153) -- but with every tensor on the GPU and the chunked 256-row no-grad passes replaced by full-batch forwards.
 SURVEY 2.3 names this number as part of the bar ("what moving the reference's own code to the GPU would give").
 
     python tools/torch_eager_context.py [--envs 4096] [--steps 2]
@@ -92,7 +92,7 @@ def run(E: int = 4096, T: int = 128, bs: int = 16384, repeat: int = 10, steps: i
     torch.cuda.synchronize()
     dt = (time.perf_counter() - t0) / steps
     return {"value": N / dt, "unit": "transitions/s", "ms_per_update": 1e3 * dt, "what": "stock PyTorch eager + autograd + torch.optim.Adam on the "
-            f"B200, {E} envs x {T} steps, minibatch {bs}, repeat {repeat}, return scaling omitted, full-batch no-grad passes: context only"}
+            f"{torch.cuda.get_device_name()}, {E} envs x {T} steps, minibatch {bs}, repeat {repeat}, return scaling omitted, full-batch no-grad passes: context only"}
 
 
 if __name__ == "__main__":

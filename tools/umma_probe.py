@@ -1,5 +1,5 @@
-"""Diagnostic: run the tcgen05 self-test kernel over dtype / M / major-ness variants and report
-the error of the accumulator against an f64 matmul under both candidate lane mappings."""
+"""Diagnostic: run the wgmma self-test kernel over M / major-ness variants and report the error of the product
+against an f64 matmul."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
@@ -10,31 +10,17 @@ _cabi.use_diagnostics_library()      # ts_umma_selftest lives in the diagnostics
 dev = "cuda:0"
 rng = np.random.default_rng(0)
 
-
-def lanes_for(M, mapping):
-    if M == 128:
-        return np.arange(128)
-    if mapping == "half":      # rows 16q..16q+15 -> lanes 32q..32q+15 (cute tmem_frg_1sm, M = 64)
-        r = np.arange(64)
-        return (r // 16) * 32 + r % 16
-    return np.arange(64)       # "linear": rows -> lanes 0..63
-
-
-for dtype in (1,):
-    for M in (128, 64):
-        for a_mn, b_mn in ((0, 0), (1, 0), (0, 1), (1, 1)):
-            for N, K in ((64, 64), (16, 128), (8, 128) if M == 64 else (32, 32)):
-                a = rng.standard_normal((M, K)).astype(np.float32); b = rng.standard_normal((N, K)).astype(np.float32)
-                ref = a.astype(np.float64) @ b.astype(np.float64).T
-                for swap in (0,):
-                    d = torch.full((128, N), float("nan"), dtype=torch.float32, device=dev)
-                    ta, tb = torch.from_numpy(a).to(dev), torch.from_numpy(b).to(dev)
-                    try:
-                        call("ts_umma_selftest", ptr(ta), ptr(tb), ptr(d), M, N, K, dtype, a_mn, b_mn, swap, stream_ptr())
-                        torch.cuda.synchronize()
-                        raw = d.cpu().numpy()
-                        errs = {mp: float(np.abs(raw[lanes_for(M, mp)] - ref).max() / np.abs(ref).max())
-                                for mp in (("full",) if M == 128 else ("half", "linear"))}
-                    except Exception as e:  # noqa: BLE001
-                        errs = f"ERR {e}"
-                    print(f"dtype={'tf32x3' if dtype == 0 else 'bf16x3'} M={M} a_mn={a_mn} b_mn={b_mn} N={N} K={K} swap={swap}: {errs}", flush=True)
+for M in (128, 64):
+    for a_mn, b_mn in ((0, 0), (1, 0), (0, 1), (1, 1)):
+        for N, K in ((64, 64), (16, 128), (8, 32), (128, 48)):
+            a = rng.standard_normal((M, K)).astype(np.float32); b = rng.standard_normal((N, K)).astype(np.float32)
+            ref = a.astype(np.float64) @ b.astype(np.float64).T
+            d = torch.full((M, N), float("nan"), dtype=torch.float32, device=dev)
+            ta, tb = torch.from_numpy(a).to(dev), torch.from_numpy(b).to(dev)
+            try:
+                call("ts_umma_selftest", ptr(ta), ptr(tb), ptr(d), M, N, K, 1, a_mn, b_mn, 0, stream_ptr())
+                torch.cuda.synchronize()
+                err = float(np.abs(d.cpu().numpy() - ref).max() / np.abs(ref).max())
+            except Exception as e:  # noqa: BLE001
+                err = f"ERR {e}"
+            print(f"bf16x3 M={M} a_mn={a_mn} b_mn={b_mn} N={N} K={K}: {err}", flush=True)
