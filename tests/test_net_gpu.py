@@ -73,6 +73,91 @@ def test_net_gemm_weight_gradient_arrangement(rows, out_f, in_f):
     np.testing.assert_allclose(gb.cpu().numpy(), dy.double().sum(0).cpu().numpy(), rtol=1e-5, atol=1e-4)
 
 
+# operand arrangements (A MN-major, B MN-major): forward X W^T, input gradient dY W, A MN-major with B K-major, weight
+# gradient dY^T X -- with the fp64 tolerance of the existing test of the same arrangement (the A-MN-major-only one has
+# none and takes the forward's)
+ARRANGEMENTS = {"fwd": (0, 0, 5e-6, 5e-6), "dx": (0, 1, 2e-6, 2e-6), "amn": (1, 0, 5e-6, 5e-6), "dw": (1, 1, 2e-6, 3e-6)}
+# M, N around the 128-wide tile edges, K around the 16-deep MMA step and the 64-deep staged chunk; K = 3136 walks the two
+# shared-memory stages 49 times (unsplit) -- tiles < 64 and K > 64 split along K when a workspace is given
+EDGE_SHAPES = [(1, 1, 1), (63, 64, 15), (64, 63, 16), (127, 129, 17), (128, 127, 64), (129, 257, 65), (257, 128, 3136),
+               (1, 257, 3136), (257, 1, 65), (129, 63, 1)]
+# epilogues: (bias, act, mask kind (0 = none), accumulate)
+EPILOGUES = [(True, 0, 0, False), (True, 1, 1, True), (False, 2, 2, False), (True, 2, 0, True), (False, 0, 1, False)]
+
+
+def _strided(store, off, rows, cols, ld):
+    return store.as_strided((rows, cols), (ld, 1), off)
+
+
+@pytest.mark.parametrize("arr", list(ARRANGEMENTS))
+@pytest.mark.parametrize("M,N,K", EDGE_SHAPES)
+def test_net_gemm_arrangements_edges_vs_fp64(M, N, K, arr):
+    """Every operand arrangement at tile-edge shapes, split and unsplit (which one ran is asserted), dense operands and
+    views (pointers an odd number of floats into the allocation, ld > extent, ldc > N, ld_mask > N: the scalar-load
+    fallback and the unpaired epilogue stores), every epilogue; C outside the M x N view must stay untouched, and two
+    identical calls must give bit-identical results."""
+    from tianshou_b200._cabi import call, load_library, stream_ptr
+    a_mn, b_mn, rtol, atol_rel = ARRANGEMENTS[arr]
+    g = torch.Generator(device="cpu").manual_seed(M * 131 + N * 17 + K)
+    A64 = torch.randn(M, K, generator=g, dtype=torch.float64)
+    B64 = torch.randn(N, K, generator=g, dtype=torch.float64) / K ** 0.5
+    bias = torch.randn(N, generator=g).to(DEV)
+    prod = (A64.float().double() @ B64.float().double().T).to(DEV)      # fp64 product of the fp32 operands
+    tiles = ((M + 127) // 128) * ((N + 127) // 128)
+    expect_split = (K + 63) // 64 >= 2 and tiles < 64
+    lib = load_library()
+    for view in (False, True):
+        pad, off = (5, 3) if view else (0, 0)
+        # A logical [M][K], B logical [N][K]; MN-major storage holds the transpose
+        a_rows, a_cols = (K, M) if a_mn else (M, K)
+        b_rows, b_cols = (K, N) if b_mn else (N, K)
+        lda, ldb, ldc, ldm = a_cols + pad, b_cols + pad, N + (3 if view else 0), N + (2 if view else 0)
+        a_st = torch.full((off + a_rows * lda,), float("nan"), device=DEV)
+        b_st = torch.full((off + b_rows * ldb,), float("nan"), device=DEV)
+        _strided(a_st, off, a_rows, a_cols, lda).copy_((A64.T if a_mn else A64).float())
+        _strided(b_st, off, b_rows, b_cols, ldb).copy_((B64.T if b_mn else B64).float())
+        # (the padding of the views stays NaN: an element read from outside an operand poisons the result)
+        y_st = torch.randn(off + M * ldm, generator=g).to(DEV)
+        y = _strided(y_st, off, M, N, ldm)
+        for has_bias, act, mask_kind, accumulate in EPILOGUES:
+            ref = prod + (bias.double() if has_bias else 0.0)
+            ref = torch.relu(ref) if act == 1 else (torch.tanh(ref) if act == 2 else ref)
+            if mask_kind == 1:
+                ref = ref * (y.double() > 0)
+            elif mask_kind == 2:
+                ref = ref * (1.0 - y.double() ** 2)
+            c0 = torch.randn(off + M * ldc, generator=g).to(DEV)
+            if accumulate:
+                ref = ref + _strided(c0, off, M, N, ldc).double()
+            outs = []
+            for split in (False, True):
+                ws_n = int(lib.ts_net_gemm_workspace_floats(M, N, K)) if split else 0
+                assert (ws_n > 0) == (split and expect_split)
+                ws = torch.empty(max(ws_n, 1), device=DEV)
+                for _ in range(2):
+                    c = c0.clone()
+                    call("ts_net_gemm", a_st.data_ptr() + 4 * off, lda, a_mn, b_st.data_ptr() + 4 * off, ldb, b_mn,
+                         c.data_ptr() + 4 * off, ldc, M, N, K, bias.data_ptr() if has_bias else None, act,
+                         y.data_ptr() if mask_kind else None, ldm if mask_kind else 0, mask_kind or 1, int(accumulate),
+                         ws.data_ptr() if ws_n else None, ws_n, stream_ptr())
+                    outs.append((split, c))
+                key = (f"net_gemm_edges/{arr}/{M}x{N}x{K}/{'view' if view else 'dense'}/b{int(has_bias)}a{act}m{mask_kind}"
+                       f"acc{int(accumulate)}/split{int(ws_n > 0)}")
+                got = _strided(outs[-1][1], off, M, N, ldc)
+                # Unsplit, one register accumulator takes all K / 16 * 6 MMA additions; each may round by up to ~2^-24 of
+                # the running sum, so the bound grows with K (at K = 3136: 7e-5 of max |C|, observed 2.7e-5; split-K
+                # partials are summed in fp32 and stay within the existing bar)
+                acc_bound = 0.0 if ws_n else (K + 15) // 16 * 6 * 2.0 ** -24
+                record_parity(key, got.cpu().numpy(), ref.cpu().numpy(), rtol=rtol,
+                              atol=max(atol_rel, acc_bound) * float(ref.abs().max()))
+                # nothing outside the M x N view is written
+                untouched = torch.ones_like(c0, dtype=torch.bool)
+                _strided(untouched, off, M, N, ldc).fill_(False)
+                assert torch.equal(outs[-1][1][untouched], c0[untouched]), key
+                # deterministic: two identical calls, bit-identical output
+                assert torch.equal(outs[-2][1], outs[-1][1]), key
+
+
 def test_conv_stack_forward_backward_vs_torch():
     """NatureCNN-shaped stack (env/atari/atari_network.py:77-96) on uint8 frame stacks: forward and all parameter
     gradients of sum(q * coef) against torch autograd on the same weights."""

@@ -359,9 +359,20 @@ def test_policy_forward_fused_inference_matches_torch_modules():
 def test_wide_observation_runs_simt_kernels_vs_oracle():
     """obs_dim = 40 is outside the tensor-core kernels' envelope (<= 32): value / log-prob passes and the whole update run
     the fp32 SIMT kernels (per-step ts_ppo_grad -> ts_clip_adam_step); same parity bar against the numpy oracle."""
+    _simt_update_vs_oracle(40, 5)
+
+
+@pytest.mark.parametrize("OBS,ACT", [(33, 1), (60, 16), (64, 4)])
+def test_simt_envelope_edges_vs_oracle(OBS, ACT):
+    """The same SIMT update at the edges of its envelope: 33 is the first width past the tensor-core kernels; (60, 16) and
+    (64, 4) are the widest shapes whose training tile fits in the H100's 227 KB of shared memory per block."""
+    _simt_update_vs_oracle(OBS, ACT)
+
+
+def _simt_update_vs_oracle(OBS, ACT):
     from tianshou_b200.data import Batch, VectorReplayBuffer
     from tianshou_b200.utils import policy_within_training_step
-    E, T, OBS, ACT = 24, 20, 40, 5
+    E, T = 24, 20
     kw = dict(gamma=0.99, gae_lambda=0.95, max_grad_norm=0.5, vf_coef=0.25, ent_coef=0.01, return_scaling=True,
               eps_clip=0.2, value_clip=True, dual_clip=None, advantage_normalization=True, recompute_advantage=True)
     algo, actor, critic = build_ppo(OBS, ACT, DEV, **kw)
@@ -392,6 +403,21 @@ def test_wide_observation_runs_simt_kernels_vs_oracle():
         np.testing.assert_allclose(getattr(stats, name).mean, res["losses"][:, col].mean(), rtol=1e-3, atol=2e-5, err_msg=name)
     for k, pv in named_params(actor, critic).items():
         np.testing.assert_allclose(pv.detach().cpu().numpy(), p[k], rtol=2e-3, atol=3e-5, err_msg=k)
+
+
+def test_simt_shape_past_shared_memory_is_refused():
+    """obs 64 / act 16 passes the descriptor check but its SIMT training tile needs 235 KB of shared memory: the update
+    must fail with a message naming the size, not an opaque launch-configuration error."""
+    from tianshou_b200.data import Batch, VectorReplayBuffer
+    from tianshou_b200.utils import policy_within_training_step
+    algo, _, _ = build_ppo(64, 16, DEV, gamma=0.99, gae_lambda=0.95, max_grad_norm=0.5, vf_coef=0.25, ent_coef=0.0,
+                           eps_clip=0.2, value_clip=False, advantage_normalization=False)
+    buf = VectorReplayBuffer(4 * 8, 4, device=DEV)
+    for s in synth_rollout(np.random.default_rng(0), 4, 8, 64, 16):
+        buf.add(Batch(**s), buffer_ids=np.arange(4))
+    with pytest.raises(RuntimeError, match="bytes of shared memory per block"):
+        with policy_within_training_step(algo.policy):
+            algo.update(buffer=buf, batch_size=16, repeat=1)
 
 
 def test_a2c_update_matches_reference():

@@ -84,6 +84,78 @@ def build_ppo(obs_dim, act_dim, device, lr=3e-4, params=None, **kw):
     return algo, actor, critic
 
 
+def perturb_params(actor, critic, seed: int = 0) -> None:
+    """Move the parameters of ``build_actor_critic`` away from values that hide indexing bugs: every bias ~ N(0, 0.3)
+    (zero biases cannot tell one bias column from another), a distinct log-std per action dimension (a constant log-std
+    cannot tell one dimension's 1 / sigma^2 from another's) and the actor head at full orthogonal scale instead of x0.01
+    (so mu depends on the observation and the ratios spread over the clip range).  In place: works on the flat views."""
+    import torch
+    g = torch.Generator(device="cpu").manual_seed(seed)
+    named = named_params(actor, critic)
+    with torch.no_grad():
+        for k, p in named.items():
+            if k[2] == "b":
+                p.copy_(0.3 * torch.randn(p.shape, generator=g, dtype=torch.float64))
+        ls = named["a_logstd"]
+        ls.copy_(torch.linspace(-1.2, 0.3, ls.numel(), dtype=torch.float64).reshape(ls.shape))
+        named["a_w3"].mul_(100.0)
+
+
+def param_offsets(flat, actor, critic) -> dict:
+    """Offset of every module parameter inside the flat parameter buffer (the parameters are views of it)."""
+    base = flat.data_ptr()
+    return {k: (p.data.data_ptr() - base) // 4 for k, p in named_params(actor, critic).items()}
+
+
+def ppo_reference_fp64(actor, critic, mb: dict, hp: dict) -> dict:
+    """One minibatch of the PPO / A2C loss (modelfree/ppo.py:183-211, modelfree/a2c.py:262-266) in float64 with torch
+    autograd on CPU, on deep copies of the SAME modules (their Linear layers and log-std parameter, so the gradients
+    come back under the modules' own parameter names).  Independent of oracle_np's hand-written backward.
+
+    mb: obs, act, adv, returns, logp_old, v_s (numpy).  hp: eps_clip, dual_clip (None / 0 = off), value_clip,
+    advantage_normalization, adv_eps, vf_coef, ent_coef, loss_kind ("ppo" | "a2c").
+    Returns v, mu, logp, ratio, value delta (value - v_s), the loss parts (loss, clip, vf, ent) and ``grads`` (13 arrays)."""
+    import copy
+
+    import torch
+    a = copy.deepcopy(actor).to("cpu", torch.float64)
+    c = copy.deepcopy(critic).to("cpu", torch.float64)
+    t = {k: torch.as_tensor(np.asarray(v), dtype=torch.float64) for k, v in mb.items()}
+    obs = t["obs"]
+    # the modules' forward casts observations to float32; run their layers directly in float64 instead
+    mu = a.mu.model(a.preprocess.model.model(obs))
+    sigma = a.sigma_param.reshape(-1).exp().expand_as(mu)
+    dist = torch.distributions.Independent(torch.distributions.Normal(mu, sigma), 1)
+    logp = dist.log_prob(t["act"])
+    value = c.last.model(c.preprocess.model.model(obs)).flatten()
+    adv = t["adv"]
+    ratio = (logp - t["logp_old"]).exp()
+    if hp.get("loss_kind", "ppo") == "a2c":
+        clip_loss = -(logp * adv).mean()
+    else:
+        if hp["advantage_normalization"]:
+            adv = (adv - adv.mean()) / (adv.std() + hp["adv_eps"])          # torch std: ddof = 1
+        eps = hp["eps_clip"]
+        surr1, surr2 = ratio * adv, ratio.clamp(1.0 - eps, 1.0 + eps) * adv
+        obj = torch.min(surr1, surr2)
+        if hp.get("dual_clip"):
+            obj = torch.where(adv < 0, torch.max(obj, hp["dual_clip"] * adv), obj)
+        clip_loss = -obj.mean()
+    R, vs = t["returns"], t["v_s"]
+    if hp.get("value_clip"):
+        v_clip = vs + (value - vs).clamp(-hp["eps_clip"], hp["eps_clip"])
+        vf_loss = torch.max((R - value).pow(2), (R - v_clip).pow(2)).mean()
+    else:
+        vf_loss = (R - value).pow(2).mean()
+    ent = dist.entropy().mean()
+    loss = clip_loss + hp["vf_coef"] * vf_loss - hp["ent_coef"] * ent
+    loss.backward()
+    grads = {k: p.grad.numpy().copy() for k, p in named_params(a, c).items()}
+    d = lambda x: x.detach().numpy().copy()
+    return dict(v=d(value), mu=d(mu), logp=d(logp), ratio=d(ratio), delta=d(value - vs), loss=loss.item(),
+                clip=clip_loss.item(), vf=vf_loss.item(), ent=ent.item(), grads=grads)
+
+
 def restore_vector_buffer(g, prefix: str, E: int, cap: int, device=None):
     """Rebuild a tianshou_b200 VectorReplayBuffer in the exact state stored in a golden file."""
     from tianshou_b200.data import Batch, VectorReplayBuffer

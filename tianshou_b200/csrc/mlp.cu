@@ -877,10 +877,15 @@ int set_smem(K kernel, size_t bytes, const char* fn) {
     static thread_local size_t configured[tsb::kMaxDevices] = {};  // per kernel instantiation and device
     const int dev = tsb::device_ordinal();
     if (bytes > configured[dev]) {
+        // the tile layout grows with obs_dim and act_dim: a shape past the per-block opt-in limit (227 KB on H100, e.g. the
+        // training layout at obs 64 / act 16) is refused with its size instead of an opaque cudaErrorInvalidValue
+        int optin = 0;
+        TS_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+        TS_REQUIRE(bytes <= (size_t)optin, "%s: this network shape needs %zu bytes of shared memory per block, the device allows %d",
+                   fn, bytes, optin);
         TS_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
         configured[dev] = bytes;
     }
-    (void)fn;
     return 0;
 }
 
