@@ -1,7 +1,9 @@
 // Non-GEMM pieces of the off-policy update bodies (SAC / DDPG-family critics, DQN with the NatureCNN):
 // frame-stack + im2col gathers, col2im, layout permutes, loss rows with their analytic backward, Adam, Polyak.
 // All HBM / latency bound elementwise or gather work: coalesced along the fastest output dimension, grid sized
-// in multiples of the SM count, no atomics (every output element has one owner -> deterministic).
+// in multiples of the SM count, no atomics (every output element has one owner -> deterministic).  grid_for caps the
+// grid at 16 blocks per SM, so every kernel launched through TS_LAUNCH_1D is a grid-stride loop: a one-thread-per-row
+// kernel would leave the rows past num_sms * 16 * 256 unwritten.
 //
 // Reference code replaced: ReplayBuffer.get frame stacking (data/buffer/buffer_base.py:557-603), DQNet conv stack
 // (env/atari/atari_network.py:77-84), SACPolicy.forward tanh-squashed Gaussian (modelfree/sac.py:108-131),
@@ -29,20 +31,20 @@ inline unsigned grid_for(int64_t n, int threads = 256) {
 __global__ void stack_prev_kernel(const int64_t* __restrict__ idx, int64_t n, int S, const int64_t* __restrict__ offset, int64_t E,
                                   const uint8_t* __restrict__ done, const int64_t* __restrict__ last_index,
                                   const int64_t* __restrict__ lengths, int64_t* __restrict__ out) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
     const int64_t total = offset[E];
-    int64_t cur = tsb::pymod(idx[i], total);
-    const int64_t e = tsb::find_subbuffer(offset, E, cur);
-    const int64_t start = offset[e];
-    const int64_t L = lengths[e] > 1 ? lengths[e] : 1;
-    const int64_t last = last_index[e];
-    out[i * S + (S - 1)] = cur;
-    for (int s = S - 2; s >= 0; --s) {
-        const int64_t p = tsb::pymod(cur - start - 1, L);
-        const int64_t end = (done[p + start] | (p + start == last)) ? 1 : 0;
-        cur = tsb::pymod(p + end, L) + start;
-        out[i * S + s] = cur;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        int64_t cur = tsb::pymod(idx[i], total);
+        const int64_t e = tsb::find_subbuffer(offset, E, cur);
+        const int64_t start = offset[e];
+        const int64_t L = lengths[e] > 1 ? lengths[e] : 1;
+        const int64_t last = last_index[e];
+        out[i * S + (S - 1)] = cur;
+        for (int s = S - 2; s >= 0; --s) {
+            const int64_t p = tsb::pymod(cur - start - 1, L);
+            const int64_t end = (done[p + start] | (p + start == last)) ? 1 : 0;
+            cur = tsb::pymod(p + end, L) + start;
+            out[i * S + s] = cur;
+        }
     }
 }
 
@@ -146,22 +148,22 @@ __global__ void concat2_kernel(const float* __restrict__ a, int wa, const float*
 __global__ void squashed_gaussian_kernel(const float* __restrict__ head, int64_t ld, const float* __restrict__ noise,
                                          int64_t B, int A, float sig_min, float sig_max, float eps, float* __restrict__ act,
                                          float* __restrict__ logp, float* __restrict__ sigma_out) {
-    const int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (b >= B) return;
-    float lp = 0.0f, corr = 0.0f;
-    for (int a = 0; a < A; ++a) {
-        const float m = head[b * ld + a];
-        const float ls = fminf(fmaxf(head[b * ld + A + a], sig_min), sig_max);
-        const float sg = expf(ls);
-        const float x = fmaf(sg, noise[b * A + a], m);      // loc + eps * scale
-        const float d = x - m;
-        lp += -(d * d) / (2.0f * (sg * sg)) - logf(sg) - 0.9189385332046727f;
-        const float t = tanhf(x);
-        corr += logf(1.0f - t * t + eps);
-        act[b * A + a] = t;
-        if (sigma_out) sigma_out[b * A + a] = sg;
+    for (int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; b < B; b += (int64_t)gridDim.x * blockDim.x) {
+        float lp = 0.0f, corr = 0.0f;
+        for (int a = 0; a < A; ++a) {
+            const float m = head[b * ld + a];
+            const float ls = fminf(fmaxf(head[b * ld + A + a], sig_min), sig_max);
+            const float sg = expf(ls);
+            const float x = fmaf(sg, noise[b * A + a], m);      // loc + eps * scale
+            const float d = x - m;
+            lp += -(d * d) / (2.0f * (sg * sg)) - logf(sg) - 0.9189385332046727f;
+            const float t = tanhf(x);
+            corr += logf(1.0f - t * t + eps);
+            act[b * A + a] = t;
+            if (sigma_out) sigma_out[b * A + a] = sg;
+        }
+        logp[b] = lp - corr;
     }
-    logp[b] = lp - corr;
 }
 // Backward of  L = mean_b( alpha * logp_b - min(q1_b, q2_b) )  w.r.t. (mu, raw log-sigma), given dq_da = d(-min(q1,q2))/d act
 // already summed into `dact` by the critics' input-gradient GEMMs (scaled by 1/B) and alpha/B for the log-prob part.
@@ -172,82 +174,82 @@ __global__ void squashed_gaussian_bwd_kernel(const float* __restrict__ head, int
                                              const float* __restrict__ act, const float* __restrict__ sigma, const float* __restrict__ dact,
                                              int64_t B, int A, float sig_min, float sig_max, float eps, float alpha_over_b,
                                              float* __restrict__ dhead) {
-    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= B * A) return;
-    const int64_t b = t / A;
-    const int a = (int)(t - b * A);
-    const float tt = act[t], one_m = 1.0f - tt * tt;
-    const float dlp_dx = 2.0f * tt * one_m / (one_m + eps);
-    const float gx = alpha_over_b * dlp_dx + dact[t] * one_m;          // dL/dx
-    const float sg = sigma[t], nz = noise[t];
-    const float gsig = gx * nz - alpha_over_b / sg;
-    const float r = head[b * ld + A + a];
-    dhead[b * ld + a] = gx;
-    dhead[b * ld + A + a] = (r >= sig_min && r <= sig_max) ? gsig * sg : 0.0f;
+    for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < B * A; t += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t b = t / A;
+        const int a = (int)(t - b * A);
+        const float tt = act[t], one_m = 1.0f - tt * tt;
+        const float dlp_dx = 2.0f * tt * one_m / (one_m + eps);
+        const float gx = alpha_over_b * dlp_dx + dact[t] * one_m;          // dL/dx
+        const float sg = sigma[t], nz = noise[t];
+        const float gsig = gx * nz - alpha_over_b / sg;
+        const float r = head[b * ld + A + a];
+        dhead[b * ld + a] = gx;
+        dhead[b * ld + A + a] = (r >= sig_min && r <= sig_max) ? gsig * sg : 0.0f;
+    }
 }
 
 // ---- per-row losses ----------------------------------------------------------------------------------------------
 // critic: td = q - target ; loss = mean(td^2 * w) ; dq = 2 td w / B          (ddpg.py:279-284)
 __global__ void critic_mse_kernel(const float* __restrict__ q, const float* __restrict__ target, const float* __restrict__ weight, int64_t B,
                                   float* __restrict__ td_out, float* __restrict__ dq, float* __restrict__ loss_rows) {
-    const int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (b >= B) return;
-    const float td = q[b] - target[b];
-    const float w = weight ? weight[b] : 1.0f;
-    td_out[b] = td;
-    dq[b] = 2.0f * td * w / (float)B;
-    loss_rows[b] = td * td * w;
+    for (int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; b < B; b += (int64_t)gridDim.x * blockDim.x) {
+        const float td = q[b] - target[b];
+        const float w = weight ? weight[b] : 1.0f;
+        td_out[b] = td;
+        dq[b] = 2.0f * td * w / (float)B;
+        loss_rows[b] = td * td * w;
+    }
 }
 // DQN: q_sel = q[b][act[b]] ; td = returns - q_sel ; MSE (weighted) or Huber(delta) ; dq only at the taken action (dqn.py:384-399)
 __global__ void dqn_loss_kernel(const float* __restrict__ q, const int64_t* __restrict__ act, const float* __restrict__ returns,
                                 const float* __restrict__ weight, int64_t B, int A, float huber_delta, float* __restrict__ td_out,
                                 float* __restrict__ dq, float* __restrict__ loss_rows) {
-    const int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (b >= B) return;
-    const int a_sel = (int)act[b];
-    const float qs = q[b * A + a_sel];
-    const float td = returns[b] - qs;
-    float lrow, g;       // g = d loss_row / d q_sel (before the 1 / B of the mean)
-    if (huber_delta > 0.0f) {       // F.huber_loss(y = q, t = returns, delta), reduction mean, unweighted (dqn.py:388-394)
-        const float d = qs - returns[b], ad = fabsf(d);
-        if (ad < huber_delta) { lrow = 0.5f * d * d; g = d; }
-        else { lrow = huber_delta * (ad - 0.5f * huber_delta); g = d > 0.0f ? huber_delta : -huber_delta; }
-    } else {
-        const float w = weight ? weight[b] : 1.0f;
-        lrow = td * td * w;
-        g = -2.0f * td * w;
+    for (int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; b < B; b += (int64_t)gridDim.x * blockDim.x) {
+        const int a_sel = (int)act[b];
+        const float qs = q[b * A + a_sel];
+        const float td = returns[b] - qs;
+        float lrow, g;       // g = d loss_row / d q_sel (before the 1 / B of the mean)
+        if (huber_delta > 0.0f) {       // F.huber_loss(y = q, t = returns, delta), reduction mean, unweighted (dqn.py:388-394)
+            const float d = qs - returns[b], ad = fabsf(d);
+            if (ad < huber_delta) { lrow = 0.5f * d * d; g = d; }
+            else { lrow = huber_delta * (ad - 0.5f * huber_delta); g = d > 0.0f ? huber_delta : -huber_delta; }
+        } else {
+            const float w = weight ? weight[b] : 1.0f;
+            lrow = td * td * w;
+            g = -2.0f * td * w;
+        }
+        td_out[b] = td;
+        loss_rows[b] = lrow;
+        for (int a = 0; a < A; ++a) dq[b * A + a] = a == a_sel ? g / (float)B : 0.0f;
     }
-    td_out[b] = td;
-    loss_rows[b] = lrow;
-    for (int a = 0; a < A; ++a) dq[b * A + a] = a == a_sel ? g / (float)B : 0.0f;
 }
 // out[b] = argmax_a q[b][a] (first maximum, torch.max(dim=1)) ; val[b] = q2[b][out[b]] (double DQN) or max_a q2[b][a]
 __global__ void dqn_target_kernel(const float* __restrict__ q_online, const float* __restrict__ q_target, int64_t B, int A, int is_double,
                                   float* __restrict__ out) {
-    const int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (b >= B) return;
     const float* src = is_double ? q_online : q_target;
-    int best = 0;
-    float bv = src[b * A];
-    for (int a = 1; a < A; ++a) { const float v = src[b * A + a]; if (v > bv) { bv = v; best = a; } }
-    out[b] = q_target[b * A + best];
+    for (int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; b < B; b += (int64_t)gridDim.x * blockDim.x) {
+        int best = 0;
+        float bv = src[b * A];
+        for (int a = 1; a < A; ++a) { const float v = src[b * A + a]; if (v > bv) { bv = v; best = a; } }
+        out[b] = q_target[b * A + best];
+    }
 }
 // SAC target: min(q1, q2) - alpha * logp   (td3.py:94-102, sac.py:298-302)
 __global__ void sac_target_kernel(const float* __restrict__ q1, const float* __restrict__ q2, const float* __restrict__ logp, float alpha,
                                   int64_t B, float* __restrict__ out) {
-    const int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (b >= B) return;
-    out[b] = fminf(q1[b], q2[b]) - alpha * logp[b];
+    for (int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; b < B; b += (int64_t)gridDim.x * blockDim.x)
+        out[b] = fminf(q1[b], q2[b]) - alpha * logp[b];
 }
 // d(-min(q1, q2))/d(q1, q2) / B with torch.minimum's tie rule (equal -> half each); also the actor-loss rows
 __global__ void sac_actor_q_grad_kernel(const float* __restrict__ q1, const float* __restrict__ q2, const float* __restrict__ logp, float alpha,
                                         int64_t B, float* __restrict__ dq1, float* __restrict__ dq2, float* __restrict__ loss_rows) {
-    const int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (b >= B) return;
-    const float a = q1[b], c = q2[b], g = -1.0f / (float)B;
-    dq1[b] = a < c ? g : (a == c ? 0.5f * g : 0.0f);
-    dq2[b] = c < a ? g : (a == c ? 0.5f * g : 0.0f);
-    loss_rows[b] = alpha * logp[b] - fminf(a, c);
+    const float g = -1.0f / (float)B;
+    for (int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; b < B; b += (int64_t)gridDim.x * blockDim.x) {
+        const float a = q1[b], c = q2[b];
+        dq1[b] = a < c ? g : (a == c ? 0.5f * g : 0.0f);
+        dq2[b] = c < a ? g : (a == c ? 0.5f * g : 0.0f);
+        loss_rows[b] = alpha * logp[b] - fminf(a, c);
+    }
 }
 // mean of n values in a fixed order: one block, pairwise tree over 1024 lanes (the values are per-row loss terms)
 __global__ void mean_kernel(const float* __restrict__ x, int64_t n, float* __restrict__ out) {
@@ -276,9 +278,11 @@ __global__ void sumsq_kernel(const float* __restrict__ g, int64_t n, double* __r
     }
     if (threadIdx.x == 0) partial[blockIdx.x] = s[0];
 }
-// torch.optim.Adam single-tensor step (lerp / addcmul / addcdiv order), optional clip_grad_norm_ from `partial` block sums
+// torch.optim.Adam single-tensor step (lerp / addcmul / addcdiv order), optional clip_grad_norm_ from `partial` block sums.
+// w1 = 1 - beta1 and w2 = 1 - beta2 are formed in double and rounded once, as torch passes them (lerp weight, addcmul
+// value): 1.0f - (float)0.999 would be 1.3e-5 off in relative terms.
 __global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v, int64_t n,
-                            float step_size, float bc2_sqrt, float beta1, float beta2, float eps, float wd, float max_norm,
+                            float step_size, float bc2_sqrt, float beta2, float w1, float w2, float eps, float wd, float max_norm,
                             const double* __restrict__ partial, int n_partial) {
     float coef = 1.0f;
     if (max_norm > 0.0f && partial) {
@@ -286,7 +290,6 @@ __global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, 
         for (int i = 0; i < n_partial; ++i) t += partial[i];
         coef = fminf(max_norm / ((float)sqrt(t) + 1e-6f), 1.0f);
     }
-    const float w1 = 1.0f - beta1, w2 = 1.0f - beta2;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
         float gi = g[i] * coef;
         float pv = p[i];
@@ -319,8 +322,8 @@ __global__ void adam_dev_kernel(float* __restrict__ p, const float* __restrict__
     }
     __syncthreads();
     const float step_size = s_step_size, bc2_sqrt = s_bc2_sqrt, coef = s_coef;
-    const float beta1 = (float)beta1d, beta2 = (float)beta2d;
-    const float w1 = 1.0f - beta1, w2 = 1.0f - beta2;
+    const float beta2 = (float)beta2d;
+    const float w1 = (float)(1.0 - beta1d), w2 = (float)(1.0 - beta2d);
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
         float gi = g[i] * coef;
         float pv = p[i];
@@ -439,8 +442,8 @@ extern "C" int ts_adam_step(float* params, const float* grad, float* exp_avg, fl
         if (tsb::check_launch("ts_adam_step/norm")) return 1;
     }
     const double bc1 = 1.0 - pow(beta1, (double)step), bc2 = 1.0 - pow(beta2, (double)step);
-    adam_kernel<<<grid_for(n), 256, 0, st>>>(params, grad, exp_avg, exp_avg_sq, n, (float)(lr / bc1), (float)sqrt(bc2), (float)beta1,
-                                             (float)beta2, (float)eps, (float)weight_decay, (float)max_grad_norm, norm_scratch, n_partial);
+    adam_kernel<<<grid_for(n), 256, 0, st>>>(params, grad, exp_avg, exp_avg_sq, n, (float)(lr / bc1), (float)sqrt(bc2), (float)beta2,
+                                             (float)(1.0 - beta1), (float)(1.0 - beta2), (float)eps, (float)weight_decay, (float)max_grad_norm, norm_scratch, n_partial);
     return tsb::check_launch("ts_adam_step");
 }
 extern "C" int ts_adam_step_dev(float* params, const float* grad, float* exp_avg, float* exp_avg_sq, int64_t n, int64_t* step_dev, double lr,
