@@ -431,6 +431,45 @@ int ts_ppo_rows(const float* head, const float* value, const float* logstd, cons
 /* stats row (loss, actor loss, vf loss, entropy, -, rows) from loss_rows */
 int ts_ppo_rows_stats(const float* loss_rows, int64_t B, const ts_ppo_hparams* hp, float* stats_row, ts_stream_t stream);
 
+/* NPG / TRPO on a layered actor (modelfree/npg.py:123-224, modelfree/trpo.py:132-191).  head [B][A] = mu (Gaussian,
+ * sigma = exp(logstd[A])) or logits (categorical, Categorical(probs = softmax(logits))); act as in ts_ppo_rows.
+ *
+ * Fisher-vector product rows (npg.py:195-200 without the damping term): the Gauss-Newton product J^T H J of the actor, H the
+ * Hessian of the row's KL(old || new) w.r.t. the head outputs at old = new.  tangent [B][A] = J v on the head; out [B][A] =
+ * (H tangent) / B feeds the backward GEMMs; Gaussian: out_logstd[A] = 2 * tangent_logstd (the whole log-std part, not rows). */
+int ts_npg_fvp_rows(const float* head, const float* tangent, const float* logstd, const float* tangent_logstd, int64_t B,
+                    int32_t A, int32_t categorical, float* out, float* out_logstd, ts_stream_t stream);
+/* surrogate rows: loss_rows[B] = -logp * adv (npg.py:155-156) or, ratio_surrogate, -exp(logp - logp_old) * adv
+ * (trpo.py:135-138); with dhead != NULL d(mean loss)/d head [B][A] and, Gaussian, per-row d / d logstd [B][A] */
+int ts_npg_rows(const float* head, const float* logstd, const float* act, const float* adv, const float* logp_old, int64_t B,
+                int32_t A, int32_t categorical, int32_t ratio_surrogate, float* loss_rows, float* dhead, float* dlogstd_rows,
+                ts_stream_t stream);
+/* kl_rows[B] = KL(old || new) per row with torch's kl_divergence formulas (npg.py:172-174, trpo.py:177), categorical: inf
+ * where a new probability is exactly 0 */
+int ts_npg_kl_rows(const float* head_old, const float* logstd_old, const float* head_new, const float* logstd_new, int64_t B,
+                   int32_t A, int32_t categorical, float* kl_rows, ts_stream_t stream);
+/* *out = mean of rows[B], fixed summation order */
+int ts_npg_mean_rows(const float* rows, int64_t B, float* out, ts_stream_t stream);
+/* conjugate gradient (npg.py:202-224) with its scalars in device memory: state[3] doubles = (r.r, done flag, iterations).
+ * ts_cg_init: x = 0, r = p = g.  ts_cg_step: z = F p on entry (damping added here: z += damping p), then alpha, x, r, the new
+ * r.r in fp64, the residual test (done: this and every later step is a no-op) and p.  iters_out (nullable) <- iterations. */
+int ts_cg_init(const float* g, float* x, float* r, float* p, int64_t n, double* state, ts_stream_t stream);
+int ts_cg_step(float* x, float* r, float* p, float* z, int64_t n, double damping, double residual_tol, double* state,
+               float* iters_out, ts_stream_t stream);
+/* trpo.py:152-159: z = F s on entry; *step = sqrt(2 max_kl / (s . (z + damping s))); stats_row[2] = 0 (kl), [3] = *step,
+ * [5] = -1 (accepted candidate), [6] = 0 (line search failed) */
+int ts_trpo_step_size(const float* s, const float* z, int64_t n, double damping, double max_kl, float* step, float* stats_row,
+                      ts_stream_t stream);
+/* out = theta + coef * (scale ? *scale : 1) * dir  (npg.py:168-170 natural step, trpo.py:165 line-search candidate) */
+int ts_npg_axpy(float* out, const float* theta, const float* dir, double coef, const float* scale, int64_t n, ts_stream_t stream);
+/* trpo.py:170-186 for candidate i < max_backtracks: mean new loss / kl from the rows, stats_row[2] = kl; accepted when
+ * kl < max_kl and new loss < stats_row[0] (*flag = 1, stats_row[3] = *step, [5] = i); else *step *= backtrack_coeff
+ * (*flag = 0) or, at the last candidate, stats_row[3] = 0, [6] = 1 (*flag = 2) */
+int ts_trpo_decide(const float* loss_rows, const float* kl_rows, int64_t B, int32_t i, int32_t max_backtracks, double max_kl,
+                   double backtrack_coeff, float* step, float* stats_row, int32_t* flag, ts_stream_t stream);
+/* npg.py:136-137: adv = (adv - mean) / std over the whole batch, unbiased std, no epsilon */
+int ts_npg_normalize_adv(float* adv, int64_t n, ts_stream_t stream);
+
 /* Frame stacking on the device (ReplayBuffer.get, data/buffer/buffer_base.py:557-603): out[i][s] for s = 0..S-1 is
  * the slot of the s-th oldest frame of the stacked observation of index[i] (out[i][S-1] = index[i], each earlier
  * one = prev() of the next, manager.py:311-336). */

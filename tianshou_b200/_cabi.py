@@ -108,6 +108,17 @@ SIGNATURES: dict[str, list[Any]] = {
     "ts_ppo_rows": [_P, _P, _P, _P, _P, _P, _P, _P, _I64, _I32, _I32, _P, _I64, _P, _P, _P, _P, _P, _P, _P],
     "ts_ppo_rows_stats": [_P, _I64, _P, _P, _P],
     "ts_net_colsum": [_P, _I64, _I32, _I32, _P, _I32, _P],
+    # NPG / TRPO (npg.cu)
+    "ts_npg_fvp_rows": [_P, _P, _P, _P, _I64, _I32, _I32, _P, _P, _P],
+    "ts_npg_rows": [_P, _P, _P, _P, _P, _I64, _I32, _I32, _I32, _P, _P, _P, _P],
+    "ts_npg_kl_rows": [_P, _P, _P, _P, _I64, _I32, _I32, _P, _P],
+    "ts_npg_mean_rows": [_P, _I64, _P, _P],
+    "ts_cg_init": [_P, _P, _P, _P, _I64, _P, _P],
+    "ts_cg_step": [_P, _P, _P, _P, _I64, _D, _D, _P, _P, _P],
+    "ts_trpo_step_size": [_P, _P, _I64, _D, _D, _P, _P, _P],
+    "ts_npg_axpy": [_P, _P, _P, _D, _P, _I64, _P],
+    "ts_trpo_decide": [_P, _P, _I64, _I32, _I32, _D, _D, _P, _P, _P, _P],
+    "ts_npg_normalize_adv": [_P, _I64, _P],
     "ts_stack_prev_indices": [_P, _I64, _I32, _P, _I64, _P, _P, _P, _P, _P],
     "ts_im2col_u8": [_P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _D, _P, _P],
     "ts_im2col_f32": [_P, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P],

@@ -1,13 +1,15 @@
 from .base import Algorithm, OffPolicyAlgorithm, OnPolicyAlgorithm, Policy, TrainingStats
 from .flat_params import UnsupportedModelError
 from .modelfree.a2c import A2CTrainingStats, ActorCriticOnPolicyAlgorithm
+from .modelfree.npg import NPG, NPGTrainingStats
 from .modelfree.ppo import A2C, PPO
 from .modelfree.reinforce import DiscreteActorPolicy, ProbabilisticActorPolicy
+from .modelfree.trpo import TRPO, TRPOTrainingStats
 from .optim import AdamOptimizerFactory, LRSchedulerFactoryLinear, OptimizerFactory, RMSpropOptimizerFactory
 
 __all__ = [
     "Algorithm", "OffPolicyAlgorithm", "OnPolicyAlgorithm", "Policy", "TrainingStats",
-    "UnsupportedModelError", "A2CTrainingStats", "ActorCriticOnPolicyAlgorithm", "PPO", "A2C",
+    "UnsupportedModelError", "A2CTrainingStats", "ActorCriticOnPolicyAlgorithm", "PPO", "A2C", "NPG", "TRPO", "NPGTrainingStats", "TRPOTrainingStats",
     "ProbabilisticActorPolicy", "DiscreteActorPolicy", "AdamOptimizerFactory", "LRSchedulerFactoryLinear", "OptimizerFactory",
     "RMSpropOptimizerFactory",
 ]

@@ -29,7 +29,9 @@ _CHUNK = 131072          # rows per forward chunk of the whole-rollout passes (b
 
 
 class LayeredActorCritic:
-    def __init__(self, actor: Any, critic: Any, device: torch.device) -> None:
+    def __init__(self, actor: Any, critic: Any, device: torch.device, split: bool = False) -> None:
+        """``split``: the actor and the critic get one ``FlatGroup`` each (``group`` / ``critic_group``) -- NPG / TRPO step the
+        actor along the natural gradient and the critic with its own optimiser; otherwise both share ``group``."""
         self.device = device
         self.categorical = hasattr(actor, "softmax_output")
         if self.categorical and not actor.softmax_output:
@@ -45,6 +47,9 @@ class LayeredActorCritic:
             if getattr(net, "softmax", False):
                 raise UnsupportedModelError(f"{what}: softmax trunk output unsupported")
         self.shared = actor.preprocess is critic.preprocess
+        if split and self.shared:
+            raise UnsupportedModelError("a critic-only optimiser (NPG / TRPO) needs separate actor and critic trunks; "
+                                        "shared trunks are unsupported")
         a_mods = module_layers(actor.preprocess)
         first = next((m for m in a_mods if isinstance(m, nn.Linear)), None)
         if first is None:
@@ -65,15 +70,18 @@ class LayeredActorCritic:
             if id(p) not in seen:
                 seen.add(id(p))
                 params.append(p)
-        self.group = FlatGroup(params, device)
         covered = {id(L.weight) for L in (*a_trunk, *c_trunk, *a_head, *c_head)} | {id(L.bias) for L in (*a_trunk, *c_trunk, *a_head, *c_head)}
         extra = [p for p in params if id(p) not in covered]
         self.sigma_param = None if self.categorical else actor.sigma_param
         if [id(p) for p in extra] != ([] if self.categorical else [id(self.sigma_param)]):
             raise UnsupportedModelError("actor / critic hold parameters outside the Linear layers")
+        if split:      # npg.py:195-224 works on policy.actor.parameters() in their order
+            self.group, self.critic_group = FlatGroup(list(actor.parameters()), device), FlatGroup(list(critic.parameters()), device)
+        else:
+            self.group = self.critic_group = FlatGroup(params, device)
         self.a_trunk, self.a_head = FusedStack(a_trunk, self.group, "a_trunk"), FusedStack(a_head, self.group, "a_head")
-        self.c_trunk = self.a_trunk if self.shared else FusedStack(c_trunk, self.group, "c_trunk")
-        self.c_head = FusedStack(c_head, self.group, "c_head")
+        self.c_trunk = self.a_trunk if self.shared else FusedStack(c_trunk, self.critic_group, "c_trunk")
+        self.c_head = FusedStack(c_head, self.critic_group, "c_head")
         self._a_act, self._c_act = a_trunk[-1].act, c_trunk[-1].act
         self._scratch: dict[str, torch.Tensor] = {}
 
@@ -159,11 +167,11 @@ class LayeredActorCritic:
         self.group.adam_step(optimizer, max_grad_norm)
 
 
-def try_layered(actor: Any, critic: Any) -> LayeredActorCritic:
+def try_layered(actor: Any, critic: Any, split: bool = False) -> LayeredActorCritic:
     plist = list(actor.parameters())
     if not plist or plist[0].device.type != "cuda":
         raise UnsupportedModelError("actor/critic must live on a CUDA device; tianshou_b200 has no CPU path")
-    return LayeredActorCritic(actor, critic, plist[0].device)
+    return LayeredActorCritic(actor, critic, plist[0].device, split=split)
 
 
 def layered_update(algo: Any, batch: Any, batch_size: int | None, repeat: int) -> torch.Tensor:

@@ -67,25 +67,30 @@ class ActorCriticOnPolicyAlgorithm(OnPolicyAlgorithm, ABC):
         assert 0.0 <= gamma <= 1.0, f"discount factor gamma should be in [0, 1] but got: {gamma}"
         self.gae_lambda = gae_lambda
         self.max_batchsize = max_batchsize  # kept for API parity; the fused pass needs no chunking
-        if not optim_include_actor:
-            raise UnsupportedModelError("critic-only optimizers (optim_include_actor=False) are not fused yet")
         self._actor_critic = ActorCritic(self.policy.actor, self.critic)
         # kernel-side view of the networks: validate structure, flatten parameters.  Shapes outside the fused kernels' envelope
         # (two 64-wide layers, obs <= 64) run layer by layer on the tensor-core GEMM (algorithm/layered.py); anything that is
         # not a Linear / ReLU | Tanh actor-critic raises -- there is no eager-PyTorch path.
         self._layered = None
-        try:
-            import os as _os
-            if _os.environ.get("TS_B200_FORCE_LAYERED", "0") == "1":      # tests: run the layer-wise path on any shape
-                raise UnsupportedModelError("TS_B200_FORCE_LAYERED=1")
-            self._desc, plist = describe_actor_critic(self.policy.actor, self.critic)
-        except UnsupportedModelError as fused_err:
+        if not optim_include_actor:
+            # critic-only optimiser (NPG / TRPO, a2c.py:102-109): the actor moves along the natural gradient, so the fused
+            # kernels (one Adam step over both networks) do not apply; the layer-wise path runs whatever the shape
             from ..layered import try_layered
+            self._layered = try_layered(self.policy.actor, self.critic, split=True)
+            self._desc, plist = None, self._layered.critic_group.params
+        else:
             try:
-                self._layered = try_layered(self.policy.actor, self.critic)
-            except UnsupportedModelError as layered_err:
-                raise UnsupportedModelError(f"{fused_err}; layer-wise path: {layered_err}") from layered_err
-            self._desc, plist = None, self._layered.group.params
+                import os as _os
+                if _os.environ.get("TS_B200_FORCE_LAYERED", "0") == "1":      # tests: run the layer-wise path on any shape
+                    raise UnsupportedModelError("TS_B200_FORCE_LAYERED=1")
+                self._desc, plist = describe_actor_critic(self.policy.actor, self.critic)
+            except UnsupportedModelError as fused_err:
+                from ..layered import try_layered
+                try:
+                    self._layered = try_layered(self.policy.actor, self.critic)
+                except UnsupportedModelError as layered_err:
+                    raise UnsupportedModelError(f"{fused_err}; layer-wise path: {layered_err}") from layered_err
+                self._desc, plist = None, self._layered.group.params
         dev = plist[0].device
         if dev.type != "cuda":
             raise UnsupportedModelError(
@@ -99,7 +104,7 @@ class ActorCriticOnPolicyAlgorithm(OnPolicyAlgorithm, ABC):
         if self._layered is not None:
             if self._world_size() > 1 and getattr(self, "data_parallel", True):
                 raise UnsupportedModelError("the layer-wise actor-critic path is single-GPU")
-            self._flat = self._layered.group
+            self._flat = self._layered.critic_group        # the optimiser's parameters (``group`` unless split)
             self._flat.weight_image = None
         else:
             self._flat = FlatParams(plist, dev, GRAD_EXTRA)
@@ -115,7 +120,8 @@ class ActorCriticOnPolicyAlgorithm(OnPolicyAlgorithm, ABC):
                 from ...parallel import broadcast_params_
                 broadcast_params_(self._flat.flat)
         # a real torch Adam (+ scheduler) keeps lr schedules and state_dict round trips unchanged
-        self.optim = self._create_optimizer(self._actor_critic, optim, max_grad_norm=max_grad_norm)
+        self.optim = self._create_optimizer(self._actor_critic if optim_include_actor else self.critic, optim,
+                                            max_grad_norm=max_grad_norm)
         adam_hyperparams(self.optim._optim)  # validates optimizer family early
         self.optim._flat = self._flat
         self.max_grad_norm = max_grad_norm

@@ -279,6 +279,30 @@ class FusedStack:
             cur = y
         return acts
 
+    # ------------------------------------------------------------------ tangent (forward-mode) pass
+    def jvp(self, acts: list[torch.Tensor], tangent: torch.Tensor, rows: int, tag: str = "a",
+            x_dot: torch.Tensor | None = None) -> list[torch.Tensor]:
+        """Tangents ``[y1', ..., yL']`` of the layer outputs of ``forward`` (its activation list ``acts``) along the parameter
+        direction ``tangent`` (a flat buffer in the group's layout), plus the input tangent ``x_dot`` (None: the input is
+        data).  Per Linear layer ``y' = act'(y) * (x W'^T + b' + x' W^T)``: two GEMM launches, the second accumulating (one when
+        ``x_dot`` is None)."""
+        out: list[torch.Tensor] = []
+        cur = x_dot
+        for i, L in enumerate(self.layers):
+            if L.kind != "linear":
+                raise UnsupportedModelError("tangent passes support Linear layers only")
+            yd = self._buf((tag, "t", i), rows * L.out_dim)[: rows * L.out_dim].view(rows, L.out_dim)
+            mask = ptr(acts[i + 1]) if L.act != ACT_NONE else None
+            kind = L.act if L.act != ACT_NONE else ACT_RELU
+            self._gemm(ptr(acts[i]), L.in_dim, 0, self._w(L, tangent), L.in_dim, 0, ptr(yd), L.out_dim, rows, L.out_dim, L.in_dim,
+                       bias=self._b(L, tangent), mask=mask, ld_mask=L.out_dim, mask_kind=kind)
+            if cur is not None:
+                self._gemm(ptr(cur), L.in_dim, 0, self._w(L), L.in_dim, 0, ptr(yd), L.out_dim, rows, L.out_dim, L.in_dim,
+                           mask=mask, ld_mask=L.out_dim, mask_kind=kind, accumulate=True)
+            out.append(yd)
+            cur = yd
+        return out
+
     # ------------------------------------------------------------------ backward
     def backward(self, acts: list[torch.Tensor], dy: torch.Tensor, rows: int, tag: str = "a", *, param_grads: bool = True,
                  input_grad: bool = False, input_cols: tuple[int, int] | None = None, dy_preact: bool = False,

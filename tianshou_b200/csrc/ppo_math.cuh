@@ -87,5 +87,41 @@ __device__ __forceinline__ float normal_logp_term(float x, float mu, float sigma
     return -(diff * diff) / (2.0f * var) - logf(sigma) - 0.9189385332046727f;
 }
 
+// Categorical(probs = softmax(z)) of one row (utils/net/discrete.py:69-92 + torch.distributions.Categorical), shared by
+// the PPO loss rows (ppo_rows.cu) and the NPG / TRPO rows (npg.cu).
+constexpr int kCatMaxA = 64;
+struct Cat { float p[kCatMaxA], pn[kCatMaxA], lg[kCatMaxA]; float s2; };
+// p = softmax(z); Categorical renormalises (pn = p / sum p), logits = log(clamp(pn, eps, 1 - eps)); entropy = -sum pn * logits
+__device__ __forceinline__ void cat_forward(const float* z, int A, int action, Cat& c, float& logp, float& ent) {
+    constexpr float eps = 1.1920928955078125e-07f;
+    float m = z[0];
+    for (int a = 1; a < A; ++a) m = fmaxf(m, z[a]);
+    float s = 0.0f;
+    for (int a = 0; a < A; ++a) { c.p[a] = expf(z[a] - m); s += c.p[a]; }
+    float s2 = 0.0f;
+    for (int a = 0; a < A; ++a) { c.p[a] = c.p[a] / s; s2 += c.p[a]; }
+    c.s2 = s2;
+    ent = 0.0f;
+    for (int a = 0; a < A; ++a) {
+        c.pn[a] = c.p[a] / s2;
+        c.lg[a] = logf(fminf(fmaxf(c.pn[a], eps), 1.0f - eps));
+        ent -= c.pn[a] * c.lg[a];
+    }
+    logp = (action >= 0 && action < A) ? c.lg[action] : 0.0f;
+}
+// autograd's chain: gather + entropy -> log o clamp -> renormalisation -> softmax
+__device__ __forceinline__ void cat_backward(const Cat& c, int A, int action, float gl, float ge, float* dz) {
+    constexpr float eps = 1.1920928955078125e-07f;
+    float dot = 0.0f;
+    for (int a = 0; a < A; ++a) {
+        const float dlg = (a == action ? gl : 0.0f) - ge * c.pn[a];
+        const bool pass = c.pn[a] >= eps && c.pn[a] <= 1.0f - eps;
+        dz[a] = -ge * c.lg[a] + (pass ? dlg / c.pn[a] : 0.0f);
+        dot += dz[a] * c.pn[a];
+    }
+    float dot2 = 0.0f;
+    for (int a = 0; a < A; ++a) { dz[a] = (dz[a] - dot) / c.s2; dot2 += dz[a] * c.p[a]; }
+    for (int a = 0; a < A; ++a) dz[a] = c.p[a] * (dz[a] - dot2);
+}
 
 }  // namespace ppo

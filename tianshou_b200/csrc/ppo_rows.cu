@@ -12,41 +12,7 @@
 
 namespace {
 
-constexpr int kMaxA = 64;
-
-struct Cat { float p[kMaxA], pn[kMaxA], lg[kMaxA]; float s2; };
-// p = softmax(z); Categorical renormalises (pn = p / sum p), logits = log(clamp(pn, eps, 1 - eps)); entropy = -sum pn * logits
-__device__ __forceinline__ void cat_forward(const float* z, int A, int action, Cat& c, float& logp, float& ent) {
-    constexpr float eps = 1.1920928955078125e-07f;
-    float m = z[0];
-    for (int a = 1; a < A; ++a) m = fmaxf(m, z[a]);
-    float s = 0.0f;
-    for (int a = 0; a < A; ++a) { c.p[a] = expf(z[a] - m); s += c.p[a]; }
-    float s2 = 0.0f;
-    for (int a = 0; a < A; ++a) { c.p[a] = c.p[a] / s; s2 += c.p[a]; }
-    c.s2 = s2;
-    ent = 0.0f;
-    for (int a = 0; a < A; ++a) {
-        c.pn[a] = c.p[a] / s2;
-        c.lg[a] = logf(fminf(fmaxf(c.pn[a], eps), 1.0f - eps));
-        ent -= c.pn[a] * c.lg[a];
-    }
-    logp = (action >= 0 && action < A) ? c.lg[action] : 0.0f;
-}
-// autograd's chain: gather + entropy -> log o clamp -> renormalisation -> softmax
-__device__ __forceinline__ void cat_backward(const Cat& c, int A, int action, float gl, float ge, float* dz) {
-    constexpr float eps = 1.1920928955078125e-07f;
-    float dot = 0.0f;
-    for (int a = 0; a < A; ++a) {
-        const float dlg = (a == action ? gl : 0.0f) - ge * c.pn[a];
-        const bool pass = c.pn[a] >= eps && c.pn[a] <= 1.0f - eps;
-        dz[a] = -ge * c.lg[a] + (pass ? dlg / c.pn[a] : 0.0f);
-        dot += dz[a] * c.pn[a];
-    }
-    float dot2 = 0.0f;
-    for (int a = 0; a < A; ++a) { dz[a] = (dz[a] - dot) / c.s2; dot2 += dz[a] * c.p[a]; }
-    for (int a = 0; a < A; ++a) dz[a] = c.p[a] * (dz[a] - dot2);
-}
+constexpr int kMaxA = ppo::kCatMaxA;
 
 // head: [B][A] (mu or logits); value: [B]; act: [B][A] (Gaussian) or [B] (categorical, float-coded index).
 // Outputs (all nullable except logp_out): logp_out [B]; dhead [B][A]; dvalue [B]; dlogstd_rows [B][A] (Gaussian: per-row
@@ -67,12 +33,12 @@ __global__ void ppo_rows_kernel(const float* __restrict__ head, const float* __r
         float z[kMaxA];
         for (int a = 0; a < A; ++a) z[a] = head[b * A + a];
         const int action = (int)act[b];
-        Cat c;
-        cat_forward(z, A, action, c, lp, ent);
+        ppo::Cat c;
+        ppo::cat_forward(z, A, action, c, lp, ent);
         if (grads) {
             ppo::actor_row(sc, lp, logp_old[b], adv[b], obj, gl);
             float dz[kMaxA];
-            cat_backward(c, A, action, gl, -sc.ent_coef * sc.inv_b, dz);
+            ppo::cat_backward(c, A, action, gl, -sc.ent_coef * sc.inv_b, dz);
             for (int a = 0; a < A; ++a) dhead[b * A + a] = dz[a];
         }
     } else {
