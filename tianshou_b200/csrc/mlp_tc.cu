@@ -25,6 +25,8 @@
 #include <cuda_bf16.h>
 #include <math.h>
 
+#include <type_traits>
+
 #include "common.cuh"
 #include "ppo_math.cuh"
 #include "wgmma.cuh"
@@ -62,7 +64,7 @@ struct Mat {
     uint32_t part;   // bytes between pieces
     uint32_t RS;     // bytes between 8-row groups (= cols/8 * 128)
 };
-__host__ __device__ inline uint32_t mat_bytes(int rows, int cols) { return (uint32_t)rows * cols * 2u; }
+__host__ __device__ constexpr uint32_t mat_bytes(int rows, int cols) { return (uint32_t)rows * cols * 2u; }
 __device__ __forceinline__ uint32_t moff(uint32_t r, uint32_t c, uint32_t RS) {
     return (r >> 3) * RS + (c >> 3) * 128u + (r & 7u) * 16u + (c & 7u) * 2u;
 }
@@ -89,10 +91,14 @@ __device__ __forceinline__ void store_chunk8(uint8_t* sm0, const Mat& m, uint32_
     *reinterpret_cast<uint4*>(p + 2 * m.part) = make_uint4(w2[0], w2[1], w2[2], w2[3]);
 }
 
-// Layer tiles: warpgroup g = tid / 128 computes rows [64 (g & 1), + 64) x columns [32 (g >> 1), + 32) of a 128 x 64
-// product; element e of the thread's accumulator is (lay_row0() + wg::frag_row(e), lay_col0() + wg::frag_col(e)).
-__device__ __forceinline__ int lay_row0() { return 64 * ((threadIdx.x >> 7) & 1); }
-__device__ __forceinline__ int lay_col0() { return 32 * (threadIdx.x >> 8); }
+// Warpgroup index of the calling thread.  Broadcast from lane 0 so that the compiler knows it is warp-uniform: the tile
+// origins and wgmma descriptors derived from it then live in uniform registers instead of being computed per thread
+// (threadIdx.x counts as divergent), which is what keeps the 128-register kernels free of spills.
+__device__ __forceinline__ int wg_index() { return __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0); }
+// Layer tiles: warpgroup g computes rows [64 (g & 1), + 64) x columns [32 (g >> 1), + 32) of a 128 x 64 product;
+// element e of the thread's accumulator is (lay_row0() + wg::frag_row(e), lay_col0() + wg::frag_col(e)).
+__device__ __forceinline__ int lay_row0() { return 64 * (wg_index() & 1); }
+__device__ __forceinline__ int lay_col0() { return 32 * (wg_index() >> 1); }
 
 // the thread's 16 layer elements -> bf16x3 operand M (two consecutive columns per 32-bit store)
 __device__ __forceinline__ void store_frag(uint8_t* sm0, const Mat& m, const float (&v)[kCols]) {
@@ -104,6 +110,19 @@ __device__ __forceinline__ void store_frag(uint8_t* sm0, const Mat& m, const flo
         *reinterpret_cast<uint32_t*>(p) = w0;
         *reinterpret_cast<uint32_t*>(p + m.part) = w1;
         *reinterpret_cast<uint32_t*>(p + 2 * m.part) = w2;
+    }
+}
+// inverse of store_frag, bit-exact: split3_pair truncates, so every piece is exact, b0 + b1 is x with its last 8 significant
+// bits cleared (representable), and (b0 + b1) + b2 == x
+__device__ __forceinline__ void load_frag(const uint8_t* sm0, const Mat& m, float (&v)[kCols]) {
+#pragma unroll
+    for (int e = 0; e < kCols; e += 2) {
+        const uint8_t* p = sm0 + (m.base + moff((uint32_t)(lay_row0() + wg::frag_row(e)), (uint32_t)(lay_col0() + wg::frag_col(e)), m.RS));
+        const uint32_t w0 = *reinterpret_cast<const uint32_t*>(p);
+        const uint32_t w1 = *reinterpret_cast<const uint32_t*>(p + m.part);
+        const uint32_t w2 = *reinterpret_cast<const uint32_t*>(p + 2 * m.part);
+        v[e] = (__uint_as_float(w0 << 16) + __uint_as_float(w1 << 16)) + __uint_as_float(w2 << 16);
+        v[e + 1] = (__uint_as_float(w0 & 0xffff0000u) + __uint_as_float(w1 & 0xffff0000u)) + __uint_as_float(w2 & 0xffff0000u);
     }
 }
 
@@ -147,9 +166,11 @@ struct Smem {   // byte offsets from the dynamic shared memory base (all multipl
                                  // of the pre-split weight image in global memory (one bulk copy per network)
     uint32_t total;
 };
-__host__ __device__ inline Smem make_smem(int obs_dim, uint32_t sbase) {
-    Smem s;
-    s.KXP = (obs_dim + 15) & ~15;
+// The kernels are instantiated per padded obs width KXP (16 or 32), so that inside them every offset below is an immediate.
+__host__ __device__ constexpr int kxp_of(int obs_dim) { return (obs_dim + 15) & ~15; }
+__host__ __device__ constexpr Smem make_smem(int kxp, uint32_t sbase) {
+    Smem s{};
+    s.KXP = kxp;
     uint32_t o = 0;
     auto mat = [&](Mat& m, int rows, int cols) {
         m.base = sbase + o; m.part = mat_bytes(rows, cols); m.RS = (uint32_t)(cols / 8) * 128u; o += 3u * m.part;
@@ -307,22 +328,21 @@ __device__ __forceinline__ void img_scatter(const ts_actor_critic_desc& d, const
     const NetG ga{d.a_w1, d.a_b1, d.a_w2, d.a_b2, d.a_w3, d.a_b3, d.a_logstd};
     img_scatter_net(S, sbase, ga, d.obs_dim, d.act_dim, i, x, wimg + S.wblk_bytes);
 }
+template <int KXP>
 __global__ void weight_image_build_kernel(const float* __restrict__ params, const ts_actor_critic_desc d, uint8_t* __restrict__ wimg) {
-    const Smem S = make_smem(d.obs_dim, 0u);
+    const Smem S = make_smem(KXP, 0u);
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < d.n_params; i += (int64_t)gridDim.x * blockDim.x)
         img_scatter(d, S, 0u, i, params[i], wimg);
 }
 
-// h = tanh(acc + bias) -> bf16x3 operand OUT; h stays in registers for the backward pass
-__device__ __forceinline__ void epi_tanh(uint8_t* sm0, const Mat& OUT, const float (&acc)[kCols], const float* __restrict__ bias,
-                                         float (&h)[kCols]) {
+// acc := h = tanh(acc + bias) -> bf16x3 operand OUT (the backward pass reads h back from there: load_frag)
+__device__ __forceinline__ void epi_tanh(uint8_t* sm0, const Mat& OUT, float (&acc)[kCols], const float* __restrict__ bias) {
 #pragma unroll
-    for (int e = 0; e < kCols; ++e) h[e] = tanh_mufu(acc[e] + bias[lay_col0() + wg::frag_col(e)]);
-    store_frag(sm0, OUT, h);
+    for (int e = 0; e < kCols; ++e) acc[e] = tanh_mufu(acc[e] + bias[lay_col0() + wg::frag_col(e)]);
+    store_frag(sm0, OUT, acc);
 }
 // dZ2 = (dOut W3) * (1 - H2^2) for the thread's layer elements (K = out_dim is tiny: SIMT)
-__device__ __forceinline__ void head_input_grad(uint8_t* sm, const Smem& S, int out_dim, const float (&h)[kCols],
-                                                float (&acc)[kCols]) {
+__device__ __forceinline__ void head_input_grad(uint8_t* sm, uint8_t* sm0, const Smem& S, int out_dim, float (&acc)[kCols]) {
     const int r0 = lay_row0() + wg::frag_row(0);        // rows r0 (elements 4 i, 4 i + 1) and r0 + 8 (4 i + 2, 4 i + 3)
     const float* dof = reinterpret_cast<const float*>(sm + S.dof);
     const float* w3f = reinterpret_cast<const float*>(sm + S.w3f) + lay_col0();
@@ -337,6 +357,8 @@ __device__ __forceinline__ void head_input_grad(uint8_t* sm, const Smem& S, int 
             acc[4 * i + 2] = fmaf(d1, w.x, acc[4 * i + 2]); acc[4 * i + 3] = fmaf(d1, w.y, acc[4 * i + 3]);
         }
     }
+    float h[kCols];
+    load_frag(sm0, S.H2, h);
 #pragma unroll
     for (int e = 0; e < kCols; ++e) acc[e] = acc[e] * fmaf(-h[e], h[e], 1.0f);
 }
@@ -418,20 +440,19 @@ __device__ __forceinline__ float warp_transpose_sum32(float (&v)[32]) {
     return v[0];
 }
 
-// forward of one trunk: X -> H1 -> H2 -> head D3 (fp32 [a][r] in shared memory, without bias); h1 / h2 of the thread's
-// layer elements stay in registers
-__device__ __forceinline__ void trunk_forward(uint8_t* sm, uint8_t* sm0, const Smem& S, float (&h1)[kCols], float (&h2)[kCols]) {
+// forward of one trunk: X -> H1 -> H2 -> head D3 (fp32 [a][r] in shared memory, without bias)
+__device__ __forceinline__ void trunk_forward(uint8_t* sm, uint8_t* sm0, const Smem& S) {
     float acc[kCols];
     publish();
     if (S.KXP == 16) wg_gemm<2 * kCols, 1, 0, 0>(acc, S.X, lay_row0(), S.W1, lay_col0());
     else wg_gemm<2 * kCols, 2, 0, 0>(acc, S.X, lay_row0(), S.W1, lay_col0());
-    epi_tanh(sm0, S.H1, acc, reinterpret_cast<const float*>(sm + S.b1), h1);
+    epi_tanh(sm0, S.H1, acc, reinterpret_cast<const float*>(sm + S.b1));
     publish();
     wg_gemm<2 * kCols, H / 16, 0, 0>(acc, S.H1, lay_row0(), S.W2, lay_col0());
-    epi_tanh(sm0, S.H2, acc, reinterpret_cast<const float*>(sm + S.b2), h2);
+    epi_tanh(sm0, S.H2, acc, reinterpret_cast<const float*>(sm + S.b2));
     publish();
     float d3[4];                                          // head: warpgroup g -> rows 64 (g & 1) .., columns 8 (g >> 1) ..
-    const int c0 = 8 * (threadIdx.x >> 8);
+    const int c0 = 8 * (wg_index() >> 1);
     wg_gemm<8, H / 16, 0, 0>(d3, S.H2, lay_row0(), S.W3, c0);
     float* out = reinterpret_cast<float*>(sm + S.d3);
 #pragma unroll
@@ -443,13 +464,12 @@ __device__ __forceinline__ void trunk_forward(uint8_t* sm, uint8_t* sm0, const S
 // `weights_dead()` is called (all threads) once nothing reads the network's weight block any more.
 template <class F>
 __device__ __forceinline__ void trunk_backward(uint8_t* sm, uint8_t* sm0, const Smem& S, const NetG& g, int obs_dim, int out_dim,
-                                               float* __restrict__ grad, const float (&h1)[kCols], const float (&h2)[kCols],
-                                               bool first, F&& weights_dead) {
-    const int wgi = threadIdx.x >> 7;
+                                               float* __restrict__ grad, bool first, F&& weights_dead) {
+    const int wgi = wg_index();
     float* scr = grad_scratch(sm0, S);
     publish();                                                 // dOut (fp32 and operand) complete
     float dz2[kCols];
-    head_input_grad(sm, S, out_dim, h2, dz2);
+    head_input_grad(sm, sm0, S, out_dim, dz2);
     float dw3[NO / 2];
     if (wgi == 3) wg_gemm<NO, kRows / 16, 1, 1, kWgradFull>(dw3, S.H2, 0u, S.DO, 0u);        // dW3^T = H2^T dOut
     tstamp(16);
@@ -474,8 +494,12 @@ __device__ __forceinline__ void trunk_backward(uint8_t* sm, uint8_t* sm0, const 
 #pragma unroll
         for (int e = 0; e < NO / 2; ++e) scr[kScrW3 + wg::frag_col(e) * kLdW2 + wg::frag_row(e)] = dw3[e];   // dW3^T [k][a] -> [a][k]
     }
+    {
+        float h1[kCols];
+        load_frag(sm0, S.H1, h1);
 #pragma unroll
-    for (int e = 0; e < kCols; ++e) dh1[e] *= fmaf(-h1[e], h1[e], 1.0f);
+        for (int e = 0; e < kCols; ++e) dh1[e] *= fmaf(-h1[e], h1[e], 1.0f);
+    }
     store_frag(sm0, S.H1, dh1);                                // H1 := dZ1
     tstamp(19);
     publish();
@@ -579,7 +603,10 @@ __device__ __noinline__ float peer_gather_sum(const unsigned long long* src0, in
     return sum;
 }
 
-struct TileIn { float xv[8]; float av[kMaxAct]; float rv[4]; };   // one thread's share of a tile's gathers
+// one thread's share of a tile's gathers: an (8-column chunk) of X, and for row r = tid % 128, group q = tid / 128, the
+// actions q + 4 u and row value q (adv, ret, logp_old, v_s) -- spread over all 512 threads, so that the prefetch that is
+// held in registers across the grid barrier stays small
+struct TileIn { float xv[8]; float av[kMaxAct / 4]; float rv; };
 
 // The minibatches of one launch are [lo0 + m * mb_size, lo0 + (m + 1) * mb_size) for m < n_mb - 1 and
 // [lo0 + (n_mb - 1) * mb_size, end) for the last one (Batch.split with merge_last, batch.py:1196-1215).
@@ -590,14 +617,14 @@ struct TileIn { float xv[8]; float av[kMaxAct]; float rv[4]; };   // one thread'
 // forward/backward -> grid barrier -> every CTA folds its slice of the gradient over the partial rows ->
 // barrier (global sum of squares) -> clip + Adam on the slice -> barrier (parameters visible).  The gathers
 // of the NEXT minibatch's tile are issued before the first barrier and land while the CTA waits.
-template <bool EPOCH>
+template <bool EPOCH, int KXP>
 __global__ void __launch_bounds__(kThreads, 1) ppo_tc_kernel(
     const float* params, const ts_actor_critic_desc d, const ts_ppo_hparams hp,
     const float* __restrict__ obs, const float* __restrict__ act, const float* __restrict__ adv,
     const float* __restrict__ ret, const float* __restrict__ logp_old, const float* __restrict__ v_s,
     const int32_t* __restrict__ perm, int64_t lo0, int64_t mb_size, int64_t end, int n_mb, int64_t global_rows,
     const float* __restrict__ adv_moments, float* __restrict__ partials, const AdamArgs opt, uint8_t* wimg /* nullable */,
-    const tsb::PeerArgs px) {
+    const __grid_constant__ tsb::PeerArgs px) {
     extern __shared__ __align__(1024) uint8_t sm[];
     __shared__ __align__(8) uint64_t s_wbar;
     __shared__ float s_coef, s_norm, s_step_size, s_bc2_sqrt;
@@ -620,7 +647,7 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_tc_kernel(
     if ((int64_t)blockIdx.x < mb_tiles(0)) prefetch_rows(0, blockIdx.x);
     const uint32_t sbase = wg::smem_u32(sm);
     uint8_t* sm0 = sm - sbase;     // so that (sm0 + shared_address) is the generic pointer
-    const Smem S = make_smem(d.obs_dim, sbase);
+    const Smem S = make_smem(KXP, sbase);
     const int A = d.act_dim;
     const NetG ga{d.a_w1, d.a_b1, d.a_w2, d.a_b2, d.a_w3, d.a_b3, d.a_logstd};
     const NetG gc{d.c_w1, d.c_b1, d.c_w2, d.c_b2, d.c_w3, d.c_b3, -1};
@@ -669,22 +696,23 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_tc_kernel(
         chunk_load(kRows, d.obs_dim, S.KXP, [&](int r) {
             return r < nrows ? obs + (int64_t)s_row[r] * d.obs_dim : (const float*)nullptr;
         }, in.xv);
-        if (tid < kRows) {
-            const int64_t row = tid < nrows ? (int64_t)s_row[tid] : -1;
+        const int r = tid & (kRows - 1), q = tid >> 7;
+        const int64_t row = r < nrows ? (int64_t)s_row[r] : -1;
 #pragma unroll
-            for (int a = 0; a < kMaxAct; ++a) in.av[a] = (row >= 0 && a < A) ? __ldg(act + row * A + a) : 0.0f;
-            in.rv[0] = in.rv[1] = in.rv[2] = in.rv[3] = 0.0f;
-            if (row >= 0) { in.rv[0] = __ldg(adv + row); in.rv[1] = __ldg(ret + row); in.rv[2] = __ldg(logp_old + row); in.rv[3] = __ldg(v_s + row); }
+        for (int u = 0; u < kMaxAct / 4; ++u) {
+            const int a = q + 4 * u;
+            in.av[u] = (row >= 0 && a < A) ? __ldg(act + row * A + a) : 0.0f;
         }
+        const float* rsrc = q == 0 ? adv : (q == 1 ? ret : (q == 2 ? logp_old : v_s));
+        in.rv = row >= 0 ? __ldg(rsrc + row) : 0.0f;
     };
     // ... and their conversion into the tile's operands
     auto store_inputs = [&](const TileIn& in) {
         chunk_store(sm0, S.X, kRows, S.KXP, in.xv);
-        if (tid < kRows) {
+        const int r = tid & (kRows - 1), q = tid >> 7;
 #pragma unroll
-            for (int a = 0; a < kMaxAct; ++a) actt[a * kRows + tid] = in.av[a];      // [a][r]: rows on consecutive banks
-            rowv[tid] = in.rv[0]; rowv[kRows + tid] = in.rv[1]; rowv[2 * kRows + tid] = in.rv[2]; rowv[3 * kRows + tid] = in.rv[3];
-        }
+        for (int u = 0; u < kMaxAct / 4; ++u) actt[(q + 4 * u) * kRows + r] = in.av[u];      // [a][r]: rows on consecutive banks
+        rowv[q * kRows + r] = in.rv;
     };
 
     double beta1_pow = 1.0, beta2_pow = 1.0;
@@ -695,7 +723,11 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_tc_kernel(
         const int64_t lo = mb_lo(m), hi = mb_hi(m);
         const int64_t tiles = (hi - lo + kRows - 1) / kRows;
         // the loss is the mean over the GLOBAL minibatch: every rank contributes hi - lo rows of its own shard
-        const ppo::Scalars sc = ppo::make_scalars(hp, EPOCH ? (hi - lo) * px.world : global_rows, adv_moments ? adv_moments + 2 * m : nullptr);
+        // in shared memory rather than in 13 registers held across the tile: the loss epilogues read it from there (the first
+        // read is behind trunk_forward's barriers; the previous minibatch's last read is behind the optimiser half's barriers)
+        __shared__ ppo::Scalars s_sc;
+        if (tid == 0) s_sc = ppo::make_scalars(hp, EPOCH ? (hi - lo) * px.world : global_rows, adv_moments ? adv_moments + 2 * m : nullptr);
+        const ppo::Scalars& sc = s_sc;
 #ifdef TS_B200_DIAGNOSTICS
         if (tid == 0 && g_tc_timeline_on && (int)blockIdx.x == g_tc_timeline_on - 1) g_tc_timeline_gate = (n_mb == 1 || m == n_mb - 2);   // a step WITH barrier 3
 #endif
@@ -729,13 +761,12 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_tc_kernel(
             }
 
             // ================= critic ================================================================
-            float h1[kCols], h2[kCols];
             tstamp(1);
             if (!critic_issued) issue_weights(0);
             critic_issued = false;
             wait_weights(gc, 1);
             tstamp(2);
-            trunk_forward(sm, sm0, S, h1, h2);
+            trunk_forward(sm, sm0, S);
             tstamp(3);
             float vf_row = 0.0f;
             if (tid < kRows) {
@@ -751,7 +782,7 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_tc_kernel(
                 if (lane == 0) red[warp] = sdv;                    // db3 (critic), one slot per warp
             }
             tstamp(4);
-            trunk_backward(sm, sm0, S, gc, d.obs_dim, 1, grad, h1, h2, first, [&] { issue_weights(1); });
+            trunk_backward(sm, sm0, S, gc, d.obs_dim, 1, grad, first, [&] { issue_weights(1); });
             tstamp(5);
             __syncthreads();
             if (tid == 0) out_acc(grad + gc.b3, (red[0] + red[1]) + (red[2] + red[3]), first);
@@ -762,7 +793,7 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_tc_kernel(
             // ================= actor =================================================================
             wait_weights(ga, A);
             tstamp(6);
-            trunk_forward(sm, sm0, S, h1, h2);
+            trunk_forward(sm, sm0, S);
             tstamp(7);
             // Actor loss epilogue on all 16 warps: thread (row r = 32 q + lane, group cq) owns the actions a = cq + 4 u -- the
             // four groups' log-prob partials meet in shared memory, every thread then evaluates the row's surrogate and writes
@@ -814,7 +845,7 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_tc_kernel(
                 }
             }
             tstamp(8);
-            trunk_backward(sm, sm0, S, ga, d.obs_dim, A, grad, h1, h2, first, [] {});
+            trunk_backward(sm, sm0, S, ga, d.obs_dim, A, grad, first, [] {});
             tstamp(9);
 
             // ================= loss sums + small gradients ===========================================
@@ -1000,9 +1031,9 @@ struct SmemF {
     uint32_t w3f, b1, b2, b3, ls, part;
     uint32_t total;
 };
-__host__ __device__ inline SmemF make_smem_f(int obs_dim, uint32_t sbase) {
-    SmemF s;
-    s.KXP = (obs_dim + 15) & ~15;
+__host__ __device__ constexpr SmemF make_smem_f(int kxp, uint32_t sbase) {
+    SmemF s{};
+    s.KXP = kxp;
     uint32_t o = 0;
     auto mat = [&](Mat& m, int rows, int cols) {
         m.base = sbase + o; m.part = mat_bytes(rows, cols); m.RS = (uint32_t)(cols / 8) * 128u; o += 3u * m.part;
@@ -1023,7 +1054,7 @@ __host__ __device__ inline SmemF make_smem_f(int obs_dim, uint32_t sbase) {
 
 // MODE 0: out0[r] = critic(in0[r]) and (if in1) out1[r] = critic(in1[r])      (a2c.py:123-126)
 // MODE 1: out0[r] = log N(in1[r] | mu(in0[r]), exp(logstd)), out1 = mu (nullable)   (ppo.py:157-161)
-template <int MODE>
+template <int MODE, int KXP>
 __global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(
     const float* __restrict__ params, const ts_actor_critic_desc d, const float* __restrict__ in0,
     float* __restrict__ out0, const float* __restrict__ in1, float* __restrict__ out1, int64_t n) {
@@ -1031,7 +1062,7 @@ __global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(
     const int tid = threadIdx.x, lane = tid & 31;
     const uint32_t sbase = wg::smem_u32(sm);
     uint8_t* sm0 = sm - sbase;
-    const SmemF S = make_smem_f(d.obs_dim, sbase);
+    const SmemF S = make_smem_f(KXP, sbase);
     const int out_dim = MODE == 0 ? 1 : d.act_dim;
     const NetG g = MODE == 0 ? NetG{d.c_w1, d.c_b1, d.c_w2, d.c_b2, d.c_w3, d.c_b3, -1}
                              : NetG{d.a_w1, d.a_b1, d.a_w2, d.a_b2, d.a_w3, d.a_b3, d.a_logstd};
@@ -1084,7 +1115,7 @@ __global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(
         float acc[kCols], h[kCols];
         if (S.KXP == 16) wg_gemm<2 * kCols, 1, 0, 0>(acc, S.X, lay_row0(), S.W1, lay_col0());
         else wg_gemm<2 * kCols, 2, 0, 0>(acc, S.X, lay_row0(), S.W1, lay_col0());
-        epi_tanh(sm0, S.H1, acc, b1, h);
+        epi_tanh(sm0, S.H1, acc, b1);
         publish();
         wg_gemm<2 * kCols, H / 16, 0, 0>(acc, S.H1, lay_row0(), S.W2, lay_col0());
 #pragma unroll
@@ -1142,28 +1173,39 @@ bool tc_supported(const ts_actor_critic_desc& d) {
            d.a_w1 != d.c_w1 && d.a_logstd >= 0;
 }
 
-static int configure_ppo_smem(size_t smem) {
-    static size_t configured[kMaxDevices] = {};       // the opt-in is a per-device function attribute
+// the dynamic shared memory opt-in is a per-device attribute of each kernel instantiation
+template <auto Kernel>
+static int opt_in_smem(size_t smem) {
+    static bool configured[kMaxDevices] = {};
     const int dev = device_ordinal();
-    if (smem > configured[dev]) {
-        TS_CUDA(cudaFuncSetAttribute(ppo_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        TS_CUDA(cudaFuncSetAttribute(ppo_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        configured[dev] = smem;
+    if (!configured[dev]) {
+        TS_CUDA(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        configured[dev] = true;
     }
     return 0;
+}
+
+// f(std::integral_constant<int, KXP>) for the instantiation that serves obs_dim (tc_supported: obs_dim <= 32)
+template <class F>
+static int with_kxp(int obs_dim, F&& f) {
+    return kxp_of(obs_dim) == 16 ? f(std::integral_constant<int, 16>{}) : f(std::integral_constant<int, 32>{});
 }
 
 int launch_ppo_grad_tc(const float* params, const ts_actor_critic_desc& d, const ts_ppo_hparams& hp, const float* obs,
                        const float* act, const float* adv, const float* ret, const float* logp_old, const float* v_s,
                        const int32_t* perm, int64_t lo, int64_t hi, int64_t global_rows, const float* adv_moments,
                        float* grad, cudaStream_t st) {
-    const size_t smem = make_smem(d.obs_dim, 0).total;
-    if (int e = configure_ppo_smem(smem)) return e;
-    const int64_t tiles = (hi - lo + kRows - 1) / kRows;
-    const unsigned grid = (unsigned)imin(tiles, num_sms());
-    ppo_tc_kernel<false><<<grid, kThreads, smem, st>>>(params, d, hp, obs, act, adv, ret, logp_old, v_s, perm, lo, hi - lo, hi, 1,
-                                                       global_rows, adv_moments, grad, AdamArgs{}, (uint8_t*)nullptr, PeerArgs{});
-    return check_launch("ts_ppo_grad(tc)");
+    return with_kxp(d.obs_dim, [&](auto kxp) {
+        constexpr int KXP = decltype(kxp)::value;
+        constexpr size_t smem = make_smem(KXP, 0).total;
+        if (int e = opt_in_smem<ppo_tc_kernel<false, KXP>>(smem)) return e;
+        const int64_t tiles = (hi - lo + kRows - 1) / kRows;
+        const unsigned grid = (unsigned)imin(tiles, num_sms());
+        ppo_tc_kernel<false, KXP><<<grid, kThreads, smem, st>>>(params, d, hp, obs, act, adv, ret, logp_old, v_s, perm, lo, hi - lo,
+                                                                hi, 1, global_rows, adv_moments, grad, AdamArgs{}, (uint8_t*)nullptr,
+                                                                PeerArgs{});
+        return check_launch("ts_ppo_grad(tc)");
+    });
 }
 
 // n_mb consecutive optimiser steps (minibatch fwd/bwd + gradient fold + clip + Adam + stats each) in ONE
@@ -1173,50 +1215,53 @@ int launch_ppo_epoch_tc(float* params, const ts_actor_critic_desc& d, const ts_p
                         const int32_t* perm, int64_t lo0, int64_t mb_size, int64_t end, int n_mb, const float* adv_moments,
                         float* partials, float* grad_scratch, float* exp_avg, float* exp_avg_sq, int64_t* step_count,
                         float* stats, void* weight_image, const PeerArgs& px, cudaStream_t st) {
-    const size_t smem = make_smem(d.obs_dim, 0).total;
-    if (int e = configure_ppo_smem(smem)) return e;
-    const int64_t last = end - (lo0 + (int64_t)(n_mb - 1) * mb_size);
-    const int64_t widest = n_mb > 1 ? (mb_size > last ? mb_size : last) : last;
-    const unsigned grid = (unsigned)imin((widest + kRows - 1) / kRows, num_sms());
-    const AdamArgs opt{params, grad_scratch, exp_avg, exp_avg_sq, step_count, stats};
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeCooperative;
-    attr[0].val.cooperative = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-    const int64_t zero = 0;
-    // scratch layout: [128-byte control block (grid-barrier state, zero between launches)][critic block][actor block]
-    uint8_t* wimg = weight_image ? static_cast<uint8_t*>(weight_image) + kCtlBytes : nullptr;
-    if (wimg) {   // (re)build the pre-split image from the current parameters: the host may have changed them
-        const Smem S = make_smem(d.obs_dim, 0);
-        TS_CUDA(cudaMemsetAsync(wimg, 0, 2 * (size_t)S.wblk_bytes, st));
-        weight_image_build_kernel<<<(unsigned)((d.n_params + 255) / 256), 256, 0, st>>>(params, d, wimg);
-        if (int e = check_launch("ts_ppo_update(weight image)")) return e;
-    }
-    TS_CUDA(cudaLaunchKernelEx(&cfg, ppo_tc_kernel<true>, (const float*)params, d, hp, obs, act, adv, ret, logp_old, v_s, perm,
-                               lo0, mb_size, end, n_mb, zero, adv_moments, partials, opt, wimg, px));
-    return check_launch("ts_ppo_epoch(tc)");
+    return with_kxp(d.obs_dim, [&](auto kxp) {
+        constexpr int KXP = decltype(kxp)::value;
+        constexpr Smem S = make_smem(KXP, 0);
+        if (int e = opt_in_smem<ppo_tc_kernel<true, KXP>>(S.total)) return e;
+        const int64_t last = end - (lo0 + (int64_t)(n_mb - 1) * mb_size);
+        const int64_t widest = n_mb > 1 ? (mb_size > last ? mb_size : last) : last;
+        const unsigned grid = (unsigned)imin((widest + kRows - 1) / kRows, num_sms());
+        const AdamArgs opt{params, grad_scratch, exp_avg, exp_avg_sq, step_count, stats};
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = S.total; cfg.stream = st;
+        cudaLaunchAttribute attr[1];
+        attr[0].id = cudaLaunchAttributeCooperative;
+        attr[0].val.cooperative = 1;
+        cfg.attrs = attr; cfg.numAttrs = 1;
+        const int64_t zero = 0;
+        // scratch layout: [128-byte control block (grid-barrier state, zero between launches)][critic block][actor block]
+        uint8_t* wimg = weight_image ? static_cast<uint8_t*>(weight_image) + kCtlBytes : nullptr;
+        if (wimg) {   // (re)build the pre-split image from the current parameters: the host may have changed them
+            TS_CUDA(cudaMemsetAsync(wimg, 0, 2 * (size_t)S.wblk_bytes, st));
+            weight_image_build_kernel<KXP><<<(unsigned)((d.n_params + 255) / 256), 256, 0, st>>>(params, d, wimg);
+            if (int e = check_launch("ts_ppo_update(weight image)")) return e;
+        }
+        TS_CUDA(cudaLaunchKernelEx(&cfg, ppo_tc_kernel<true, KXP>, (const float*)params, d, hp, obs, act, adv, ret, logp_old, v_s,
+                                   perm, lo0, mb_size, end, n_mb, zero, adv_moments, partials, opt, wimg, px));
+        return check_launch("ts_ppo_epoch(tc)");
+    });
 }
 
 int64_t weight_image_bytes(const ts_actor_critic_desc& d) {
-    return tc_supported(d) ? (int64_t)kCtlBytes + 2 * (int64_t)make_smem(d.obs_dim, 0).wblk_bytes : 0;
+    return tc_supported(d) ? (int64_t)kCtlBytes + 2 * (int64_t)make_smem(kxp_of(d.obs_dim), 0).wblk_bytes : 0;
 }
 
 int launch_forward_tc(int mode, const float* params, const ts_actor_critic_desc& d, const float* in0, float* out0,
                       const float* in1, float* out1, int64_t n, cudaStream_t st) {
-    const size_t smem = make_smem_f(d.obs_dim, 0).total;
-    static size_t configured[kMaxDevices][2] = {};
-    const int dev = device_ordinal();
-    if (smem > configured[dev][mode]) {
-        if (mode == 0) TS_CUDA(cudaFuncSetAttribute(forward_tc_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        else TS_CUDA(cudaFuncSetAttribute(forward_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        configured[dev][mode] = smem;
-    }
-    const int64_t tiles = ((n + kRows - 1) / kRows) * ((mode == 0 && in1) ? 2 : 1);
-    const unsigned grid = (unsigned)imin(tiles, num_sms());
-    if (mode == 0) forward_tc_kernel<0><<<grid, kThreads, smem, st>>>(params, d, in0, out0, in1, out1, n);
-    else forward_tc_kernel<1><<<grid, kThreads, smem, st>>>(params, d, in0, out0, in1, out1, n);
-    return check_launch(mode == 0 ? "ts_critic_forward(tc)" : "ts_actor_logp(tc)");
+    return with_kxp(d.obs_dim, [&](auto kxp) {
+        constexpr int KXP = decltype(kxp)::value;
+        constexpr size_t smem = make_smem_f(KXP, 0).total;
+        const int64_t tiles = ((n + kRows - 1) / kRows) * ((mode == 0 && in1) ? 2 : 1);
+        const unsigned grid = (unsigned)imin(tiles, num_sms());
+        if (mode == 0) {
+            if (int e = opt_in_smem<forward_tc_kernel<0, KXP>>(smem)) return e;
+            forward_tc_kernel<0, KXP><<<grid, kThreads, smem, st>>>(params, d, in0, out0, in1, out1, n);
+        } else {
+            if (int e = opt_in_smem<forward_tc_kernel<1, KXP>>(smem)) return e;
+            forward_tc_kernel<1, KXP><<<grid, kThreads, smem, st>>>(params, d, in0, out0, in1, out1, n);
+        }
+        return check_launch(mode == 0 ? "ts_critic_forward(tc)" : "ts_actor_logp(tc)");
+    });
 }
 }  // namespace tsb
