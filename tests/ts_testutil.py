@@ -156,6 +156,87 @@ def ppo_reference_fp64(actor, critic, mb: dict, hp: dict) -> dict:
                 clip=clip_loss.item(), vf=vf_loss.item(), ent=ent.item(), grads=grads)
 
 
+F32_EPS = float(np.finfo(np.float32).eps)
+
+
+def ac_named_params(actor, critic) -> dict:
+    """``named_params`` for every actor-critic the fused kernels accept: Gaussian (``mu`` head + ``a_logstd``) or
+    categorical (DiscreteActor, ``last`` head, no log-std) and separate or shared trunks.  A shared trunk has one set of
+    slots, reported under the ``a_*`` names only."""
+    import torch
+    a1, a2 = [m for m in actor.preprocess.model.model if isinstance(m, torch.nn.Linear)]
+    c1, c2 = [m for m in critic.preprocess.model.model if isinstance(m, torch.nn.Linear)]
+    categorical = hasattr(actor, "softmax_output")
+    a3 = actor.last.model[0] if categorical else actor.mu.model[0]
+    d = {"a_w1": a1.weight, "a_b1": a1.bias, "a_w2": a2.weight, "a_b2": a2.bias, "a_w3": a3.weight, "a_b3": a3.bias}
+    if not categorical:
+        d["a_logstd"] = actor.sigma_param
+    if c1 is not a1:
+        d.update({"c_w1": c1.weight, "c_b1": c1.bias, "c_w2": c2.weight, "c_b2": c2.bias})
+    c3 = critic.last.model[0]
+    d.update({"c_w3": c3.weight, "c_b3": c3.bias})
+    return d
+
+
+def actor_critic_reference_fp64(actor, critic, mb: dict, hp: dict) -> dict:
+    """``ppo_reference_fp64`` for the whole fused family: Tanh or ReLU trunks, a shared trunk (actor and critic copied
+    together, so autograd adds both losses' gradients into the same leaves) and the categorical head as
+    ``Categorical(probs=softmax(z))`` computes it -- renormalise, clamp with the FLOAT32 eps the reference's fp32 run
+    uses (torch's own ``clamp_probs`` would take the float64 eps here), log.  Runs the modules' own Linear layers in
+    float64 on CPU.  Returns v, mu (Gaussian: the mean; categorical: softmax(z) before renormalisation), pn (categorical:
+    the renormalised probabilities), logp, the loss parts and ``grads`` keyed like ``ac_named_params``."""
+    import copy
+
+    import torch
+    a, c = copy.deepcopy((actor, critic))        # one deepcopy: a shared trunk stays shared
+    a.to("cpu", torch.float64)
+    c.to("cpu", torch.float64)
+    t = {k: torch.as_tensor(np.asarray(v), dtype=torch.float64) for k, v in mb.items()}
+    obs = t["obs"]
+    categorical = hasattr(a, "softmax_output")
+    pn = None
+    if categorical:
+        z = a.last.model(a.preprocess.model.model(obs))
+        mu = torch.softmax(z, dim=-1)
+        pn = mu / mu.sum(-1, keepdim=True)
+        lg = torch.log(pn.clamp(F32_EPS, 1.0 - F32_EPS))
+        act = t["act"].reshape(obs.shape[0], -1)[:, 0].long()
+        logp = lg.gather(1, act.view(-1, 1)).view(-1)
+        ent = -(pn * lg).sum(-1)
+    else:
+        mu = a.mu.model(a.preprocess.model.model(obs))
+        sigma = a.sigma_param.reshape(-1).exp().expand_as(mu)
+        dist = torch.distributions.Independent(torch.distributions.Normal(mu, sigma), 1)
+        logp = dist.log_prob(t["act"])
+        ent = dist.entropy()
+    value = c.last.model(c.preprocess.model.model(obs)).flatten()
+    adv = t["adv"]
+    ratio = (logp - t["logp_old"]).exp()
+    if hp.get("loss_kind", "ppo") == "a2c":
+        clip_loss = -(logp * adv).mean()
+    else:
+        if hp["advantage_normalization"]:
+            adv = (adv - adv.mean()) / (adv.std() + hp["adv_eps"])
+        eps = hp["eps_clip"]
+        obj = torch.min(ratio * adv, ratio.clamp(1.0 - eps, 1.0 + eps) * adv)
+        if hp.get("dual_clip"):
+            obj = torch.where(adv < 0, torch.max(obj, hp["dual_clip"] * adv), obj)
+        clip_loss = -obj.mean()
+    R, vs = t["returns"], t["v_s"]
+    if hp.get("value_clip"):
+        v_clip = vs + (value - vs).clamp(-hp["eps_clip"], hp["eps_clip"])
+        vf_loss = torch.max((R - value).pow(2), (R - v_clip).pow(2)).mean()
+    else:
+        vf_loss = (R - value).pow(2).mean()
+    ent = ent.mean()
+    loss = clip_loss + hp["vf_coef"] * vf_loss - hp["ent_coef"] * ent
+    loss.backward()
+    grads = {k: p.grad.numpy().copy() for k, p in ac_named_params(a, c).items()}
+    d = lambda x: None if x is None else x.detach().numpy().copy()
+    return dict(v=d(value), mu=d(mu), pn=d(pn), logp=d(logp), loss=loss.item(), clip=clip_loss.item(), vf=vf_loss.item(),
+                ent=ent.item(), grads=grads)
+
+
 def restore_vector_buffer(g, prefix: str, E: int, cap: int, device=None):
     """Rebuild a tianshou_b200 VectorReplayBuffer in the exact state stored in a golden file."""
     from tianshou_b200.data import Batch, VectorReplayBuffer
