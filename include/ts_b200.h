@@ -533,6 +533,15 @@ int ts_adam_step_dev(float* params, const float* grad, float* exp_avg, float* ex
 /* target = tau * source + (1 - tau) * target   (utils/lagged_network.py:8-18) */
 int ts_polyak_update(float* target, const float* source, int64_t n, double tau, ts_stream_t stream);
 
+/* GAIL discriminator rows (imitation/gail.py).  Rewards (gail.py:193-206): rew[n] = -log_sigmoid(-logits[n]) evaluated in fp32
+ * as torch does (min(0, z) - log1p(exp(-|z|)), z = -logit), widened to f64 for GAE; grid-stride over any n. */
+int ts_gail_reward_rows(const float* logits, int64_t n, double* rew, ts_stream_t stream);
+/* one discriminator step (gail.py:226-235): logits [n_pi + n_exp] = [policy rows | expert rows];
+ * dlogits = d loss / d logit with loss = -log_sigmoid(-logits_pi).mean() + -log_sigmoid(logits_exp).mean()
+ * (sigmoid(x) / n_pi, -sigmoid(-x) / n_exp); stats_row[4] = (loss, (logits_pi < 0).mean(), (logits_exp > 0).mean(), n_pi).
+ * Fixed-order reduction, no atomics: two calls on the same input are bit-identical. */
+int ts_gail_disc_rows(const float* logits, int64_t n_pi, int64_t n_exp, float* dlogits, float* stats_row, ts_stream_t stream);
+
 #ifdef TS_B200_DIAGNOSTICS
 /* Diagnostics build only (libts_b200_diag.so, `python -m tianshou_b200.csrc.build --diag`): not part of the product library. */
 /* Hardware self-test of the wgmma building blocks (csrc/wgmma.cuh), one CTA:

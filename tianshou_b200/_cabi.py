@@ -119,6 +119,9 @@ SIGNATURES: dict[str, list[Any]] = {
     "ts_npg_axpy": [_P, _P, _P, _D, _P, _I64, _P],
     "ts_trpo_decide": [_P, _P, _I64, _I32, _I32, _D, _D, _P, _P, _P, _P],
     "ts_npg_normalize_adv": [_P, _I64, _P],
+    # GAIL (gail.cu)
+    "ts_gail_reward_rows": [_P, _I64, _P, _P],
+    "ts_gail_disc_rows": [_P, _I64, _I64, _P, _P, _P],
     "ts_stack_prev_indices": [_P, _I64, _I32, _P, _I64, _P, _P, _P, _P, _P],
     "ts_im2col_u8": [_P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _D, _P, _P],
     "ts_im2col_f32": [_P, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P],

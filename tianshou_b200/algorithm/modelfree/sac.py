@@ -245,15 +245,8 @@ class SAC(OffPolicyAlgorithm):
     def _rows(self, buffer: ReplayBuffer, key: str, indices: np.ndarray | torch.Tensor) -> torch.Tensor:
         """buffer[key][indices] as a dense fp32 [I, width] device tensor: gathered from the device mirror when the
         buffer keeps one (no host traffic), else a host gather of the sampled rows + one upload."""
-        cols = self._cols_override if self._cols_override is not None else (
-            buffer.device_columns() if hasattr(buffer, "device_columns") else None)
-        if cols is not None and key in cols:
-            from ... import ops
-            idx = indices if isinstance(indices, torch.Tensor) else to_device(np.asarray(indices, dtype=np.int64), self._dev)
-            src = cols[key]
-            return ops.gather_rows(src.reshape(src.shape[0], -1), idx).to(torch.float32)
-        arr = np.asarray(buffer._meta[key])[np.asarray(indices)]
-        return to_device(np.ascontiguousarray(arr.reshape(len(arr), -1)), self._dev, dtype=torch.float32)
+        from ... import ops
+        return ops.buffer_rows(buffer, key, indices, self._dev, cols=self._cols_override)
 
     def _actor_forward(self, obs: torch.Tensor, tag: str) -> tuple[list[torch.Tensor], torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
         """policy(batch) on the device: returns (activations, act, log_prob, sigma, noise)."""

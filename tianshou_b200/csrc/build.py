@@ -8,7 +8,7 @@ import sys
 from concurrent.futures import ThreadPoolExecutor
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-SOURCES = ["capi.cu", "gae.cu", "nstep.cu", "index.cu", "segtree.cu", "mlp.cu", "mlp_tc.cu", "peer.cu", "hostperm.cu", "net_gemm.cu", "net_ops.cu", "ppo_rows.cu", "npg.cu",
+SOURCES = ["capi.cu", "gae.cu", "nstep.cu", "index.cu", "segtree.cu", "mlp.cu", "mlp_tc.cu", "peer.cu", "hostperm.cu", "net_gemm.cu", "net_ops.cu", "ppo_rows.cu", "npg.cu", "gail.cu",
            "hostperm_simd.cpp"]      # .cpp = host-only, compiled by g++
 DIAG_SOURCES = ["umma_selftest.cu"]       # diagnostics library only (-DTS_B200_DIAGNOSTICS: phase timeline + wgmma self-test)
 LIB = os.path.join(os.path.dirname(HERE), "libts_b200.so")

@@ -209,6 +209,20 @@ def gather_rows(src: torch.Tensor, idx: torch.Tensor, out: torch.Tensor | None =
     return out
 
 
+def buffer_rows(buffer, key: str, indices: np.ndarray | torch.Tensor, device: torch.device,
+                cols: dict[str, torch.Tensor] | None = None) -> torch.Tensor:
+    """buffer[key][indices] as a dense fp32 [I, width] device tensor: gathered from the device mirror ``cols`` (default: the
+    buffer's own, when it keeps one) with no host traffic, else a host gather of the sampled rows + one upload."""
+    if cols is None and hasattr(buffer, "device_columns"):
+        cols = buffer.device_columns()
+    if cols is not None and key in cols:
+        idx = indices if isinstance(indices, torch.Tensor) else to_device(np.asarray(indices, dtype=np.int64), device)
+        src = cols[key]
+        return gather_rows(src.reshape(src.shape[0], -1), idx).to(torch.float32)
+    arr = np.asarray(buffer._meta[key])[np.asarray(indices)]
+    return to_device(np.ascontiguousarray(arr.reshape(len(arr), -1)), device, dtype=torch.float32)
+
+
 def value_mask_rows(target_q: torch.Tensor, terminated: torch.Tensor, idx: torch.Tensor) -> None:
     I = idx.numel()
     A = target_q.numel() // max(I, 1)
