@@ -126,22 +126,38 @@ def test_wide_network_runs_the_tensor_core_gemm_path_vs_oracle():
 
 
 def test_three_layer_relu_trunk_gradients_vs_autograd():
-    """A deeper trunk (three hidden layers, different widths) -- gradients of one layered minibatch step vs torch autograd of
-    the same PPO loss on the same modules."""
+    """A deeper trunk (three hidden layers, different widths) per network."""
+    _trunk_gradients_vs_fp64_autograd("three-layer")
+
+
+def test_two_net_wrappers_around_one_trunk_gradients_vs_autograd():
+    """Actor and critic hold two different ``Net`` wrappers around ONE (128, 128) MLP: the trunk is shared, and its gradient
+    is the sum of both losses' gradients (not the critic's alone)."""
+    _trunk_gradients_vs_fp64_autograd("two-wrappers")
+
+
+def _trunk_gradients_vs_fp64_autograd(trunk):
+    """Gradients of one layered minibatch step vs float64 torch autograd of the same PPO loss on copies of the same modules."""
+    import copy
+
     from tianshou_b200.algorithm import PPO, AdamOptimizerFactory, ProbabilisticActorPolicy
-    from tianshou_b200.utils.net.common import Net
+    from tianshou_b200.utils.net.common import ActorCritic, Net
     from tianshou_b200.utils.net.continuous import ContinuousActorProbabilistic, ContinuousCritic
     from ts_testutil import Box, gaussian_dist
-    O, A, H = 29, 4, (96, 80, 40)
+    O, A, H = (29, 4, (96, 80, 40)) if trunk == "three-layer" else (17, 6, (128, 128))
     torch.manual_seed(1)
-    actor = ContinuousActorProbabilistic(preprocess_net=Net(state_shape=(O,), hidden_sizes=H), action_shape=(A,), unbounded=True).to(DEV)
-    critic = ContinuousCritic(preprocess_net=Net(state_shape=(O,), hidden_sizes=H)).to(DEV)
+    a_net = Net(state_shape=(O,), hidden_sizes=H)
+    c_net = Net(state_shape=(O,), hidden_sizes=H)
+    if trunk == "two-wrappers":
+        c_net.model = a_net.model
+    actor = ContinuousActorProbabilistic(preprocess_net=a_net, action_shape=(A,), unbounded=True).to(DEV)
+    critic = ContinuousCritic(preprocess_net=c_net).to(DEV)
     policy = ProbabilisticActorPolicy(actor=actor, dist_fn=gaussian_dist, action_scaling=True, action_bound_method="clip",
                                       action_space=Box(A))
     algo = PPO(policy=policy, critic=critic, optim=AdamOptimizerFactory(lr=0.0), eps_clip=0.2, vf_coef=0.5, ent_coef=0.02,
                value_clip=False, advantage_normalization=False, max_grad_norm=None)
     L = algo._layered
-    assert L is not None and len(L.a_trunk.layers) == 3
+    assert L is not None and len(L.a_trunk.layers) == len(H) and L.shared == (trunk == "two-wrappers")
     B = 200
     g = torch.Generator().manual_seed(0)
     obs = torch.randn(B, O, generator=g).to(DEV)
@@ -158,21 +174,26 @@ def test_three_layer_relu_trunk_gradients_vs_autograd():
     batch.obs, batch.act, batch.adv, batch.returns, batch.logp_old, batch.v_s = obs, act, adv, ret, lpo.contiguous(), vso
     stats_row = torch.zeros(8, device=DEV)
     L.minibatch_step(batch, torch.arange(B, device=DEV), algo._loss_hparams(), None, algo.optim._optim, None, stats_row)
-    # torch autograd reference of ppo.py:183-211 on the same modules (lr = 0: the step did not move the parameters)
-    (mu, sig), _ = actor(obs)
-    dist = gaussian_dist((mu, sig))
+    # float64 autograd of ppo.py:183-211 on copies of the modules (lr = 0: the step did not move the parameters), through
+    # their Sequentials: MLP.forward casts its input to float32
+    actor64, critic64 = copy.deepcopy((actor, critic))
+    actor64.double()
+    critic64.double()
+    obs, act, adv, ret, lpo = (t.double() for t in (obs, act, adv, ret, lpo))
+    mu = actor64.mu.model(actor64.preprocess.model.model(obs))
+    dist = gaussian_dist((mu, (actor64.sigma_param.view(1, -1) + torch.zeros_like(mu)).exp()))
     ratio = (dist.log_prob(act) - lpo).exp()
     surr = torch.min(ratio * adv, ratio.clamp(0.8, 1.2) * adv)
-    value = critic(obs).flatten()
+    value = critic64.last.model(critic64.preprocess.model.model(obs)).flatten()
     loss = -surr.mean() + 0.5 * (ret - value).pow(2).mean() - 0.02 * dist.entropy().mean()
-    for p_ in L.group.params:
-        p_.grad = None
     loss.backward()
-    record_parity("layered_deep/loss", stats_row[:1].cpu().numpy(), np.array([float(loss)]), rtol=2e-5, atol=1e-6)
-    for i, p_ in enumerate(L.group.params):
+    tag = f"layered_{trunk}"
+    record_parity(f"{tag}/loss", stats_row[:1].cpu().numpy(), np.array([float(loss)]), rtol=2e-5, atol=1e-6)
+    params64 = list(ActorCritic(actor64, critic64).parameters())      # the group's order: ActorCritic order, shared once
+    for i, (p_, p64) in enumerate(zip(L.group.params, params64, strict=True)):
         got = L.group.view(L.group.grad, p_).view(p_.shape).cpu().numpy()
-        ref = p_.grad.cpu().numpy()
-        record_parity(f"layered_deep/grad{i}", got, ref, rtol=2e-4, atol=2e-5 * float(np.abs(ref).max()) + 1e-9)
+        ref = p64.grad.cpu().numpy()
+        record_parity(f"{tag}/grad{i}", got, ref, rtol=2e-4, atol=2e-5 * float(np.abs(ref).max()) + 1e-9)
 
 
 # ------------------------------------------------------------------------------------------- ts_ppo_rows per row

@@ -163,7 +163,8 @@ def test_conv_stack_forward_backward_vs_torch():
     gradients of sum(q * coef) against torch autograd on the same weights."""
     from torch import nn
 
-    from tianshou_b200.algorithm.netgraph import FlatGroup, FusedStack, compile_sequential
+    from tianshou_b200.algorithm.flat_params import FlatGroup
+    from tianshou_b200.algorithm.netgraph import FusedStack, compile_sequential
     torch.manual_seed(0)
     B, A = 6, 5
     net = nn.Sequential(

@@ -262,7 +262,7 @@ def _check_grads(tag, mod, group, grad, ref_mod):
 def _sac_grad_case(O, A, H, separate_critic2, per, auto_alpha, seed):
     from tianshou_b200.algorithm import AdamOptimizerFactory
     from tianshou_b200.algorithm.modelfree.sac import SAC, AutoAlpha, SACPolicy
-    from tianshou_b200.algorithm.netgraph import FlatGroup
+    from tianshou_b200.algorithm.flat_params import FlatGroup
     from tianshou_b200.data import Batch, PrioritizedVectorReplayBuffer, VectorReplayBuffer
     from tianshou_b200.utils import policy_within_training_step
     from tianshou_b200.utils.net.common import Net

@@ -139,8 +139,8 @@ class Algorithm(nn.Module, ABC):
 
     class Optimizer:
         """torch optimizer + optional global-norm clipping (algorithm_base.py:457-511).
-        ``step(loss)`` is the generic eager path kept for API users; the fused PPO update drives
-        the same optimizer state through ``FlatParams`` instead."""
+        ``step(loss)`` is the generic eager path kept for API users; the device updates drive the
+        same optimizer state through the ``FlatGroup`` that ``bind_optimizer`` sets as ``_flat``."""
 
         def __init__(self, optim: torch.optim.Optimizer, module: nn.Module, max_grad_norm: float | None = None):
             self._optim = optim

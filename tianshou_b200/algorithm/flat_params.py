@@ -1,10 +1,10 @@
-"""Flat f32 parameter / Adam-moment storage shared between torch modules and the CUDA kernels.
+"""Flat f32 parameter / gradient / Adam-moment storage shared between torch modules and the CUDA kernels.
 
-The kernels (csrc/mlp.cu) address all 11k parameters of the actor-critic through ONE flat buffer
-plus the offsets of ``ts_actor_critic_desc``.  To keep ``state_dict()`` / ``load_state_dict()`` /
-the Collector's torch forward working unchanged (SURVEY 5: checkpoint/resume), every
-``nn.Parameter`` is re-pointed at a view of that buffer: kernels update the flat buffer in place
-and the modules see the new weights without copies.
+The kernels address an optimiser's parameters through ONE flat buffer: the fused actor-critic kernels (csrc/mlp.cu,
+mlp_tc.cu) through the offsets of ``ts_actor_critic_desc``, the layer-wise networks (netgraph.py) through per-layer
+offsets.  To keep ``state_dict()`` / ``load_state_dict()`` / the Collector's torch forward working unchanged (SURVEY 5:
+checkpoint/resume), every ``nn.Parameter`` is re-pointed at a view of that buffer: kernels update the flat buffer in
+place and the modules see the new weights without copies.
 """
 from __future__ import annotations
 
@@ -15,100 +15,12 @@ import torch
 from torch import nn
 from torch.distributions import Categorical, Independent, Normal
 
-from .._cabi import AC_CATEGORICAL, AC_RELU, ActorCriticDesc
+from .._cabi import call, ptr, stream_ptr
 
 
 class UnsupportedModelError(NotImplementedError):
     """Raised when actor / critic / dist_fn / optimizer are outside the fused kernel family.
     There is deliberately no eager-PyTorch fallback."""
-
-
-def _single_linear(mlp: Any, what: str) -> nn.Linear:
-    mods = list(mlp.model)
-    if len(mods) != 1 or not isinstance(mods[0], nn.Linear):
-        raise UnsupportedModelError(f"{what}: expected a single Linear head, got {mods}")
-    return mods[0]
-
-
-def _trunk(net: Any, what: str) -> tuple[nn.Linear, nn.Linear, bool]:
-    """Net(obs -> 64 -> 64, Tanh | ReLU) -> its two Linear layers and whether the activation is ReLU."""
-    mlp = getattr(net, "model", None)
-    seq = getattr(mlp, "model", None)
-    if seq is None:
-        raise UnsupportedModelError(f"{what}: preprocess net must be a tianshou_b200 Net/MLP")
-    mods = list(seq)
-    lin = [m for m in mods if isinstance(m, nn.Linear)]
-    act = [m for m in mods if not isinstance(m, nn.Linear)]
-    tanh = all(isinstance(a, nn.Tanh) for a in act)
-    relu = all(type(a) is nn.ReLU for a in act)
-    if len(lin) != 2 or len(mods) != 4 or not (tanh or relu):
-        raise UnsupportedModelError(
-            f"{what}: fused kernels support exactly Linear-Act-Linear-Act trunks with Act = Tanh or ReLU, got {mods}")
-    if getattr(net, "softmax", False):
-        raise UnsupportedModelError(f"{what}: softmax trunk output unsupported")
-    return lin[0], lin[1], relu
-
-
-def describe_actor_critic(actor: Any, critic: Any) -> tuple[ActorCriticDesc, list[nn.Parameter]]:
-    """Validate the module structure and return (desc, parameters in flat-buffer order).
-
-    Two families: the MuJoCo one (ContinuousActorProbabilistic + ContinuousCritic, separate trunks, Gaussian head)
-    and the reference's discrete PPO test net (DiscreteActor(softmax_output=True) + DiscreteCritic, optionally on ONE
-    shared preprocess Net; test/discrete/test_ppo_discrete.py:90-100).  A shared trunk appears once in the flat
-    buffer and both networks' descriptor offsets alias it."""
-    discrete = hasattr(actor, "softmax_output")
-    if discrete:
-        if not actor.softmax_output:
-            raise UnsupportedModelError("actor: DiscreteActor needs softmax_output=True (Categorical over probabilities)")
-        head = _single_linear(actor.last, "actor.last")
-    else:
-        if getattr(actor, "_c_sigma", False) or not hasattr(actor, "sigma_param"):
-            raise UnsupportedModelError("actor: conditioned sigma unsupported (need state-independent sigma_param)")
-        if not getattr(actor, "_unbounded", False):
-            raise UnsupportedModelError("actor: only unbounded=True (mu without tanh) is supported")
-        head = _single_linear(actor.mu, "actor.mu")
-    a1, a2, a_relu = _trunk(actor.preprocess, "actor")
-    a3 = head
-    c1, c2, c_relu = _trunk(critic.preprocess, "critic")
-    c3 = _single_linear(critic.last, "critic.last")
-    if a_relu != c_relu:
-        raise UnsupportedModelError("actor and critic trunks must use the same activation")
-    if getattr(critic, "apply_preprocess_net_to_obs_only", False):
-        raise UnsupportedModelError("critic: apply_preprocess_net_to_obs_only unsupported")
-    H, obs = a1.out_features, a1.in_features
-    act = a3.out_features
-    ok = (H == 64 and a2.in_features == H and a2.out_features == H and a3.in_features == H and
-          c1.in_features == obs and c1.out_features == H and c2.in_features == H and c2.out_features == H and
-          c3.in_features == H and c3.out_features == 1)
-    if not ok:
-        raise UnsupportedModelError("fused kernels support obs -> 64 -> 64 -> {act, 1} shapes only")
-    if obs > 64 or act > 16:
-        raise UnsupportedModelError(f"obs_dim {obs} > 64 or act_dim {act} > 16 unsupported")
-    for lin in (a1, a2, a3, c1, c2, c3):
-        if lin.bias is None:
-            raise UnsupportedModelError("Linear layers need a bias")
-    shared = a1 is c1 and a2 is c2
-    if not shared and (a1 is c1 or a2 is c2):
-        raise UnsupportedModelError("partially shared trunks are unsupported")
-    named = [("a_w1", a1.weight), ("a_b1", a1.bias), ("a_w2", a2.weight), ("a_b2", a2.bias), ("a_w3", a3.weight),
-             ("a_b3", a3.bias)]
-    if not discrete:
-        named.append(("a_logstd", actor.sigma_param))
-    if not shared:
-        named += [("c_w1", c1.weight), ("c_b1", c1.bias), ("c_w2", c2.weight), ("c_b2", c2.bias)]
-    named += [("c_w3", c3.weight), ("c_b3", c3.bias)]
-    d = ActorCriticDesc()
-    d.obs_dim, d.act_dim, d.hidden = obs, act, H
-    d.flags = (AC_RELU if a_relu else 0) | (AC_CATEGORICAL if discrete else 0)
-    d.a_logstd = -1
-    off = 0
-    for name, p in named:
-        setattr(d, name, off)
-        off += p.numel()
-    if shared:
-        d.c_w1, d.c_b1, d.c_w2, d.c_b2 = d.a_w1, d.a_b1, d.a_w2, d.a_b2
-    d.n_params = off
-    return d, [p for _, p in named]
 
 
 def check_categorical_dist_fn(dist_fn: Any, act_dim: int, device: torch.device) -> None:
@@ -129,76 +41,6 @@ def check_gaussian_dist_fn(dist_fn: Any, act_dim: int, device: torch.device) -> 
         raise UnsupportedModelError(f"dist_fn must build Independent(Normal(loc, scale), 1); got {d}")
 
 
-class FlatParams:
-    """Owns the flat parameter, gradient and Adam-moment buffers."""
-
-    def __init__(self, params: list[nn.Parameter], device: torch.device, grad_extra: int) -> None:
-        self.params = params
-        self.device = device
-        self.n = sum(p.numel() for p in params)
-        self.flat = torch.empty(self.n, dtype=torch.float32, device=device)
-        self.grad = torch.zeros(self.n + grad_extra, dtype=torch.float32, device=device)
-        # per-CTA partial gradient rows written by ts_ppo_grad (folded by ts_clip_adam_step)
-        from .._cabi import load_library
-        self.partial_rows = int(load_library().ts_ppo_partial_rows())
-        self.partials = torch.zeros((self.partial_rows, self.n + grad_extra), dtype=torch.float32, device=device)
-        self.exp_avg = torch.zeros(self.n, dtype=torch.float32, device=device)
-        self.exp_avg_sq = torch.zeros(self.n, dtype=torch.float32, device=device)
-        self.step = torch.zeros(1, dtype=torch.int64, device=device)
-        self.weight_image: torch.Tensor | None = None   # set by the algorithm (needs the network descriptor)
-        self._ptrs: list[int] = []
-        self.adopt()
-
-    def _views(self, buf: torch.Tensor) -> list[torch.Tensor]:
-        out, off = [], 0
-        for p in self.params:
-            out.append(buf[off:off + p.numel()].view(p.shape))
-            off += p.numel()
-        return out
-
-    def adopt(self) -> None:
-        """Copy current parameter values into the flat buffer and re-point ``p.data`` at views."""
-        with torch.no_grad():
-            for p, v in zip(self.params, self._views(self.flat), strict=True):
-                if p.data.data_ptr() != v.data_ptr():
-                    v.copy_(p.data.to(self.device, torch.float32))
-                    p.data = v
-        self._ptrs = [p.data.data_ptr() for p in self.params]
-
-    def ensure_adopted(self) -> None:
-        if [p.data.data_ptr() for p in self.params] != self._ptrs:
-            self.adopt()
-
-    # -- torch.optim.Adam state interop ----------------------------------------------------
-    def export_state(self, optimizer: torch.optim.Optimizer) -> None:
-        """Expose the flat moments as the torch optimizer's per-parameter state (views)."""
-        step = float(self.step.item())
-        if step == 0 and len(optimizer.state) == 0:
-            return
-        for p, m, v in zip(self.params, self._views(self.exp_avg), self._views(self.exp_avg_sq), strict=True):
-            optimizer.state[p] = {"step": torch.tensor(step, dtype=torch.float32), "exp_avg": m, "exp_avg_sq": v}
-
-    def import_state(self, optimizer: torch.optim.Optimizer) -> None:
-        """After ``optimizer.load_state_dict``: pull its moments / step into the flat buffers."""
-        steps = []
-        with torch.no_grad():
-            for p, m, v in zip(self.params, self._views(self.exp_avg), self._views(self.exp_avg_sq), strict=True):
-                st = optimizer.state.get(p)
-                if not st:
-                    m.zero_(); v.zero_()
-                    continue
-                m.copy_(st["exp_avg"].to(self.device, torch.float32))
-                v.copy_(st["exp_avg_sq"].to(self.device, torch.float32))
-                steps.append(float(st["step"]))
-        if steps:
-            if max(steps) != min(steps):
-                raise UnsupportedModelError("per-parameter Adam step counts differ; cannot fuse")
-            self.step.fill_(int(round(steps[0])))
-        else:
-            self.step.zero_()
-        self.export_state(optimizer)
-
-
 def adam_hyperparams(optimizer: torch.optim.Optimizer) -> dict[str, float]:
     if type(optimizer) is not torch.optim.Adam:
         raise UnsupportedModelError(f"fused update supports torch.optim.Adam only, got {type(optimizer).__name__}")
@@ -214,3 +56,130 @@ def adam_hyperparams(optimizer: torch.optim.Optimizer) -> dict[str, float]:
         raise ValueError("non-finite Adam hyper-parameters")
     return dict(lr=lr, beta1=float(b1), beta2=float(b2), adam_eps=float(g["eps"]),
                 weight_decay=float(g["weight_decay"]))
+
+
+def bind_optimizer(optim: Any, group: FlatGroup) -> None:
+    """Let ``group`` hold the state of ``optim`` (an ``Algorithm.Optimizer``): the kernels step the flat buffers with the
+    torch optimiser's hyper-parameters, and ``state_dict()`` / ``load_state_dict()`` go through ``group``."""
+    adam_hyperparams(optim._optim)
+    if set(map(id, optim._optim.param_groups[0]["params"])) != set(map(id, group.params)):
+        raise UnsupportedModelError("optimizer parameters differ from the fused network's parameters")
+    optim._flat = group
+
+
+class FlatGroup:
+    """Flat fp32 storage (parameters, gradient, Adam moments) of one optimiser's parameters.
+
+    The Adam step count has one owner: a host int that ``adam_step`` advances, or -- once ``step_dev`` exists -- the
+    int64[1] device counter that kernels advance without a host round trip.  ``device_step`` creates that counter up front
+    (the fused actor-critic kernels); ``adam_step_device`` creates it on first use (CUDA-graph mode).  ``grad_extra``
+    floats past the ``n`` parameters of ``grad`` are kernel scratch; ``partials`` and ``weight_image`` are scratch of the
+    fused actor-critic kernels, set by the algorithm that runs them."""
+
+    def __init__(self, params: list[nn.Parameter], device: torch.device, *, grad_extra: int = 0,
+                 device_step: bool = False) -> None:
+        self.params = list(params)
+        self.device = device
+        self.n = sum(p.numel() for p in self.params)
+        self.flat = torch.empty(self.n, dtype=torch.float32, device=device)
+        self.grad = torch.zeros(self.n + grad_extra, dtype=torch.float32, device=device)
+        self.exp_avg = torch.zeros(self.n, dtype=torch.float32, device=device)
+        self.exp_avg_sq = torch.zeros(self.n, dtype=torch.float32, device=device)
+        self.norm_scratch = torch.zeros(256, dtype=torch.float64, device=device)
+        self.partials: torch.Tensor | None = None
+        self.weight_image: torch.Tensor | None = None
+        self._step = 0
+        self.step_dev = torch.zeros(1, dtype=torch.int64, device=device) if device_step else None
+        self._offsets: dict[int, int] = {}
+        off = 0
+        for p in self.params:
+            self._offsets[id(p)] = off
+            off += p.numel()
+        self._ptrs: list[int] = []
+        self.adopt()
+
+    @property
+    def step(self) -> int | torch.Tensor:
+        """The Adam step count where it lives: ``step_dev`` when it exists, else the host int."""
+        return self.step_dev if self.step_dev is not None else self._step
+
+    def offset(self, p: nn.Parameter) -> int:
+        return self._offsets[id(p)]
+
+    def view(self, buf: torch.Tensor, p: nn.Parameter) -> torch.Tensor:
+        o = self._offsets[id(p)]
+        return buf[o:o + p.numel()]
+
+    def adopt(self) -> None:
+        """Copy current parameter values into the flat buffer and re-point ``p.data`` at views."""
+        with torch.no_grad():
+            for p in self.params:
+                v = self.view(self.flat, p).view(p.shape)
+                if p.data.data_ptr() != v.data_ptr():
+                    v.copy_(p.data.to(self.device, torch.float32))
+                    p.data = v
+        self._ptrs = [p.data.data_ptr() for p in self.params]
+
+    def ensure_adopted(self) -> None:
+        if [p.data.data_ptr() for p in self.params] != self._ptrs:
+            self.adopt()
+
+    def adam_step(self, optimizer: torch.optim.Optimizer, max_grad_norm: float | None) -> None:
+        """``Algorithm.Optimizer.step`` after backward: clip_grad_norm_ (optional) + Adam (algorithm_base.py:496-500)."""
+        hp = adam_hyperparams(optimizer)
+        step = self.sync_step_from_device() + 1
+        if self.step_dev is not None:
+            self.step_dev.fill_(step)
+        else:
+            self._step = step
+        call("ts_adam_step", ptr(self.flat), ptr(self.grad), ptr(self.exp_avg), ptr(self.exp_avg_sq), self.n, step,
+             hp["lr"], hp["beta1"], hp["beta2"], hp["adam_eps"], hp["weight_decay"], float(max_grad_norm or 0.0),
+             ptr(self.norm_scratch), stream_ptr(self.device))
+
+    def adam_step_device(self, optimizer: torch.optim.Optimizer, max_grad_norm: float | None) -> None:
+        """Same step with the step number read from / advanced in DEVICE memory: nothing in the launch depends on host state,
+        so it can live inside a captured CUDA graph."""
+        hp = adam_hyperparams(optimizer)
+        if self.step_dev is None:
+            self.step_dev = torch.tensor([self._step], dtype=torch.int64, device=self.device)
+        call("ts_adam_step_dev", ptr(self.flat), ptr(self.grad), ptr(self.exp_avg), ptr(self.exp_avg_sq), self.n, ptr(self.step_dev),
+             hp["lr"], hp["beta1"], hp["beta2"], hp["adam_eps"], hp["weight_decay"], float(max_grad_norm or 0.0),
+             ptr(self.norm_scratch), stream_ptr(self.device))
+
+    def sync_step_from_device(self) -> int:
+        """The step count as a host int: one read of ``step_dev`` when the device counter owns it."""
+        return int(self.step_dev.item()) if self.step_dev is not None else self._step
+
+    # -- torch.optim.Adam state interop ----------------------------------------------------
+    def export_state(self, optimizer: torch.optim.Optimizer) -> None:
+        """Expose the flat moments as the torch optimizer's per-parameter state (views)."""
+        step = self.sync_step_from_device()
+        if step == 0 and len(optimizer.state) == 0:
+            return
+        for p in self.params:
+            optimizer.state[p] = {"step": torch.tensor(float(step), dtype=torch.float32),
+                                  "exp_avg": self.view(self.exp_avg, p).view(p.shape),
+                                  "exp_avg_sq": self.view(self.exp_avg_sq, p).view(p.shape)}
+
+    def import_state(self, optimizer: torch.optim.Optimizer) -> None:
+        """After ``optimizer.load_state_dict`` or an eager ``optimizer.step()``: pull its moments / step into the flat
+        buffers, then expose them as the optimizer's state again."""
+        steps = []
+        with torch.no_grad():
+            for p in self.params:
+                st = optimizer.state.get(p)
+                m, v = self.view(self.exp_avg, p), self.view(self.exp_avg_sq, p)
+                if not st:
+                    m.zero_(); v.zero_()
+                    continue
+                m.copy_(st["exp_avg"].to(self.device, torch.float32).reshape(-1))
+                v.copy_(st["exp_avg_sq"].to(self.device, torch.float32).reshape(-1))
+                steps.append(float(st["step"]))
+        if steps and max(steps) != min(steps):
+            raise UnsupportedModelError("per-parameter Adam step counts differ; cannot fuse")
+        step = int(round(steps[0])) if steps else 0
+        if self.step_dev is not None:
+            self.step_dev.fill_(step)
+        else:
+            self._step = step
+        self.export_state(optimizer)

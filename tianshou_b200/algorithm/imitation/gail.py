@@ -28,12 +28,12 @@ from ...data import Batch, ReplayBuffer, SequenceSummaryStats
 from ...data.batch import minibatch_bounds, numpy_global_permutation_
 from ...utils.net.common import ModuleWithVectorOutput
 from ..base import _space_kind
-from ..flat_params import UnsupportedModelError, adam_hyperparams
+from ..flat_params import FlatGroup, UnsupportedModelError, bind_optimizer
 from ..modelfree.a2c import A2CTrainingStats, ActorCriticOnPolicyAlgorithm
 from ..modelfree.ppo import PPO
 from ..modelfree.reinforce import ProbabilisticActorPolicy
 from ..modelfree.sac import describe_q_critic
-from ..netgraph import FlatGroup, FusedStack
+from ..netgraph import FusedStack
 from ..optim import OptimizerFactory
 
 # columns of the per-step discriminator table ``last_disc_table``
@@ -89,19 +89,13 @@ class GAIL(PPO):
         self.expert_buffer = expert_buffer
         self.action_dim = self.policy.actor.get_output_dim()
 
-        if self._layered is not None:
-            self._obs_dim, self._act_dim = self._layered.obs_dim, self._layered.act_dim
-        else:
-            self._obs_dim, self._act_dim = int(self._desc.obs_dim), int(self._desc.act_dim)
+        self._obs_dim, self._act_dim = self._spec.obs_dim, self._spec.act_dim
         try:
             layers, params = describe_q_critic(disc_net, self._obs_dim, self._act_dim)
         except AttributeError as e:
             raise UnsupportedModelError(f"discriminator: expected ContinuousCritic(preprocess_net=Net(concat=True)): {e}") from e
-        adam_hyperparams(self.disc_optim._optim)
         self._g_disc = FlatGroup(params, self.device)
-        if set(map(id, self.disc_optim._optim.param_groups[0]["params"])) != set(map(id, self._g_disc.params)):
-            raise UnsupportedModelError("discriminator optimizer parameters differ from the discriminator's Linear layers")
-        self.disc_optim._flat = self._g_disc
+        bind_optimizer(self.disc_optim, self._g_disc)
         self._disc = FusedStack(layers, self._g_disc, "disc")
         self._check_expert_buffer()
         self._disc_order: torch.Tensor | None = None

@@ -1,9 +1,10 @@
-"""Actor-critic networks OUTSIDE the fused 17-64-64 kernels' shape envelope, layer by layer on the tensor cores.
+"""Actor-critic structure, and the networks OUTSIDE the fused 17-64-64 kernels' shape envelope layer by layer on the tensor cores.
 
-``describe_actor_critic`` (flat_params.py) accepts exactly the shapes the persistent tensor-core / SIMT update kernels were
-written for (two-layer 64-wide trunks, obs <= 64).  Everything else that is still a Linear / ReLU | Tanh actor-critic --
-wider or deeper trunks, large observations (Humanoid: 376), the reference's shared-trunk discrete PPO net at other widths
--- runs here: every Linear forward / input gradient / weight gradient is one ``ts_net_gemm`` launch (wgmma,
+``parse_actor_critic`` reads the actor / critic modules once: every on-policy algorithm runs what it accepts, and
+``fused_descriptor`` picks out the shapes the persistent tensor-core / SIMT update kernels were written for (two-layer
+64-wide trunks, obs <= 64).  Everything else that is still a Linear / ReLU | Tanh actor-critic -- wider or deeper trunks,
+large observations (Humanoid: 376), the reference's shared-trunk discrete PPO net at other widths -- runs in
+``LayeredActorCritic``: every Linear forward / input gradient / weight gradient is one ``ts_net_gemm`` launch (wgmma,
 fp32-faithful), the PPO / A2C loss between them is ``ts_ppo_rows``, the optimiser ``ts_adam_step`` (global-norm clip + Adam).
 Same public behaviour as the fused path (ppo.py:146-224, a2c.py:115-153); single GPU.
 
@@ -14,75 +15,139 @@ separate or ONE shared ``Net`` (utils/net/discrete.py:29-123, test/discrete/test
 from __future__ import annotations
 
 import ctypes as C
+from dataclasses import dataclass
 from typing import Any
 
-import numpy as np
 import torch
 from torch import nn
 
 from .. import ops
-from .._cabi import STATS_STRIDE, call, ptr, stream_ptr
-from .flat_params import UnsupportedModelError
-from .netgraph import ACT_NONE, FlatGroup, FusedStack, compile_sequential, module_layers
+from .._cabi import AC_CATEGORICAL, AC_RELU, STATS_STRIDE, ActorCriticDesc, call, ptr, stream_ptr
+from .flat_params import FlatGroup, UnsupportedModelError
+from .netgraph import ACT_NONE, ACT_RELU, FusedStack, _Layer, compile_sequential, module_layers
 
 _CHUNK = 131072          # rows per forward chunk of the whole-rollout passes (bounds the activation scratch)
 
 
+@dataclass
+class ActorCriticSpec:
+    """The structure of an accepted actor-critic.  ``group_params``: the parameters of each layer-wise ``FlatGroup`` in
+    module order -- one group (``ActorCritic(actor, critic).parameters()``, a shared trunk once), or the actor's and the
+    critic's when ``split``."""
+    obs_dim: int
+    act_dim: int
+    categorical: bool
+    shared: bool
+    sigma_param: nn.Parameter | None
+    a_trunk: list[_Layer]
+    a_head: list[_Layer]
+    c_trunk: list[_Layer]
+    c_head: list[_Layer]
+    group_params: list[list[nn.Parameter]]
+
+
+def _layer_params(layers: list[_Layer]) -> list[nn.Parameter]:
+    return [p for L in layers if L.weight is not None for p in (L.weight, L.bias)]
+
+
+def parse_actor_critic(actor: Any, critic: Any, *, split: bool) -> ActorCriticSpec:
+    """Validate the actor / critic modules and compile their layers; raises ``UnsupportedModelError`` for anything the
+    kernels do not run.  Pure: allocates nothing and works on modules on any device.  ``split``: the actor and the critic
+    get one parameter group each (NPG / TRPO step the actor along the natural gradient and the critic with its own
+    optimiser).  A trunk is shared when actor and critic hold the very same trunk parameters; sharing only some of them is
+    refused (the two backward passes would overwrite each other's gradient in the shared slots)."""
+    categorical = hasattr(actor, "softmax_output")
+    if categorical and not actor.softmax_output:
+        raise UnsupportedModelError("actor: DiscreteActor needs softmax_output=True (Categorical over probabilities)")
+    if not categorical:
+        if getattr(actor, "_c_sigma", False) or not hasattr(actor, "sigma_param"):
+            raise UnsupportedModelError("actor: conditioned sigma unsupported (need state-independent sigma_param)")
+        if not getattr(actor, "_unbounded", False):
+            raise UnsupportedModelError("actor: only unbounded=True (mu without tanh) is supported")
+    if getattr(critic, "apply_preprocess_net_to_obs_only", False):
+        raise UnsupportedModelError("critic: apply_preprocess_net_to_obs_only unsupported")
+    for net, what in ((actor.preprocess, "actor"), (critic.preprocess, "critic")):
+        if getattr(net, "softmax", False):
+            raise UnsupportedModelError(f"{what}: softmax trunk output unsupported")
+    a_mods = module_layers(actor.preprocess)
+    first = next((m for m in a_mods if isinstance(m, nn.Linear)), None)
+    if first is None:
+        raise UnsupportedModelError("actor trunk has no Linear layer")
+    obs_dim = int(first.in_features)
+    a_trunk = compile_sequential(a_mods, (obs_dim,))
+    c_trunk = compile_sequential(module_layers(critic.preprocess), (obs_dim,))
+    a_head = compile_sequential(module_layers(actor.last if categorical else actor.mu), (a_trunk[-1].out_dim,))
+    c_head = compile_sequential(module_layers(critic.last), (c_trunk[-1].out_dim,))
+    if a_head[-1].act != ACT_NONE or c_head[-1].act != ACT_NONE or c_head[-1].out_dim != 1:
+        raise UnsupportedModelError("heads must end in a linear layer (critic: one output)")
+    act_dim = int(a_head[-1].out_dim)
+    if act_dim > 64:
+        raise UnsupportedModelError("action width > 64 unsupported")
+    a_ids, c_ids = set(map(id, actor.parameters())), set(map(id, critic.parameters()))
+    trunk_ids = [id(p) for p in _layer_params(a_trunk)]
+    shared = trunk_ids == [id(p) for p in _layer_params(c_trunk)] and [L.act for L in a_trunk] == [L.act for L in c_trunk]
+    if (a_ids & c_ids) != (set(trunk_ids) if shared else set()):
+        raise UnsupportedModelError("partially shared trunks are unsupported")
+    if split and shared:
+        raise UnsupportedModelError("a critic-only optimiser (NPG / TRPO) needs separate actor and critic trunks; "
+                                    "shared trunks are unsupported")
+    params = list({id(p): p for p in [*actor.parameters(), *critic.parameters()]}.values())   # ActorCritic order, shared once
+    sigma_param = None if categorical else actor.sigma_param
+    covered = {id(p) for p in _layer_params([*a_trunk, *c_trunk, *a_head, *c_head])}
+    if [id(p) for p in params if id(p) not in covered] != ([] if categorical else [id(sigma_param)]):
+        raise UnsupportedModelError("actor / critic hold parameters outside the Linear layers")
+    return ActorCriticSpec(obs_dim, act_dim, categorical, shared, sigma_param, a_trunk, a_head, c_trunk, c_head,
+                           [list(actor.parameters()), list(critic.parameters())] if split else [params])
+
+
+def fused_descriptor(spec: ActorCriticSpec) -> tuple[ActorCriticDesc, list[nn.Parameter]] | None:
+    """(descriptor, parameters in flat-buffer order) for the fused tensor-core / SIMT kernels, or None when the networks are
+    outside their envelope: trunks exactly Linear+act -> Linear+act, 64 wide, one activation (Tanh or ReLU) in both, each
+    head a single Linear, obs_dim <= 64, act_dim <= 16.  Two families: the MuJoCo one (Gaussian head, separate trunks) and
+    the reference's discrete PPO test net (test/discrete/test_ppo_discrete.py:90-100), optionally on ONE shared trunk, which
+    appears once in the flat buffer while both networks' descriptor offsets alias it."""
+    trunks = (spec.a_trunk, spec.c_trunk)
+    if any(len(t) != 2 or any(L.kind != "linear" or L.act == ACT_NONE or L.out_dim != 64 for L in t) for t in trunks):
+        return None
+    if len({L.act for t in trunks for L in t}) != 1 or len(spec.a_head) != 1 or len(spec.c_head) != 1:
+        return None
+    if spec.obs_dim > 64 or spec.act_dim > 16:
+        return None
+    (a1, a2), (c1, c2), a3, c3 = spec.a_trunk, spec.c_trunk, spec.a_head[0], spec.c_head[0]
+    named = [("a_w1", a1.weight), ("a_b1", a1.bias), ("a_w2", a2.weight), ("a_b2", a2.bias), ("a_w3", a3.weight),
+             ("a_b3", a3.bias)]
+    if not spec.categorical:
+        named.append(("a_logstd", spec.sigma_param))
+    if not spec.shared:
+        named += [("c_w1", c1.weight), ("c_b1", c1.bias), ("c_w2", c2.weight), ("c_b2", c2.bias)]
+    named += [("c_w3", c3.weight), ("c_b3", c3.bias)]
+    d = ActorCriticDesc()
+    d.obs_dim, d.act_dim, d.hidden = spec.obs_dim, spec.act_dim, 64
+    d.flags = (AC_RELU if a1.act == ACT_RELU else 0) | (AC_CATEGORICAL if spec.categorical else 0)
+    d.a_logstd = -1
+    off = 0
+    for name, p in named:
+        setattr(d, name, off)
+        off += p.numel()
+    if spec.shared:
+        d.c_w1, d.c_b1, d.c_w2, d.c_b2 = d.a_w1, d.a_b1, d.a_w2, d.a_b2
+    d.n_params = off
+    return d, [p for _, p in named]
+
+
 class LayeredActorCritic:
-    def __init__(self, actor: Any, critic: Any, device: torch.device, split: bool = False) -> None:
-        """``split``: the actor and the critic get one ``FlatGroup`` each (``group`` / ``critic_group``) -- NPG / TRPO step the
-        actor along the natural gradient and the critic with its own optimiser; otherwise both share ``group``."""
+    def __init__(self, spec: ActorCriticSpec, device: torch.device) -> None:
+        """One ``FlatGroup`` per entry of ``spec.group_params``: ``group`` holds the actor, ``critic_group`` the critic
+        (the same group unless the spec is split)."""
         self.device = device
-        self.categorical = hasattr(actor, "softmax_output")
-        if self.categorical and not actor.softmax_output:
-            raise UnsupportedModelError("actor: DiscreteActor needs softmax_output=True (Categorical over probabilities)")
-        if not self.categorical:
-            if getattr(actor, "_c_sigma", False) or not hasattr(actor, "sigma_param"):
-                raise UnsupportedModelError("actor: conditioned sigma unsupported (need state-independent sigma_param)")
-            if not getattr(actor, "_unbounded", False):
-                raise UnsupportedModelError("actor: only unbounded=True (mu without tanh) is supported")
-        if getattr(critic, "apply_preprocess_net_to_obs_only", False):
-            raise UnsupportedModelError("critic: apply_preprocess_net_to_obs_only unsupported")
-        for net, what in ((actor.preprocess, "actor"), (critic.preprocess, "critic")):
-            if getattr(net, "softmax", False):
-                raise UnsupportedModelError(f"{what}: softmax trunk output unsupported")
-        self.shared = actor.preprocess is critic.preprocess
-        if split and self.shared:
-            raise UnsupportedModelError("a critic-only optimiser (NPG / TRPO) needs separate actor and critic trunks; "
-                                        "shared trunks are unsupported")
-        a_mods = module_layers(actor.preprocess)
-        first = next((m for m in a_mods if isinstance(m, nn.Linear)), None)
-        if first is None:
-            raise UnsupportedModelError("actor trunk has no Linear layer")
-        self.obs_dim = int(first.in_features)
-        a_trunk = compile_sequential(a_mods, (self.obs_dim,))
-        c_trunk = a_trunk if self.shared else compile_sequential(module_layers(critic.preprocess), (self.obs_dim,))
-        a_head = compile_sequential(module_layers(actor.last if self.categorical else actor.mu), (a_trunk[-1].out_dim,))
-        c_head = compile_sequential(module_layers(critic.last), (c_trunk[-1].out_dim,))
-        if a_head[-1].act != ACT_NONE or c_head[-1].act != ACT_NONE or c_head[-1].out_dim != 1:
-            raise UnsupportedModelError("heads must end in a linear layer (critic: one output)")
-        self.act_dim = int(a_head[-1].out_dim)
-        if self.act_dim > 64:
-            raise UnsupportedModelError("action width > 64 unsupported")
-        seen: set[int] = set()
-        params: list[nn.Parameter] = []
-        for p in [*actor.parameters(), *critic.parameters()]:      # ActorCritic(actor, critic).parameters() order, shared once
-            if id(p) not in seen:
-                seen.add(id(p))
-                params.append(p)
-        covered = {id(L.weight) for L in (*a_trunk, *c_trunk, *a_head, *c_head)} | {id(L.bias) for L in (*a_trunk, *c_trunk, *a_head, *c_head)}
-        extra = [p for p in params if id(p) not in covered]
-        self.sigma_param = None if self.categorical else actor.sigma_param
-        if [id(p) for p in extra] != ([] if self.categorical else [id(self.sigma_param)]):
-            raise UnsupportedModelError("actor / critic hold parameters outside the Linear layers")
-        if split:      # npg.py:195-224 works on policy.actor.parameters() in their order
-            self.group, self.critic_group = FlatGroup(list(actor.parameters()), device), FlatGroup(list(critic.parameters()), device)
-        else:
-            self.group = self.critic_group = FlatGroup(params, device)
-        self.a_trunk, self.a_head = FusedStack(a_trunk, self.group, "a_trunk"), FusedStack(a_head, self.group, "a_head")
-        self.c_trunk = self.a_trunk if self.shared else FusedStack(c_trunk, self.critic_group, "c_trunk")
-        self.c_head = FusedStack(c_head, self.critic_group, "c_head")
-        self._a_act, self._c_act = a_trunk[-1].act, c_trunk[-1].act
+        self.categorical, self.shared, self.act_dim = spec.categorical, spec.shared, spec.act_dim
+        groups = [FlatGroup(p, device) for p in spec.group_params]
+        self.group, self.critic_group = groups[0], groups[-1]
+        self.a_trunk, self.a_head = FusedStack(spec.a_trunk, self.group, "a_trunk"), FusedStack(spec.a_head, self.group, "a_head")
+        self.c_trunk = self.a_trunk if self.shared else FusedStack(spec.c_trunk, self.critic_group, "c_trunk")
+        self.c_head = FusedStack(spec.c_head, self.critic_group, "c_head")
+        self.sigma_param = spec.sigma_param
+        self._a_act, self._c_act = spec.a_trunk[-1].act, spec.c_trunk[-1].act
         self._scratch: dict[str, torch.Tensor] = {}
 
     # ------------------------------------------------------------------ helpers
@@ -165,13 +230,6 @@ class LayeredActorCritic:
         if dls is not None:
             call("ts_net_colsum", ptr(dls), A, B, A, self._logstd_ptr(self.group.grad), 0, st)
         self.group.adam_step(optimizer, max_grad_norm)
-
-
-def try_layered(actor: Any, critic: Any, split: bool = False) -> LayeredActorCritic:
-    plist = list(actor.parameters())
-    if not plist or plist[0].device.type != "cuda":
-        raise UnsupportedModelError("actor/critic must live on a CUDA device; tianshou_b200 has no CPU path")
-    return LayeredActorCritic(actor, critic, plist[0].device, split=split)
 
 
 def layered_update(algo: Any, batch: Any, batch_size: int | None, repeat: int) -> torch.Tensor:

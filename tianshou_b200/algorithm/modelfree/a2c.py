@@ -14,6 +14,8 @@ What changes (same signatures, same 3-phase structure as ``Algorithm._update``):
 """
 from __future__ import annotations
 
+import ctypes as C
+import os
 from abc import ABC
 from dataclasses import dataclass
 from typing import Any
@@ -22,19 +24,20 @@ import numpy as np
 import torch
 
 from ... import ops
-from ..._cabi import AC_CATEGORICAL, GRAD_EXTRA, STATS_STRIDE, PPOHParams, to_device
+from ..._cabi import GRAD_EXTRA, STATS_STRIDE, PPOHParams, load_library, to_device
 from ...data import Batch, ReplayBuffer, SequenceSummaryStats
 from ...utils import RunningMeanStd
 from ...utils.net.common import ActorCritic
 from ..base import OnPolicyAlgorithm, TrainingStats
 from ..flat_params import (
-    FlatParams,
+    FlatGroup,
     UnsupportedModelError,
     adam_hyperparams,
+    bind_optimizer,
     check_categorical_dist_fn,
     check_gaussian_dist_fn,
-    describe_actor_critic,
 )
+from ..layered import LayeredActorCritic, fused_descriptor, parse_actor_critic
 from ..optim import OptimizerFactory
 from .reinforce import ProbabilisticActorPolicy
 
@@ -68,51 +71,37 @@ class ActorCriticOnPolicyAlgorithm(OnPolicyAlgorithm, ABC):
         self.gae_lambda = gae_lambda
         self.max_batchsize = max_batchsize  # kept for API parity; the fused pass needs no chunking
         self._actor_critic = ActorCritic(self.policy.actor, self.critic)
-        # kernel-side view of the networks: validate structure, flatten parameters.  Shapes outside the fused kernels' envelope
-        # (two 64-wide layers, obs <= 64) run layer by layer on the tensor-core GEMM (algorithm/layered.py); anything that is
-        # not a Linear / ReLU | Tanh actor-critic raises -- there is no eager-PyTorch path.
-        self._layered = None
-        if not optim_include_actor:
-            # critic-only optimiser (NPG / TRPO, a2c.py:102-109): the actor moves along the natural gradient, so the fused
-            # kernels (one Adam step over both networks) do not apply; the layer-wise path runs whatever the shape
-            from ..layered import try_layered
-            self._layered = try_layered(self.policy.actor, self.critic, split=True)
-            self._desc, plist = None, self._layered.critic_group.params
-        else:
-            try:
-                import os as _os
-                if _os.environ.get("TS_B200_FORCE_LAYERED", "0") == "1":      # tests: run the layer-wise path on any shape
-                    raise UnsupportedModelError("TS_B200_FORCE_LAYERED=1")
-                self._desc, plist = describe_actor_critic(self.policy.actor, self.critic)
-            except UnsupportedModelError as fused_err:
-                from ..layered import try_layered
-                try:
-                    self._layered = try_layered(self.policy.actor, self.critic)
-                except UnsupportedModelError as layered_err:
-                    raise UnsupportedModelError(f"{fused_err}; layer-wise path: {layered_err}") from layered_err
-                self._desc, plist = None, self._layered.group.params
-        dev = plist[0].device
+        # kernel-side view of the networks.  Shapes outside the fused kernels' envelope (two 64-wide layers, obs <= 64) run
+        # layer by layer on the tensor-core GEMM (algorithm/layered.py), and so does a critic-only optimiser (NPG / TRPO,
+        # a2c.py:102-109: the actor moves along the natural gradient, while the fused kernels take one Adam step over both
+        # networks); anything that is not a Linear / ReLU | Tanh actor-critic raises -- there is no eager-PyTorch path.
+        self._spec = parse_actor_critic(self.policy.actor, self.critic, split=not optim_include_actor)
+        dev = next(self.policy.actor.parameters()).device
         if dev.type != "cuda":
             raise UnsupportedModelError(
                 f"actor/critic live on {dev}; tianshou_b200 has no CPU path -- move them to a CUDA device first")
-        categorical = self._layered.categorical if self._layered is not None else bool(self._desc.flags & AC_CATEGORICAL)
-        act_dim = self._layered.act_dim if self._layered is not None else self._desc.act_dim
-        if categorical:
-            check_categorical_dist_fn(self.policy.dist_fn, act_dim, dev)
+        if self._spec.categorical:
+            check_categorical_dist_fn(self.policy.dist_fn, self._spec.act_dim, dev)
         else:
-            check_gaussian_dist_fn(self.policy.dist_fn, act_dim, dev)
-        if self._layered is not None:
+            check_gaussian_dist_fn(self.policy.dist_fn, self._spec.act_dim, dev)
+        force_layered = os.environ.get("TS_B200_FORCE_LAYERED", "0") == "1"      # tests: the layer-wise path on any shape
+        fused = fused_descriptor(self._spec) if optim_include_actor and not force_layered else None
+        if fused is None:
+            self._desc, self._layered = None, LayeredActorCritic(self._spec, dev)
             if self._world_size() > 1 and getattr(self, "data_parallel", True):
                 raise UnsupportedModelError("the layer-wise actor-critic path is single-GPU")
             self._flat = self._layered.critic_group        # the optimiser's parameters (``group`` unless split)
-            self._flat.weight_image = None
         else:
-            self._flat = FlatParams(plist, dev, GRAD_EXTRA)
+            self._desc, plist = fused
+            self._layered = None
+            self._flat = FlatGroup(plist, dev, grad_extra=GRAD_EXTRA, device_step=True)
+            lib = load_library()
+            # per-CTA partial gradient rows written by ts_ppo_grad (folded by ts_clip_adam_step)
+            self._flat.partials = torch.zeros((int(lib.ts_ppo_partial_rows()), self._flat.n + GRAD_EXTRA), dtype=torch.float32,
+                                              device=dev)
             # scratch for the pre-split (bf16x3) weight image of the tensor-core update kernel; None -> the
             # kernels gather + split the weights themselves (networks the tensor-core path does not cover)
-            import ctypes as _C
-            from ..._cabi import load_library
-            nbytes = int(load_library().ts_ppo_weight_image_bytes(_C.byref(self._desc)))
+            nbytes = int(lib.ts_ppo_weight_image_bytes(C.byref(self._desc)))
             self._flat.weight_image = torch.zeros(nbytes, dtype=torch.uint8, device=dev) if nbytes > 0 else None
             if hasattr(self.policy, "_fused_inference"):      # Collector-side inference through the same forward kernel
                 self.policy._fused_inference = (self._flat, self._desc)
@@ -122,8 +111,7 @@ class ActorCriticOnPolicyAlgorithm(OnPolicyAlgorithm, ABC):
         # a real torch Adam (+ scheduler) keeps lr schedules and state_dict round trips unchanged
         self.optim = self._create_optimizer(self._actor_critic if optim_include_actor else self.critic, optim,
                                             max_grad_norm=max_grad_norm)
-        adam_hyperparams(self.optim._optim)  # validates optimizer family early
-        self.optim._flat = self._flat
+        bind_optimizer(self.optim, self._flat)
         self.max_grad_norm = max_grad_norm
         self.gamma = gamma
         self.return_scaling = return_scaling
@@ -160,10 +148,7 @@ class ActorCriticOnPolicyAlgorithm(OnPolicyAlgorithm, ABC):
                                         "by the MLP actor-critic kernels")
         obs_w = int(np.prod(meta_host.obs.shape[1:], dtype=np.int64))
         act_w = int(np.prod(meta_host.act.shape[1:], dtype=np.int64))
-        if self._layered is not None:
-            net_obs, want_act = self._layered.obs_dim, (1 if self._layered.categorical else self._layered.act_dim)
-        else:
-            net_obs, want_act = int(self._desc.obs_dim), (1 if self._desc.flags & AC_CATEGORICAL else int(self._desc.act_dim))
+        net_obs, want_act = self._spec.obs_dim, (1 if self._spec.categorical else self._spec.act_dim)
         if obs_w != net_obs or act_w != want_act:
             raise ValueError(f"buffer rows (obs width {obs_w}, act width {act_w}) do not match the networks "
                              f"(obs_dim {net_obs}, action width {want_act})")

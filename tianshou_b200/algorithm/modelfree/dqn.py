@@ -27,8 +27,8 @@ from ... import ops
 from ..._cabi import call, ptr, stream_ptr, to_device
 from ...data import Batch, ReplayBuffer, to_numpy
 from ..base import OffPolicyAlgorithm, Policy, TrainingStats
-from ..flat_params import UnsupportedModelError
-from ..netgraph import ACT_NONE, FlatGroup, FusedStack, compile_sequential, module_layers
+from ..flat_params import FlatGroup, UnsupportedModelError, bind_optimizer
+from ..netgraph import ACT_NONE, FusedStack, compile_sequential, module_layers
 from ..optim import OptimizerFactory
 
 
@@ -144,9 +144,7 @@ class DQN(OffPolicyAlgorithm):
         self._group = FlatGroup(params, dev)
         self._net = FusedStack(layers, self._group, "q")
         self.optim = self._create_optimizer(policy, optim)
-        if set(map(id, self.optim._optim.param_groups[0]["params"])) != set(map(id, params)):
-            raise UnsupportedModelError("optimizer parameters differ from the fused network's parameters")
-        self.optim._flat = self._group
+        bind_optimizer(self.optim, self._group)
         self.model_old = deepcopy(policy.model).eval() if self.use_target_network else None
         self._target_flat = self._group.flat.clone() if self.use_target_network else None
         self._scratch: dict[str, torch.Tensor] = {}

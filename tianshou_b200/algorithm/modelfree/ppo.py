@@ -278,7 +278,7 @@ class FusedActorCriticUpdate(ActorCriticOnPolicyAlgorithm):
         adv_tmp = self._buf("adv_tmp", 32 + 8 * n_mb, torch.uint8)
         adv_tmp.zero_()
         bounds_c = (C.c_int64 * (2 * n_mb))(*[x for b in bounds for x in b])
-        call("ts_ppo_update", ptr(f.flat), ptr(f.grad), ptr(f.partials), ptr(f.exp_avg), ptr(f.exp_avg_sq), ptr(f.step),
+        call("ts_ppo_update", ptr(f.flat), ptr(f.grad), ptr(f.partials), ptr(f.exp_avg), ptr(f.exp_avg_sq), ptr(f.step_dev),
              C.byref(self._desc), C.byref(hp), ptr(batch.obs), ptr(batch.obs_next), ptr(batch.act),
              ptr(batch.rew), ptr(batch.terminated), ptr(batch.truncated), ptr(batch.get("_unfinished")),
              ptr(batch.v_s), ptr(batch.returns), ptr(batch.adv), ptr(batch.logp_old),
@@ -323,7 +323,7 @@ class FusedActorCriticUpdate(ActorCriticOnPolicyAlgorithm):
             allreduce_sum_(sums)
             adv_mom = self._buf("epoch_adv_mom", 2 * n_mb, torch.float32)
             call("ts_epoch_adv_finalize", ptr(sums), lo0, size, end, n_mb, wsize, ptr(adv_mom), st)
-        call("ts_ppo_epoch_multi", ptr(f.flat), ptr(f.grad), ptr(f.partials), ptr(f.exp_avg), ptr(f.exp_avg_sq), ptr(f.step),
+        call("ts_ppo_epoch_multi", ptr(f.flat), ptr(f.grad), ptr(f.partials), ptr(f.exp_avg), ptr(f.exp_avg_sq), ptr(f.step_dev),
              C.byref(self._desc), C.byref(hp), ptr(batch.obs), ptr(batch.act), ptr(batch.adv), ptr(batch.returns),
              ptr(batch.logp_old), ptr(batch.v_s), ptr(perm), lo0, size, end, n_mb, ptr(adv_mom), ptr(f.weight_image),
              ptr(stats), rank, wsize, ex.ptrs, st)
@@ -351,7 +351,7 @@ class FusedActorCriticUpdate(ActorCriticOnPolicyAlgorithm):
                  global_rows, ptr(adv_mom), ptr(f.partials), C.byref(n_part), st)
             call("ts_grad_reduce", ptr(f.partials), n_part.value, C.byref(self._desc), ptr(f.grad), st)
             allreduce_sum_(f.grad)   # ONE collective per optimiser step: grads + loss sums
-            call("ts_clip_adam_step", ptr(f.flat), ptr(f.grad), None, 0, ptr(f.exp_avg), ptr(f.exp_avg_sq), ptr(f.step),
+            call("ts_clip_adam_step", ptr(f.flat), ptr(f.grad), None, 0, ptr(f.exp_avg), ptr(f.exp_avg_sq), ptr(f.step_dev),
                  C.byref(self._desc), C.byref(hp), ptr(stats[m]), st)
 
 

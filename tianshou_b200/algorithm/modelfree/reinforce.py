@@ -34,7 +34,7 @@ class ProbabilisticActorPolicy(Policy):
         self.dist_fn = dist_fn
         self._eps = 1e-8
         self.deterministic_eval = deterministic_eval
-        # set by the owning algorithm when the actor belongs to the fused kernel family: (FlatParams, desc).
+        # set by the owning algorithm when the actor belongs to the fused kernel family: (FlatGroup, desc).
         # Inference under torch.no_grad() then runs ONE kernel (the update path's forward kernel) instead of the
         # module-by-module torch forward (SURVEY 8(f) rank 4: Collector._compute_action_policy_hidden).
         self._fused_inference: Any = None

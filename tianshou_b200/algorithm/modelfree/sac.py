@@ -27,8 +27,8 @@ from torch.distributions import Independent, Normal
 from ..._cabi import call, ptr, stream_ptr, to_device
 from ...data import Batch, ReplayBuffer
 from ..base import OffPolicyAlgorithm, Policy, TrainingStats
-from ..flat_params import UnsupportedModelError
-from ..netgraph import ACT_NONE, FlatGroup, FusedStack, _Layer, compile_sequential, module_layers, polyak_update
+from ..flat_params import FlatGroup, UnsupportedModelError, bind_optimizer
+from ..netgraph import ACT_NONE, FusedStack, _Layer, compile_sequential, module_layers, polyak_update
 from ..optim import OptimizerFactory
 
 SIGMA_MIN, SIGMA_MAX = -20.0, 2.0          # utils/net/continuous.py:17-18
@@ -222,9 +222,7 @@ class SAC(OffPolicyAlgorithm):
         self.critic_optim = self._create_optimizer(self.critic, critic_optim)
         self.critic2_optim = self._create_optimizer(self.critic2, critic2_optim or critic_optim)
         for o, g in ((self.policy_optim, self._g_actor), (self.critic_optim, self._g_c[0]), (self.critic2_optim, self._g_c[1])):
-            if set(map(id, o._optim.param_groups[0]["params"])) != set(map(id, g.params)):
-                raise UnsupportedModelError("optimizer parameters differ from the fused network's parameters")
-            o._flat = g
+            bind_optimizer(o, g)
         self._scratch: dict[str, torch.Tensor] = {}
         # opt-in: the device work of one update() (~85 launches) captured once into a CUDA graph and replayed -- the eager call
         # sequence is Python-launch bound.  Needs a buffer with a device mirror, uniform replay and a fixed alpha.

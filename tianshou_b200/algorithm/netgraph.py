@@ -4,7 +4,7 @@ A ``FusedStack`` is the kernel-side view of a torch module stack made of ``nn.Li
 ``nn.ReLU`` / ``nn.Flatten`` (the reference's ``MLP`` / ``Net`` / ``ContinuousCritic`` / ``DQNet``,
 utils/net/common.py:76-369, utils/net/continuous.py:96-238, env/atari/atari_network.py:60-122): every layer's
 forward, input gradient and weight gradient is ONE ``ts_net_gemm`` launch (wgmma, fp32-faithful), convolutions
-run as implicit GEMM over im2col rows.  Parameters live in a ``FlatGroup`` (one flat fp32 buffer per optimiser,
+run as implicit GEMM over im2col rows.  Parameters live in a ``FlatGroup`` (flat_params.py: one flat fp32 buffer per optimiser,
 ``nn.Parameter``s are views of it) so Adam and the Polyak update are single kernels and ``state_dict()`` keeps
 working.  There is no autograd graph and no eager-PyTorch path: unsupported layers raise ``UnsupportedModelError``.
 """
@@ -18,104 +18,9 @@ import torch
 from torch import nn
 
 from .._cabi import call, load_library, ptr, stream_ptr
-from .flat_params import UnsupportedModelError, adam_hyperparams
+from .flat_params import FlatGroup, UnsupportedModelError
 
 ACT_NONE, ACT_RELU, ACT_TANH = 0, 1, 2
-
-
-class FlatGroup:
-    """Flat fp32 storage (parameters, gradient, Adam moments) of one optimiser's parameters."""
-
-    def __init__(self, params: list[nn.Parameter], device: torch.device) -> None:
-        self.params = list(params)
-        self.device = device
-        self.n = sum(p.numel() for p in self.params)
-        self.flat = torch.empty(self.n, dtype=torch.float32, device=device)
-        self.grad = torch.zeros(self.n, dtype=torch.float32, device=device)
-        self.exp_avg = torch.zeros(self.n, dtype=torch.float32, device=device)
-        self.exp_avg_sq = torch.zeros(self.n, dtype=torch.float32, device=device)
-        self.norm_scratch = torch.zeros(256, dtype=torch.float64, device=device)
-        self.step = 0
-        self.step_dev: torch.Tensor | None = None     # device-resident step counter (CUDA-graph mode: see adam_step_device)
-        self._offsets: dict[int, int] = {}
-        off = 0
-        for p in self.params:
-            self._offsets[id(p)] = off
-            off += p.numel()
-        self._ptrs: list[int] = []
-        self.adopt()
-
-    def offset(self, p: nn.Parameter) -> int:
-        return self._offsets[id(p)]
-
-    def view(self, buf: torch.Tensor, p: nn.Parameter) -> torch.Tensor:
-        o = self._offsets[id(p)]
-        return buf[o:o + p.numel()]
-
-    def adopt(self) -> None:
-        with torch.no_grad():
-            for p in self.params:
-                v = self.view(self.flat, p).view(p.shape)
-                if p.data.data_ptr() != v.data_ptr():
-                    v.copy_(p.data.to(self.device, torch.float32))
-                    p.data = v
-        self._ptrs = [p.data.data_ptr() for p in self.params]
-
-    def ensure_adopted(self) -> None:
-        if [p.data.data_ptr() for p in self.params] != self._ptrs:
-            self.adopt()
-
-    def adam_step(self, optimizer: torch.optim.Optimizer, max_grad_norm: float | None) -> None:
-        """``Algorithm.Optimizer.step`` after backward: clip_grad_norm_ (optional) + Adam (algorithm_base.py:496-500)."""
-        hp = adam_hyperparams(optimizer)
-        self.sync_step_from_device()
-        self.step += 1
-        if self.step_dev is not None:
-            self.step_dev.fill_(self.step)
-        call("ts_adam_step", ptr(self.flat), ptr(self.grad), ptr(self.exp_avg), ptr(self.exp_avg_sq), self.n, self.step,
-             hp["lr"], hp["beta1"], hp["beta2"], hp["adam_eps"], hp["weight_decay"], float(max_grad_norm or 0.0),
-             ptr(self.norm_scratch), stream_ptr(self.device))
-
-    def adam_step_device(self, optimizer: torch.optim.Optimizer, max_grad_norm: float | None) -> None:
-        """Same step with the step number read from / advanced in DEVICE memory: nothing in the launch depends on host state,
-        so it can live inside a captured CUDA graph (the host mirror ``self.step`` is re-read by ``sync_step_from_device``)."""
-        hp = adam_hyperparams(optimizer)
-        if self.step_dev is None:
-            self.step_dev = torch.tensor([self.step], dtype=torch.int64, device=self.device)
-        call("ts_adam_step_dev", ptr(self.flat), ptr(self.grad), ptr(self.exp_avg), ptr(self.exp_avg_sq), self.n, ptr(self.step_dev),
-             hp["lr"], hp["beta1"], hp["beta2"], hp["adam_eps"], hp["weight_decay"], float(max_grad_norm or 0.0),
-             ptr(self.norm_scratch), stream_ptr(self.device))
-
-    def sync_step_from_device(self) -> None:
-        if self.step_dev is not None:
-            self.step = int(self.step_dev.item())
-
-    def export_state(self, optimizer: torch.optim.Optimizer) -> None:
-        self.sync_step_from_device()
-        if self.step == 0 and len(optimizer.state) == 0:
-            return
-        for p in self.params:
-            optimizer.state[p] = {"step": torch.tensor(float(self.step), dtype=torch.float32),
-                                  "exp_avg": self.view(self.exp_avg, p).view(p.shape),
-                                  "exp_avg_sq": self.view(self.exp_avg_sq, p).view(p.shape)}
-
-    def import_state(self, optimizer: torch.optim.Optimizer) -> None:
-        steps = []
-        with torch.no_grad():
-            for p in self.params:
-                st = optimizer.state.get(p)
-                m, v = self.view(self.exp_avg, p), self.view(self.exp_avg_sq, p)
-                if not st:
-                    m.zero_(); v.zero_()
-                    continue
-                m.copy_(st["exp_avg"].to(self.device, torch.float32).reshape(-1))
-                v.copy_(st["exp_avg_sq"].to(self.device, torch.float32).reshape(-1))
-                steps.append(float(st["step"]))
-        if steps and max(steps) != min(steps):
-            raise UnsupportedModelError("per-parameter Adam step counts differ; cannot fuse")
-        self.step = int(round(steps[0])) if steps else 0
-        if self.step_dev is not None:
-            self.step_dev.fill_(self.step)
 
 
 def polyak_update(target: FlatGroup, source: FlatGroup, tau: float) -> None:

@@ -1,8 +1,8 @@
 """MLP / Net building blocks (API of tianshou/utils/net/common.py:76-369, :457-470).
 
 These are ordinary ``nn.Module``s: the Collector runs them for action inference and
-``state_dict()`` round-trips unchanged.  The PPO update does not call them -- it reads the very
-same parameter storage through a flat view (tianshou_b200/algorithm/flat_params.py).
+``state_dict()`` round-trips unchanged.  The device updates do not call them -- they read the very
+same parameter storage through the flat view of a ``FlatGroup`` (tianshou_b200/algorithm/flat_params.py).
 """
 from __future__ import annotations
 

@@ -14,6 +14,6 @@ with policy_within_training_step(algo.policy):
     stats = algo.update(buffer=buf, batch_size=128, repeat=1)
 torch.cuda.synchronize()
 print("fused disabled:", os.environ.get("TS_B200_NO_FUSED_STEP"))
-print("loss mean", stats.loss.mean, "ref", g["u0_losses"][:4, 0].mean(), "step", int(algo._flat.step.item()))
+print("loss mean", stats.loss.mean, "ref", g["u0_losses"][:4, 0].mean(), "step", int(algo._flat.step_dev.item()))
 print("param delta", float((algo._flat.flat - p0).abs().max()), "ref delta", float(np.abs(g["u0_p_c_w2"] - g["p0_c_w2"]).max()))
 print("grad scratch extras", algo._flat.grad[-4:].cpu().numpy())
