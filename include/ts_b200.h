@@ -268,9 +268,11 @@ int ts_ppo_grad(const float* params, const ts_actor_critic_desc* desc, const ts_
  * gradient + loss sums a multi-GPU caller all-reduces before ts_clip_adam_step. */
 int ts_grad_reduce(const float* partials, int32_t n_partials, const ts_actor_critic_desc* desc,
                    float* grad, ts_stream_t stream);
-/* mean and unbiased std of adv[perm[lo..hi)] (ppo.py:184-186) -> out[0..1]; partial sums go to
- * sums (device double[2]) first so a multi-GPU caller can allreduce them; pass finalize=1 to
- * turn (sum, sumsq, count=global_rows) into {mean, std}. */
+/* mean and unbiased std of adv[perm[lo..hi)] (ppo.py:184-186) -> out[0..1]: ts_minibatch_adv_sums
+ * WRITES (sum, sum of squares) of the rows to sums (device double[2]; fixed summation order, the same
+ * as ts_epoch_adv_sums) so a multi-GPU caller can allreduce them; ts_adv_moments_finalize turns
+ * (sum, sumsq, count=global_rows) into {mean, std} and leaves sums as they are.  A single row gives
+ * std 0 (torch: NaN). */
 int ts_minibatch_adv_sums(const float* adv, const int32_t* perm, int64_t lo, int64_t hi,
                           double* sums, ts_stream_t stream);
 int ts_adv_moments_finalize(const double* sums, int64_t global_rows, float* out,
@@ -295,7 +297,7 @@ int ts_clip_adam_step(float* params, float* grad, const float* partials, int32_t
  * rewritten when recompute_adv).  stats: repeat*n_mb rows.  rms_state as in ts_gae (nullable
  * when return_scaling is off).  v_next_tmp: N f32 scratch.  gae_ws: ts_gae_workspace_bytes(N).
  * grad: n_params + TS_PPO_GRAD_EXTRA floats scratch; partials: ts_ppo_partial_rows() rows of the
- * same width.  adv_tmp: 32 + 8 * n_minibatch bytes of zero-initialised scratch (double[2] sums, float[2] moments,
+ * same width.  adv_tmp: 32 + 8 * n_minibatch bytes of scratch (double[2] sums, float[2] moments,
  * then one (mean, std) float pair per minibatch).  weight_image: ts_ppo_weight_image_bytes(desc) bytes of scratch
  * (nullable: the kernels then gather + split the weights themselves every step); rebuilt from `params` on entry.
  * row_feed: NULL, or a feed from ts_host_perm_feed_start whose dev_rows == perm: pass r then waits (on `stream`, not on the

@@ -261,7 +261,6 @@ def layered_update(algo: Any, batch: Any, batch_size: int | None, repeat: int) -
                 adv_mom = None
                 if algo.advantage_normalization:
                     sums = L._buf("adv_sums", 2, torch.float64)
-                    sums.zero_()
                     call("ts_minibatch_adv_sums", ptr(batch.adv), ptr(perm), lo, hi, ptr(sums), st)
                     adv_mom = L._buf("adv_mom", 2)
                     call("ts_adv_moments_finalize", ptr(sums), hi - lo, ptr(adv_mom), st)

@@ -340,7 +340,6 @@ class FusedActorCriticUpdate(ActorCriticOnPolicyAlgorithm):
             adv_mom = None
             if self.advantage_normalization:
                 sums = self._buf("adv_sums", 2, torch.float64)
-                sums.zero_()
                 call("ts_minibatch_adv_sums", ptr(batch.adv), ptr(perm), lo, hi, ptr(sums), st)
                 allreduce_sum_(sums)
                 adv_mom = self._buf("adv_mom", 2, torch.float32)

@@ -364,7 +364,7 @@ extern "C" int ts_gather_rows(const void* src, int64_t row_bytes, const int64_t*
         const int64_t rw = row_bytes / 16;
         const unsigned grid = (unsigned)tsb::imin((int64_t)blocks_for(n * rw, 256), tsb::num_sms() * 32);
         gather_rows_kernel<uint4><<<grid, 256, 0, st>>>(static_cast<const uint4*>(src), rw, idx, n, static_cast<uint4*>(dst));
-    } else if (row_bytes % 4 == 0) {
+    } else if (row_bytes % 4 == 0 && (((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 3u) == 0)) {
         const int64_t rw = row_bytes / 4;
         const unsigned grid = (unsigned)tsb::imin((int64_t)blocks_for(n * rw, 256), tsb::num_sms() * 32);
         gather_rows_kernel<uint32_t><<<grid, 256, 0, st>>>(static_cast<const uint32_t*>(src), rw, idx, n, static_cast<uint32_t*>(dst));

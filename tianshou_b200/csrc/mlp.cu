@@ -736,32 +736,13 @@ __global__ void grad_reduce_kernel(const float* __restrict__ partials, int n_par
     grad[i] = ((acc[0] + acc[1]) + (acc[2] + acc[3])) + ((acc[4] + acc[5]) + (acc[6] + acc[7]));
 }
 
-__global__ void adv_sums_kernel(const float* __restrict__ adv, const int32_t* __restrict__ perm,
-                                int64_t lo, int64_t hi, double* __restrict__ sums) {
-    __shared__ double s1[8], s2[8];
-    double a = 0.0, b = 0.0;
-    for (int64_t p = lo + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < hi;
-         p += (int64_t)gridDim.x * blockDim.x) {
-        const double v = adv[perm ? (int64_t)perm[p] : p];
-        a += v; b += v * v;
-    }
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) { a += tsb::shfl_xor_f64(a, off); b += tsb::shfl_xor_f64(b, off); }
-    if ((threadIdx.x & 31) == 0) { s1[threadIdx.x >> 5] = a; s2[threadIdx.x >> 5] = b; }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double x = 0.0, y = 0.0;
-        for (int w = 0; w < (int)(blockDim.x >> 5); ++w) { x += s1[w]; y += s2[w]; }
-        atomicAdd(sums + 0, x); atomicAdd(sums + 1, y);
-    }
-}
-__global__ void adv_finalize_kernel(double* __restrict__ sums, int64_t n, float* __restrict__ out) {
+// One row: std 0, where torch's adv.std() of a single element is NaN (see DESIGN.md section 4).
+__global__ void adv_finalize_kernel(const double* __restrict__ sums, int64_t n, float* __restrict__ out) {
     if (threadIdx.x != 0) return;
     const double mean = sums[0] / (double)n;
     double var = (sums[1] - sums[0] * mean) / (double)(n > 1 ? n - 1 : 1);   // unbiased (torch .std())
     if (var < 0.0) var = 0.0;
     out[0] = (float)mean; out[1] = (float)sqrt(var);
-    sums[0] = 0.0; sums[1] = 0.0;
 }
 
 // mean / unbiased std of the advantages of EVERY minibatch of one pass (one CTA per minibatch, fixed
@@ -973,17 +954,17 @@ extern "C" int ts_ppo_grad(const float* params, const ts_actor_critic_desc* desc
 
 extern "C" int ts_minibatch_adv_sums(const float* adv, const int32_t* perm, int64_t lo, int64_t hi,
                                      double* sums, ts_stream_t stream) {
-    if (hi <= lo) return 0;
     TS_REQUIRE(adv && sums, "ts_minibatch_adv_sums: null pointer");
-    const unsigned grid = (unsigned)tsb::imin((int64_t)(hi - lo + 255) / 256, tsb::num_sms());
-    adv_sums_kernel<<<grid, 256, 0, tsb::as_stream(stream)>>>(adv, perm, lo, hi, sums);
+    // one minibatch of the epoch kernel: the same fixed summation order as ts_epoch_adv_sums and the fused path's
+    // epoch_adv_moments_kernel, so all three give bit-identical moments.  An empty range writes (0, 0).
+    epoch_adv_sums_kernel<<<1, 1024, 0, tsb::as_stream(stream)>>>(adv, perm, lo, hi - lo, hi, 1, sums);
     return tsb::check_launch("ts_minibatch_adv_sums");
 }
 
 extern "C" int ts_adv_moments_finalize(const double* sums, int64_t global_rows, float* out,
                                        ts_stream_t stream) {
     TS_REQUIRE(sums && out && global_rows > 0, "ts_adv_moments_finalize: bad arguments");
-    adv_finalize_kernel<<<1, 32, 0, tsb::as_stream(stream)>>>(const_cast<double*>(sums), global_rows, out);
+    adv_finalize_kernel<<<1, 32, 0, tsb::as_stream(stream)>>>(sums, global_rows, out);
     return tsb::check_launch("ts_adv_moments_finalize");
 }
 
