@@ -232,9 +232,16 @@ typedef struct ts_ppo_hparams {
     int32_t advantage_normalization;
     int32_t loss_kind;    /* TS_LOSS_PPO (0): clipped surrogate, ppo.py:184-196; TS_LOSS_A2C (1): actor loss
                            * -mean(log_prob * adv) (a2c.py:262-266), eps_clip / dual_clip / logp_old / v_s unused */
+    int32_t optimizer;    /* TS_OPT_ADAM (0) or TS_OPT_RMSPROP (1): torch.optim.RMSprop's single-tensor step without
+                           * momentum or centering (examples/mujoco/mujoco_a2c.py:117-121).  RMSprop reads lr, beta2 as its
+                           * smoothing constant alpha, adam_eps as its eps and weight_decay; beta1 is unused.  square_avg
+                           * lives in exp_avg_sq, exp_avg is untouched.  (The field fills the struct's tail padding: the
+                           * layout and size are those of the Adam-only struct.) */
 } ts_ppo_hparams;
 #define TS_LOSS_PPO 0
 #define TS_LOSS_A2C 1
+#define TS_OPT_ADAM 0
+#define TS_OPT_RMSPROP 1
 
 /* Per-optimiser-step device statistics: {loss, clip_loss, vf_loss, ent_loss, grad_norm, n_rows,
  * 0, 0} -- 8 floats per step (ppo.py:213-216 without the 4 host syncs). */
@@ -278,7 +285,7 @@ int ts_minibatch_adv_sums(const float* adv, const int32_t* perm, int64_t lo, int
 int ts_adv_moments_finalize(const double* sums, int64_t global_rows, float* out,
                             ts_stream_t stream);
 /* clip_grad_norm_ + Adam.step (algorithm_base.py:496-500; torch/optim/adam.py single-tensor
- * path) on the flat buffers, and one row of per-step statistics.  If partials != NULL the
+ * path; RMSprop.step when hp->optimizer == TS_OPT_RMSPROP) on the flat buffers, and one row of per-step statistics.  If partials != NULL the
  * gradient is first folded from the n_partials rows (single-GPU fast path: reduce + norm + clip
  * + Adam in ONE launch); otherwise `grad` must already hold the (all-reduced) gradient.
  * grad: n_params + TS_PPO_GRAD_EXTRA floats (scratch / input).  step_count: device int64[1],
@@ -532,6 +539,13 @@ int ts_adam_step(float* params, const float* grad, float* exp_avg, float* exp_av
 int ts_adam_step_dev(float* params, const float* grad, float* exp_avg, float* exp_avg_sq, int64_t n, int64_t* step_dev, double lr,
                      double beta1, double beta2, double eps, double weight_decay, double max_grad_norm, double* norm_scratch,
                      ts_stream_t stream);
+/* clip_grad_norm_ (optional) + torch.optim.RMSprop step without momentum or centering on a flat parameter vector
+ * (algorithm_base.py:496-500, optim.py RMSpropOptimizerFactory; torch/optim/rmsprop.py _single_tensor_rmsprop):
+ *   g = clipped grad (+ weight_decay * p);  square_avg = square_avg * alpha + (1 - alpha) * g * g;
+ *   p -= lr * g / (sqrt(square_avg) + eps)
+ * No bias correction, so the step count is the caller's (torch's `step` state). */
+int ts_rmsprop_step(float* params, const float* grad, float* square_avg, int64_t n, double lr, double alpha, double eps,
+                    double weight_decay, double max_grad_norm, double* norm_scratch, ts_stream_t stream);
 /* target = tau * source + (1 - tau) * target   (utils/lagged_network.py:8-18) */
 int ts_polyak_update(float* target, const float* source, int64_t n, double tau, ts_stream_t stream);
 

@@ -19,6 +19,7 @@ LIB_PATH = os.path.join(_HERE, "libts_b200.so")
 TS_F32, TS_F64 = 0, 1
 AC_RELU, AC_CATEGORICAL = 1, 2
 LOSS_PPO, LOSS_A2C = 0, 1
+OPT_ADAM, OPT_RMSPROP = 0, 1
 STATS_STRIDE = 8
 GRAD_EXTRA = 4
 
@@ -45,6 +46,7 @@ class PPOHParams(C.Structure):
         ("lr", C.c_double), ("beta1", C.c_double), ("beta2", C.c_double), ("adam_eps", C.c_double),
         ("weight_decay", C.c_double),
         ("value_clip", C.c_int32), ("advantage_normalization", C.c_int32), ("loss_kind", C.c_int32),
+        ("optimizer", C.c_int32),
     ]
 
 
@@ -139,6 +141,7 @@ SIGNATURES: dict[str, list[Any]] = {
     "ts_mean": [_P, _I64, _P, _P],
     "ts_adam_step": [_P, _P, _P, _P, _I64, _I64, _D, _D, _D, _D, _D, _D, _P, _P],
     "ts_adam_step_dev": [_P, _P, _P, _P, _I64, _P, _D, _D, _D, _D, _D, _D, _P, _P],
+    "ts_rmsprop_step": [_P, _P, _P, _I64, _D, _D, _D, _D, _D, _P, _P],
     "ts_polyak_update": [_P, _P, _I64, _D, _P],
 }
 # diagnostics build only (libts_b200_diag.so, tools/): not part of the product library

@@ -15,7 +15,7 @@ import torch
 from torch import nn
 from torch.distributions import Categorical, Independent, Normal
 
-from .._cabi import call, ptr, stream_ptr
+from .._cabi import OPT_ADAM, OPT_RMSPROP, call, ptr, stream_ptr
 
 
 class UnsupportedModelError(NotImplementedError):
@@ -41,27 +41,46 @@ def check_gaussian_dist_fn(dist_fn: Any, act_dim: int, device: torch.device) -> 
         raise UnsupportedModelError(f"dist_fn must build Independent(Normal(loc, scale), 1); got {d}")
 
 
-def adam_hyperparams(optimizer: torch.optim.Optimizer) -> dict[str, float]:
-    if type(optimizer) is not torch.optim.Adam:
-        raise UnsupportedModelError(f"fused update supports torch.optim.Adam only, got {type(optimizer).__name__}")
+def optimizer_hyperparams(optimizer: torch.optim.Optimizer, *, rmsprop: bool = True) -> dict[str, Any]:
+    """The device step's hyper-parameters, keyed by ``ts_ppo_hparams`` field, for a torch Adam or (``rmsprop``) RMSprop;
+    ``optimizer`` is ``OPT_ADAM`` or ``OPT_RMSPROP``.  RMSprop's ``alpha`` travels in ``beta2`` and its ``eps`` in
+    ``adam_eps`` (include/ts_b200.h).  Every optimiser or option the kernels do not implement raises
+    ``UnsupportedModelError``."""
+    kind = type(optimizer)
+    if kind is not torch.optim.Adam and not (rmsprop and kind is torch.optim.RMSprop):
+        allowed = "torch.optim.Adam / torch.optim.RMSprop" if rmsprop else "torch.optim.Adam"
+        raise UnsupportedModelError(f"fused update supports {allowed} only, got {kind.__name__}")
     if len(optimizer.param_groups) != 1:
         raise UnsupportedModelError("fused update supports a single param group")
     g = optimizer.param_groups[0]
-    if g.get("amsgrad") or g.get("maximize") or g.get("decoupled_weight_decay"):
-        raise UnsupportedModelError("amsgrad / maximize / decoupled weight decay unsupported")
     lr = g["lr"]
     lr = float(lr.item()) if isinstance(lr, torch.Tensor) else float(lr)
+    if kind is torch.optim.RMSprop:
+        # momentum and centered would each need a third state vector next to the parameters and square_avg; no reference
+        # example uses them (examples/mujoco/mujoco_a2c.py:117-121 builds RMSprop(lr, eps, alpha))
+        if g.get("momentum") or g.get("centered"):
+            raise UnsupportedModelError("RMSprop momentum != 0 / centered=True unsupported: the device step keeps square_avg "
+                                        "as its only state vector")
+        if g.get("maximize"):
+            raise UnsupportedModelError("RMSprop maximize=True unsupported")
+        alpha = float(g["alpha"])
+        if not all(math.isfinite(x) for x in (lr, alpha)):
+            raise ValueError("non-finite RMSprop hyper-parameters")
+        return dict(optimizer=OPT_RMSPROP, lr=lr, beta2=alpha, adam_eps=float(g["eps"]), weight_decay=float(g["weight_decay"]))
+    if g.get("amsgrad") or g.get("maximize") or g.get("decoupled_weight_decay"):
+        raise UnsupportedModelError("amsgrad / maximize / decoupled weight decay unsupported")
     b1, b2 = g["betas"]
     if not all(math.isfinite(x) for x in (lr, b1, b2)):
         raise ValueError("non-finite Adam hyper-parameters")
-    return dict(lr=lr, beta1=float(b1), beta2=float(b2), adam_eps=float(g["eps"]),
+    return dict(optimizer=OPT_ADAM, lr=lr, beta1=float(b1), beta2=float(b2), adam_eps=float(g["eps"]),
                 weight_decay=float(g["weight_decay"]))
 
 
-def bind_optimizer(optim: Any, group: FlatGroup) -> None:
+def bind_optimizer(optim: Any, group: FlatGroup, *, rmsprop: bool = False) -> None:
     """Let ``group`` hold the state of ``optim`` (an ``Algorithm.Optimizer``): the kernels step the flat buffers with the
-    torch optimiser's hyper-parameters, and ``state_dict()`` / ``load_state_dict()`` go through ``group``."""
-    adam_hyperparams(optim._optim)
+    torch optimiser's hyper-parameters, and ``state_dict()`` / ``load_state_dict()`` go through ``group``.  ``rmsprop``:
+    the caller steps through ``FlatGroup.optimizer_step`` or the actor-critic kernels, which also take torch RMSprop."""
+    optimizer_hyperparams(optim._optim, rmsprop=rmsprop)
     if set(map(id, optim._optim.param_groups[0]["params"])) != set(map(id, group.params)):
         raise UnsupportedModelError("optimizer parameters differ from the fused network's parameters")
     optim._flat = group
@@ -124,22 +143,37 @@ class FlatGroup:
         if [p.data.data_ptr() for p in self.params] != self._ptrs:
             self.adopt()
 
-    def adam_step(self, optimizer: torch.optim.Optimizer, max_grad_norm: float | None) -> None:
-        """``Algorithm.Optimizer.step`` after backward: clip_grad_norm_ (optional) + Adam (algorithm_base.py:496-500)."""
-        hp = adam_hyperparams(optimizer)
+    def _advance_step(self) -> int:
         step = self.sync_step_from_device() + 1
         if self.step_dev is not None:
             self.step_dev.fill_(step)
         else:
             self._step = step
+        return step
+
+    def adam_step(self, optimizer: torch.optim.Optimizer, max_grad_norm: float | None) -> None:
+        """``Algorithm.Optimizer.step`` after backward: clip_grad_norm_ (optional) + Adam (algorithm_base.py:496-500)."""
+        hp = optimizer_hyperparams(optimizer, rmsprop=False)
+        step = self._advance_step()
         call("ts_adam_step", ptr(self.flat), ptr(self.grad), ptr(self.exp_avg), ptr(self.exp_avg_sq), self.n, step,
              hp["lr"], hp["beta1"], hp["beta2"], hp["adam_eps"], hp["weight_decay"], float(max_grad_norm or 0.0),
              ptr(self.norm_scratch), stream_ptr(self.device))
 
+    def optimizer_step(self, optimizer: torch.optim.Optimizer, max_grad_norm: float | None) -> None:
+        """``adam_step``, or for a torch RMSprop clip_grad_norm_ (optional) + RMSprop (``ts_rmsprop_step``; square_avg in
+        ``exp_avg_sq``)."""
+        hp = optimizer_hyperparams(optimizer)
+        if hp["optimizer"] == OPT_ADAM:
+            self.adam_step(optimizer, max_grad_norm)
+            return
+        self._advance_step()
+        call("ts_rmsprop_step", ptr(self.flat), ptr(self.grad), ptr(self.exp_avg_sq), self.n, hp["lr"], hp["beta2"],
+             hp["adam_eps"], hp["weight_decay"], float(max_grad_norm or 0.0), ptr(self.norm_scratch), stream_ptr(self.device))
+
     def adam_step_device(self, optimizer: torch.optim.Optimizer, max_grad_norm: float | None) -> None:
         """Same step with the step number read from / advanced in DEVICE memory: nothing in the launch depends on host state,
         so it can live inside a captured CUDA graph."""
-        hp = adam_hyperparams(optimizer)
+        hp = optimizer_hyperparams(optimizer, rmsprop=False)
         if self.step_dev is None:
             self.step_dev = torch.tensor([self._step], dtype=torch.int64, device=self.device)
         call("ts_adam_step_dev", ptr(self.flat), ptr(self.grad), ptr(self.exp_avg), ptr(self.exp_avg_sq), self.n, ptr(self.step_dev),
@@ -150,21 +184,28 @@ class FlatGroup:
         """The step count as a host int: one read of ``step_dev`` when the device counter owns it."""
         return int(self.step_dev.item()) if self.step_dev is not None else self._step
 
-    # -- torch.optim.Adam state interop ----------------------------------------------------
+    # -- torch.optim.Adam / RMSprop state interop --------------------------------------------
     def export_state(self, optimizer: torch.optim.Optimizer) -> None:
-        """Expose the flat moments as the torch optimizer's per-parameter state (views)."""
+        """Expose the flat moments as the torch optimizer's per-parameter state (views): Adam's exp_avg / exp_avg_sq, or
+        RMSprop's square_avg (``exp_avg_sq``)."""
         step = self.sync_step_from_device()
         if step == 0 and len(optimizer.state) == 0:
             return
+        rmsprop = type(optimizer) is torch.optim.RMSprop
         for p in self.params:
-            optimizer.state[p] = {"step": torch.tensor(float(step), dtype=torch.float32),
-                                  "exp_avg": self.view(self.exp_avg, p).view(p.shape),
-                                  "exp_avg_sq": self.view(self.exp_avg_sq, p).view(p.shape)}
+            st = {"step": torch.tensor(float(step), dtype=torch.float32)}
+            if rmsprop:
+                st["square_avg"] = self.view(self.exp_avg_sq, p).view(p.shape)
+            else:
+                st["exp_avg"] = self.view(self.exp_avg, p).view(p.shape)
+                st["exp_avg_sq"] = self.view(self.exp_avg_sq, p).view(p.shape)
+            optimizer.state[p] = st
 
     def import_state(self, optimizer: torch.optim.Optimizer) -> None:
         """After ``optimizer.load_state_dict`` or an eager ``optimizer.step()``: pull its moments / step into the flat
         buffers, then expose them as the optimizer's state again."""
         steps = []
+        rmsprop = type(optimizer) is torch.optim.RMSprop
         with torch.no_grad():
             for p in self.params:
                 st = optimizer.state.get(p)
@@ -172,11 +213,14 @@ class FlatGroup:
                 if not st:
                     m.zero_(); v.zero_()
                     continue
-                m.copy_(st["exp_avg"].to(self.device, torch.float32).reshape(-1))
-                v.copy_(st["exp_avg_sq"].to(self.device, torch.float32).reshape(-1))
+                if rmsprop:
+                    v.copy_(st["square_avg"].to(self.device, torch.float32).reshape(-1))
+                else:
+                    m.copy_(st["exp_avg"].to(self.device, torch.float32).reshape(-1))
+                    v.copy_(st["exp_avg_sq"].to(self.device, torch.float32).reshape(-1))
                 steps.append(float(st["step"]))
         if steps and max(steps) != min(steps):
-            raise UnsupportedModelError("per-parameter Adam step counts differ; cannot fuse")
+            raise UnsupportedModelError("per-parameter optimiser step counts differ; cannot fuse")
         step = int(round(steps[0])) if steps else 0
         if self.step_dev is not None:
             self.step_dev.fill_(step)

@@ -5,7 +5,7 @@
 64-wide trunks, obs <= 64).  Everything else that is still a Linear / ReLU | Tanh actor-critic -- wider or deeper trunks,
 large observations (Humanoid: 376), the reference's shared-trunk discrete PPO net at other widths -- runs in
 ``LayeredActorCritic``: every Linear forward / input gradient / weight gradient is one ``ts_net_gemm`` launch (wgmma,
-fp32-faithful), the PPO / A2C loss between them is ``ts_ppo_rows``, the optimiser ``ts_adam_step`` (global-norm clip + Adam).
+fp32-faithful), the PPO / A2C loss between them is ``ts_ppo_rows``, the optimiser ``ts_adam_step`` / ``ts_rmsprop_step`` (global-norm clip + Adam or RMSprop).
 Same public behaviour as the fused path (ppo.py:146-224, a2c.py:115-153); single GPU.
 
 Reference structures covered: ``ContinuousActorProbabilistic(unbounded=True, conditioned_sigma=False)`` +
@@ -229,7 +229,7 @@ class LayeredActorCritic:
             self.c_trunk.backward(ct, dz_c, B, "up", dy_preact=True)
         if dls is not None:
             call("ts_net_colsum", ptr(dls), A, B, A, self._logstd_ptr(self.group.grad), 0, st)
-        self.group.adam_step(optimizer, max_grad_norm)
+        self.group.optimizer_step(optimizer, max_grad_norm)
 
 
 def layered_update(algo: Any, batch: Any, batch_size: int | None, repeat: int) -> torch.Tensor:

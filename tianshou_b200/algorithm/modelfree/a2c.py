@@ -32,10 +32,10 @@ from ..base import OnPolicyAlgorithm, TrainingStats
 from ..flat_params import (
     FlatGroup,
     UnsupportedModelError,
-    adam_hyperparams,
     bind_optimizer,
     check_categorical_dist_fn,
     check_gaussian_dist_fn,
+    optimizer_hyperparams,
 )
 from ..layered import LayeredActorCritic, fused_descriptor, parse_actor_critic
 from ..optim import OptimizerFactory
@@ -108,10 +108,10 @@ class ActorCriticOnPolicyAlgorithm(OnPolicyAlgorithm, ABC):
             if self._world_size() > 1 and getattr(self, "data_parallel", True):  # replicas start bit-identical
                 from ...parallel import broadcast_params_
                 broadcast_params_(self._flat.flat)
-        # a real torch Adam (+ scheduler) keeps lr schedules and state_dict round trips unchanged
+        # a real torch Adam / RMSprop (+ scheduler) keeps lr schedules and state_dict round trips unchanged
         self.optim = self._create_optimizer(self._actor_critic if optim_include_actor else self.critic, optim,
                                             max_grad_norm=max_grad_norm)
-        bind_optimizer(self.optim, self._flat)
+        bind_optimizer(self.optim, self._flat, rmsprop=True)
         self.max_grad_norm = max_grad_norm
         self.gamma = gamma
         self.return_scaling = return_scaling
@@ -276,7 +276,7 @@ class ActorCriticOnPolicyAlgorithm(OnPolicyAlgorithm, ABC):
         hp.eps_clip, hp.dual_clip, hp.vf_coef, hp.ent_coef = 0.0, 0.0, 0.5, 0.01
         hp.max_grad_norm = float(self.max_grad_norm) if self.max_grad_norm is not None else 0.0
         hp.adv_eps = self._eps
-        for k, v in adam_hyperparams(self.optim._optim).items():
+        for k, v in optimizer_hyperparams(self.optim._optim).items():   # the scheduler's lr of this update
             setattr(hp, k, v)
         hp.value_clip, hp.advantage_normalization = 0, 0
         for k, v in over.items():

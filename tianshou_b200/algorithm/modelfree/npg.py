@@ -178,7 +178,7 @@ class NPG(ActorCriticOnPolicyAlgorithm):
         self._actor_backward(at, ah, rows, B)
 
     def _critic_steps(self, obs: torch.Tensor, ret: torch.Tensor, B: int, row: torch.Tensor) -> None:
-        """optim_critic_iters x (F.mse_loss(returns, critic(obs)), Adam step) (npg.py:175-179); vf_loss = the last one."""
+        """optim_critic_iters x (F.mse_loss(returns, critic(obs)), optimiser step) (npg.py:175-179); vf_loss = the last one."""
         L, st = self._layered, stream_ptr(self.device)
         td, dval, vrows = L._buf("vf_td", B), L._buf("dval", (B, 1)), L._buf("vf_rows", B)
         dz = L._buf("dz_c", (B, L.c_trunk.layers[-1].out_dim))
@@ -190,4 +190,4 @@ class NPG(ActorCriticOnPolicyAlgorithm):
             L.c_head.backward(ch, dval, B, "up", input_grad=True, input_act=(L._c_act, ct[-1]) if L._c_act != ACT_NONE else None,
                               dx_out=dz)
             L.c_trunk.backward(ct, dz, B, "up", dy_preact=True)
-            L.critic_group.adam_step(self.optim._optim, None)
+            L.critic_group.optimizer_step(self.optim._optim, None)

@@ -685,16 +685,28 @@ __global__ void __launch_bounds__(kAdamElems * kAdamGroups) clip_adam_kernel(
             coef = fminf(coef, 1.0f);
         }
         s_coef = coef; s_norm = total_norm;
-        const double bc1 = 1.0 - pow(hp.beta1, (double)step);
-        const double bc2 = 1.0 - pow(hp.beta2, (double)step);
-        s_step_size = (float)(hp.lr / bc1);
-        s_bc2_sqrt = (float)sqrt(bc2);
+        if (hp.optimizer != TS_OPT_RMSPROP) {       // RMSprop has no bias correction
+            const double bc1 = 1.0 - pow(hp.beta1, (double)step);
+            const double bc2 = 1.0 - pow(hp.beta2, (double)step);
+            s_step_size = (float)(hp.lr / bc1);
+            s_bc2_sqrt = (float)sqrt(bc2);
+        }
     }
     __syncthreads();
     const float coef = s_coef, step_size = s_step_size, bc2_sqrt = s_bc2_sqrt;
     const float w1 = (float)(1.0 - hp.beta1), w2 = (float)(1.0 - hp.beta2);
     const float beta2 = (float)hp.beta2, adam_eps = (float)hp.adam_eps, wd = (float)hp.weight_decay;
-    if (q == 0 && i < n_params) {
+    if (hp.optimizer == TS_OPT_RMSPROP) {
+        if (q == 0 && i < n_params) {
+            g *= coef;
+            float p = params[i];
+            if (wd != 0.0f) g = fmaf(wd, p, g);
+            float v = exp_avg_sq[i];
+            v = v * beta2 + w2 * g * g;             // square_avg.mul_(alpha).addcmul_(grad, grad, 1 - alpha): beta2 holds alpha
+            p = p - (float)hp.lr * (g / (sqrtf(v) + adam_eps));         // addcdiv_(grad, square_avg.sqrt().add_(eps), -lr)
+            exp_avg_sq[i] = v; params[i] = p;
+        }
+    } else if (q == 0 && i < n_params) {
         g *= coef;
         float p = params[i];
         if (wd != 0.0f) g = fmaf(wd, p, g);

@@ -716,7 +716,8 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_tc_kernel(
     };
 
     double beta1_pow = 1.0, beta2_pow = 1.0;
-    if (EPOCH && tid == 256) { beta1_pow = pow(hp.beta1, (double)step0); beta2_pow = pow(hp.beta2, (double)step0); }
+    const bool rmsprop = hp.optimizer == TS_OPT_RMSPROP;       // block-uniform: RMSprop has no bias correction
+    if (EPOCH && tid == 256 && !rmsprop) { beta1_pow = pow(hp.beta1, (double)step0); beta2_pow = pow(hp.beta2, (double)step0); }
     bool staged = false;        // the tile's inputs were already stored by the previous step's prefetch
     tstamp(0);
     for (int m = 0; m < n_mb; ++m) {
@@ -732,7 +733,7 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_tc_kernel(
         if (tid == 0 && g_tc_timeline_on && (int)blockIdx.x == g_tc_timeline_on - 1) g_tc_timeline_gate = (n_mb == 1 || m == n_mb - 2);   // a step WITH barrier 3
 #endif
         tstamp(22);
-        if (EPOCH && tid == 256) {    // Adam bias corrections of this step, off the critical path
+        if (EPOCH && tid == 256 && !rmsprop) {    // Adam bias corrections of this step, off the critical path
             beta1_pow *= hp.beta1; beta2_pow *= hp.beta2;          // beta^(step0 + m + 1)
             s_step_size = (float)(hp.lr / (1.0 - beta1_pow));
             s_bc2_sqrt = (float)sqrt(1.0 - beta2_pow);
@@ -967,9 +968,18 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_tc_kernel(
         const float coef = s_coef, step_size = s_step_size, bc2_sqrt = s_bc2_sqrt;
         const float w1 = (float)(1.0 - hp.beta1), w2 = (float)(1.0 - hp.beta2);
         const float beta2 = (float)hp.beta2, adam_eps = (float)hp.adam_eps, wd = (float)hp.weight_decay;
+        // RMSprop: beta2 holds alpha; 1 - alpha formed in double and rounded once, as torch passes addcmul's value
+        const float alpha = (float)hp.beta2, w_sq = (float)(1.0 - hp.beta2), lr = (float)hp.lr;
         auto adam_elem = [&](int64_t i, float g, float pv, float mm, float v) {
             g *= coef;
             if (wd != 0.0f) g = fmaf(wd, pv, g);
+            if (rmsprop) {
+                v = v * alpha + w_sq * g * g;           // square_avg.mul_(alpha).addcmul_(grad, grad, 1 - alpha)
+                pv = pv - lr * (g / (sqrtf(v) + adam_eps));   // addcdiv_(grad, square_avg.sqrt().add_(eps), -lr)
+                opt.exp_avg_sq[i] = v; opt.params_w[i] = pv;
+                if (wimg != nullptr) img_scatter(d, S, sbase, i, pv, wimg);
+                return;
+            }
             mm = mm + w1 * (g - mm);                    // exp_avg.lerp_(grad, 1 - beta1)
             v = v * beta2 + w2 * g * g;                 // mul_(beta2).addcmul_(grad, grad, 1 - beta2)
             const float denom = sqrtf(v) / bc2_sqrt + adam_eps;

@@ -278,18 +278,23 @@ __global__ void sumsq_kernel(const float* __restrict__ g, int64_t n, double* __r
     }
     if (threadIdx.x == 0) partial[blockIdx.x] = s[0];
 }
-// torch.optim.Adam single-tensor step (lerp / addcmul / addcdiv order), optional clip_grad_norm_ from `partial` block sums.
-// w1 = 1 - beta1 and w2 = 1 - beta2 are formed in double and rounded once, as torch passes them (lerp weight, addcmul
-// value): 1.0f - (float)0.999 would be 1.3e-5 off in relative terms.
-__global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v, int64_t n,
-                            float step_size, float bc2_sqrt, float beta2, float w1, float w2, float eps, float wd, float max_norm,
-                            const double* __restrict__ partial, int n_partial) {
+// clip_grad_norm_'s coefficient from sumsq_kernel's `partial` block sums (1 when clipping is off)
+__device__ __forceinline__ float clip_coef(float max_norm, const double* __restrict__ partial, int n_partial) {
     float coef = 1.0f;
     if (max_norm > 0.0f && partial) {
         double t = 0.0;
         for (int i = 0; i < n_partial; ++i) t += partial[i];
         coef = fminf(max_norm / ((float)sqrt(t) + 1e-6f), 1.0f);
     }
+    return coef;
+}
+// torch.optim.Adam single-tensor step (lerp / addcmul / addcdiv order), optional clip_grad_norm_ from `partial` block sums.
+// w1 = 1 - beta1 and w2 = 1 - beta2 are formed in double and rounded once, as torch passes them (lerp weight, addcmul
+// value): 1.0f - (float)0.999 would be 1.3e-5 off in relative terms.
+__global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v, int64_t n,
+                            float step_size, float bc2_sqrt, float beta2, float w1, float w2, float eps, float wd, float max_norm,
+                            const double* __restrict__ partial, int n_partial) {
+    const float coef = clip_coef(max_norm, partial, n_partial);
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
         float gi = g[i] * coef;
         float pv = p[i];
@@ -312,13 +317,7 @@ __global__ void adam_dev_kernel(float* __restrict__ p, const float* __restrict__
         const double step = (double)(*step_dev + 1);
         s_step_size = (float)(lr / (1.0 - pow(beta1d, step)));
         s_bc2_sqrt = (float)sqrt(1.0 - pow(beta2d, step));
-        float coef = 1.0f;
-        if (max_norm > 0.0f && partial) {
-            double t = 0.0;
-            for (int i = 0; i < n_partial; ++i) t += partial[i];
-            coef = fminf(max_norm / ((float)sqrt(t) + 1e-6f), 1.0f);
-        }
-        s_coef = coef;
+        s_coef = clip_coef(max_norm, partial, n_partial);
     }
     __syncthreads();
     const float step_size = s_step_size, bc2_sqrt = s_bc2_sqrt, coef = s_coef;
@@ -334,6 +333,22 @@ __global__ void adam_dev_kernel(float* __restrict__ p, const float* __restrict__
         const float denom = sqrtf(vv) / bc2_sqrt + eps;
         pv = pv - step_size * (mm / denom);
         m[i] = mm; v[i] = vv; p[i] = pv;
+    }
+}
+// torch.optim.RMSprop single-tensor step without momentum / centering (mul_ / addcmul_ / sqrt / add_ / addcdiv_ order), the
+// clip as adam_kernel.  w_sq = 1 - alpha is formed in double and rounded once, as torch passes addcmul's value.
+__global__ void rmsprop_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ sq, int64_t n, float lr,
+                               float alpha, float w_sq, float eps, float wd, float max_norm, const double* __restrict__ partial,
+                               int n_partial) {
+    const float coef = clip_coef(max_norm, partial, n_partial);
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        float gi = g[i] * coef;
+        float pv = p[i];
+        if (wd != 0.0f) gi = fmaf(wd, pv, gi);
+        float vv = sq[i];
+        vv = vv * alpha + w_sq * gi * gi;
+        pv = pv - lr * (gi / (sqrtf(vv) + eps));
+        sq[i] = vv; p[i] = pv;
     }
 }
 __global__ void step_inc_kernel(int64_t* step_dev) { *step_dev += 1; }
@@ -464,6 +479,25 @@ extern "C" int ts_adam_step_dev(float* params, const float* grad, float* exp_avg
     if (tsb::check_launch("ts_adam_step_dev")) return 1;
     step_inc_kernel<<<1, 1, 0, st>>>(step_dev);
     return tsb::check_launch("ts_adam_step_dev/inc");
+}
+// replaces clip_grad_norm_ + RMSprop.step (algorithm_base.py:496-500; torch/optim/rmsprop.py _single_tensor_rmsprop:
+// square_avg.mul_(alpha).addcmul_(grad, grad, value=1 - alpha); avg = square_avg.sqrt().add_(eps);
+// param.addcdiv_(grad, avg, value=-lr))
+extern "C" int ts_rmsprop_step(float* params, const float* grad, float* square_avg, int64_t n, double lr, double alpha, double eps,
+                               double weight_decay, double max_grad_norm, double* norm_scratch, ts_stream_t stream) {
+    TS_REQUIRE(params && grad && square_avg, "ts_rmsprop_step: null pointer");
+    if (n <= 0) return 0;
+    cudaStream_t st = tsb::as_stream(stream);
+    int n_partial = 0;
+    if (max_grad_norm > 0.0) {
+        TS_REQUIRE(norm_scratch, "ts_rmsprop_step: clipping needs norm_scratch");
+        n_partial = (int)tsb::imin((n + 255) / 256, 256);
+        sumsq_kernel<<<n_partial, 256, 0, st>>>(grad, n, norm_scratch);
+        if (tsb::check_launch("ts_rmsprop_step/norm")) return 1;
+    }
+    rmsprop_kernel<<<grid_for(n), 256, 0, st>>>(params, grad, square_avg, n, (float)lr, (float)alpha, (float)(1.0 - alpha), (float)eps,
+                                                (float)weight_decay, (float)max_grad_norm, norm_scratch, n_partial);
+    return tsb::check_launch("ts_rmsprop_step");
 }
 extern "C" int ts_polyak_update(float* target, const float* source, int64_t n, double tau, ts_stream_t stream) {
     TS_REQUIRE(target && source, "ts_polyak_update: null pointer");
