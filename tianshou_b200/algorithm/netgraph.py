@@ -80,6 +80,8 @@ def compile_sequential(mods: list[nn.Module], input_shape: tuple[int, ...]) -> l
                     or m.bias is None or m.in_channels != shape[0]):
                 raise UnsupportedModelError(f"unsupported Conv2d configuration {m}")
             Cc, H, W = shape
+            if H < k[0] or W < k[0]:
+                raise UnsupportedModelError(f"{m} on a {H} x {W} input: the kernel is larger than the input")
             Ho, Wo = (H - k[0]) // s[0] + 1, (W - k[0]) // s[0] + 1
             layers.append(_Layer("conv", m.weight, m.bias, ACT_NONE, Cc * k[0] * k[0], m.out_channels, C=Cc, H=H, W=W, k=k[0],
                                  s=s[0], Ho=Ho, Wo=Wo))
@@ -98,6 +100,11 @@ def compile_sequential(mods: list[nn.Module], input_shape: tuple[int, ...]) -> l
             continue
         else:
             raise UnsupportedModelError(f"layer {m} is outside the fused layered-network family")
+    # FusedStack.backward masks a convolution's or a flatten's input gradient with ReLU only: refuse a Tanh there now
+    # rather than in the middle of the first update
+    for prev, L in zip(layers, layers[1:]):
+        if L.kind in ("conv", "flatten") and prev.act == ACT_TANH:
+            raise UnsupportedModelError(f"tanh in front of a {'convolution' if L.kind == 'conv' else 'flatten'} is not supported")
     return layers
 
 
