@@ -80,7 +80,7 @@ def test_two_rank_shared_rollout_matches_reference(variant, tmp_path):
     """Strong scaling (SURVEY 8(e)): ONE rollout, the same ``np.random.permutation`` stream on both ranks, every minibatch split
     into two contiguous slices, gradient sum inside the epoch kernel -> the reference run's results, loss table row by row.
     Variant B's golden uses a minibatch size that does not divide the rollout (ragged last minibatch): a shared rollout
-    refuses that split loudly (``ValueError`` from ``PPO._shared_slice``) instead of changing the minibatch composition."""
+    refuses that split loudly (``ValueError`` from ``minibatch_order.shared_slice``) instead of changing the minibatch composition."""
     if torch.cuda.device_count() < 2:
         pytest.skip("needs 2 GPUs")
     import torch.multiprocessing as mp

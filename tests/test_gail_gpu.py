@@ -309,9 +309,9 @@ def test_state_dict_round_trip_continues_training():
 
 # ---------------------------------------------------------------------------------------------------------- API
 @gpu
-def test_refusals_and_errors(monkeypatch):
+def test_constructor_refusals_and_update_errors(monkeypatch):
     from tianshou_b200.algorithm import AdamOptimizerFactory, RMSpropOptimizerFactory, UnsupportedModelError
-    from tianshou_b200.algorithm.modelfree.a2c import ActorCriticOnPolicyAlgorithm
+    from tianshou_b200.algorithm.imitation import gail as gail_module
     from tianshou_b200.data import ReplayBuffer
     from tianshou_b200.utils import policy_within_training_step
     O, A = 11, 3
@@ -346,7 +346,7 @@ def test_refusals_and_errors(monkeypatch):
                                   np.zeros(4, bool), np.zeros(4, bool), np.zeros((4, O + 1), np.float32))
     with pytest.raises(UnsupportedModelError, match="do not match"):
         _gail(actor, critic, disc, wide, A)
-    monkeypatch.setattr(ActorCriticOnPolicyAlgorithm, "_world_size", staticmethod(lambda: 2))
+    monkeypatch.setattr(gail_module, "world", lambda: (0, 2))
     with pytest.raises(UnsupportedModelError, match="single-GPU"):
         _gail(actor, critic, disc, expert, A)
     monkeypatch.undo()

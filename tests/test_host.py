@@ -280,23 +280,6 @@ def test_numpy_permutation_job_many_jobs_and_fork():
     assert os.WIFEXITED(status) and os.WEXITSTATUS(status) == 0
 
 
-def test_numpy_state_pack_roundtrip():
-    """Shared rollout on several GPUs: rank 0's generator state travels to the other ranks as 627 float64 (PPO._broadcast_numpy_state)."""
-    from tianshou_b200.algorithm.modelfree.ppo import PPO
-    np.random.seed(123)
-    np.random.standard_normal(3)                  # has_gauss = 1, a cached gaussian
-    np.random.permutation(1000)
-    st = np.random.get_state()
-    a = np.random.rand(5)
-    np.random.seed(0)
-    np.random.set_state(PPO._unpack_numpy_state(st[0], PPO._pack_numpy_state(st)))
-    assert np.array_equal(np.random.rand(5), a)
-    np.random.set_state(st)
-    g1 = np.random.standard_normal(1)
-    np.random.set_state(PPO._unpack_numpy_state(st[0], PPO._pack_numpy_state(st)))
-    assert np.array_equal(np.random.standard_normal(1), g1)       # the cached gaussian survived
-
-
 def test_numpy_permutation_job_numa_confinement(tmp_path):
     """The crew is confined to the CPUs of the caller's NUMA node (csrc/hostperm.cu caller_node_cpus).  Fake two-node topology
     through TS_B200_SYSFS_NODE_DIR: the job reports the confinement and still reproduces numpy's stream."""

@@ -82,25 +82,3 @@ def test_single_process_defaults():
     t = torch.ones(4)
     assert allreduce_sum_(t) is t
     assert allgather_moments(torch.tensor([1.0, 2.0, 3.0], dtype=torch.float64)).shape == (1, 3)
-
-
-def test_shared_rollout_slices_partition_every_minibatch():
-    """rollout_partition='shared' (SURVEY 8(e)): with the SAME permutation on every rank, rank r takes the r-th contiguous
-    1 / world slice of every minibatch -- the ranks' local minibatches tile the global one in order, nothing else."""
-    from tianshou_b200.algorithm.modelfree.ppo import FusedActorCriticUpdate
-    from tianshou_b200.data.batch import minibatch_bounds
-    N, B = 4096, 512
-    perm = torch.randperm(N, generator=torch.Generator().manual_seed(0)).to(torch.int32)
-    bounds = minibatch_bounds(N, B, merge_last=True)
-    for w in (2, 4, 8):
-        parts = [FusedActorCriticUpdate._shared_slice(None, perm, bounds, r, w) for r in range(w)]
-        local = B // w
-        for r, (sl, lb) in enumerate(parts):
-            assert sl.numel() == N // w and lb == [(m * local, (m + 1) * local) for m in range(len(bounds))]
-        for m, (lo, hi) in enumerate(bounds):
-            glued = torch.cat([parts[r][0][m * local:(m + 1) * local] for r in range(w)])
-            assert torch.equal(glued, perm[lo:hi])
-    with pytest.raises(ValueError):       # a merged tail / a minibatch that does not divide: refused, not silently re-balanced
-        FusedActorCriticUpdate._shared_slice(None, perm[:4000], minibatch_bounds(4000, 512, merge_last=True), 0, 2)
-    with pytest.raises(ValueError):
-        FusedActorCriticUpdate._shared_slice(None, perm, minibatch_bounds(N, 512, merge_last=True), 0, 3)

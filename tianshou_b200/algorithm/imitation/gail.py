@@ -26,10 +26,11 @@ from ... import ops
 from ..._cabi import call, ptr, stream_ptr, to_device
 from ...data import Batch, ReplayBuffer, SequenceSummaryStats
 from ...data.batch import minibatch_bounds, numpy_global_permutation_
+from ...parallel import world
 from ...utils.net.common import ModuleWithVectorOutput
 from ..base import _space_kind
 from ..flat_params import FlatGroup, UnsupportedModelError, bind_optimizer
-from ..modelfree.a2c import A2CTrainingStats, ActorCriticOnPolicyAlgorithm
+from ..modelfree.a2c import A2CTrainingStats
 from ..modelfree.ppo import PPO
 from ..modelfree.reinforce import ProbabilisticActorPolicy
 from ..modelfree.sac import describe_q_critic
@@ -75,7 +76,7 @@ class GAIL(PPO):
     ) -> None:
         if not isinstance(policy.actor, ModuleWithVectorOutput):
             raise TypeError("GAIL requires the policy to use an actor with known output dimension.")
-        if ActorCriticOnPolicyAlgorithm._world_size() > 1:
+        if world()[1] > 1:
             raise UnsupportedModelError("GAIL is single-GPU")
         if _space_kind(policy.action_space) != "continuous":
             raise UnsupportedModelError("GAIL needs a Box action space: the discriminator reads concat(obs, act) rows")

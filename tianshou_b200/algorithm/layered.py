@@ -232,41 +232,23 @@ class LayeredActorCritic:
         self.group.optimizer_step(optimizer, max_grad_norm)
 
 
-def layered_update(algo: Any, batch: Any, batch_size: int | None, repeat: int) -> torch.Tensor:
-    """The repeat x minibatch loop (ppo.py:164-224) on a layered actor-critic; returns the device loss table [steps, 8]."""
-    from ..data.batch import NumpyGlobalPermutationJob, minibatch_bounds
+def layered_update(algo: Any, batch: Any, batch_size: int | None, repeat: int, order: Any) -> torch.Tensor:
+    """The repeat x minibatch loop (ppo.py:164-224) on a layered actor-critic in the passes' ``MinibatchOrder``; returns the
+    device loss table [steps, 8]."""
+    from ..data.batch import minibatch_bounds
     L: LayeredActorCritic = algo._layered
-    dev = L.device
     N = batch.obs.shape[0]
     bounds = minibatch_bounds(N, batch_size or N, merge_last=True)
     n_mb = len(bounds)
     hp = algo._loss_hparams()
-    stats = torch.zeros((repeat * n_mb, STATS_STRIDE), dtype=torch.float32, device=dev)
-    st = stream_ptr(dev)
-    if algo.minibatch_shuffle == "device":
-        perms = ops.make_permutation(algo._shuffle_seed, algo._shuffle_epoch, repeat, N, dev)
-        algo._shuffle_epoch += repeat
-        job = None
-    else:
-        job = getattr(algo, "_perm_job", None)
-        own_job = job is None or job.shape != (repeat, N)
-        if own_job:
-            job = NumpyGlobalPermutationJob(algo._host_perm_rows(repeat, N), repeat)
-    try:
-        for r in range(repeat):
-            if algo.recompute_adv and r > 0:
-                algo._add_returns_and_advantages(batch, None, None)
-            perm = perms[r] if job is None else job.wait(r).to(dev, non_blocking=True)
-            for m, (lo, hi) in enumerate(bounds):
-                adv_mom = None
-                if algo.advantage_normalization:
-                    sums = L._buf("adv_sums", 2, torch.float64)
-                    call("ts_minibatch_adv_sums", ptr(batch.adv), ptr(perm), lo, hi, ptr(sums), st)
-                    adv_mom = L._buf("adv_mom", 2)
-                    call("ts_adv_moments_finalize", ptr(sums), hi - lo, ptr(adv_mom), st)
-                idx = perm[lo:hi].to(torch.int64)
-                L.minibatch_step(batch, idx, hp, adv_mom, algo.optim._optim, algo.optim._max_grad_norm, stats[r * n_mb + m])
-    finally:
-        if job is not None and algo.minibatch_shuffle != "device" and getattr(algo, "_perm_job", None) is not job:
-            job.__exit__(None, None, None)
+    stats = torch.zeros((repeat * n_mb, STATS_STRIDE), dtype=torch.float32, device=L.device)
+    for r in range(repeat):
+        if algo.recompute_adv and r > 0:
+            algo._add_returns_and_advantages(batch, None, None)
+        order.ready(r)
+        perm = order.rows[r]
+        for m, (lo, hi) in enumerate(bounds):
+            adv_mom = algo._minibatch_adv_moments(batch, perm, lo, hi, 1) if algo.advantage_normalization else None
+            idx = perm[lo:hi].to(torch.int64)
+            L.minibatch_step(batch, idx, hp, adv_mom, algo.optim._optim, algo.optim._max_grad_norm, stats[r * n_mb + m])
     return stats

@@ -14,6 +14,7 @@ What changes (same signatures, same 3-phase structure as ``Algorithm._update``):
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import os
 from abc import ABC
@@ -26,6 +27,7 @@ import torch
 from ... import ops
 from ..._cabi import GRAD_EXTRA, STATS_STRIDE, PPOHParams, load_library, to_device
 from ...data import Batch, ReplayBuffer, SequenceSummaryStats
+from ...parallel import world
 from ...utils import RunningMeanStd
 from ...utils.net.common import ActorCritic
 from ..base import OnPolicyAlgorithm, TrainingStats
@@ -38,6 +40,7 @@ from ..flat_params import (
     optimizer_hyperparams,
 )
 from ..layered import LayeredActorCritic, fused_descriptor, parse_actor_critic
+from ..minibatch_order import MinibatchOrder
 from ..optim import OptimizerFactory
 from .reinforce import ProbabilisticActorPolicy
 
@@ -59,12 +62,28 @@ def _upload(arr: np.ndarray, dev: torch.device, dtype: torch.dtype | None = None
 
 
 class ActorCriticOnPolicyAlgorithm(OnPolicyAlgorithm, ABC):
-    """GAE-based actor-critic base (a2c.py:32-153) on the fused device path."""
+    """GAE-based actor-critic base (a2c.py:32-153) on the fused device path.
+
+    Multi-GPU data parallelism (one process per GPU).  ``rollout_partition="per_rank"``: every rank's buffer is ITS OWN shard
+    of the rollout (weak scaling: the global minibatch is the union of the ranks' local minibatches).  ``"shared"``: every
+    rank holds the SAME rollout and draws the SAME permutation; each minibatch of B rows is split into world_size contiguous
+    slices of B / world_size (SURVEY 8(e): a fixed problem, results comparable with a single-GPU / reference run on the same
+    inputs).  ``data_parallel=False`` ignores an initialised process group (single-rank execution)."""
+
+    minibatch_shuffle: str = "numpy"
+    _shuffle_seed: int = 0
+    _shuffle_epoch: int = 0
 
     def __init__(self, *, policy: ProbabilisticActorPolicy, critic: torch.nn.Module, optim: OptimizerFactory,
                  optim_include_actor: bool, max_grad_norm: float | None = None, gae_lambda: float = 0.95,
-                 max_batchsize: int = 256, gamma: float = 0.99, return_scaling: bool = False) -> None:
+                 max_batchsize: int = 256, gamma: float = 0.99, return_scaling: bool = False,
+                 rollout_partition: str = "per_rank", data_parallel: bool = True) -> None:
         super().__init__(policy=policy)
+        if rollout_partition not in ("per_rank", "shared"):
+            raise ValueError(f"rollout_partition must be 'per_rank' or 'shared', got {rollout_partition!r}")
+        self.rollout_partition = rollout_partition
+        self.data_parallel = bool(data_parallel)
+        self._active_order: MinibatchOrder | None = None
         self.critic = critic
         assert 0.0 <= gae_lambda <= 1.0, f"GAE lambda should be in [0, 1] but got: {gae_lambda}"
         assert 0.0 <= gamma <= 1.0, f"discount factor gamma should be in [0, 1] but got: {gamma}"
@@ -88,7 +107,7 @@ class ActorCriticOnPolicyAlgorithm(OnPolicyAlgorithm, ABC):
         fused = fused_descriptor(self._spec) if optim_include_actor and not force_layered else None
         if fused is None:
             self._desc, self._layered = None, LayeredActorCritic(self._spec, dev)
-            if self._world_size() > 1 and getattr(self, "data_parallel", True):
+            if self._ranks()[1] > 1:
                 raise UnsupportedModelError("the layer-wise actor-critic path is single-GPU")
             self._flat = self._layered.critic_group        # the optimiser's parameters (``group`` unless split)
         else:
@@ -105,7 +124,7 @@ class ActorCriticOnPolicyAlgorithm(OnPolicyAlgorithm, ABC):
             self._flat.weight_image = torch.zeros(nbytes, dtype=torch.uint8, device=dev) if nbytes > 0 else None
             if hasattr(self.policy, "_fused_inference"):      # Collector-side inference through the same forward kernel
                 self.policy._fused_inference = (self._flat, self._desc)
-            if self._world_size() > 1 and getattr(self, "data_parallel", True):  # replicas start bit-identical
+            if self._ranks()[1] > 1:      # replicas start bit-identical
                 from ...parallel import broadcast_params_
                 broadcast_params_(self._flat.flat)
         # a real torch Adam / RMSprop (+ scheduler) keeps lr schedules and state_dict round trips unchanged
@@ -130,6 +149,46 @@ class ActorCriticOnPolicyAlgorithm(OnPolicyAlgorithm, ABC):
         if t is None or t.shape != shape or t.dtype != dtype:
             t = self._scratch[name] = torch.empty(shape, dtype=dtype, device=self.device)
         return t
+
+    def _ranks(self) -> tuple[int, int]:
+        """(rank, world size) of the data-parallel update; (0, 1) without a process group or with ``data_parallel=False``."""
+        return world() if self.data_parallel else (0, 1)
+
+    # ------------------------------------------------------------------ update
+    def update(self, buffer: ReplayBuffer, batch_size: int | None, repeat: int) -> TrainingStats:
+        """``OnPolicyAlgorithm.update`` (algorithm_base.py:854-865).  The ``repeat`` minibatch orders are started here, so that
+        the reference-exact draws of ``Batch.split`` (batch.py:1209) overlap the upload / value pass / GAE that precede the
+        first pass (nothing in between touches numpy's global stream: ``sample(0)`` draws nothing)."""
+        with self._minibatch_order_job(buffer, repeat):
+            return super().update(buffer=buffer, batch_size=batch_size, repeat=repeat)
+
+    @contextlib.contextmanager
+    def _minibatch_order_job(self, buffer: Any, repeat: int) -> Any:
+        """Open (and on exit close) this update's ``MinibatchOrder``; ``_update_with_batch`` picks it up."""
+        if buffer is None or not self.policy.is_within_training_step or len(buffer) == 0 or repeat <= 0:
+            yield None        # update() raises or returns before any pass: no draw
+            return
+        with self._minibatch_order(repeat, len(buffer)) as order:
+            self._active_order = order
+            try:
+                yield order
+            finally:
+                self._active_order = None
+
+    @contextlib.contextmanager
+    def _minibatch_order(self, repeat: int, n: int) -> Any:
+        """The running order if it covers (repeat, n), else one opened for the duration of the block (direct calls)."""
+        order = self._active_order
+        if order is not None and order.shape == (repeat, n):
+            yield order
+            return
+        order = MinibatchOrder(self, repeat, n)
+        completed = False
+        try:
+            yield order
+            completed = True
+        finally:
+            order.close(completed)
 
     # ------------------------------------------------------------------ rollout -> device
     def _sample(self, buffer: ReplayBuffer, sample_size: int | None) -> tuple[Batch, Any]:
@@ -198,14 +257,14 @@ class ActorCriticOnPolicyAlgorithm(OnPolicyAlgorithm, ABC):
         n = batch.obs.shape[0]
         v_s = self._buf("v_s", n, torch.float32)
         v_next = self._buf("v_next", n, torch.float32)
+        r, w = self._ranks()
         if self._layered is not None:
             self._layered.critic_values(batch.obs, v_s)
             self._layered.critic_values(batch.obs_next, v_next)
-        elif self._shared_world() > 1 and n % self._shared_world() == 0:
+        elif self.rollout_partition == "shared" and w > 1 and n % w == 0:
             # shared rollout on several GPUs: every rank evaluates the critic on ITS 1 / world of the rows (contiguous env range),
             # one all-gather makes v_s / v_s_ complete everywhere; the 17 us scan below runs redundantly (replicas identical)
             import torch.distributed as dist
-            w, r = self._shared_world(), dist.get_rank()
             lo, hi = r * (n // w), (r + 1) * (n // w)
             pair = self._buf("v_pair_local", (2, n // w), torch.float32)
             ops.critic_forward(self._flat.flat, self._desc, batch.obs[lo:hi], batch.obs_next[lo:hi], out=pair[0], out2=pair[1])
@@ -221,8 +280,7 @@ class ActorCriticOnPolicyAlgorithm(OnPolicyAlgorithm, ABC):
         moments = None
         # per-rank rollout shards: the ranks' batch moments are merged in rank order; a shared rollout needs no exchange
         # (every rank scans the same transitions)
-        if (rms is not None and self._world_size() > 1 and getattr(self, "data_parallel", True)
-                and getattr(self, "rollout_partition", "per_rank") == "per_rank"):
+        if rms is not None and w > 1 and self.rollout_partition == "per_rank":
             moments = self._buf("rms_moments", 3, torch.float64)
         ops.gae(v_s, v_next, batch.rew, batch.terminated, batch.truncated, batch.get("_unfinished"),
                 gamma=self.gamma, gae_lambda=self.gae_lambda, rms_state=rms, rms_eps=self._eps,
@@ -253,17 +311,6 @@ class ActorCriticOnPolicyAlgorithm(OnPolicyAlgorithm, ABC):
             self.ret_rms.load_device_state(self._scratch.pop("rms"))
 
     # ------------------------------------------------------------------ multi-GPU hooks
-    def _shared_world(self) -> int:
-        """World size if this algorithm runs data-parallel on ONE shared rollout (rollout_partition='shared'), else 1."""
-        if getattr(self, "data_parallel", True) and getattr(self, "rollout_partition", "per_rank") == "shared":
-            return self._world_size()
-        return 1
-
-    @staticmethod
-    def _world_size() -> int:
-        import torch.distributed as dist
-        return dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
-
     def _merge_rms_across_ranks(self, rms: torch.Tensor, moments: torch.Tensor) -> None:
         from ...parallel import allgather_moments
         from ..._cabi import call, ptr, stream_ptr

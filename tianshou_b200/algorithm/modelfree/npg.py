@@ -22,7 +22,7 @@ import torch
 from ... import ops
 from ..._cabi import call, ptr, stream_ptr
 from ...data import Batch, ReplayBuffer, SequenceSummaryStats
-from ...data.batch import NumpyGlobalPermutationJob, minibatch_bounds
+from ...data.batch import minibatch_bounds
 from ..base import TrainingStats
 from ..flat_params import UnsupportedModelError
 from ..netgraph import ACT_NONE
@@ -46,8 +46,6 @@ class NPGTrainingStats(TrainingStats):
 class NPG(ActorCriticOnPolicyAlgorithm):
     """Natural Policy Gradient (https://proceedings.neurips.cc/paper/2001/file/4b86abe48d358ecf194c56c69108433e-Paper.pdf)."""
 
-    # the reference's minibatch order (np.random.permutation on the global stream, batch.py:1209) is the only one supported
-    minibatch_shuffle: str = "numpy"
     _ratio_surrogate = False
 
     def __init__(self, *, policy: ProbabilisticActorPolicy, critic: torch.nn.Module, optim: OptimizerFactory,
@@ -80,20 +78,16 @@ class NPG(ActorCriticOnPolicyAlgorithm):
         if self.minibatch_shuffle != "numpy":
             raise UnsupportedModelError("NPG / TRPO draw the reference's minibatch order (numpy's global stream) only; "
                                         "the device-generated order is unsupported")
-        dev = self.device
         N = batch.obs.shape[0]
         bounds = minibatch_bounds(N, batch_size or N, merge_last=True)
         n_mb = len(bounds)
         stats = self._alloc_stats(repeat * n_mb)
-        rows = self._scratch.get("host_perms")
-        if rows is None or rows.shape[0] < repeat or rows.shape[1] != N:
-            rows = self._scratch["host_perms"] = torch.empty((repeat, N), dtype=torch.int32, pin_memory=True)
-        with NumpyGlobalPermutationJob(rows, repeat) as job:
+        with self._minibatch_order(repeat, N) as order:
             for r in range(repeat):
-                perm = job.wait(r).to(dev, non_blocking=True)
+                order.ready(r)
                 for m, (lo, hi) in enumerate(bounds):
-                    self._minibatch(batch, perm[lo:hi].to(torch.int64), stats[r * n_mb + m])
-            table = stats.cpu().numpy().astype(np.float64)      # the only host sync (pinned rows are read before the job ends)
+                    self._minibatch(batch, order.rows[r, lo:hi].to(torch.int64), stats[r * n_mb + m])
+            table = stats.cpu().numpy().astype(np.float64)      # the only host sync
         self._rms_end()
         self._flat.export_state(self.optim._optim)
         self.last_stats_table = table

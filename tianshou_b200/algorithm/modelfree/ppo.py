@@ -13,24 +13,22 @@ Per ``update(buffer, batch_size, repeat)``:
          minibatch and one all-reduce of (gradient, loss sums) precedes the Adam step.
 
 ``minibatch_shuffle="device"`` replaces the host permutation by a keyed bijection generated on
-the GPU (``ts_make_permutation``); the update is then a single asynchronous C call.  The index
-stream then differs from the reference's (same distribution, different RNG) -- opt-in.
+the GPU (algorithm/minibatch_order.py).  The index stream then differs from the reference's (same
+distribution, different RNG) -- opt-in.
 """
 from __future__ import annotations
-
-import contextlib
 
 import ctypes as C
 from typing import Any, Literal
 
-import numpy as np
 import torch
 
 from ... import ops
-from ..._cabi import LOSS_A2C, STATS_STRIDE, call, ptr, stream_ptr
+from ..._cabi import LOSS_A2C, call, ptr, stream_ptr
 from ...data import Batch, ReplayBuffer
-from ...data.batch import NumpyGlobalPermutationJob, minibatch_bounds
-from ...parallel import allreduce_sum_, shard_bounds, world
+from ...data.batch import minibatch_bounds
+from ...parallel import allreduce_sum_
+from ..minibatch_order import shared_slice
 from ..optim import OptimizerFactory
 from .a2c import A2CTrainingStats, ActorCriticOnPolicyAlgorithm
 from .reinforce import ProbabilisticActorPolicy
@@ -41,233 +39,59 @@ class FusedActorCriticUpdate(ActorCriticOnPolicyAlgorithm):
     optimiser step (single GPU), the same launch with the gradient all-reduce fused in (multi GPU, NVLink peer memory),
     or the per-step NCCL fallback.  Subclasses provide ``_preprocess_batch`` and ``_loss_hparams``."""
 
-    minibatch_shuffle: str = "numpy"
-    _shuffle_seed: int = 0
-    _shuffle_epoch: int = 0
     recompute_adv: bool = False
     advantage_normalization: bool = False
-    # Multi-GPU data parallelism (one process per GPU).  "per_rank": every rank's buffer is ITS OWN shard of the rollout
-    # (weak scaling: the global minibatch is the union of the ranks' local minibatches).  "shared": every rank holds the
-    # SAME rollout and draws the SAME permutation; each minibatch of B rows is split into world_size contiguous slices of
-    # B / world_size (SURVEY 8(e): a fixed problem, results comparable with a single-GPU / reference run on the same inputs).
-    rollout_partition: str = "per_rank"
-    data_parallel: bool = True          # False: ignore an initialised process group (single-rank execution)
-
-    def _ranks(self) -> tuple[int, int]:
-        return world() if self.data_parallel else (0, 1)
-
-    def _shared_slice(self, perm_r: torch.Tensor, bounds: list[tuple[int, int]], rank: int, wsize: int
-                      ) -> tuple[torch.Tensor, list[tuple[int, int]]]:
-        """This rank's contiguous 1 / wsize slice of every minibatch of ``perm_r`` as a local permutation + bounds."""
-        n_mb = len(bounds)
-        size = bounds[0][1] - bounds[0][0]
-        regular = all(lo == m * size and hi == lo + size for m, (lo, hi) in enumerate(bounds))
-        if not regular or size % wsize != 0:
-            raise ValueError(f"rollout_partition='shared' needs len(buffer) % batch_size == 0 and batch_size % world_size == 0 "
-                             f"(got {bounds[-1][1]} transitions, minibatch {size}, {wsize} ranks)")
-        local = size // wsize
-        sl = perm_r[: n_mb * size].view(n_mb, wsize, local)[:, rank, :].contiguous().view(-1)
-        return sl, [(m * local, (m + 1) * local) for m in range(n_mb)]
 
     def _loss_hparams(self) -> Any:
         raise NotImplementedError
-
-    def update(self, buffer: ReplayBuffer, batch_size: int | None, repeat: int) -> A2CTrainingStats:
-        """``OnPolicyAlgorithm.update`` (algorithm_base.py:854-865).  With the default reference-exact minibatch order
-        the ``repeat`` permutation draws of ``Batch.split`` (batch.py:1209) are started here, in the background, so that
-        they overlap the upload / value pass / GAE that precede the first pass (nothing in between touches numpy's
-        global stream: ``sample(0)`` draws nothing)."""
-        with self._minibatch_order_job(buffer, repeat):
-            return super().update(buffer=buffer, batch_size=batch_size, repeat=repeat)
-
-    @contextlib.contextmanager
-    def _minibatch_order_job(self, buffer: Any, repeat: int) -> Any:
-        """Start (and on exit join) the background job that draws this update's ``repeat`` minibatch orders from numpy's
-        global stream.  ``update()`` enters it first thing; ``_update_with_batch`` picks the running job up."""
-        job = None
-        wanted = (self.minibatch_shuffle == "numpy" and buffer is not None and self.policy.is_within_training_step
-                  and len(buffer) > 0 and repeat > 0 and torch.cuda.is_available())
-        # ONE shared rollout on several GPUs: every rank would draw the very same rows from the very same stream.  Rank 0 draws,
-        # the rows travel over NVLink (one broadcast per pass), and the advanced generator state is broadcast at the end.
-        remote = wanted and self._shared_order_from_rank0()
-        if wanted and (not remote or self._ranks()[0] == 0):
-            job = NumpyGlobalPermutationJob(self._host_perm_rows(repeat, len(buffer)), repeat)
-        self._perm_job = job if not (remote and job is None) else "rank0"
-        completed = False
-        try:
-            yield job
-            completed = True
-        finally:
-            self._perm_job = None
-            if job is not None:
-                job.__exit__(None, None, None)      # joins the threads, writes the advanced state back into numpy
-            if remote and completed:                # (not while an exception unwinds: the other ranks may never reach the collective)
-                self._broadcast_numpy_state()
-
-    def _shared_order_from_rank0(self) -> bool:
-        import torch.distributed as dist
-        return (self.rollout_partition == "shared" and self._ranks()[1] > 1 and dist.is_available() and dist.is_initialized()
-                and dist.get_backend() == "nccl")
-
-    @staticmethod
-    def _pack_numpy_state(st: tuple) -> np.ndarray:
-        """numpy's legacy MT19937 state tuple as 627 float64 (every field is exactly representable: 32-bit words, small ints)."""
-        out = np.empty(627, dtype=np.float64)
-        out[:624] = np.asarray(st[1], dtype=np.float64)
-        out[624], out[625], out[626] = float(st[2]), float(st[3]), float(st[4])
-        return out
-
-    @staticmethod
-    def _unpack_numpy_state(kind: str, h: np.ndarray) -> tuple:
-        return (kind, h[:624].astype(np.uint32), int(h[624]), int(h[625]), float(h[626]))
-
-    def _broadcast_numpy_state(self) -> None:
-        """numpy's global legacy state of rank 0 -> every rank (they all consumed the same draws: rank 0 made them)."""
-        import torch.distributed as dist
-        st = np.random.get_state()
-        t = torch.zeros(627, dtype=torch.float64, device=self.device)
-        if dist.get_rank() == 0:
-            t.copy_(torch.from_numpy(self._pack_numpy_state(st)))
-        dist.broadcast(t, 0)
-        if dist.get_rank() != 0:
-            np.random.set_state(self._unpack_numpy_state(st[0], t.cpu().numpy()))
 
     def _one_pass(self, batch: Batch, perm_r: torch.Tensor, bounds: list[tuple[int, int]], hp: Any, stats: torch.Tensor,
                   r: int, rank: int, wsize: int) -> None:
         """Pass r over the minibatches in the order ``perm_r`` (optional advantage recompute first, ppo.py:174-178)."""
         if self.recompute_adv and r > 0:
             self._add_returns_and_advantages(batch, None, None)
-        if wsize > 1 and self.rollout_partition == "shared":
-            perm_r, bounds = self._shared_slice(perm_r, bounds, rank, wsize)
-        if wsize == 1:
-            self._device_passes(batch, perm_r, bounds, hp, stats, 1, False)
-        elif self._peer_exchange(bounds) is not None:
+        if self.rollout_partition == "shared":
+            perm_r, bounds = shared_slice(perm_r, bounds, rank, wsize)
+        if self._peer_exchange(bounds) is not None:
             self._fused_distributed_pass(batch, perm_r, bounds, hp, stats, rank, wsize)
         else:
             self._distributed_repeat(batch, perm_r, bounds, hp, stats, rank, wsize)
 
-    def _host_perm_rows(self, repeat: int, n: int) -> torch.Tensor:
-        t = self._scratch.get("host_perms")
-        if t is None or t.shape[0] < repeat or t.shape[1] != n:
-            t = self._scratch["host_perms"] = torch.empty((repeat, n), dtype=torch.int32, pin_memory=True)
-        return t
-
     # ------------------------------------------------------------------ update
     def _update_with_batch(self, batch: Batch, batch_size: int | None, repeat: int) -> A2CTrainingStats:
         """The repeat x minibatch loop of ppo.py:164-224 as device work."""
-        if self._layered is not None:        # networks outside the fused kernels' envelope: layer-wise tensor-core path
-            from ..layered import layered_update
-            result = self._stats_from_device(layered_update(self, batch, batch_size, repeat))
-            self._rms_end()
-            self._flat.export_state(self.optim._optim)
-            return result
-        dev = self.device
         N = batch.obs.shape[0]
-        size = batch_size or N
-        bounds = minibatch_bounds(N, size, merge_last=True)
-        n_mb = len(bounds)
-        hp = self._loss_hparams()
-        stats = self._alloc_stats(repeat * n_mb)
-        rank, wsize = self._ranks()
-        single_call = self.minibatch_shuffle == "device" and wsize == 1
-        feed = None
-
-        if self.minibatch_shuffle == "device":
-            perms = ops.make_permutation(self._shuffle_seed, self._shuffle_epoch, repeat, N, dev)
-            self._shuffle_epoch += repeat
-        else:
-            perms = None
-
-        if single_call:      # every pass of the update in ONE asynchronous C call
-            self._device_passes(batch, perms, bounds, hp, stats, repeat, self.recompute_adv)
-        elif perms is not None:
-            for r in range(repeat):
-                self._one_pass(batch, perms[r], bounds, hp, stats[r * n_mb:], r, rank, wsize)
-        else:
-            # the reference's RNG draws (np.random.permutation on the global stream once per pass, batch.py:1209),
-            # bit-identical, produced ahead of the passes by background threads straight into pinned memory (one row per
-            # pass, so a pending async copy is never overwritten) and overlapped with the GPU work enqueued so far
-            job = getattr(self, "_perm_job", None)
-            if isinstance(job, str) or (wsize > 1 and self._shared_order_from_rank0() and job is not None and rank == 0
-                                        and job.shape == (repeat, N)):
-                # shared rollout: rank 0's rows, broadcast pass by pass (job is "rank0" on the other ranks)
-                feed = self._rank0_order_passes(None if isinstance(job, str) else job, batch, bounds, hp, stats, repeat, rank, wsize)
-            elif job is not None and job.shape == (repeat, N):       # started by update(), already running
-                feed = self._numpy_order_passes(job, batch, bounds, hp, stats, repeat, rank, wsize)
-            else:                                                    # _update_with_batch called directly
-                with NumpyGlobalPermutationJob(self._host_perm_rows(repeat, N), repeat) as job:
-                    feed = self._numpy_order_passes(job, batch, bounds, hp, stats, repeat, rank, wsize)
-                    if feed is not None:                             # the job must outlive its feed
-                        torch.cuda.current_stream(dev).synchronize()
-                        call("ts_host_perm_feed_finish", feed)
-                        feed = None
-        try:
+        with self._minibatch_order(repeat, N) as order:
+            if self._layered is not None:    # networks outside the fused kernels' envelope: layer-wise tensor-core path
+                from ..layered import layered_update
+                stats = layered_update(self, batch, batch_size, repeat, order)
+            else:
+                bounds = minibatch_bounds(N, batch_size or N, merge_last=True)
+                n_mb = len(bounds)
+                hp = self._loss_hparams()
+                stats = self._alloc_stats(repeat * n_mb)
+                rank, wsize = self._ranks()
+                if wsize == 1:       # every pass of the update in ONE asynchronous C call
+                    self._device_passes(batch, order.rows, bounds, hp, stats, repeat, self.recompute_adv, feed=order.feed)
+                else:                # pass by pass: the exchange set-up is host-driven
+                    for r in range(repeat):
+                        order.ready(r)
+                        self._one_pass(batch, order.rows[r], bounds, hp, stats[r * n_mb:], r, rank, wsize)
             result = self._stats_from_device(stats)   # the only host sync of the update
-        finally:
-            if feed is not None:
-                torch.cuda.current_stream(dev).synchronize()
-                call("ts_host_perm_feed_finish", feed)
         self._rms_end()
         self._flat.export_state(self.optim._optim)
         return result
 
-    def _rank0_order_passes(self, job: NumpyGlobalPermutationJob | None, batch: Batch, bounds: list[tuple[int, int]], hp: Any,
-                            stats: torch.Tensor, repeat: int, rank: int, wsize: int) -> Any:
-        """Shared rollout on several GPUs: rank 0 feeds its job's rows to its device and broadcasts each one (NCCL, on the
-        compute stream, 4 N bytes over NVLink) before the pass that uses it; the other ranks run no host job at all."""
-        import torch.distributed as dist
-        dev, N, n_mb = self.device, batch.obs.shape[0], len(bounds)
-        perms = self._buf("perms_dev", (repeat, N), torch.int32)
-        feed = None
-        if job is not None:
-            if job._job is None:
-                perms.copy_(job._rows[:repeat], non_blocking=True)
-            else:
-                feed = C.c_void_p()
-                call("ts_host_perm_feed_start", job._job, C.c_void_p(job._rows.data_ptr()), ptr(perms), N, repeat, C.byref(feed))
-        try:
-            for r in range(repeat):
-                if feed is not None:
-                    call("ts_host_perm_feed_wait_row", feed, r, stream_ptr(dev))
-                dist.broadcast(perms[r], 0)
-                self._one_pass(batch, perms[r], bounds, hp, stats[r * n_mb:], r, rank, wsize)
-        except BaseException:
-            if feed is not None:
-                torch.cuda.current_stream(dev).synchronize()
-                call("ts_host_perm_feed_finish", feed)
-            raise
-        return feed
-
-    def _numpy_order_passes(self, job: NumpyGlobalPermutationJob, batch: Batch, bounds: list[tuple[int, int]], hp: Any,
-                            stats: torch.Tensor, repeat: int, rank: int, wsize: int) -> Any:
-        """All passes in the order of the running host job.  One GPU: ONE asynchronous C call -- the rows reach the device
-        through the job's feed (``ts_host_perm_feed_*``: copy stream + events), the host does not wait for any of them; returns
-        the feed handle, to be finished after the update's final sync.  Several GPUs: pass by pass (the exchange set-up is
-        host-driven), each pass ordered after its row's event on the stream."""
-        dev, N, n_mb = self.device, batch.obs.shape[0], len(bounds)
-        perms = self._buf("perms_dev", (repeat, N), torch.int32)
-        if job._job is None:                 # no background job (foreign bit generator): the rows are complete already
-            perms.copy_(job._rows[:repeat], non_blocking=True)
-            if wsize > 1:
-                for r in range(repeat):
-                    self._one_pass(batch, perms[r], bounds, hp, stats[r * n_mb:], r, rank, wsize)
-            else:
-                self._device_passes(batch, perms, bounds, hp, stats, repeat, self.recompute_adv)
-            return None
-        feed = C.c_void_p()
-        call("ts_host_perm_feed_start", job._job, C.c_void_p(job._rows.data_ptr()), ptr(perms), N, repeat, C.byref(feed))
-        try:
-            if wsize > 1:      # pass by pass (the exchange set-up is host-driven), but the STREAM waits for row r, not the host
-                for r in range(repeat):
-                    call("ts_host_perm_feed_wait_row", feed, r, stream_ptr(dev))
-                    self._one_pass(batch, perms[r], bounds, hp, stats[r * n_mb:], r, rank, wsize)
-            else:
-                self._device_passes(batch, perms, bounds, hp, stats, repeat, self.recompute_adv, feed=feed)
-        except BaseException:
-            torch.cuda.current_stream(dev).synchronize()
-            call("ts_host_perm_feed_finish", feed)
-            raise
-        return feed
+    def _minibatch_adv_moments(self, batch: Batch, perm: torch.Tensor, lo: int, hi: int, world: int) -> torch.Tensor:
+        """Advantage mean / std of minibatch ``perm[lo:hi]`` over every rank's slice (rows hi - lo per rank)."""
+        st = stream_ptr(self.device)
+        sums = self._buf("adv_sums", 2, torch.float64)
+        call("ts_minibatch_adv_sums", ptr(batch.adv), ptr(perm), lo, hi, ptr(sums), st)
+        if world > 1:
+            allreduce_sum_(sums)
+        adv_mom = self._buf("adv_mom", 2, torch.float32)
+        call("ts_adv_moments_finalize", ptr(sums), (hi - lo) * world, ptr(adv_mom), st)
+        return adv_mom
 
     def _device_passes(self, batch: Batch, perm_rows: torch.Tensor | None, bounds: list[tuple[int, int]], hp: Any,
                        stats: torch.Tensor, nrep: int, recompute: bool, feed: Any = None) -> None:
@@ -337,13 +161,7 @@ class FusedActorCriticUpdate(ActorCriticOnPolicyAlgorithm):
         st = stream_ptr(dev)
         for m, (lo, hi) in enumerate(bounds):
             global_rows = (hi - lo) * wsize
-            adv_mom = None
-            if self.advantage_normalization:
-                sums = self._buf("adv_sums", 2, torch.float64)
-                call("ts_minibatch_adv_sums", ptr(batch.adv), ptr(perm), lo, hi, ptr(sums), st)
-                allreduce_sum_(sums)
-                adv_mom = self._buf("adv_mom", 2, torch.float32)
-                call("ts_adv_moments_finalize", ptr(sums), global_rows, ptr(adv_mom), st)
+            adv_mom = self._minibatch_adv_moments(batch, perm, lo, hi, wsize) if self.advantage_normalization else None
             n_part = C.c_int32(0)
             call("ts_ppo_grad", ptr(f.flat), C.byref(self._desc), C.byref(hp), ptr(batch.obs), ptr(batch.act),
                  ptr(batch.adv), ptr(batch.returns), ptr(batch.logp_old), ptr(batch.v_s), ptr(perm), lo, hi,
@@ -384,10 +202,10 @@ class PPO(FusedActorCriticUpdate):
     ) -> None:
         assert dual_clip is None or dual_clip > 1.0, (
             f"Dual-clip PPO parameter should greater than 1.0 but got {dual_clip}")
-        object.__setattr__(self, "data_parallel", bool(data_parallel))     # read by the base constructor (replica broadcast)
         super().__init__(policy=policy, critic=critic, optim=optim, optim_include_actor=True,
                          max_grad_norm=max_grad_norm, gae_lambda=gae_lambda, max_batchsize=max_batchsize,
-                         gamma=gamma, return_scaling=return_scaling)
+                         gamma=gamma, return_scaling=return_scaling, rollout_partition=rollout_partition,
+                         data_parallel=data_parallel)
         self.vf_coef = vf_coef
         self.ent_coef = ent_coef
         self.eps_clip = eps_clip
@@ -399,10 +217,6 @@ class PPO(FusedActorCriticUpdate):
             raise ValueError(f"minibatch_shuffle must be 'numpy' or 'device', got {minibatch_shuffle!r}")
         self.minibatch_shuffle = minibatch_shuffle
         self._shuffle_seed = shuffle_seed
-        self._shuffle_epoch = 0
-        if rollout_partition not in ("per_rank", "shared"):
-            raise ValueError(f"rollout_partition must be 'per_rank' or 'shared', got {rollout_partition!r}")
-        self.rollout_partition = rollout_partition
 
     # ------------------------------------------------------------------ preprocess
     def _preprocess_batch(self, batch: Batch, buffer: ReplayBuffer, indices: Any) -> Batch:

@@ -739,7 +739,8 @@ class NumpyGlobalPermutationJob:
     (``ts_host_perm_job_*``, csrc/hostperm.cu): bit-identical rows and final generator state, but row r is
     ready ~4 + 2 r ms after the start instead of after (r + 1) x 14 ms of ``np.random.permutation + astype``.
     ``rows``: int32 host tensor [>= repeat, n] (pinned).  Use as a context manager; ``wait(r)`` blocks until row r is
-    complete; leaving the context joins the threads and writes the advanced state back into numpy."""
+    complete; leaving the context joins the threads and writes the advanced state back into numpy.  ``handle``: the C
+    job (what ``ts_host_perm_feed_start`` takes), None when the rows were drawn up front."""
 
     def __init__(self, rows: "torch.Tensor", repeat: int, n_workers: int | None = None) -> None:
         import ctypes as C
@@ -747,10 +748,10 @@ class NumpyGlobalPermutationJob:
 
         from .._cabi import call
         assert rows.dtype == torch.int32 and not rows.is_cuda and rows.is_contiguous() and rows.shape[0] >= repeat
-        self._rows, self._repeat, self._n = rows, repeat, rows.shape[1]
+        self.rows, self._repeat, self._n = rows, repeat, rows.shape[1]
         self.shape = (repeat, self._n)
         self._st = np.random.get_state()
-        self._job = None
+        self.handle = None
         if self._st[0] != "MT19937":          # not the legacy MT19937 state: plain numpy draws, in order, up front
             self._draw_serially()
             return
@@ -767,20 +768,20 @@ class NumpyGlobalPermutationJob:
         try:
             call("ts_host_perm_job_start", self._key.ctypes.data_as(C.c_void_p), int(self._st[2]), self._n, repeat,
                  C.c_void_p(rows.data_ptr()), nw, C.byref(h))
-            self._job = h
+            self.handle = h
         except RuntimeError:      # no threads / memory for the job: same stream, drawn serially (in order) right now
-            self._job = None
+            self.handle = None
             self._draw_serially()
 
     def _draw_serially(self) -> None:
         for r in range(self._repeat):
-            numpy_global_permutation_(self._rows[r])
+            numpy_global_permutation_(self.rows[r])
 
     def wait(self, r: int) -> "torch.Tensor":
         from .._cabi import call
-        if self._job is not None:
-            call("ts_host_perm_job_wait", self._job, r)
-        return self._rows[r]
+        if self.handle is not None:
+            call("ts_host_perm_job_wait", self.handle, r)
+        return self.rows[r]
 
     def __enter__(self) -> "NumpyGlobalPermutationJob":
         return self
@@ -789,10 +790,10 @@ class NumpyGlobalPermutationJob:
         import ctypes as C
 
         from .._cabi import call
-        if self._job is not None:
+        if self.handle is not None:
             pos = C.c_int32(0)
-            call("ts_host_perm_job_finish", self._job, self._key.ctypes.data_as(C.c_void_p), C.byref(pos))
-            self._job = None
+            call("ts_host_perm_job_finish", self.handle, self._key.ctypes.data_as(C.c_void_p), C.byref(pos))
+            self.handle = None
             cur = np.random.get_state()
             if cur[2] != self._st[2] or not np.array_equal(cur[1], self._st[1]):
                 # somebody drew from numpy's GLOBAL stream while the update was running (an lr-scheduler lambda, user

@@ -1,5 +1,5 @@
 """Host timeline of ONE default-order `PPO.update()`-equivalent (device-resident rollout): when each C entry point is called
-and how long the call blocks the host, plus the job constructor / exit.  Diagnostics only; needs a GPU."""
+and how long the call blocks the host, plus the order's open / close.  Diagnostics only; needs a GPU."""
 import os
 import sys
 import time
@@ -12,6 +12,7 @@ import bench
 import tianshou_b200._cabi as cabi
 import tianshou_b200.algorithm.modelfree.ppo as ppo_mod
 import tianshou_b200.algorithm.modelfree.a2c as a2c_mod
+import tianshou_b200.algorithm.minibatch_order as order_mod
 import tianshou_b200.data.batch as batch_mod
 import tianshou_b200.ops as ops_mod
 from tianshou_b200.synthetic import build_mujoco_ppo
@@ -36,7 +37,7 @@ def main() -> None:
     buf = bench.build_host_buffer(E, T, seed=0, device=dev)
     np.random.seed(1000)
     algo, _, _ = build_mujoco_ppo(bench.OBS, bench.ACT, dev, minibatch_shuffle="numpy")
-    for mod in (ppo_mod, a2c_mod, batch_mod, ops_mod):
+    for mod in (ppo_mod, a2c_mod, order_mod, batch_mod, ops_mod):
         if hasattr(mod, "call"):
             mod.call = traced_call
     batch_mod_call_patch = batch_mod.__dict__.get("call")
@@ -51,12 +52,12 @@ def main() -> None:
             s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             s.record()
             with algo._minibatch_order_job(buf, REPEAT):
-                LOG.append(("<job constructed>", 1e3 * (time.perf_counter() - T0[0]), 0.0))
+                LOG.append(("<order opened>", 1e3 * (time.perf_counter() - T0[0]), 0.0))
                 b = algo._preprocess_batch(batch, buf, idx)
                 LOG.append(("<preprocess enqueued>", 1e3 * (time.perf_counter() - T0[0]), 0.0))
                 algo._update_with_batch(b, BS, REPEAT)
                 LOG.append(("<_update_with_batch returned>", 1e3 * (time.perf_counter() - T0[0]), 0.0))
-            LOG.append(("<job exited>", 1e3 * (time.perf_counter() - T0[0]), 0.0))
+            LOG.append(("<order closed>", 1e3 * (time.perf_counter() - T0[0]), 0.0))
             e.record()
             sync()
             if it == 3:

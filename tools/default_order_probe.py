@@ -52,10 +52,10 @@ def main() -> None:
                 algo._update_with_batch(b, BS, REPEAT)
 
         def c_default_rows_ready_first():
-            with algo._minibatch_order_job(buf, REPEAT) as job:
-                job.wait(REPEAT - 1)
+            with algo._minibatch_order_job(buf, REPEAT) as order:
                 for r in range(REPEAT):
-                    job.wait(r)
+                    order.ready(r)
+                torch.cuda.current_stream().synchronize()       # every row is on the device
                 b = algo._preprocess_batch(batch, buf, idx)
                 algo._update_with_batch(b, BS, REPEAT)
 
@@ -63,8 +63,10 @@ def main() -> None:
             algo._preprocess_batch(batch, buf, idx)
 
         def e_job_only():
-            with algo._minibatch_order_job(buf, REPEAT) as job:
-                job.wait(REPEAT - 1)
+            with algo._minibatch_order_job(buf, REPEAT) as order:
+                for r in range(REPEAT):
+                    order.ready(r)
+                torch.cuda.current_stream().synchronize()
 
         def f_default_no_early_start():
             b = algo._preprocess_batch(batch, buf, idx)
@@ -72,8 +74,8 @@ def main() -> None:
 
         for name, fn in (("a device order", a_device_order), ("b default (job started first, as update() does)", b_default),
                          ("c default, every row complete before the update is enqueued", c_default_rows_ready_first),
-                         ("d _preprocess_batch only", d_preprocess_only), ("e permutation job only (host)", e_job_only),
-                         ("f default, job started inside _update_with_batch", f_default_no_early_start)):
+                         ("d _preprocess_batch only", d_preprocess_only), ("e minibatch orders only (host job + feed)", e_job_only),
+                         ("f default, order opened inside _update_with_batch", f_default_no_early_start)):
             ev, wall = timed(fn)
             print(f"{name:70s} events {ev:8.3f} ms   wall {wall:8.3f} ms")
 
