@@ -558,6 +558,17 @@ int ts_gail_reward_rows(const float* logits, int64_t n, double* rew, ts_stream_t
  * Fixed-order reduction, no atomics: two calls on the same input are bit-identical. */
 int ts_gail_disc_rows(const float* logits, int64_t n_pi, int64_t n_exp, float* dlogits, float* stats_row, ts_stream_t stream);
 
+/* ---- discrete SAC (discrete_sac.cu) ---- */
+/* The categorical rows of discrete SAC (discrete_sac.py:147-155 target value, :176-184 actor loss), in torch's fp32
+ * Categorical(logits=...) formulation: per row b with p = softmax(logits[b]), log p = logits[b] - logsumexp(logits[b]),
+ * m = min(q1[b], q2[b]): probs[b] = p; entropy[b] = H = -sum clamp(log p, finfo.min) * p; v[b] = sum p * m + alpha * H;
+ * dlogits[b] (nullable: the target needs none) = dlogit_scale * d(-v[b]) / dlogits[b]
+ *                                              = dlogit_scale * (alpha p (log p + H) - p (m - sum p * m)).
+ * [B, A] row-major, any A >= 1, any B (warps stride over the rows).  Fixed-order reductions, no atomics: two calls on the
+ * same input are bit-identical. */
+int ts_discrete_sac_rows(const float* logits, const float* q1, const float* q2, float alpha, int64_t B, int32_t A, float* v,
+                         float* entropy, float* probs, float* dlogits, float dlogit_scale, ts_stream_t stream);
+
 #ifdef TS_B200_DIAGNOSTICS
 /* Diagnostics build only (libts_b200_diag.so, `python -m tianshou_b200.csrc.build --diag`): not part of the product library. */
 /* Hardware self-test of the wgmma building blocks (csrc/wgmma.cuh), one CTA:

@@ -2,6 +2,7 @@ from .base import Algorithm, OffPolicyAlgorithm, OnPolicyAlgorithm, Policy, Trai
 from .flat_params import UnsupportedModelError
 from .imitation import GAIL, GailTrainingStats
 from .modelfree.a2c import A2CTrainingStats, ActorCriticOnPolicyAlgorithm
+from .modelfree.discrete_sac import DiscreteSAC
 from .modelfree.npg import NPG, NPGTrainingStats
 from .modelfree.ppo import A2C, PPO
 from .modelfree.reinforce import DiscreteActorPolicy, ProbabilisticActorPolicy
@@ -11,7 +12,7 @@ from .optim import AdamOptimizerFactory, LRSchedulerFactoryLinear, OptimizerFact
 __all__ = [
     "Algorithm", "OffPolicyAlgorithm", "OnPolicyAlgorithm", "Policy", "TrainingStats",
     "UnsupportedModelError", "A2CTrainingStats", "ActorCriticOnPolicyAlgorithm", "PPO", "A2C", "NPG", "TRPO", "NPGTrainingStats", "TRPOTrainingStats",
-    "GAIL", "GailTrainingStats",
+    "GAIL", "GailTrainingStats", "DiscreteSAC",
     "ProbabilisticActorPolicy", "DiscreteActorPolicy", "AdamOptimizerFactory", "LRSchedulerFactoryLinear", "OptimizerFactory",
     "RMSpropOptimizerFactory",
 ]

@@ -23,12 +23,12 @@ import numpy as np
 import torch
 from torch import nn
 
-from ... import ops
 from ..._cabi import call, ptr, stream_ptr, to_device
 from ...data import Batch, ReplayBuffer, to_numpy
 from ..base import OffPolicyAlgorithm, Policy, TrainingStats
 from ..flat_params import FlatGroup, UnsupportedModelError, bind_optimizer
 from ..netgraph import ACT_NONE, FusedStack, compile_sequential, module_layers
+from ..obs_source import DeviceObsSource, device_obs_source
 from ..optim import OptimizerFactory
 
 
@@ -85,19 +85,6 @@ class DiscreteQLearningPolicy(Policy):
             act[rand_mask] = rand_act[rand_mask]
             return act
         raise NotImplementedError(f"Currently only numpy array is supported for action, but got {type(act)}")
-
-
-class DeviceObsSource:
-    """``buffer[indices].obs`` as the kernels read it: either dense fp32 rows ``x`` or (uint8 frames, frame slots per
-    sample, scale) for the first convolution's fused frame-stack + im2col gather.  Sized like the batch it stands for."""
-
-    ndim = 1
-
-    def __init__(self, rows: int, x: torch.Tensor | None = None, frames: tuple | None = None) -> None:
-        self.rows, self.x, self.frames = rows, x, frames
-
-    def __len__(self) -> int:
-        return self.rows
 
 
 def describe_q_network(model: Any) -> tuple[Any, tuple[int, ...], float]:
@@ -162,41 +149,8 @@ class DQN(OffPolicyAlgorithm):
 
     # ------------------------------------------------------------------ observations -> first-layer input
     def _obs_source(self, buffer: ReplayBuffer, indices: np.ndarray | torch.Tensor, key: str = "obs") -> DeviceObsSource:
-        """How the network reads ``buffer[indices].<key>`` without materialising it on the host.
-        Convolutional input from a frame-stacking buffer: the S frame slots per sample (prev() chain) + the uint8 frame
-        column of the device mirror (or a version-cached upload).  Flat observations: gathered fp32 rows."""
-        idx = ops._idx(np.asarray(indices) if not isinstance(indices, torch.Tensor) else indices, self._dev)
-        if key == "obs_next":
-            if buffer._save_obs_next:
-                col = "obs_next"
-            else:        # obs_next = obs[next(index)] (buffer_base.py:627-629)
-                idx, col = ops.next_index(buffer.device_meta(), idx), "obs"
-        else:
-            col = "obs"
-        n = idx.numel()
-        if len(self._in_shape) == 3:
-            C, H, W = self._in_shape
-            frames = buffer.device_array(col)
-            S = int(buffer.stack_num)
-            if frames.dim() == 3 and S == C:                      # single frames [slot, H, W]: stack through prev()
-                m = buffer.device_meta()
-                sidx = self._buf(f"sidx_{key}", (n, S), torch.int64)
-                o, E, d, l, ln = m._args()
-                call("ts_stack_prev_indices", ptr(idx), n, S, o, E, d, l, ln, ptr(sidx), stream_ptr(self._dev))
-                if frames.dtype != torch.uint8:
-                    raise UnsupportedModelError("frame-stacked image observations must be stored as uint8")
-                return DeviceObsSource(n, frames=(frames, sidx, self._in_scale))
-            if frames.dim() == 4 and frames.shape[1] == C and S == 1:   # stored stacks [slot, C, H, W]
-                if frames.dtype != torch.uint8:
-                    raise UnsupportedModelError("image observations must be stored as uint8")
-                sidx = (idx.view(n, 1) * C + torch.arange(C, device=self._dev).view(1, C)).contiguous()
-                return DeviceObsSource(n, frames=(frames.view(-1, H, W), sidx, self._in_scale))
-            raise UnsupportedModelError(f"observation storage {tuple(frames.shape)} / stack_num {S} does not match the network input {self._in_shape}")
-        src = buffer.device_array(col)
-        x = ops.gather_rows(src.reshape(src.shape[0], -1), idx).to(torch.float32)
-        if self._in_scale != 1.0:
-            x = (x.to(torch.float64) / self._in_scale).to(torch.float32)
-        return DeviceObsSource(n, x=x.contiguous())
+        """How the network reads ``buffer[indices].<key>`` without materialising it on the host (obs_source.py)."""
+        return device_obs_source(buffer, indices, key, self._in_shape, self._in_scale, self._dev, self._buf)
 
     def _q_values(self, src: DeviceObsSource, tag: str, target: bool = False) -> tuple[list[torch.Tensor], torch.Tensor]:
         acts = self._net.forward(src.x, src.rows, tag, frames=src.frames, params=self._target_flat if target else None)
