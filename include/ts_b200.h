@@ -569,6 +569,33 @@ int ts_gail_disc_rows(const float* logits, int64_t n_pi, int64_t n_exp, float* d
 int ts_discrete_sac_rows(const float* logits, const float* q1, const float* q2, float alpha, int64_t B, int32_t A, float* v,
                          float* entropy, float* probs, float* dlogits, float dlogit_scale, ts_stream_t stream);
 
+/* ---- CQL (cql.cu) ---- */
+/* Per-row pieces of CQL's critic step (imitation/cql.py:295-365; CalQL calibration :331-346).  q1 / q2: each critic's outputs
+ * on one forward over B + 3N rows, N = B * R, ordered [data B | random N | current-pi N | next-pi N].  target [B]: the one-step
+ * target.  Block row i (observation i / R) has the values v_j = q_j - c_j with c = (rand_logp, logp_cur[i], logp_next[i]);
+ * cal_ret (nullable: uncalibrated) [B]: v_j = max(v_j, cal_ret[i / R]).  With x_j = v_j / T and the multiplier
+ * scale = log_alpha ? clamp(exp(*log_alpha), alpha_min, alpha_max) : 1 (device scalar):
+ *   sq_rows [2][B]   (q - target)^2 of the data rows;  lse_rows [2][N]   logsumexp over the THREE values x_j of the row (the
+ *                    reference concatenates three (N, 1) blocks along dim 1)
+ *   dq1 / dq2 [B+3N] d critic loss / d q: data rows 2 (q - target) / B - scale w / B; block rows
+ *                    (scale T w / N) exp(x_j - lse) / T times 1, 1/2 or 0 as v_j is above, equal to or below cal_ret (torch.maximum).
+ * Any R >= 1, any B (grid-stride). */
+int ts_cql_rows(const float* q1, const float* q2, const float* target, int64_t B, int32_t R, const float* logp_cur,
+                const float* logp_next, float rand_logp, const float* cal_ret, float temperature, float cql_weight,
+                const float* log_alpha, float alpha_min, float alpha_max, float* dq1, float* dq2, float* sq_rows,
+                float* lse_rows, ts_stream_t stream);
+/* The losses of ts_cql_rows' rows (cql.py:353-384), one block, fixed-order sums (bit-identical from run to run):
+ * penalty_k = mean(lse_k) w T - mean(q_k data) w; with log_alpha (Lagrange): a = clamp(exp(*log_alpha)), c_k = a (penalty_k -
+ * threshold), out[2] = a, out[3] = cql_alpha_loss = -(c1 + c2) 0.5, *grad_log_alpha = its derivative (clamp passes the gradient
+ * inside [alpha_min, alpha_max]); out[0], out[1] = mean (q_k - target)^2 + (c_k or penalty_k). */
+int ts_cql_losses(const float* q1, const float* q2, const float* sq_rows, const float* lse_rows, int64_t B, int64_t N,
+                  float temperature, float cql_weight, const float* log_alpha, float alpha_min, float alpha_max,
+                  float threshold, float* grad_log_alpha, float* out, ts_stream_t stream);
+/* One-step target of CQL (cql.py:282-292): out = rew + logical_not(done) * gamma * (min(q1, q2) - alpha * logp) in fp32, in
+ * the reference's operation order; rew / done are fp32 rows (to_torch(batch, dtype=torch.float)). */
+int ts_cql_target(const float* q1, const float* q2, const float* logp, float alpha, const float* rew, const float* done,
+                  float gamma, int64_t B, float* out, ts_stream_t stream);
+
 #ifdef TS_B200_DIAGNOSTICS
 /* Diagnostics build only (libts_b200_diag.so, `python -m tianshou_b200.csrc.build --diag`): not part of the product library. */
 /* Hardware self-test of the wgmma building blocks (csrc/wgmma.cuh), one CTA:

@@ -126,6 +126,10 @@ SIGNATURES: dict[str, list[Any]] = {
     "ts_gail_disc_rows": [_P, _I64, _I64, _P, _P, _P],
     # discrete SAC (discrete_sac.cu)
     "ts_discrete_sac_rows": [_P, _P, _P, C.c_float, _I64, _I32, _P, _P, _P, _P, C.c_float, _P],
+    # CQL (cql.cu)
+    "ts_cql_rows": [_P, _P, _P, _I64, _I32, _P, _P, C.c_float, _P, C.c_float, C.c_float, _P, C.c_float, C.c_float, _P, _P, _P, _P, _P],
+    "ts_cql_losses": [_P, _P, _P, _P, _I64, _I64, C.c_float, C.c_float, _P, C.c_float, C.c_float, C.c_float, _P, _P, _P],
+    "ts_cql_target": [_P, _P, _P, C.c_float, _P, _P, C.c_float, _I64, _P, _P],
     "ts_stack_prev_indices": [_P, _I64, _I32, _P, _I64, _P, _P, _P, _P, _P],
     "ts_im2col_u8": [_P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _D, _P, _P],
     "ts_im2col_f32": [_P, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P],

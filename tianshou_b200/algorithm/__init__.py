@@ -1,6 +1,6 @@
-from .base import Algorithm, OffPolicyAlgorithm, OnPolicyAlgorithm, Policy, TrainingStats
+from .base import Algorithm, OfflineAlgorithm, OffPolicyAlgorithm, OnPolicyAlgorithm, Policy, TrainingStats
 from .flat_params import UnsupportedModelError
-from .imitation import GAIL, GailTrainingStats
+from .imitation import CQL, GAIL, CQLTrainingStats, GailTrainingStats
 from .modelfree.a2c import A2CTrainingStats, ActorCriticOnPolicyAlgorithm
 from .modelfree.discrete_sac import DiscreteSAC
 from .modelfree.npg import NPG, NPGTrainingStats
@@ -10,9 +10,9 @@ from .modelfree.trpo import TRPO, TRPOTrainingStats
 from .optim import AdamOptimizerFactory, LRSchedulerFactoryLinear, OptimizerFactory, RMSpropOptimizerFactory
 
 __all__ = [
-    "Algorithm", "OffPolicyAlgorithm", "OnPolicyAlgorithm", "Policy", "TrainingStats",
+    "Algorithm", "OfflineAlgorithm", "OffPolicyAlgorithm", "OnPolicyAlgorithm", "Policy", "TrainingStats",
     "UnsupportedModelError", "A2CTrainingStats", "ActorCriticOnPolicyAlgorithm", "PPO", "A2C", "NPG", "TRPO", "NPGTrainingStats", "TRPOTrainingStats",
-    "GAIL", "GailTrainingStats", "DiscreteSAC",
+    "GAIL", "GailTrainingStats", "DiscreteSAC", "CQL", "CQLTrainingStats",
     "ProbabilisticActorPolicy", "DiscreteActorPolicy", "AdamOptimizerFactory", "LRSchedulerFactoryLinear", "OptimizerFactory",
     "RMSpropOptimizerFactory",
 ]

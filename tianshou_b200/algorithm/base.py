@@ -349,3 +349,18 @@ class OffPolicyAlgorithm(Algorithm, ABC):
     def update(self, buffer: ReplayBuffer, sample_size: int | None) -> TrainingStats:
         return self._update(sample_size=sample_size, buffer=buffer,
                             update_with_batch_fn=lambda batch: self._update_with_batch(batch))
+
+
+class OfflineAlgorithm(Algorithm, ABC):
+    """Learns from a fixed buffer: ``process_buffer`` once, then update(buffer, sample_size) (algorithm_base.py:906-951)."""
+
+    def process_buffer(self, buffer: ReplayBuffer) -> ReplayBuffer:
+        """Prepare the buffer for offline learning, e.g. add keys to it (algorithm_base.py:913-915)."""
+        return buffer
+
+    @abstractmethod
+    def _update_with_batch(self, batch: Batch) -> TrainingStats: ...
+
+    def update(self, buffer: ReplayBuffer, sample_size: int | None) -> TrainingStats:
+        return self._update(sample_size=sample_size, buffer=buffer,
+                            update_with_batch_fn=lambda batch: self._update_with_batch(batch))

@@ -1,3 +1,4 @@
+from .cql import CQL, CQLTrainingStats
 from .gail import GAIL, GailTrainingStats
 
-__all__ = ["GAIL", "GailTrainingStats"]
+__all__ = ["CQL", "CQLTrainingStats", "GAIL", "GailTrainingStats"]
