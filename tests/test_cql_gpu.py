@@ -280,6 +280,7 @@ def test_update_gradients_vs_fp64_autograd(O, A, H, R):
     before its Adam step, against float64 autograd of the eager restatement on copies of the modules with the same batch,
     noise and random actions.  Adam's first step is lr * sign(g); this is the check that sees a gradient off by a factor."""
     from oracle.oracle_cql import cql_nets, cql_update
+    from tianshou_b200.algorithm.flat_params import FlatGroup
     from tianshou_b200.utils import policy_within_training_step
     cfg = dict(obs=O, act=A, hidden=H, critic2=True, critic2_lr=1e-3, auto=False, alpha=0.2, cql_alpha_lr=1e-3, cql_weight=1.0,
                tau=0.005, gamma=0.99, temperature=1.0, with_lagrange=True, lagrange_threshold=10.0, min_action=-0.5, max_action=1.0,
@@ -309,16 +310,14 @@ def test_update_gradients_vs_fp64_autograd(O, A, H, R):
         return noises[-1]
 
     algo._noise_fn = noise
-    groups = {"actor": algo._g_actor, "c1": algo._g_c[0], "c2": algo._g_c[1], "la": algo._g_la}
+    names = {id(algo._g_actor): "actor", id(algo._g_c[0]): "c1", id(algo._g_c[1]): "c2", id(algo._g_la): "la"}
     cap = {}
-    for name, grp in groups.items():
-        real = grp.adam_step
 
-        def step(optimizer, mgn, _n=name, _g=grp, _real=real):
-            cap[_n] = _g.grad[:_g.n].detach().cpu().double().clone()
-            _real(optimizer, mgn)
+    def adam(group, optimizer, mgn):
+        cap[names[id(group)]] = group.grad[:group.n].detach().cpu().double().clone()
+        FlatGroup.adam_step(group, optimizer, mgn)
 
-        grp.adam_step = step
+    algo._adam = adam
     orig = algo._preprocess_batch
     algo._preprocess_batch = lambda b, buffer, idx: (cap.update(indices=np.asarray(idx).copy()), orig(b, buffer, idx))[1]
     torch.manual_seed(9)

@@ -330,6 +330,7 @@ def test_update_gradients_vs_fp64_autograd(kind, per, auto, separate_critic2, la
     returns; the 1-step returns against float64 of the target value; alpha's loss and step.  Adam's first step is lr * sign(g),
     so a gradient off by a constant factor leaves the parameters unchanged; this is the check that sees it."""
     from tianshou_b200.algorithm import AdamOptimizerFactory, DiscreteSAC
+    from tianshou_b200.algorithm.flat_params import FlatGroup
     from tianshou_b200.algorithm.modelfree.discrete_sac import DiscreteSACPolicy
     from tianshou_b200.algorithm.modelfree.sac import AutoAlpha
     from tianshou_b200.utils import policy_within_training_step
@@ -344,14 +345,12 @@ def test_update_gradients_vs_fp64_autograd(kind, per, auto, separate_critic2, la
     groups = [algo._g_c[0], algo._g_c[1], algo._g_actor]
     init = [copy.deepcopy(m).to("cpu", torch.float64) for m in (actor, algo.critic_old, algo.critic2_old)]
     cap = {"adam": []}
-    for grp in groups:
-        real = grp.adam_step
 
-        def step(optimizer, mgn, _g=grp, _real=real):
-            cap["adam"].append((_g, _g.grad.clone(), [x.flat.clone() for x in groups]))
-            _real(optimizer, mgn)
+    def adam(group, optimizer, mgn):
+        cap["adam"].append((group, group.grad.clone(), [x.flat.clone() for x in groups]))
+        FlatGroup.adam_step(group, optimizer, mgn)
 
-        grp.adam_step = step
+    algo._adam = adam
     orig_pre, orig_post = algo._preprocess_batch, algo._postprocess_batch
 
     def pre(batch, buffer, indices):

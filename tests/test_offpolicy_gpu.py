@@ -139,6 +139,22 @@ def test_sac_policy_forward_collector_path():
     assert algo.policy.map_action(out.act.detach().cpu().numpy()).shape == (7, int(g["cfg_act"]))
 
 
+def test_sac_refuses_networks_off_one_cuda_device():
+    """A critic outside the actor's CUDA device is refused, not silently moved there."""
+    from tianshou_b200.algorithm import AdamOptimizerFactory, UnsupportedModelError
+    from tianshou_b200.algorithm.modelfree.sac import SAC, SACPolicy
+    from tianshou_b200.utils.net.common import Net
+    from tianshou_b200.utils.net.continuous import ContinuousActorProbabilistic, ContinuousCritic
+    O, A = 4, 2
+    actor = ContinuousActorProbabilistic(preprocess_net=Net(state_shape=(O,), hidden_sizes=(8,)), action_shape=(A,), unbounded=True,
+                                         conditioned_sigma=True).to(DEV)
+    critic = ContinuousCritic(preprocess_net=Net(state_shape=(O,), action_shape=(A,), hidden_sizes=(8,), concat=True))
+    with pytest.raises(UnsupportedModelError, match="no CPU path"):
+        SAC(policy=SACPolicy(actor=actor, action_space=_Box(A)), policy_optim=AdamOptimizerFactory(lr=1e-3), critic=critic,
+            critic_optim=AdamOptimizerFactory(lr=1e-3))
+    assert next(critic.parameters()).device.type == "cpu"
+
+
 # ------------------------------------------------------------------------------------------------------------ DQN
 def _build_dqn(g):
     from tianshou_b200.algorithm import AdamOptimizerFactory

@@ -227,3 +227,20 @@ class FlatGroup:
         else:
             self._step = step
         self.export_state(optimizer)
+
+
+class DeviceScratch(dict):
+    """An algorithm's named scratch: ``tensor`` returns the cached device tensor of that name while its shape and dtype still
+    fit, so the update loop does no allocator traffic.  Other per-update state (pinned host buffers, the running-mean
+    state of one update) may sit under names of its own."""
+
+    def __init__(self, device: torch.device) -> None:
+        super().__init__()
+        self.device = device
+
+    def tensor(self, name: str, shape: tuple[int, ...] | int, dtype: torch.dtype = torch.float32) -> torch.Tensor:
+        shape = (shape,) if isinstance(shape, int) else tuple(shape)
+        t = self.get(name)
+        if t is None or t.shape != shape or t.dtype != dtype:
+            t = self[name] = torch.empty(shape, dtype=dtype, device=self.device)
+        return t

@@ -28,10 +28,8 @@ from torch import nn
 from ..._cabi import call, ptr, stream_ptr
 from ...data import Batch, ReplayBuffer
 from ..base import OfflineAlgorithm
-from ..flat_params import FlatGroup, UnsupportedModelError, bind_optimizer
-from ..modelfree.sac import (_F32_EPS, SIGMA_MAX, SIGMA_MIN, Alpha, SACPolicy, SACTrainingStats, describe_gaussian_actor,
-                             describe_q_critic)
-from ..netgraph import FusedStack, module_layers, polyak_update
+from ..flat_params import FlatGroup
+from ..modelfree.sac import Alpha, ContinuousTwinCritic, SACPolicy, SACTrainingStats
 from ..optim import OptimizerFactory
 
 
@@ -59,7 +57,7 @@ class _EvalModeModule(nn.Module):
         return self.module(*args, **kwargs)
 
 
-class CQL(OfflineAlgorithm):
+class CQL(ContinuousTwinCritic, OfflineAlgorithm):
     """Conservative Q-learning (arXiv:2006.04779), reference API and semantics (cql.py:32-400).
 
     The update reproduces what ``CQL._update_with_batch`` computes:
@@ -119,73 +117,20 @@ class CQL(OfflineAlgorithm):
         self.calibrated = calibrated
         if int(num_repeat_actions) < 1:
             raise ValueError(f"num_repeat_actions must be at least 1, got {num_repeat_actions}")
-        devs = {p.device for m in (policy.actor, self.critic, self.critic2) for p in m.parameters()}
-        if len(devs) != 1 or next(iter(devs)).type != "cuda":
-            raise UnsupportedModelError(f"networks live on {sorted(map(str, devs))}; tianshou_b200 has no CPU path -- move them to "
-                                        "one CUDA device")
-        dev = self._dev = next(iter(devs))
-        first = module_layers(policy.actor.preprocess)[0]
-        self.obs_dim = int(first.in_features)
-        a_layers, a_params, self.act_dim = describe_gaussian_actor(policy.actor, self.obs_dim)
-        self._g_actor = FlatGroup(a_params, dev)
-        self._actor = FusedStack(a_layers, self._g_actor, "actor")
-        self._g_c, self._c, self._g_ct = [], [], []
-        for src, tgt in ((self.critic, self.critic_old), (self.critic2, self.critic2_old)):
-            layers, params = describe_q_critic(src, self.obs_dim, self.act_dim)
-            _, tparams = describe_q_critic(tgt.module, self.obs_dim, self.act_dim)
-            g = FlatGroup(params, dev)
-            self._g_c.append(g)
-            self._c.append(FusedStack(layers, g, "critic"))
-            self._g_ct.append(FlatGroup(tparams, dev))
-        self.policy_optim = self._create_optimizer(self.policy, policy_optim)
-        self.critic_optim = self._create_optimizer(self.critic, critic_optim, max_grad_norm=max_grad_norm)
-        self.critic2_optim = self._create_optimizer(self.critic2, critic2_optim or critic_optim, max_grad_norm=max_grad_norm)
-        for o, g in ((self.policy_optim, self._g_actor), (self.critic_optim, self._g_c[0]), (self.critic2_optim, self._g_c[1])):
-            bind_optimizer(o, g)
+        self._build_networks(lagged=(self.critic_old.module, self.critic2_old.module), policy_optim=policy_optim,
+                             critic_optim=critic_optim, critic2_optim=critic2_optim, max_grad_norm=max_grad_norm)
+        dev = self._dev
         # the Lagrange multiplier: a plain tensor (not a module attribute, so not in state_dict(), as in the reference) whose
         # storage is a one-element flat group on the device
         self.cql_log_alpha = torch.tensor([0.0], requires_grad=True)
         self.cql_alpha_optim = torch.optim.Adam([self.cql_log_alpha], lr=cql_alpha_lr)
         self._g_la = FlatGroup([self.cql_log_alpha], dev)
         self._g_la.export_state(self.cql_alpha_optim)
-        self._scratch: dict[str, torch.Tensor] = {}
         # rsample noise source: torch's generator on the networks' device, the standard-normal draw Normal.rsample makes there
         # (randn: no host-side validity check, so no synchronisation)
         self._noise_fn = lambda shape: torch.randn(shape, device=dev)
 
     # ------------------------------------------------------------------ helpers
-    def _buf(self, name: str, shape: tuple[int, ...] | int, dtype: torch.dtype = torch.float32) -> torch.Tensor:
-        shape = (shape,) if isinstance(shape, int) else tuple(shape)
-        t = self._scratch.get(name)
-        if t is None or t.shape != shape or t.dtype != dtype:
-            t = self._scratch[name] = torch.empty(shape, dtype=dtype, device=self._dev)
-        return t
-
-    def _actor_forward(self, obs: torch.Tensor, tag: str) -> tuple[list[torch.Tensor], torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
-        """policy(batch) on the device (sac.py:108-131): returns (activations, act, log_prob, sigma, noise)."""
-        B, A = obs.shape[0], self.act_dim
-        acts = self._actor.forward(obs, B, tag)
-        noise = self._noise_fn((B, A)).to(self._dev, torch.float32).contiguous()
-        act, logp, sigma = self._buf(tag + "_act", (B, A)), self._buf(tag + "_logp", B), self._buf(tag + "_sigma", (B, A))
-        call("ts_squashed_gaussian", ptr(acts[-1]), 2 * A, ptr(noise), B, A, SIGMA_MIN, SIGMA_MAX, _F32_EPS, ptr(act), ptr(logp),
-             ptr(sigma), stream_ptr(self._dev))
-        return acts, act, logp, sigma, noise
-
-    def _concat(self, obs: torch.Tensor, act: torch.Tensor, out: torch.Tensor) -> None:
-        call("ts_concat2", ptr(obs), self.obs_dim, ptr(act), self.act_dim, obs.shape[0], ptr(out), stream_ptr(self._dev))
-
-    def _q_pair(self, obs: torch.Tensor, act: torch.Tensor, tag: str, target: bool = False) -> list[list[torch.Tensor]]:
-        """Both critics (or both lagged critics) on concat(obs, act): their activation lists."""
-        B = obs.shape[0]
-        x = self._buf(f"{tag}_x", (B, self.obs_dim + self.act_dim))
-        self._concat(obs, act, x)
-        out = []
-        for k in range(2):
-            if target:
-                self._g_ct[k].ensure_adopted()
-            out.append(self._c[k].forward(x, B, tag, params=self._g_ct[k].flat if target else None))
-        return out
-
     def _repeat_rows(self, x: torch.Tensor, R: int, tag: str) -> torch.Tensor:
         """x.unsqueeze(1).repeat(1, R, 1).view(B * R, -1) (cql.py:309-313): row b * R + j is x[b]."""
         from ... import ops
@@ -252,22 +197,7 @@ class CQL(OfflineAlgorithm):
         losses = self._buf("losses", 5)
 
         # actor: mean(alpha log pi - min(Q1, Q2)) against the current critics (cql.py:208-216, 275-276)
-        alpha = float(self.alpha.value)
-        a_acts, new_act, logp, sigma, noise = self._actor_forward(obs, "au")
-        c_acts = self._q_pair(obs, new_act, "aq")
-        dq1, dq2, rows = self._buf("adq1", (B, 1)), self._buf("adq2", (B, 1)), self._buf("actor_rows", B)
-        call("ts_sac_actor_q_grad", ptr(c_acts[0][-1]), ptr(c_acts[1][-1]), ptr(logp), alpha, B, ptr(dq1), ptr(dq2), ptr(rows), st)
-        call("ts_mean", ptr(rows), B, ptr(losses[0:1]), st)
-        cols = (self.obs_dim, self.obs_dim + A)
-        dact = self._buf("dact", (B, A))            # d loss / d act of both critics, the second one accumulated
-        for k, d in enumerate((dq1, dq2)):
-            self._c[k].backward(c_acts[k], d, B, "aq", param_grads=False, input_grad=True, input_cols=cols, dx_out=dact,
-                                dx_accumulate=k == 1)
-        dhead = self._buf("dhead", (B, 2 * A))
-        call("ts_squashed_gaussian_bwd", ptr(a_acts[-1]), 2 * A, ptr(noise), ptr(new_act), ptr(sigma), ptr(dact), B, A,
-             SIGMA_MIN, SIGMA_MAX, _F32_EPS, alpha / B, ptr(dhead), st)
-        self._actor.backward(a_acts, dhead, B, "au")
-        self._g_actor.adam_step(self.policy_optim._optim, self.policy_optim._max_grad_norm)
+        logp = self._actor_step(obs, float(self.alpha.value), losses[0:1])
         alpha_loss = self.alpha.update(-logp.detach().unsqueeze(-1))
 
         # target with the updated actor and alpha (cql.py:282-292)
@@ -308,15 +238,14 @@ class CQL(OfflineAlgorithm):
              float(self.cql_weight), ptr(log_alpha), float(self.alpha_min), float(self.alpha_max), float(self.lagrange_threshold),
              ptr(self._g_la.grad) if log_alpha is not None else None, ptr(losses[1:5]), st)
         if log_alpha is not None:                           # cql.py:378-381
-            self._g_la.adam_step(self.cql_alpha_optim, None)
+            self._adam(self._g_la, self.cql_alpha_optim, None)
             self._g_la.export_state(self.cql_alpha_optim)
 
         # critics: parameter gradients only (cql.py:383-388), clipped Adam
         for k, optim in enumerate((self.critic_optim, self.critic2_optim)):
             self._c[k].backward(q[k], dq[k], B + 3 * N, "cq")
-            self._g_c[k].adam_step(optim._optim, optim._max_grad_norm)
-        for k in range(2):                                  # _update_lagged_network_weights
-            polyak_update(self._g_ct[k], self._g_c[k], self.tau)
+            self._adam(self._g_c[k], optim._optim, optim._max_grad_norm)
+        self._polyak()
         return losses, alpha_loss
 
     def _sync_multiplier_state(self) -> None:

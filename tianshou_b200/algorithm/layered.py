@@ -23,7 +23,7 @@ from torch import nn
 
 from .. import ops
 from .._cabi import AC_CATEGORICAL, AC_RELU, STATS_STRIDE, ActorCriticDesc, call, ptr, stream_ptr
-from .flat_params import FlatGroup, UnsupportedModelError
+from .flat_params import DeviceScratch, FlatGroup, UnsupportedModelError
 from .netgraph import ACT_NONE, ACT_RELU, FusedStack, _Layer, compile_sequential, module_layers
 
 _CHUNK = 131072          # rows per forward chunk of the whole-rollout passes (bounds the activation scratch)
@@ -148,16 +148,10 @@ class LayeredActorCritic:
         self.c_head = FusedStack(spec.c_head, self.critic_group, "c_head")
         self.sigma_param = spec.sigma_param
         self._a_act, self._c_act = spec.a_trunk[-1].act, spec.c_trunk[-1].act
-        self._scratch: dict[str, torch.Tensor] = {}
+        self._scratch = DeviceScratch(device)
+        self._buf = self._scratch.tensor
 
     # ------------------------------------------------------------------ helpers
-    def _buf(self, name: str, shape: tuple[int, ...] | int, dtype: torch.dtype = torch.float32) -> torch.Tensor:
-        shape = (shape,) if isinstance(shape, int) else tuple(shape)
-        t = self._scratch.get(name)
-        if t is None or t.shape != shape or t.dtype != dtype:
-            t = self._scratch[name] = torch.empty(shape, dtype=dtype, device=self.device)
-        return t
-
     def _logstd_ptr(self, buf: torch.Tensor) -> int | None:
         return None if self.categorical else buf.data_ptr() + 4 * self.group.offset(self.sigma_param)
 

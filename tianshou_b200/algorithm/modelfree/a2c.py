@@ -32,6 +32,7 @@ from ...utils import RunningMeanStd
 from ...utils.net.common import ActorCritic
 from ..base import OnPolicyAlgorithm, TrainingStats
 from ..flat_params import (
+    DeviceScratch,
     FlatGroup,
     UnsupportedModelError,
     bind_optimizer,
@@ -136,19 +137,12 @@ class ActorCriticOnPolicyAlgorithm(OnPolicyAlgorithm, ABC):
         self.return_scaling = return_scaling
         self.ret_rms = RunningMeanStd()
         self._eps = 1e-8
-        self._scratch: dict[str, torch.Tensor] = {}
+        self._scratch = DeviceScratch(dev)
+        self._buf = self._scratch.tensor
 
     @property
     def device(self) -> torch.device:
         return self._flat.device
-
-    def _buf(self, name: str, shape: tuple[int, ...] | int, dtype: torch.dtype) -> torch.Tensor:
-        """Cached device scratch (no allocator traffic inside the update loop)."""
-        shape = (shape,) if isinstance(shape, int) else tuple(shape)
-        t = self._scratch.get(name)
-        if t is None or t.shape != shape or t.dtype != dtype:
-            t = self._scratch[name] = torch.empty(shape, dtype=dtype, device=self.device)
-        return t
 
     def _ranks(self) -> tuple[int, int]:
         """(rank, world size) of the data-parallel update; (0, 1) without a process group or with ``data_parallel=False``."""

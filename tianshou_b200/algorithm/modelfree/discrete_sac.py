@@ -12,7 +12,8 @@ Per ``update(buffer, sample_size)``:
          lagged critics forward on s' -> ``ts_discrete_sac_rows`` (V(s')) -> value mask + ``ts_nstep_return``; per critic
          forward -> ``ts_dqn_loss`` (gathered weighted MSE) -> backward GEMMs -> Adam; actor forward, both critics forward ->
          ``ts_discrete_sac_rows`` (V(s), H, d loss / d logits) -> actor backward -> Adam; alpha update; Polyak.
-Every Linear / Conv2d layer's forward, input gradient and weight gradient is one wgmma GEMM launch (csrc/net_gemm.cu).
+Every Linear / Conv2d layer's forward, input gradient and weight gradient is one wgmma GEMM launch (csrc/net_gemm.cu).  The
+networks, optimisers, lagged forward and Polyak are the twin-critic core's (twin_critic.py), as for SAC and CQL.
 """
 from __future__ import annotations
 
@@ -25,13 +26,14 @@ import torch
 from torch import nn
 from torch.distributions import Categorical
 
-from ..._cabi import call, ptr, stream_ptr, to_device
+from ..._cabi import call, ptr, stream_ptr
 from ...data import Batch, ReplayBuffer
 from ..base import OffPolicyAlgorithm, Policy
-from ..flat_params import FlatGroup, UnsupportedModelError, bind_optimizer
-from ..netgraph import ACT_NONE, FusedStack, _Layer, compile_sequential, module_layers, polyak_update
+from ..flat_params import UnsupportedModelError
+from ..netgraph import ACT_NONE, _Layer, compile_sequential, module_layers
 from ..obs_source import DeviceObsSource, device_obs_source
 from ..optim import OptimizerFactory
+from ..twin_critic import TwinCriticAlgorithm, pop_batch_weight, sample_discrete
 from .dqn import describe_q_network
 from .sac import Alpha, SACTrainingStats
 
@@ -84,7 +86,7 @@ def describe_discrete_head_network(net: Any, role: str) -> tuple[list[_Layer], l
     return layers, params, shape, scale
 
 
-class DiscreteSAC(OffPolicyAlgorithm):
+class DiscreteSAC(TwinCriticAlgorithm, OffPolicyAlgorithm):
     """Soft actor-critic for discrete actions (arXiv:1910.07207), reference API (discrete_sac.py:83-196)."""
 
     def __init__(self, *, policy: DiscreteSACPolicy, policy_optim: OptimizerFactory, critic: nn.Module,
@@ -115,45 +117,28 @@ class DiscreteSAC(OffPolicyAlgorithm):
                     raise UnsupportedModelError(f"{owner[id(p)]} and {name} share parameters (a common preprocess trunk, as in "
                                                 "examples/atari/atari_sac.py); give each network its own trunk")
                 owner[id(p)] = name
-        devs = {p.device for _, net in nets for p in net.parameters()}
-        if len(devs) != 1 or next(iter(devs)).type != "cuda":
-            raise UnsupportedModelError(f"networks live on {sorted(map(str, devs))}; tianshou_b200 has no CPU path -- move them to "
-                                        "one CUDA device")
-        dev = self._dev = next(iter(devs))
-        a_layers, a_params, self._in_shape, self._in_scale = describe_discrete_head_network(actor, "actor")
-        self.n_actions = a_layers[-1].out_dim
-        if self.n_actions != int(policy.action_space.n):
-            raise UnsupportedModelError(f"actor has {self.n_actions} outputs for {int(policy.action_space.n)} actions")
-        self._g_actor = FlatGroup(a_params, dev)
-        self._actor_net = FusedStack(a_layers, self._g_actor, "actor")
-        self._g_c, self._c, self._g_ct = [], [], []
-        for name, src, tgt in (("critic", self.critic, self.critic_old), ("critic2", self.critic2, self.critic2_old)):
-            layers, params, shape, scale = describe_discrete_head_network(src, name)
-            if (shape, scale) != (self._in_shape, self._in_scale):
-                raise UnsupportedModelError(f"{name} reads the observation as shape {shape} / denominator {scale}, the actor as "
-                                            f"{self._in_shape} / {self._in_scale}: the networks must read it the same way")
-            if layers[-1].out_dim != self.n_actions:
-                raise UnsupportedModelError(f"{name} has {layers[-1].out_dim} outputs for {self.n_actions} actions")
-            _, tparams, _, _ = describe_discrete_head_network(tgt, name)
-            g = FlatGroup(params, dev)
-            self._g_c.append(g)
-            self._c.append(FusedStack(layers, g, name))
-            self._g_ct.append(FlatGroup(tparams, dev))
-        self.policy_optim = self._create_optimizer(policy, policy_optim)
-        self.critic_optim = self._create_optimizer(self.critic, critic_optim)
-        self.critic2_optim = self._create_optimizer(self.critic2, critic2_optim or critic_optim)
-        for o, g in ((self.policy_optim, self._g_actor), (self.critic_optim, self._g_c[0]), (self.critic2_optim, self._g_c[1])):
-            bind_optimizer(o, g)
-        self._scratch: dict[str, torch.Tensor] = {}
+        self._build_twin_critic(describe_actor=self._describe_actor, describe_critic=self._describe_critic,
+                                lagged=(self.critic_old, self.critic2_old), policy_optim=policy_optim, critic_optim=critic_optim,
+                                critic2_optim=critic2_optim)
+
+    def _describe_actor(self, actor: nn.Module) -> tuple[list[_Layer], list[nn.Parameter]]:
+        layers, params, self._in_shape, self._in_scale = describe_discrete_head_network(actor, "actor")
+        self.n_actions = layers[-1].out_dim
+        if self.n_actions != int(self.policy.action_space.n):
+            raise UnsupportedModelError(f"actor has {self.n_actions} outputs for {int(self.policy.action_space.n)} actions")
+        return layers, params
+
+    def _describe_critic(self, net: nn.Module, name: str) -> tuple[list[_Layer], list[nn.Parameter]]:
+        """A critic read as the actor reads the observation, one output per action."""
+        layers, params, shape, scale = describe_discrete_head_network(net, name)
+        if (shape, scale) != (self._in_shape, self._in_scale):
+            raise UnsupportedModelError(f"{name} reads the observation as shape {shape} / denominator {scale}, the actor as "
+                                        f"{self._in_shape} / {self._in_scale}: the networks must read it the same way")
+        if layers[-1].out_dim != self.n_actions:
+            raise UnsupportedModelError(f"{name} has {layers[-1].out_dim} outputs for {self.n_actions} actions")
+        return layers, params
 
     # ------------------------------------------------------------------ helpers
-    def _buf(self, name: str, shape: tuple[int, ...] | int, dtype: torch.dtype = torch.float32) -> torch.Tensor:
-        shape = (shape,) if isinstance(shape, int) else tuple(shape)
-        t = self._scratch.get(name)
-        if t is None or t.shape != shape or t.dtype != dtype:
-            t = self._scratch[name] = torch.empty(shape, dtype=dtype, device=self._dev)
-        return t
-
     def _obs_source(self, buffer: ReplayBuffer, indices: np.ndarray | torch.Tensor, key: str = "obs") -> DeviceObsSource:
         return device_obs_source(buffer, indices, key, self._in_shape, self._in_scale, self._dev, self._buf)
 
@@ -174,11 +159,8 @@ class DiscreteSAC(OffPolicyAlgorithm):
         """sum_a pi(a|s') min(Q1', Q2')(s', a) + alpha H(pi(.|s'))   (discrete_sac.py:147-155, ddpg.py:327-339)"""
         src = self._obs_source(buffer, indices, "obs_next")
         B = src.rows
-        logits = self._actor_net.forward(src.x, B, "tq", frames=src.frames)[-1]
-        q = []
-        for k in range(2):
-            self._g_ct[k].ensure_adopted()
-            q.append(self._c[k].forward(src.x, B, "tq", frames=src.frames, params=self._g_ct[k].flat)[-1])
+        logits = self._actor.forward(src.x, B, "tq", frames=src.frames)[-1]
+        q = [self._lagged_forward(k, src.x, B, "tq", frames=src.frames)[-1] for k in range(2)]
         v, _, _ = self._categorical_rows(logits, q[0], q[1], float(self.alpha.value), "tq", with_grad=False)
         return v
 
@@ -187,17 +169,7 @@ class DiscreteSAC(OffPolicyAlgorithm):
                                          gamma=self.gamma, n_step=self.n_step_return_horizon)
 
     def _sample(self, buffer: ReplayBuffer, sample_size: int | None) -> tuple[Batch, Any]:
-        """Indices from the buffer's host RNG streams (identical to the reference's draws); observations stay on the device."""
-        indices = buffer.sample_indices(sample_size)
-        batch = Batch()
-        batch.__dict__["obs"] = self._obs_source(buffer, indices, "obs")
-        act = np.asarray(buffer.act)[indices]
-        batch.__dict__["act"] = to_device(np.ascontiguousarray(act.reshape(-1)).astype(np.int64), self._dev)
-        if hasattr(buffer, "get_weight"):          # PrioritizedReplayBuffer.__getitem__ adds the IS weight (prio.py:104-106)
-            w = buffer.get_weight(indices)
-            batch.__dict__["weight"] = to_device(np.asarray(w / np.max(w) if buffer._weight_norm else w, dtype=np.float32), self._dev)
-        batch.__dict__["info"] = Batch()
-        return batch, indices
+        return sample_discrete(buffer, sample_size, self._obs_source, self._dev)
 
     # ------------------------------------------------------------------ update
     def _critic_step(self, k: int, src: DeviceObsSource, act: torch.Tensor, returns: torch.Tensor, weight: torch.Tensor | None,
@@ -213,18 +185,14 @@ class DiscreteSAC(OffPolicyAlgorithm):
         call("ts_dqn_loss", ptr(acts[-1]), ptr(act), ptr(returns), ptr(weight), B, A, 0.0, ptr(td), ptr(dq), ptr(rows), st)
         call("ts_mean", ptr(rows), B, ptr(out_loss), st)
         self._c[k].backward(acts, dq, B, "cu")
-        self._g_c[k].adam_step(optim._optim, optim._max_grad_norm)
+        self._adam(self._g_c[k], optim._optim, optim._max_grad_norm)
         return td
 
     def _update_with_batch(self, batch: Batch) -> DiscreteSACTrainingStats:
         dev, st = self._dev, stream_ptr(self._dev)
         src = batch.obs
         B = src.rows
-        weight = batch.__dict__.pop("weight", None)
-        if weight is not None:
-            if not isinstance(weight, torch.Tensor):
-                weight = to_device(np.asarray(weight, dtype=np.float32), dev)
-            weight = weight.reshape(-1).to(dev, torch.float32).contiguous()
+        weight = pop_batch_weight(batch, dev)
         returns = batch.returns.reshape(-1).to(dev, torch.float32).contiguous()
         losses = self._buf("losses", 3)
         td1 = self._critic_step(0, src, batch.act, returns, weight, self.critic_optim, losses[0:1])
@@ -233,17 +201,16 @@ class DiscreteSAC(OffPolicyAlgorithm):
 
         # actor: loss = -mean(alpha H + sum_a pi(a|s) min(Q1, Q2)(s, a)), the critics after their steps, no gradient into them
         alpha = float(self.alpha.value)
-        a_acts = self._actor_net.forward(src.x, B, "au", frames=src.frames)
+        a_acts = self._actor.forward(src.x, B, "au", frames=src.frames)
         q1 = self._c[0].forward(src.x, B, "aq", frames=src.frames)[-1]
         q2 = self._c[1].forward(src.x, B, "aq", frames=src.frames)[-1]
         v, entropy, dlogits = self._categorical_rows(a_acts[-1], q1, q2, alpha, "au", with_grad=True)
         call("ts_mean", ptr(v), B, ptr(losses[2:3]), st)
-        self._actor_net.backward(a_acts, dlogits, B, "au")
-        self._g_actor.adam_step(self.policy_optim._optim, self.policy_optim._max_grad_norm)
+        self._actor.backward(a_acts, dlogits, B, "au")
+        self._adam(self._g_actor, self.policy_optim._optim, self.policy_optim._max_grad_norm)
 
         alpha_loss = self.alpha.update(entropy)
-        for k in range(2):                      # _update_lagged_network_weights
-            polyak_update(self._g_ct[k], self._g_c[k], self.tau)
+        self._polyak()
         l = losses.cpu().numpy()                # the only host read of the losses
         return DiscreteSACTrainingStats(actor_loss=-float(l[2]), critic1_loss=float(l[0]), critic2_loss=float(l[1]),
                                         alpha=float(self.alpha.value), alpha_loss=alpha_loss)

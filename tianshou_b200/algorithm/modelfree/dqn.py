@@ -23,13 +23,14 @@ import numpy as np
 import torch
 from torch import nn
 
-from ..._cabi import call, ptr, stream_ptr, to_device
+from ..._cabi import call, ptr, stream_ptr
 from ...data import Batch, ReplayBuffer, to_numpy
 from ..base import OffPolicyAlgorithm, Policy, TrainingStats
-from ..flat_params import FlatGroup, UnsupportedModelError, bind_optimizer
+from ..flat_params import DeviceScratch, FlatGroup, UnsupportedModelError, bind_optimizer
 from ..netgraph import ACT_NONE, FusedStack, compile_sequential, module_layers
 from ..obs_source import DeviceObsSource, device_obs_source
 from ..optim import OptimizerFactory
+from ..twin_critic import cuda_device_of, pop_batch_weight, sample_discrete
 
 
 @dataclass(kw_only=True)
@@ -118,10 +119,7 @@ class DQN(OffPolicyAlgorithm):
         self.is_double = is_double
         self.huber_loss_delta = huber_loss_delta
         self._iter = 0
-        dev = next(policy.model.parameters()).device
-        if dev.type != "cuda":
-            raise UnsupportedModelError(f"networks live on {dev}; tianshou_b200 has no CPU path -- move them to a CUDA device")
-        self._dev = dev
+        dev = self._dev = cuda_device_of(policy.model)
         inner, self._in_shape, self._in_scale = describe_q_network(policy.model)
         layers = compile_sequential(module_layers(inner), self._in_shape)
         if layers[-1].kind != "linear" or layers[-1].act != ACT_NONE:
@@ -134,18 +132,12 @@ class DQN(OffPolicyAlgorithm):
         bind_optimizer(self.optim, self._group)
         self.model_old = deepcopy(policy.model).eval() if self.use_target_network else None
         self._target_flat = self._group.flat.clone() if self.use_target_network else None
-        self._scratch: dict[str, torch.Tensor] = {}
+        self._scratch = DeviceScratch(dev)
+        self._buf = self._scratch.tensor
 
     @property
     def use_target_network(self) -> bool:
         return self.target_update_freq > 0
-
-    def _buf(self, name: str, shape: tuple[int, ...] | int, dtype: torch.dtype = torch.float32) -> torch.Tensor:
-        shape = (shape,) if isinstance(shape, int) else tuple(shape)
-        t = self._scratch.get(name)
-        if t is None or t.shape != shape or t.dtype != dtype:
-            t = self._scratch[name] = torch.empty(shape, dtype=dtype, device=self._dev)
-        return t
 
     # ------------------------------------------------------------------ observations -> first-layer input
     def _obs_source(self, buffer: ReplayBuffer, indices: np.ndarray | torch.Tensor, key: str = "obs") -> DeviceObsSource:
@@ -172,16 +164,7 @@ class DQN(OffPolicyAlgorithm):
                                          gamma=self.gamma, n_step=self.n_step)
 
     def _sample(self, buffer: ReplayBuffer, sample_size: int | None) -> tuple[Batch, Any]:
-        indices = buffer.sample_indices(sample_size)
-        batch = Batch()
-        batch.__dict__["obs"] = self._obs_source(buffer, indices, "obs")
-        act = np.asarray(buffer.act)[indices]
-        batch.__dict__["act"] = to_device(np.ascontiguousarray(act.reshape(-1)).astype(np.int64), self._dev)
-        if hasattr(buffer, "get_weight"):          # PrioritizedReplayBuffer.__getitem__ adds the IS weight (prio.py:104-106)
-            w = buffer.get_weight(indices)
-            batch.__dict__["weight"] = to_device(np.asarray(w / np.max(w) if buffer._weight_norm else w, dtype=np.float32), self._dev)
-        batch.__dict__["info"] = Batch()
-        return batch, indices
+        return sample_discrete(buffer, sample_size, self._obs_source, self._dev)
 
     # ------------------------------------------------------------------ update
     def _periodically_update_lagged_network_weights(self) -> None:
@@ -198,9 +181,7 @@ class DQN(OffPolicyAlgorithm):
         st = stream_ptr(self._dev)
         src = batch.obs
         B = src.rows
-        weight = batch.__dict__.pop("weight", None) if "weight" in batch.__dict__ else None
-        if weight is not None and not isinstance(weight, torch.Tensor):
-            weight = to_device(np.asarray(weight, dtype=np.float32), self._dev)
+        weight = pop_batch_weight(batch, self._dev)
         acts, q = self._q_values(src, "up")
         returns = batch.returns.reshape(-1).to(self._dev, torch.float32).contiguous()
         td = self._buf("td", B)

@@ -9,8 +9,11 @@ Per ``update(buffer, sample_size)``:
          transitions are the reference's), the two ``rsample`` noise draws (torch generator), one D2H of 3 loss scalars.
   GPU  : row gathers from the buffer's device mirror (or one upload of the sampled rows), target actor + lagged critics
          forward -> ``ts_sac_target`` -> ``ts_nstep_return``; per critic forward / loss / backward (``ts_net_gemm``) + Adam;
-         actor forward, critics' input-gradient GEMMs, tanh-Gaussian head backward, actor backward + Adam; Polyak axpy.
-Every Linear layer's forward / input gradient / weight gradient is one wgmma GEMM launch (csrc/net_gemm.cu).
+         actor forward, critics' input-gradient GEMMs (the second accumulating into the first), tanh-Gaussian head backward,
+         actor backward + Adam; Polyak axpy.
+Every Linear layer's forward / input gradient / weight gradient is one wgmma GEMM launch (csrc/net_gemm.cu).  The networks,
+the actor forward, the critic pair and the actor step are ``ContinuousTwinCritic``'s, shared with CQL (imitation/cql.py); it
+stands on the twin-critic core of twin_critic.py.
 """
 from __future__ import annotations
 
@@ -24,12 +27,13 @@ import torch
 from torch import nn
 from torch.distributions import Independent, Normal
 
-from ..._cabi import call, ptr, stream_ptr, to_device
+from ..._cabi import call, ptr, stream_ptr
 from ...data import Batch, ReplayBuffer
 from ..base import OffPolicyAlgorithm, Policy, TrainingStats
-from ..flat_params import FlatGroup, UnsupportedModelError, bind_optimizer
-from ..netgraph import ACT_NONE, FusedStack, _Layer, compile_sequential, module_layers, polyak_update
+from ..flat_params import FlatGroup, UnsupportedModelError
+from ..netgraph import ACT_NONE, _Layer, compile_sequential, module_layers
 from ..optim import OptimizerFactory
+from ..twin_critic import TwinCriticAlgorithm, per_weight, pop_batch_weight
 
 SIGMA_MIN, SIGMA_MAX = -20.0, 2.0          # utils/net/continuous.py:17-18
 _F32_EPS = float(np.finfo(np.float32).eps)
@@ -180,7 +184,68 @@ def describe_gaussian_actor(actor: Any, obs_dim: int) -> tuple[list[_Layer], lis
     return [*trunk, head], params, A
 
 
-class SAC(OffPolicyAlgorithm):
+class ContinuousTwinCritic(TwinCriticAlgorithm):
+    """The tanh-squashed Gaussian actor and the two Q(s, a) critics SAC and CQL share: building them, the actor forward,
+    both critics on concat(obs, act), and SAC's actor step."""
+
+    def _build_networks(self, *, lagged: tuple[nn.Module, nn.Module], policy_optim: OptimizerFactory,
+                        critic_optim: OptimizerFactory, critic2_optim: OptimizerFactory | None,
+                        max_grad_norm: float | None = None) -> None:
+        def describe_actor(actor: nn.Module) -> tuple[list[_Layer], list[nn.Parameter]]:
+            self.obs_dim = int(module_layers(actor.preprocess)[0].in_features)
+            layers, params, self.act_dim = describe_gaussian_actor(actor, self.obs_dim)
+            return layers, params
+
+        self._build_twin_critic(describe_actor=describe_actor,
+                                describe_critic=lambda net, _: describe_q_critic(net, self.obs_dim, self.act_dim), lagged=lagged,
+                                policy_optim=policy_optim, critic_optim=critic_optim, critic2_optim=critic2_optim,
+                                max_grad_norm=max_grad_norm)
+
+    def _actor_forward(self, obs: torch.Tensor, tag: str) -> tuple[list[torch.Tensor], torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
+        """policy(batch) on the device (sac.py:108-131): returns (activations, act, log_prob, sigma, noise)."""
+        B, A = obs.shape[0], self.act_dim
+        acts = self._actor.forward(obs, B, tag)
+        noise = self._noise_fn((B, A)).to(self._dev, torch.float32).contiguous()
+        act, logp, sigma = self._buf(tag + "_act", (B, A)), self._buf(tag + "_logp", B), self._buf(tag + "_sigma", (B, A))
+        call("ts_squashed_gaussian", ptr(acts[-1]), 2 * A, ptr(noise), B, A, SIGMA_MIN, SIGMA_MAX, _F32_EPS, ptr(act), ptr(logp),
+             ptr(sigma), stream_ptr(self._dev))
+        return acts, act, logp, sigma, noise
+
+    def _concat(self, obs: torch.Tensor, act: torch.Tensor, out: torch.Tensor) -> None:
+        call("ts_concat2", ptr(obs), self.obs_dim, ptr(act), self.act_dim, obs.shape[0], ptr(out), stream_ptr(self._dev))
+
+    def _q_pair(self, obs: torch.Tensor, act: torch.Tensor, tag: str, target: bool = False) -> list[list[torch.Tensor]]:
+        """Both critics (or both lagged critics) on concat(obs, act): their activation lists."""
+        B = obs.shape[0]
+        x = self._buf(f"{tag}_x", (B, self.obs_dim + self.act_dim))
+        self._concat(obs, act, x)
+        return [self._lagged_forward(k, x, B, tag) if target else self._c[k].forward(x, B, tag) for k in range(2)]
+
+    def _actor_step(self, obs: torch.Tensor, alpha: float, out_loss: torch.Tensor) -> torch.Tensor:
+        """SAC's actor step against the current critics: L = mean(alpha * log pi(a|s) - min(Q1, Q2)(s, a)) with
+        a = tanh(mu + sigma * eps) into ``out_loss``, backward through both critics' input gradients and the tanh-Gaussian
+        head, Adam.  Returns log pi(a|s)."""
+        B, A = obs.shape[0], self.act_dim
+        st = stream_ptr(self._dev)
+        a_acts, act, logp, sigma, noise = self._actor_forward(obs, "au")
+        c_acts = self._q_pair(obs, act, "aq")
+        dq1, dq2, rows = self._buf("adq1", (B, 1)), self._buf("adq2", (B, 1)), self._buf("actor_rows", B)
+        call("ts_sac_actor_q_grad", ptr(c_acts[0][-1]), ptr(c_acts[1][-1]), ptr(logp), alpha, B, ptr(dq1), ptr(dq2), ptr(rows), st)
+        call("ts_mean", ptr(rows), B, ptr(out_loss), st)
+        cols = (self.obs_dim, self.obs_dim + A)
+        dact = self._buf("dact", (B, A))            # d loss / d act of both critics, the second one accumulated
+        for k, d in enumerate((dq1, dq2)):
+            self._c[k].backward(c_acts[k], d, B, "aq", param_grads=False, input_grad=True, input_cols=cols, dx_out=dact,
+                                dx_accumulate=k == 1)
+        dhead = self._buf("dhead", (B, 2 * A))
+        call("ts_squashed_gaussian_bwd", ptr(a_acts[-1]), 2 * A, ptr(noise), ptr(act), ptr(sigma), ptr(dact), B, A,
+             SIGMA_MIN, SIGMA_MAX, _F32_EPS, alpha / B, ptr(dhead), st)
+        self._actor.backward(a_acts, dhead, B, "au")
+        self._adam(self._g_actor, self.policy_optim._optim, self.policy_optim._max_grad_norm)
+        return logp
+
+
+class SAC(ContinuousTwinCritic, OffPolicyAlgorithm):
     """Soft Actor-Critic (arXiv:1801.01290 / 1812.05905), reference API (sac.py:218-336)."""
 
     def __init__(self, *, policy: SACPolicy, policy_optim: OptimizerFactory, critic: nn.Module, critic_optim: OptimizerFactory,
@@ -201,72 +266,22 @@ class SAC(OffPolicyAlgorithm):
         self.critic2 = critic2 or deepcopy(critic)
         self.critic_old = deepcopy(self.critic).eval()
         self.critic2_old = deepcopy(self.critic2).eval()
-        dev = next(policy.actor.parameters()).device
-        if dev.type != "cuda":
-            raise UnsupportedModelError(f"networks live on {dev}; tianshou_b200 has no CPU path -- move them to a CUDA device")
-        self._dev = dev
-        first = module_layers(policy.actor.preprocess)[0]
-        self.obs_dim = int(first.in_features)
-        a_layers, a_params, self.act_dim = describe_gaussian_actor(policy.actor, self.obs_dim)
-        self._g_actor = FlatGroup(a_params, dev)
-        self._actor = FusedStack(a_layers, self._g_actor, "actor")
-        self._g_c, self._c, self._g_ct = [], [], []
-        for src, tgt in ((self.critic, self.critic_old), (self.critic2, self.critic2_old)):
-            layers, params = describe_q_critic(src, self.obs_dim, self.act_dim)
-            _, tparams = describe_q_critic(tgt, self.obs_dim, self.act_dim)
-            g = FlatGroup(params, dev)
-            self._g_c.append(g)
-            self._c.append(FusedStack(layers, g, "critic"))
-            self._g_ct.append(FlatGroup(tparams, dev))
-        self.policy_optim = self._create_optimizer(policy, policy_optim)
-        self.critic_optim = self._create_optimizer(self.critic, critic_optim)
-        self.critic2_optim = self._create_optimizer(self.critic2, critic2_optim or critic_optim)
-        for o, g in ((self.policy_optim, self._g_actor), (self.critic_optim, self._g_c[0]), (self.critic2_optim, self._g_c[1])):
-            bind_optimizer(o, g)
-        self._scratch: dict[str, torch.Tensor] = {}
-        # opt-in: the device work of one update() (~85 launches) captured once into a CUDA graph and replayed -- the eager call
+        self._build_networks(lagged=(self.critic_old, self.critic2_old), policy_optim=policy_optim, critic_optim=critic_optim,
+                             critic2_optim=critic2_optim)
+        # opt-in: the device work of one update() (~80 launches) captured once into a CUDA graph and replayed -- the eager call
         # sequence is Python-launch bound.  Needs a buffer with a device mirror, uniform replay and a fixed alpha.
         self.cuda_graph = bool(cuda_graph)
         self._graph: dict[str, Any] = {}
-        self._adam = FlatGroup.adam_step          # the graphed body switches to the device-step variant
         # rsample noise source: torch's generator on the networks' device (what the reference draws when it runs there)
+        dev = self._dev
         self._noise_fn = lambda shape: torch.normal(torch.zeros(shape, device=dev), torch.ones(shape, device=dev))
 
     # ------------------------------------------------------------------ helpers
-    def _buf(self, name: str, shape: tuple[int, ...] | int, dtype: torch.dtype = torch.float32) -> torch.Tensor:
-        shape = (shape,) if isinstance(shape, int) else tuple(shape)
-        t = self._scratch.get(name)
-        if t is None or t.shape != shape or t.dtype != dtype:
-            t = self._scratch[name] = torch.empty(shape, dtype=dtype, device=self._dev)
-        return t
-
     def _rows(self, buffer: ReplayBuffer, key: str, indices: np.ndarray | torch.Tensor) -> torch.Tensor:
         """buffer[key][indices] as a dense fp32 [I, width] device tensor: gathered from the device mirror when the
         buffer keeps one (no host traffic), else a host gather of the sampled rows + one upload."""
         from ... import ops
         return ops.buffer_rows(buffer, key, indices, self._dev, cols=self._cols_override)
-
-    def _actor_forward(self, obs: torch.Tensor, tag: str) -> tuple[list[torch.Tensor], torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
-        """policy(batch) on the device: returns (activations, act, log_prob, sigma, noise)."""
-        B, A = obs.shape[0], self.act_dim
-        acts = self._actor.forward(obs, B, tag)
-        head = acts[-1]
-        noise = self._noise_fn((B, A)).to(self._dev, torch.float32).contiguous()
-        act = self._buf(tag + "_act", (B, A))
-        logp = self._buf(tag + "_logp", B)
-        sigma = self._buf(tag + "_sigma", (B, A))
-        call("ts_squashed_gaussian", ptr(head), 2 * A, ptr(noise), B, A, SIGMA_MIN, SIGMA_MAX, _F32_EPS, ptr(act), ptr(logp),
-             ptr(sigma), stream_ptr(self._dev))
-        return acts, act, logp, sigma, noise
-
-    def _q_forward(self, k: int, obs: torch.Tensor, act: torch.Tensor, tag: str, target: bool = False) -> tuple[list[torch.Tensor], torch.Tensor]:
-        B = obs.shape[0]
-        x = self._buf(f"{tag}_x{k}", (B, self.obs_dim + self.act_dim))
-        call("ts_concat2", ptr(obs), self.obs_dim, ptr(act), self.act_dim, B, ptr(x), stream_ptr(self._dev))
-        if target:
-            self._g_ct[k].ensure_adopted()
-        acts = self._c[k].forward(x, B, tag, params=self._g_ct[k].flat if target else None)
-        return acts, acts[-1].view(B)
 
     # ------------------------------------------------------------------ target
     def _target_q(self, buffer: ReplayBuffer, indices: np.ndarray) -> torch.Tensor:
@@ -275,12 +290,13 @@ class SAC(OffPolicyAlgorithm):
             obs_next = self._rows(buffer, "obs_next", indices)
         else:
             obs_next = self._rows(buffer, "obs", buffer.next(indices))
+        obs_next = obs_next.contiguous()
         B = obs_next.shape[0]
-        _, act, logp, _, _ = self._actor_forward(obs_next.contiguous(), "tq")
-        _, q1 = self._q_forward(0, obs_next, act, "tq", target=True)
-        _, q2 = self._q_forward(1, obs_next, act, "tq", target=True)
+        _, act, logp, _, _ = self._actor_forward(obs_next, "tq")
+        t_acts = self._q_pair(obs_next, act, "tq", target=True)
         out = self._buf("tq_out", (B, 1))
-        call("ts_sac_target", ptr(q1), ptr(q2), ptr(logp), float(self.alpha.value), B, ptr(out), stream_ptr(self._dev))
+        call("ts_sac_target", ptr(t_acts[0][-1]), ptr(t_acts[1][-1]), ptr(logp), float(self.alpha.value), B, ptr(out),
+             stream_ptr(self._dev))
         return out
 
     def _preprocess_batch(self, batch: Batch, buffer: ReplayBuffer, indices: np.ndarray) -> Batch:
@@ -293,64 +309,45 @@ class SAC(OffPolicyAlgorithm):
         batch = Batch()
         batch.__dict__["obs"] = self._rows(buffer, "obs", indices).contiguous()
         batch.__dict__["act"] = self._rows(buffer, "act", indices).contiguous()
-        if hasattr(buffer, "get_weight"):          # PrioritizedReplayBuffer.__getitem__ adds the IS weight (prio.py:104-106)
-            w = buffer.get_weight(indices)
-            batch.__dict__["weight"] = to_device(np.asarray(w / np.max(w) if buffer._weight_norm else w, dtype=np.float32), self._dev)
+        weight = per_weight(buffer, indices, self._dev)
+        if weight is not None:
+            batch.__dict__["weight"] = weight
         batch.__dict__["info"] = Batch()
         return batch, indices
 
     # ------------------------------------------------------------------ update
-    def _critic_step(self, k: int, obs: torch.Tensor, act: torch.Tensor, returns: torch.Tensor, weight: torch.Tensor | None,
-                     optim: Any, out_loss: torch.Tensor) -> torch.Tensor:
-        """``_minimize_critic_squared_loss`` (ddpg.py:267-285): forward, weighted MSE, backward, Adam."""
-        B = obs.shape[0]
+    def _critic_step(self, k: int, x: torch.Tensor, returns: torch.Tensor, weight: torch.Tensor | None, optim: Any,
+                     out_loss: torch.Tensor) -> torch.Tensor:
+        """``_minimize_critic_squared_loss`` (ddpg.py:267-285) on the critic input x = concat(obs, act): forward, weighted
+        MSE, backward, Adam."""
+        B = x.shape[0]
         st = stream_ptr(self._dev)
-        acts, q = self._q_forward(k, obs, act, "cu")
+        acts = self._c[k].forward(x, B, "cu")
         td = self._buf(f"td{k}", B)
         dq = self._buf("dq", (B, 1))
         rows = self._buf("loss_rows", B)
-        call("ts_critic_mse", ptr(q), ptr(returns), ptr(weight), B, ptr(td), ptr(dq), ptr(rows), st)
+        call("ts_critic_mse", ptr(acts[-1]), ptr(returns), ptr(weight), B, ptr(td), ptr(dq), ptr(rows), st)
         call("ts_mean", ptr(rows), B, ptr(out_loss), st)
         self._c[k].backward(acts, dq, B, "cu")
         self._adam(self._g_c[k], optim._optim, optim._max_grad_norm)
         return td
 
     def _update_with_batch(self, batch: Batch) -> SACTrainingStats:
-        dev, st = self._dev, stream_ptr(self._dev)
+        dev = self._dev
         obs, act = batch.obs, batch.act
-        B, A = obs.shape[0], self.act_dim
+        B = obs.shape[0]
         returns = batch.returns.reshape(-1).to(dev, torch.float32).contiguous()
-        weight = getattr(batch, "weight", None)
-        if weight is not None and not isinstance(weight, torch.Tensor):
-            weight = to_device(np.asarray(weight, dtype=np.float32), dev)
-        if weight is not None:
-            weight = weight.reshape(-1).to(dev, torch.float32).contiguous()
+        weight = pop_batch_weight(batch, dev)
         losses = self._buf("losses", 3)
-        td1 = self._critic_step(0, obs, act, returns, weight, self.critic_optim, losses[0:1])
-        td2 = self._critic_step(1, obs, act, returns, weight, self.critic2_optim, losses[1:2])
+        x = self._buf("cu_x", (B, self.obs_dim + self.act_dim))
+        self._concat(obs, act, x)
+        td1 = self._critic_step(0, x, returns, weight, self.critic_optim, losses[0:1])
+        td2 = self._critic_step(1, x, returns, weight, self.critic2_optim, losses[1:2])
         batch.weight = (td1 + td2) / 2.0       # prio-buffer
 
-        # actor: L = mean(alpha * log pi(a|s) - min(Q1, Q2)(s, a)),  a = tanh(mu + sigma * eps)
-        alpha = float(self.alpha.value)
-        a_acts, new_act, logp, sigma, noise = self._actor_forward(obs, "au")
-        c1_acts, q1a = self._q_forward(0, obs, new_act, "aq0")
-        c2_acts, q2a = self._q_forward(1, obs, new_act, "aq1")
-        dq1, dq2, rows = self._buf("dq1", (B, 1)), self._buf("dq2", (B, 1)), self._buf("loss_rows", B)
-        call("ts_sac_actor_q_grad", ptr(q1a), ptr(q2a), ptr(logp), alpha, B, ptr(dq1), ptr(dq2), ptr(rows), st)
-        call("ts_mean", ptr(rows), B, ptr(losses[2:3]), st)
-        cols = (self.obs_dim, self.obs_dim + A)
-        da1 = self._c[0].backward(c1_acts, dq1, B, "aq0", param_grads=False, input_grad=True, input_cols=cols)
-        da2 = self._c[1].backward(c2_acts, dq2, B, "aq1", param_grads=False, input_grad=True, input_cols=cols)
-        dact = da1 + da2
-        dhead = self._buf("dhead", (B, 2 * A))
-        call("ts_squashed_gaussian_bwd", ptr(a_acts[-1]), 2 * A, ptr(noise), ptr(new_act), ptr(sigma), ptr(dact), B, A,
-             SIGMA_MIN, SIGMA_MAX, _F32_EPS, alpha / B, ptr(dhead), st)
-        self._actor.backward(a_acts, dhead, B, "au")
-        self._adam(self._g_actor, self.policy_optim._optim, self.policy_optim._max_grad_norm)
-
+        logp = self._actor_step(obs, float(self.alpha.value), losses[2:3])
         alpha_loss = None if self._in_graph_body else self.alpha.update(-logp.detach().unsqueeze(-1))
-        for k in range(2):                      # _update_lagged_network_weights
-            polyak_update(self._g_ct[k], self._g_c[k], self.tau)
+        self._polyak()
         if self._in_graph_body:
             return None                         # the losses stay on the device; update() reads them after the replay
         l = losses.cpu().numpy()                # the only host sync of the update
