@@ -62,6 +62,19 @@ __host__ __device__ inline int64_t imin(int64_t a, int64_t b) { return a < b ? a
 __device__ __forceinline__ int lane_id() { return threadIdx.x & 31; }
 __device__ __forceinline__ int warp_id() { return threadIdx.x >> 5; }
 
+// Butterfly reductions over the warp: every lane ends with the same value, and the order of the operations is fixed by the
+// lane pattern alone, so the result is bit-identical from run to run.
+__device__ __forceinline__ float warp_sum(float v) {
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
+    return v;
+}
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, off));
+    return v;
+}
+
 __device__ __forceinline__ double shfl_down_f64(double v, int d) {
     return __shfl_down_sync(0xffffffffu, v, d);
 }

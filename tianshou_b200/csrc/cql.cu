@@ -75,13 +75,6 @@ __global__ void __launch_bounds__(kThreads) cql_rows_kernel(
     }
 }
 
-// Butterfly sum over the warp: the order of the additions is fixed by the lane pattern, so the result is bit-identical from
-// run to run.
-__device__ __forceinline__ float warp_sum(float v) {
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-
 constexpr int kLossThreads = 1024;
 constexpr int kSums = 6;
 
@@ -110,14 +103,14 @@ __global__ void __launch_bounds__(kLossThreads) cql_losses_kernel(
     }
 #pragma unroll
     for (int k = 0; k < kSums; ++k) {
-        const float v = warp_sum(acc[k]);
+        const float v = tsb::warp_sum(acc[k]);
         if (tsb::lane_id() == 0) part[k][tsb::warp_id()] = v;
     }
     __syncthreads();
     if (tsb::warp_id() != 0) return;
     float tot[kSums];
 #pragma unroll
-    for (int k = 0; k < kSums; ++k) tot[k] = warp_sum(part[k][tsb::lane_id()]);
+    for (int k = 0; k < kSums; ++k) tot[k] = tsb::warp_sum(part[k][tsb::lane_id()]);
     if (tsb::lane_id() != 0) return;
     float pen[2], loss[2];
     for (int k = 0; k < 2; ++k) {

@@ -16,17 +16,6 @@ namespace {
 constexpr int kThreads = 256;
 constexpr int kRowsPerBlock = kThreads / 32;      // one warp per row
 
-// Butterfly reductions over the warp: every lane ends with the same value, and the order of the additions is fixed by the
-// lane pattern alone, so the result is bit-identical from run to run.
-__device__ __forceinline__ float warp_max(float v) {
-    for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-    return v;
-}
-__device__ __forceinline__ float warp_sum(float v) {
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-
 // Per row b, with z = logits[b], m = min(q1[b], q2[b]), p = softmax(z), log p = z - logsumexp(z):
 //   probs[b]   = p
 //   entropy[b] = H = -sum_a clamp(log p_a, -FLT_MAX) * p_a
@@ -45,10 +34,10 @@ __global__ void __launch_bounds__(kThreads) discrete_sac_rows_kernel(
         float* p_out = probs + b * A;
         float mx = -INFINITY;
         for (int a = lane; a < A; a += 32) mx = fmaxf(mx, z[a]);
-        mx = warp_max(mx);
+        mx = tsb::warp_max(mx);
         float s = 0.0f;
         for (int a = lane; a < A; a += 32) s += expf(z[a] - mx);
-        s = warp_sum(s);
+        s = tsb::warp_sum(s);
         // torch.logsumexp: log(sum(exp(z - max))) + max, with an infinite max replaced by 0 in the final add
         const float lse = logf(s) + (isinf(mx) ? 0.0f : mx);
         float plogp = 0.0f, pm = 0.0f;
@@ -59,8 +48,8 @@ __global__ void __launch_bounds__(kThreads) discrete_sac_rows_kernel(
             plogp += lp * p;
             pm += p * fminf(qa[a], qb[a]);
         }
-        const float H = -warp_sum(plogp);
-        const float S = warp_sum(pm);
+        const float H = -tsb::warp_sum(plogp);
+        const float S = tsb::warp_sum(pm);
         if (lane == 0) {
             entropy[b] = H;
             v[b] = S + alpha * H;

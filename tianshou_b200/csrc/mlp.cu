@@ -19,6 +19,8 @@
 #include <stdlib.h>
 
 #include "common.cuh"
+#include "optim_math.cuh"
+#include "ppo_math.cuh"
 
 namespace {
 
@@ -207,53 +209,6 @@ __device__ __forceinline__ NetGlobal critic_global(const ts_actor_critic_desc& d
     return NetGlobal{d.c_w1, d.c_b1, d.c_w2, d.c_b2, d.c_w3, d.c_b3, 0};
 }
 
-// log N(x; mu, sigma) summed over the action dims, torch.distributions.Normal.log_prob order:
-//   -((x-mu)^2) / (2 var) - log(sigma) - log(sqrt(2 pi))
-__device__ __forceinline__ float normal_logp_term(float x, float mu, float sigma) {
-    const float var = sigma * sigma;
-    const float diff = x - mu;
-    return -(diff * diff) / (2.0f * var) - logf(sigma) - 0.9189385332046727f;
-}
-
-// Categorical head exactly as the reference builds it (DiscreteActor(softmax_output=True) -> torch.distributions.
-// Categorical(probs), utils/net/discrete.py:69-92, reinforce.py:167-192): p = softmax(z); Categorical renormalises
-// (pn = p / sum p) and takes logits = log(clamp(pn, eps, 1 - eps)); log_prob gathers, entropy = -sum pn * logits.
-// fwd: returns log_prob(action) and the row entropy; keeps p, pn, lg for the backward.
-struct CatRow { float p[kMaxAct], pn[kMaxAct], lg[kMaxAct]; float s2; };
-__device__ __forceinline__ void categorical_forward(const float* z, int A, int action, CatRow& c, float& logp, float& ent) {
-    constexpr float eps = 1.1920928955078125e-07f;   // torch.finfo(float32).eps
-    float m = z[0];
-    for (int a = 1; a < A; ++a) m = fmaxf(m, z[a]);
-    float s = 0.0f;
-    for (int a = 0; a < A; ++a) { c.p[a] = expf(z[a] - m); s += c.p[a]; }
-    float s2 = 0.0f;
-    for (int a = 0; a < A; ++a) { c.p[a] = c.p[a] / s; s2 += c.p[a]; }
-    c.s2 = s2;
-    ent = 0.0f;
-    for (int a = 0; a < A; ++a) {
-        c.pn[a] = c.p[a] / s2;
-        c.lg[a] = logf(fminf(fmaxf(c.pn[a], eps), 1.0f - eps));
-        ent -= c.pn[a] * c.lg[a];
-    }
-    logp = (action >= 0 && action < A) ? c.lg[action] : 0.0f;
-}
-// bwd: dz[a] = d loss / d logit a given gl = d loss / d log_prob and ge = d loss / d entropy (autograd's chain:
-// gather + entropy -> log o clamp -> renormalisation -> softmax)
-__device__ __forceinline__ void categorical_backward(const CatRow& c, int A, int action, float gl, float ge, float* dz) {
-    constexpr float eps = 1.1920928955078125e-07f;
-    float dpn[kMaxAct];
-    float dot = 0.0f;
-    for (int a = 0; a < A; ++a) {
-        const float dlg = (a == action ? gl : 0.0f) - ge * c.pn[a];
-        const bool pass = c.pn[a] >= eps && c.pn[a] <= 1.0f - eps;        // clamp backward
-        dpn[a] = -ge * c.lg[a] + (pass ? dlg / c.pn[a] : 0.0f);
-        dot += dpn[a] * c.pn[a];
-    }
-    float dot2 = 0.0f;
-    for (int a = 0; a < A; ++a) { dpn[a] = (dpn[a] - dot) / c.s2; dot2 += dpn[a] * c.p[a]; }   // now d/dp
-    for (int a = 0; a < A; ++a) dz[a] = c.p[a] * (dpn[a] - dot2);
-}
-
 // ---- kernels --------------------------------------------------------------------------------
 __global__ void __launch_bounds__(kThreads, 1) critic_forward_kernel(
     const float* __restrict__ params, const ts_actor_critic_desc d, const float* __restrict__ obs0,
@@ -304,9 +259,9 @@ __global__ void __launch_bounds__(kThreads, 1) actor_logp_kernel(
             const int r = threadIdx.x;
             float z[kMaxAct];
             for (int a = 0; a < A; ++a) z[a] = sm[L.H1 + r * LDH + a];
-            CatRow c;
+            ppo::CatT<kMaxAct> c;
             float lp, ent;
-            categorical_forward(z, A, (int)sm[L.ACT + r * kMaxAct], c, lp, ent);
+            ppo::cat_forward(z, A, (int)sm[L.ACT + r * kMaxAct], c, lp, ent);
             if (mu_out) for (int a = 0; a < A; ++a) mu_out[(row0 + r) * A + a] = c.p[a];   // the actor's output: probabilities
             logp_out[row0 + r] = lp;
         } else if (threadIdx.x < nrows) {
@@ -315,7 +270,7 @@ __global__ void __launch_bounds__(kThreads, 1) actor_logp_kernel(
             for (int a = 0; a < A; ++a) {
                 const float sigma = expf(sm[L.actor.ls + a]);
                 const float mu = sm[L.H1 + r * LDH + a];
-                lp += normal_logp_term(sm[L.ACT + r * kMaxAct + a], mu, sigma);
+                lp += ppo::normal_logp_term(sm[L.ACT + r * kMaxAct + a], mu, sigma);
                 if (mu_out) mu_out[(row0 + r) * A + a] = mu;
             }
             logp_out[row0 + r] = lp;
@@ -460,12 +415,7 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_grad_kernel(
     // (c_w1 == a_w1, ...): both backward passes add into the same gradient slots of this CTA's row.
     stage_net(sm, L.actor, params, ga, d.obs_dim, L.KX, A, true, !categorical);
     stage_net(sm, L.critic, params, gc, d.obs_dim, L.KX, 1, true, false);
-    const float inv_b = 1.0f / (float)global_rows;
-    const float eps_clip = (float)hp.eps_clip, lo_c = (float)(1.0 - hp.eps_clip), hi_c = (float)(1.0 + hp.eps_clip);
-    const float vf_coef = (float)hp.vf_coef, ent_coef = (float)hp.ent_coef, adv_eps = (float)hp.adv_eps;
-    const float dual_clip = (float)hp.dual_clip;
-    float adv_mean = 0.0f, adv_std = 1.0f;
-    if (hp.advantage_normalization && adv_moments) { adv_mean = adv_moments[0]; adv_std = adv_moments[1]; }
+    const ppo::Scalars sc = ppo::make_scalars(hp, global_rows, adv_moments);
     float* rowv = sm + L.ROWV;  // [0]=adv [1]=ret [2]=logp_old [3]=v_s, each kRows
     const int64_t B = hi - lo;
     const int64_t tiles = (B + kRows - 1) / kRows;
@@ -490,28 +440,8 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_grad_kernel(
         float vf_row = 0.0f;
         if (tid < kRows) {
             float dv = 0.0f;
-            if (tid < nrows) {
-                const float value = head_dot(sm, L, L.critic, tid, 0);
-                const float R = rowv[kRows + tid];
-                float g;  // d vf / d value
-                if (hp.value_clip) {           // ppo.py:199-206
-                    const float vs = rowv[3 * kRows + tid];
-                    const float dlt = value - vs;
-                    const float dcl = fminf(fmaxf(dlt, -eps_clip), eps_clip);
-                    const float v_clip = vs + dcl;
-                    const float e1 = R - value, e2 = R - v_clip;
-                    const float vf1 = e1 * e1, vf2 = e2 * e2;
-                    vf_row = fmaxf(vf1, vf2);
-                    const float in_range = (dlt >= -eps_clip && dlt <= eps_clip) ? 1.0f : 0.0f;
-                    const float g1 = -2.0f * e1, g2 = -2.0f * e2 * in_range;
-                    g = (vf1 > vf2) ? g1 : ((vf1 < vf2) ? g2 : 0.5f * (g1 + g2));
-                } else {
-                    const float e1 = R - value;
-                    vf_row = e1 * e1;
-                    g = -2.0f * e1;
-                }
-                dv = vf_coef * inv_b * g;
-            }
+            if (tid < nrows)
+                ppo::critic_row(sc, head_dot(sm, L, L.critic, tid, 0), rowv[kRows + tid], rowv[3 * kRows + tid], vf_row, dv);
             sm[L.DOUT + tid * LDO] = dv;
         }
         __syncthreads();
@@ -525,45 +455,20 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_grad_kernel(
         }
         __syncthreads();
         float clip_row = 0.0f, ent_row = 0.0f;
-        // PPO surrogate of one row: objective value and d loss / d log_prob           (ppo.py:184-196)
-        auto surrogate = [&](int r, float lp, float& obj) -> float {
-            float Adv = rowv[r];
-            if (hp.loss_kind == TS_LOSS_A2C) {     // a2c.py:262-266: actor_loss = -(log_prob * adv).mean()
-                obj = lp * Adv;
-                return -inv_b * Adv;
-            }
-            if (hp.advantage_normalization) Adv = (Adv - adv_mean) / (adv_std + adv_eps);
-            const float ratio = expf(lp - rowv[2 * kRows + r]);
-            const float rc = fminf(fmaxf(ratio, lo_c), hi_c);
-            const bool in_range = (ratio >= lo_c) && (ratio <= hi_c);
-            const float surr1 = ratio * Adv, surr2 = rc * Adv;
-            // d min(surr1, surr2) / d ratio with torch's tie rule (half to each branch)
-            float g_ratio;
-            if (surr1 < surr2) g_ratio = Adv;
-            else if (surr1 > surr2) g_ratio = in_range ? Adv : 0.0f;
-            else g_ratio = in_range ? Adv : 0.5f * Adv;
-            const float clip1 = fminf(surr1, surr2);
-            obj = clip1;
-            if (dual_clip > 0.0f && Adv < 0.0f) {   // ppo.py:191-194
-                const float c2 = dual_clip * Adv;
-                obj = fmaxf(clip1, c2);
-                if (clip1 < c2) g_ratio = 0.0f; else if (clip1 == c2) g_ratio *= 0.5f;
-            }
-            return -inv_b * g_ratio * ratio;
-        };
         if (tid < kRows && categorical) {
             const int r = tid;
             float z[kMaxAct], dz[kMaxAct];
             for (int a = 0; a < A; ++a) z[a] = sm[L.DOUT + r * LDO + a];
             const int action = (int)sm[L.ACT + r * kMaxAct];
-            CatRow c;
+            ppo::CatT<kMaxAct> c;
             float lp, ent;
-            categorical_forward(z, A, action, c, lp, ent);
+            ppo::cat_forward(z, A, action, c, lp, ent);
             for (int a = 0; a < A; ++a) dz[a] = 0.0f;
             if (r < nrows) {
-                const float gl = surrogate(r, lp, clip_row);
+                float gl;
+                ppo::actor_row(sc, lp, rowv[2 * kRows + r], rowv[r], clip_row, gl);
                 ent_row = ent;
-                categorical_backward(c, A, action, gl, -ent_coef * inv_b, dz);
+                ppo::cat_backward(c, A, action, gl, -sc.ent_coef * sc.inv_b, dz);
             }
             for (int a = 0; a < A; ++a) sm[L.DOUT + r * LDO + a] = dz[a];
         } else if (tid < kRows) {
@@ -576,18 +481,15 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_grad_kernel(
                 if (a < A) {
                     sig[a] = expf(sm[L.actor.ls + a]);
                     mu[a] = sm[L.DOUT + r * LDO + a];
-                    lp += normal_logp_term(sm[L.ACT + r * kMaxAct + a], mu[a], sig[a]);
+                    lp += ppo::normal_logp_term(sm[L.ACT + r * kMaxAct + a], mu[a], sig[a]);
                 }
             }
-            if (r < nrows) gl = surrogate(r, lp, clip_row);
+            if (r < nrows) ppo::actor_row(sc, lp, rowv[2 * kRows + r], rowv[r], clip_row, gl);
 #pragma unroll
             for (int a = 0; a < kMaxAct; ++a) {
-                if (a < A) {
-                    const float diff = sm[L.ACT + r * kMaxAct + a] - mu[a];
-                    const float var = sig[a] * sig[a];
-                    sm[L.DOUT + r * LDO + a] = gl * diff / var;                        // d/d mu
-                    sm[L.DOUT + r * LDO + 16 + a] = gl * (diff * diff / var - 1.0f);  // d/d logstd
-                }
+                if (a < A)
+                    ppo::normal_backward(sm[L.ACT + r * kMaxAct + a], mu[a], sig[a], gl, sm[L.DOUT + r * LDO + a],
+                                         sm[L.DOUT + r * LDO + 16 + a]);
             }
         }
         __syncthreads();
@@ -595,7 +497,7 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_grad_kernel(
         if (tid < A && !categorical) {
             float s = 0.0f;
             for (int r = 0; r < kRows; ++r) s += sm[L.DOUT + r * LDO + 16 + tid];
-            s += -ent_coef * inv_b * (float)nrows;   // d(-ent_coef * mean(entropy))/d logstd
+            s += -sc.ent_coef * sc.inv_b * (float)nrows;   // d(-ent_coef * mean(entropy))/d logstd
             atomicAdd(grad + d.a_logstd + tid, s);
         }
         trunk_backward(sm, L, L.actor, ga, A, d.obs_dim, grad, relu);
@@ -605,8 +507,8 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_grad_kernel(
         const float s_vf = block_sum_128(tid < kRows ? vf_row : 0.0f, sm + L.RED);
         const float s_ent = block_sum_128(tid < kRows ? ent_row : 0.0f, sm + L.RED);      // categorical: per-row entropies
         if (tid == 0) {
-            float ent = 0.0f;   // Normal entropy: 0.5 + 0.5 log(2 pi) + log(sigma), summed over dims
-            if (!categorical) for (int a = 0; a < A; ++a) ent += 1.4189385332046727f + logf(expf(sm[L.actor.ls + a]));
+            float ent = 0.0f;   // Normal entropy summed over dims
+            if (!categorical) for (int a = 0; a < A; ++a) ent += ppo::normal_entropy_term(expf(sm[L.actor.ls + a]));
             float* ex = grad + d.n_params;
             atomicAdd(ex + 0, s_clip);
             atomicAdd(ex + 1, s_vf);
@@ -638,7 +540,8 @@ __global__ void __launch_bounds__(kAdamElems * kAdamGroups) clip_adam_kernel(
     AdamCtl& ctl = g_adam_ctl[ctl_slot];
     __shared__ double s_red[8];
     __shared__ float s_part[kAdamGroups][kAdamElems];
-    __shared__ float s_coef, s_norm, s_step_size, s_bc2_sqrt;
+    __shared__ float s_coef, s_norm;
+    __shared__ optim::AdamBias s_bias;
     const int tid = threadIdx.x, e = tid & (kAdamElems - 1), q = tid >> 8;
     const int64_t step = *step_count + 1;
     const int64_t width = n_params + TS_PPO_GRAD_EXTRA;
@@ -679,53 +582,31 @@ __global__ void __launch_bounds__(kAdamElems * kAdamGroups) clip_adam_kernel(
         while (*((volatile unsigned int*)&ctl.arrive) < gridDim.x) {}
         __threadfence();
         const float total_norm = (float)sqrt(*((volatile double*)&ctl.ss));
-        float coef = 1.0f;
-        if (hp.max_grad_norm > 0.0) {   // torch.nn.utils.clip_grad_norm_
-            coef = (float)hp.max_grad_norm / (total_norm + 1e-6f);
-            coef = fminf(coef, 1.0f);
-        }
-        s_coef = coef; s_norm = total_norm;
-        if (hp.optimizer != TS_OPT_RMSPROP) {       // RMSprop has no bias correction
-            const double bc1 = 1.0 - pow(hp.beta1, (double)step);
-            const double bc2 = 1.0 - pow(hp.beta2, (double)step);
-            s_step_size = (float)(hp.lr / bc1);
-            s_bc2_sqrt = (float)sqrt(bc2);
-        }
+        s_coef = hp.max_grad_norm > 0.0 ? optim::clip_coef((float)hp.max_grad_norm, total_norm) : 1.0f;
+        s_norm = total_norm;
+        if (hp.optimizer != TS_OPT_RMSPROP) s_bias = optim::adam_bias(hp.lr, hp.beta1, hp.beta2, step);   // RMSprop has no bias correction
     }
     __syncthreads();
-    const float coef = s_coef, step_size = s_step_size, bc2_sqrt = s_bc2_sqrt;
+    const float coef = s_coef, step_size = s_bias.step_size, bc2_sqrt = s_bias.bc2_sqrt;
     const float w1 = (float)(1.0 - hp.beta1), w2 = (float)(1.0 - hp.beta2);
     const float beta2 = (float)hp.beta2, adam_eps = (float)hp.adam_eps, wd = (float)hp.weight_decay;
     if (hp.optimizer == TS_OPT_RMSPROP) {
-        if (q == 0 && i < n_params) {
-            g *= coef;
-            float p = params[i];
-            if (wd != 0.0f) g = fmaf(wd, p, g);
-            float v = exp_avg_sq[i];
-            v = v * beta2 + w2 * g * g;             // square_avg.mul_(alpha).addcmul_(grad, grad, 1 - alpha): beta2 holds alpha
-            p = p - (float)hp.lr * (g / (sqrtf(v) + adam_eps));         // addcdiv_(grad, square_avg.sqrt().add_(eps), -lr)
+        if (q == 0 && i < n_params) {               // beta2 holds alpha
+            float p = params[i], v = exp_avg_sq[i];
+            optim::rmsprop_elem(g * coef, p, v, (float)hp.lr, beta2, w2, adam_eps, wd);
             exp_avg_sq[i] = v; params[i] = p;
         }
     } else if (q == 0 && i < n_params) {
-        g *= coef;
-        float p = params[i];
-        if (wd != 0.0f) g = fmaf(wd, p, g);
-        float m = exp_avg[i], v = exp_avg_sq[i];
-        m = m + w1 * (g - m);                       // exp_avg.lerp_(grad, 1 - beta1)
-        v = v * beta2 + w2 * g * g;                 // mul_(beta2).addcmul_(grad, grad, 1 - beta2)
-        const float denom = sqrtf(v) / bc2_sqrt + adam_eps;
-        p = p - step_size * (m / denom);            // addcdiv_(exp_avg, denom, -step_size)
+        float p = params[i], m = exp_avg[i], v = exp_avg_sq[i];
+        optim::adam_elem(g * coef, p, m, v, step_size, bc2_sqrt, beta2, w1, w2, adam_eps, wd);
         exp_avg[i] = m; exp_avg_sq[i] = v; params[i] = p;
     }
     if (tid == 0) {
         if (blockIdx.x == 0) {
             const float e0 = __ldcg(grad + n_params), e1 = __ldcg(grad + n_params + 1);
             const float e2 = __ldcg(grad + n_params + 2), e3 = __ldcg(grad + n_params + 3);
-            const float rows = e3 > 0.0f ? e3 : 1.0f;
-            const float clip_loss = -e0 / rows, vf_loss = e1 / rows, ent_loss = e2 / rows;
             if (stats_row) {
-                stats_row[0] = clip_loss + (float)hp.vf_coef * vf_loss - (float)hp.ent_coef * ent_loss;
-                stats_row[1] = clip_loss; stats_row[2] = vf_loss; stats_row[3] = ent_loss;
+                ppo::loss_row(e0, e1, e2, e3 > 0.0f ? e3 : 1.0f, hp, stats_row);
                 stats_row[4] = s_norm; stats_row[5] = e3; stats_row[6] = 0.0f; stats_row[7] = 0.0f;
             }
             *step_count = step;
@@ -748,11 +629,30 @@ __global__ void grad_reduce_kernel(const float* __restrict__ partials, int n_par
     grad[i] = ((acc[0] + acc[1]) + (acc[2] + acc[3])) + ((acc[4] + acc[5]) + (acc[6] + acc[7]));
 }
 
-// One row: std 0, where torch's adv.std() of a single element is NaN (see DESIGN.md section 4).
-__global__ void adv_finalize_kernel(const double* __restrict__ sums, int64_t n, float* __restrict__ out) {
-    if (threadIdx.x != 0) return;
-    const double mean = sums[0] / (double)n;
-    double var = (sums[1] - sums[0] * mean) / (double)(n > 1 ? n - 1 : 1);   // unbiased (torch .std())
+// (sum, sum of squares) in f64 of adv over the positions [lo, hi) (through perm when given), in a fixed summation order that
+// depends on blockDim.x alone; the result is valid in thread 0
+__device__ __forceinline__ void adv_block_sums(const float* __restrict__ adv, const int32_t* __restrict__ perm, int64_t lo, int64_t hi,
+                                               double& x, double& y) {
+    __shared__ double s1[32], s2[32];
+    double a = 0.0, b = 0.0;
+    for (int64_t p = lo + threadIdx.x; p < hi; p += blockDim.x) {
+        const double v = adv[perm ? (int64_t)perm[p] : p];
+        a += v; b += v * v;
+    }
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) { a += tsb::shfl_xor_f64(a, off); b += tsb::shfl_xor_f64(b, off); }
+    if ((threadIdx.x & 31) == 0) { s1[threadIdx.x >> 5] = a; s2[threadIdx.x >> 5] = b; }
+    __syncthreads();
+    x = 0.0; y = 0.0;
+    if (threadIdx.x == 0)
+        for (int w = 0; w < (int)(blockDim.x >> 5); ++w) { x += s1[w]; y += s2[w]; }
+}
+
+// (mean, unbiased std) of n values from their (sum, sum of squares), as torch's adv.mean() / adv.std().  One row: std 0,
+// where torch's adv.std() of a single element is NaN (see DESIGN.md section 4).
+__device__ __forceinline__ void moments_from_sums(double x, double y, int64_t n, float* __restrict__ out) {
+    const double mean = x / (double)n;
+    double var = (y - x * mean) / (double)(n > 1 ? n - 1 : 1);
     if (var < 0.0) var = 0.0;
     out[0] = (float)mean; out[1] = (float)sqrt(var);
 }
@@ -762,61 +662,29 @@ __global__ void adv_finalize_kernel(const double* __restrict__ sums, int64_t n, 
 __global__ void __launch_bounds__(1024) epoch_adv_moments_kernel(const float* __restrict__ adv, const int32_t* __restrict__ perm,
                                                                  int64_t lo0, int64_t mb_size, int64_t end, int n_mb,
                                                                  float* __restrict__ out) {
-    __shared__ double s1[32], s2[32];
     const int m = blockIdx.x;
     const int64_t lo = lo0 + (int64_t)m * mb_size, hi = m == n_mb - 1 ? end : lo + mb_size;
-    double a = 0.0, b = 0.0;
-    for (int64_t p = lo + threadIdx.x; p < hi; p += blockDim.x) {
-        const double v = adv[perm ? (int64_t)perm[p] : p];
-        a += v; b += v * v;
-    }
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) { a += tsb::shfl_xor_f64(a, off); b += tsb::shfl_xor_f64(b, off); }
-    if ((threadIdx.x & 31) == 0) { s1[threadIdx.x >> 5] = a; s2[threadIdx.x >> 5] = b; }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double x = 0.0, y = 0.0;
-        for (int w = 0; w < (int)(blockDim.x >> 5); ++w) { x += s1[w]; y += s2[w]; }
-        const int64_t n = hi - lo;
-        const double mean = x / (double)n;
-        double var = (y - x * mean) / (double)(n > 1 ? n - 1 : 1);
-        if (var < 0.0) var = 0.0;
-        out[2 * m] = (float)mean; out[2 * m + 1] = (float)sqrt(var);
-    }
+    double x, y;
+    adv_block_sums(adv, perm, lo, hi, x, y);
+    if (threadIdx.x == 0) moments_from_sums(x, y, hi - lo, out + 2 * m);
 }
 
 // multi-GPU variant: per-minibatch (sum, sum of squares) in f64 -> all-reduce on the host side -> finalize
 __global__ void __launch_bounds__(1024) epoch_adv_sums_kernel(const float* __restrict__ adv, const int32_t* __restrict__ perm,
                                                               int64_t lo0, int64_t mb_size, int64_t end, int n_mb,
                                                               double* __restrict__ sums) {
-    __shared__ double s1[32], s2[32];
     const int m = blockIdx.x;
     const int64_t lo = lo0 + (int64_t)m * mb_size, hi = m == n_mb - 1 ? end : lo + mb_size;
-    double a = 0.0, b = 0.0;
-    for (int64_t p = lo + threadIdx.x; p < hi; p += blockDim.x) {
-        const double v = adv[perm ? (int64_t)perm[p] : p];
-        a += v; b += v * v;
-    }
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) { a += tsb::shfl_xor_f64(a, off); b += tsb::shfl_xor_f64(b, off); }
-    if ((threadIdx.x & 31) == 0) { s1[threadIdx.x >> 5] = a; s2[threadIdx.x >> 5] = b; }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double x = 0.0, y = 0.0;
-        for (int w = 0; w < (int)(blockDim.x >> 5); ++w) { x += s1[w]; y += s2[w]; }
-        sums[2 * m] = x; sums[2 * m + 1] = y;
-    }
+    double x, y;
+    adv_block_sums(adv, perm, lo, hi, x, y);
+    if (threadIdx.x == 0) { sums[2 * m] = x; sums[2 * m + 1] = y; }
 }
 __global__ void epoch_adv_finalize_kernel(const double* __restrict__ sums, int64_t lo0, int64_t mb_size, int64_t end, int n_mb,
                                           int world, float* __restrict__ out) {
     const int m = blockIdx.x * blockDim.x + threadIdx.x;
     if (m >= n_mb) return;
     const int64_t lo = lo0 + (int64_t)m * mb_size, hi = m == n_mb - 1 ? end : lo + mb_size;
-    const int64_t n = (hi - lo) * world;
-    const double mean = sums[2 * m] / (double)n;
-    double var = (sums[2 * m + 1] - sums[2 * m] * mean) / (double)(n > 1 ? n - 1 : 1);
-    if (var < 0.0) var = 0.0;
-    out[2 * m] = (float)mean; out[2 * m + 1] = (float)sqrt(var);
+    moments_from_sums(sums[2 * m], sums[2 * m + 1], (hi - lo) * world, out + 2 * m);
 }
 
 // ---- keyed bijection of [0, n): balanced Feistel on an even number of bits + cycle walking ----
@@ -976,7 +844,8 @@ extern "C" int ts_minibatch_adv_sums(const float* adv, const int32_t* perm, int6
 extern "C" int ts_adv_moments_finalize(const double* sums, int64_t global_rows, float* out,
                                        ts_stream_t stream) {
     TS_REQUIRE(sums && out && global_rows > 0, "ts_adv_moments_finalize: bad arguments");
-    adv_finalize_kernel<<<1, 32, 0, tsb::as_stream(stream)>>>(sums, global_rows, out);
+    // one minibatch [0, global_rows) of one rank
+    epoch_adv_finalize_kernel<<<1, 128, 0, tsb::as_stream(stream)>>>(sums, 0, global_rows, global_rows, 1, 1, out);
     return tsb::check_launch("ts_adv_moments_finalize");
 }
 

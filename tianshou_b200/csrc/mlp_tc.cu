@@ -28,6 +28,7 @@
 #include <type_traits>
 
 #include "common.cuh"
+#include "optim_math.cuh"
 #include "ppo_math.cuh"
 #include "wgmma.cuh"
 
@@ -65,27 +66,12 @@ struct Mat {
     uint32_t RS;     // bytes between 8-row groups (= cols/8 * 128)
 };
 __host__ __device__ constexpr uint32_t mat_bytes(int rows, int cols) { return (uint32_t)rows * cols * 2u; }
-__device__ __forceinline__ uint32_t moff(uint32_t r, uint32_t c, uint32_t RS) {
-    return (r >> 3) * RS + (c >> 3) * 128u + (r & 7u) * 16u + (c & 7u) * 2u;
-}
-
-// x = b0 + b1 + b2 with three bf16 pieces obtained by TRUNCATION (x & 0xffff0000), each capturing 8
-// more significant bits; the residuals are exact in fp32.  4 ALU ops per element + 3 PRMT per pair.
-__device__ __forceinline__ void split3_pair(float x0, float x1, uint32_t& w0, uint32_t& w1, uint32_t& w2) {
-    const uint32_t u0 = __float_as_uint(x0), u1 = __float_as_uint(x1);
-    w0 = __byte_perm(u0, u1, 0x7632);                       // high halves of (x0, x1)
-    const float r0 = x0 - __uint_as_float(u0 & 0xffff0000u), r1 = x1 - __uint_as_float(u1 & 0xffff0000u);
-    const uint32_t v0 = __float_as_uint(r0), v1 = __float_as_uint(r1);
-    w1 = __byte_perm(v0, v1, 0x7632);
-    const float s0 = r0 - __uint_as_float(v0 & 0xffff0000u), s1 = r1 - __uint_as_float(v1 & 0xffff0000u);
-    w2 = __byte_perm(__float_as_uint(s0), __float_as_uint(s1), 0x7632);
-}
 // 8 consecutive columns (one 16-byte chunk) of row r
 __device__ __forceinline__ void store_chunk8(uint8_t* sm0, const Mat& m, uint32_t r, uint32_t c0, const float* v) {
     uint32_t w0[4], w1[4], w2[4];
 #pragma unroll
-    for (int j = 0; j < 4; ++j) split3_pair(v[2 * j], v[2 * j + 1], w0[j], w1[j], w2[j]);
-    uint8_t* p = sm0 + (m.base + moff(r, c0, m.RS));
+    for (int j = 0; j < 4; ++j) wg::split3_pair(v[2 * j], v[2 * j + 1], w0[j], w1[j], w2[j]);
+    uint8_t* p = sm0 + (m.base + wg::moff(r, c0, m.RS));
     *reinterpret_cast<uint4*>(p) = make_uint4(w0[0], w0[1], w0[2], w0[3]);
     *reinterpret_cast<uint4*>(p + m.part) = make_uint4(w1[0], w1[1], w1[2], w1[3]);
     *reinterpret_cast<uint4*>(p + 2 * m.part) = make_uint4(w2[0], w2[1], w2[2], w2[3]);
@@ -105,8 +91,8 @@ __device__ __forceinline__ void store_frag(uint8_t* sm0, const Mat& m, const flo
 #pragma unroll
     for (int e = 0; e < kCols; e += 2) {
         uint32_t w0, w1, w2;
-        split3_pair(v[e], v[e + 1], w0, w1, w2);
-        uint8_t* p = sm0 + (m.base + moff((uint32_t)(lay_row0() + wg::frag_row(e)), (uint32_t)(lay_col0() + wg::frag_col(e)), m.RS));
+        wg::split3_pair(v[e], v[e + 1], w0, w1, w2);
+        uint8_t* p = sm0 + (m.base + wg::moff((uint32_t)(lay_row0() + wg::frag_row(e)), (uint32_t)(lay_col0() + wg::frag_col(e)), m.RS));
         *reinterpret_cast<uint32_t*>(p) = w0;
         *reinterpret_cast<uint32_t*>(p + m.part) = w1;
         *reinterpret_cast<uint32_t*>(p + 2 * m.part) = w2;
@@ -117,7 +103,7 @@ __device__ __forceinline__ void store_frag(uint8_t* sm0, const Mat& m, const flo
 __device__ __forceinline__ void load_frag(const uint8_t* sm0, const Mat& m, float (&v)[kCols]) {
 #pragma unroll
     for (int e = 0; e < kCols; e += 2) {
-        const uint8_t* p = sm0 + (m.base + moff((uint32_t)(lay_row0() + wg::frag_row(e)), (uint32_t)(lay_col0() + wg::frag_col(e)), m.RS));
+        const uint8_t* p = sm0 + (m.base + wg::moff((uint32_t)(lay_row0() + wg::frag_row(e)), (uint32_t)(lay_col0() + wg::frag_col(e)), m.RS));
         const uint32_t w0 = *reinterpret_cast<const uint32_t*>(p);
         const uint32_t w1 = *reinterpret_cast<const uint32_t*>(p + m.part);
         const uint32_t w2 = *reinterpret_cast<const uint32_t*>(p + 2 * m.part);
@@ -294,8 +280,8 @@ __device__ void stage_weights(uint8_t* sm, uint8_t* sm0, const Smem& S, const fl
 // rewrites.  Padding (columns >= obs_dim, head rows >= out_dim) is zero and never touched.
 __device__ __forceinline__ void img_put(uint8_t* blk, uint32_t rel, uint32_t part, uint32_t RS, uint32_t r, uint32_t c, float x) {
     uint32_t w0, w1, w2;
-    split3_pair(x, 0.0f, w0, w1, w2);
-    uint8_t* p = blk + rel + moff(r, c, RS);
+    wg::split3_pair(x, 0.0f, w0, w1, w2);
+    uint8_t* p = blk + rel + wg::moff(r, c, RS);
     *reinterpret_cast<uint16_t*>(p) = (uint16_t)w0;
     *reinterpret_cast<uint16_t*>(p + part) = (uint16_t)w1;
     *reinterpret_cast<uint16_t*>(p + 2 * part) = (uint16_t)w2;
@@ -513,12 +499,6 @@ __device__ __forceinline__ void trunk_backward(uint8_t* sm, uint8_t* sm0, const 
     grad_out<1>(sm0, S, g, obs_dim, out_dim, grad, first);
 }
 
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
-    return v;
-}
-
 // State of the in-kernel grid barriers of the fused epoch kernel (self-resetting; launches are
 // stream-ordered and every CTA of the grid is resident: cooperative launch, 1 CTA / SM).
 // They live in the 128-byte control block in front of the caller's weight image (one per model instance, so
@@ -660,7 +640,7 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_tc_kernel(
         const Mat& M = e < 3 * kRows ? S.X : S.H1;
         const uint32_t c = e < 3 * kRows ? (uint32_t)S.KXP : (uint32_t)H;
         const uint32_t w = pc == 0 ? 0x3F803F80u : 0u;
-        *reinterpret_cast<uint4*>(sm0 + (M.base + pc * M.part + moff((uint32_t)r, c, M.RS))) = make_uint4(w, w, w, w);
+        *reinterpret_cast<uint4*>(sm0 + (M.base + pc * M.part + wg::moff((uint32_t)r, c, M.RS))) = make_uint4(w, w, w, w);
     }
     __syncthreads();
     EpochCtl* ctl = wimg != nullptr ? reinterpret_cast<EpochCtl*>(wimg - kCtlBytes) : &g_ep_ctl;
@@ -779,7 +759,7 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_tc_kernel(
                     ppo::critic_row(sc, value, rowv[kRows + tid], rowv[3 * kRows + tid], vf_row, dv[0]);
                 }
                 write_dout_row(sm, sm0, S, tid, dv);
-                const float sdv = warp_sum(dv[0]);
+                const float sdv = tsb::warp_sum(dv[0]);
                 if (lane == 0) red[warp] = sdv;                    // db3 (critic), one slot per warp
             }
             tstamp(4);
@@ -834,13 +814,13 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_tc_kernel(
                         const float g_ls = gl * (d2v[u] - 1.0f);               // d loss / d logstd_a
                         dof[a * kRows + r] = g_mu;
                         uint32_t w0, w1, w2;
-                        split3_pair(g_mu, 0.0f, w0, w1, w2);
-                        uint8_t* pdo = sm0 + (S.DO.base + moff((uint32_t)r, (uint32_t)a, S.DO.RS));   // columns >= A stay zero (critic pass)
+                        wg::split3_pair(g_mu, 0.0f, w0, w1, w2);
+                        uint8_t* pdo = sm0 + (S.DO.base + wg::moff((uint32_t)r, (uint32_t)a, S.DO.RS));   // columns >= A stay zero (critic pass)
                         *reinterpret_cast<uint16_t*>(pdo) = (uint16_t)w0;
                         *reinterpret_cast<uint16_t*>(pdo + S.DO.part) = (uint16_t)w1;
                         *reinterpret_cast<uint16_t*>(pdo + 2 * S.DO.part) = (uint16_t)w2;
                         // column sums over the 32 rows of this warp: red[128 + 32 q + a] <- db3[a], red[128 + 32 q + 16 + a] <- dlogstd[a]
-                        const float s_mu = warp_sum(g_mu), s_ls = warp_sum(g_ls);
+                        const float s_mu = tsb::warp_sum(g_mu), s_ls = tsb::warp_sum(g_ls);
                         if (lane == 0) { red[128 + 32 * q + a] = s_mu; red[128 + 32 * q + 16 + a] = s_ls; }
                     }
                 }
@@ -850,8 +830,8 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_tc_kernel(
             tstamp(9);
 
             // ================= loss sums + small gradients ===========================================
-            const float s_clip = warp_sum(tid < kRows ? clip_row : 0.0f);
-            const float s_vf = warp_sum(tid < kRows ? vf_row : 0.0f);
+            const float s_clip = tsb::warp_sum(tid < kRows ? clip_row : 0.0f);
+            const float s_vf = tsb::warp_sum(tid < kRows ? vf_row : 0.0f);
             if (lane == 0 && tid < kRows) { red[4 + warp] = s_clip; red[8 + warp] = s_vf; }
             __syncthreads();
             if (tid < A) {
@@ -955,12 +935,8 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_tc_kernel(
         tstamp(13);
         if (tid == 0) {
             const float total_norm = (float)sqrt(*((volatile double*)ss_cur));
-            float coef = 1.0f;
-            if (hp.max_grad_norm > 0.0) {   // torch.nn.utils.clip_grad_norm_
-                coef = (float)hp.max_grad_norm / (total_norm + 1e-6f);
-                coef = fminf(coef, 1.0f);
-            }
-            s_coef = coef; s_norm = total_norm;
+            s_coef = hp.max_grad_norm > 0.0 ? optim::clip_coef((float)hp.max_grad_norm, total_norm) : 1.0f;
+            s_norm = total_norm;
             if (blockIdx.x == 0) ctl->ss[(m + 1) & 1] = 0.0;       // next step's accumulator (idle until barrier 3)
         }
         __syncthreads();
@@ -968,22 +944,15 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_tc_kernel(
         const float coef = s_coef, step_size = s_step_size, bc2_sqrt = s_bc2_sqrt;
         const float w1 = (float)(1.0 - hp.beta1), w2 = (float)(1.0 - hp.beta2);
         const float beta2 = (float)hp.beta2, adam_eps = (float)hp.adam_eps, wd = (float)hp.weight_decay;
-        // RMSprop: beta2 holds alpha; 1 - alpha formed in double and rounded once, as torch passes addcmul's value
-        const float alpha = (float)hp.beta2, w_sq = (float)(1.0 - hp.beta2), lr = (float)hp.lr;
+        const float lr = (float)hp.lr;     // RMSprop: beta2 holds alpha, w2 = 1 - alpha
         auto adam_elem = [&](int64_t i, float g, float pv, float mm, float v) {
-            g *= coef;
-            if (wd != 0.0f) g = fmaf(wd, pv, g);
             if (rmsprop) {
-                v = v * alpha + w_sq * g * g;           // square_avg.mul_(alpha).addcmul_(grad, grad, 1 - alpha)
-                pv = pv - lr * (g / (sqrtf(v) + adam_eps));   // addcdiv_(grad, square_avg.sqrt().add_(eps), -lr)
+                optim::rmsprop_elem(g * coef, pv, v, lr, beta2, w2, adam_eps, wd);
                 opt.exp_avg_sq[i] = v; opt.params_w[i] = pv;
                 if (wimg != nullptr) img_scatter(d, S, sbase, i, pv, wimg);
                 return;
             }
-            mm = mm + w1 * (g - mm);                    // exp_avg.lerp_(grad, 1 - beta1)
-            v = v * beta2 + w2 * g * g;                 // mul_(beta2).addcmul_(grad, grad, 1 - beta2)
-            const float denom = sqrtf(v) / bc2_sqrt + adam_eps;
-            pv = pv - step_size * (mm / denom);         // addcdiv_(exp_avg, denom, -step_size)
+            optim::adam_elem<true>(g * coef, pv, mm, v, step_size, bc2_sqrt, beta2, w1, w2, adam_eps, wd);
             opt.exp_avg[i] = mm; opt.exp_avg_sq[i] = v; opt.params_w[i] = pv;
             if (wimg != nullptr) img_scatter(d, S, sbase, i, pv, wimg);
         };
@@ -1003,12 +972,9 @@ __global__ void __launch_bounds__(kThreads, 1) ppo_tc_kernel(
             // next step's fold, i.e. after every CTA passed the NEXT barrier 1
             const float* ex = opt.grad_scratch + d.n_params;
             const float e0 = __ldcg(ex), e1 = __ldcg(ex + 1), e2 = __ldcg(ex + 2), e3 = __ldcg(ex + 3);
-            const float rows = e3 > 0.0f ? e3 : 1.0f;
-            const float clip_loss = -e0 / rows, vf_loss = e1 / rows, ent_loss = e2 / rows;
             if (opt.stats) {
                 float* sr = opt.stats + (int64_t)m * TS_PPO_STATS_STRIDE;
-                sr[0] = clip_loss + (float)hp.vf_coef * vf_loss - (float)hp.ent_coef * ent_loss;
-                sr[1] = clip_loss; sr[2] = vf_loss; sr[3] = ent_loss;
+                ppo::loss_row(e0, e1, e2, e3 > 0.0f ? e3 : 1.0f, hp, sr);
                 sr[4] = s_norm; sr[5] = e3; sr[6] = 0.0f; sr[7] = 0.0f;
             }
         }

@@ -47,19 +47,6 @@ struct GemmParams {
     int k_per_split;     // multiple of BK
 };
 
-__device__ __forceinline__ uint32_t moff(uint32_t r, uint32_t c, uint32_t RS) {
-    return (r >> 3) * RS + (c >> 3) * 128u + (r & 7u) * 16u + (c & 7u) * 2u;
-}
-__device__ __forceinline__ void split3_pair(float x0, float x1, uint32_t& w0, uint32_t& w1, uint32_t& w2) {
-    const uint32_t u0 = __float_as_uint(x0), u1 = __float_as_uint(x1);
-    w0 = __byte_perm(u0, u1, 0x7632);
-    const float r0 = x0 - __uint_as_float(u0 & 0xffff0000u), r1 = x1 - __uint_as_float(u1 & 0xffff0000u);
-    const uint32_t v0 = __float_as_uint(r0), v1 = __float_as_uint(r1);
-    w1 = __byte_perm(v0, v1, 0x7632);
-    const float s0 = r0 - __uint_as_float(v0 & 0xffff0000u), s1 = r1 - __uint_as_float(v1 & 0xffff0000u);
-    w2 = __byte_perm(__float_as_uint(s0), __float_as_uint(s1), 0x7632);
-}
-
 // Stage one 128 (mn) x 64 (k) chunk of an operand.  Shared-memory matrix = [rows = non-contiguous dim][cols =
 // contiguous dim]: K-major -> [128 mn][64 k] (RS = 1024), MN-major -> [64 k][128 mn] (RS = 2048); one task = 8
 // contiguous floats -> one 16-byte chunk per piece.  1024 tasks / 256 threads.
@@ -95,9 +82,9 @@ __device__ __forceinline__ void store_operand(uint8_t* sm0, uint32_t base, const
         const int r = mn_major ? (task >> 4) : (task >> 3), c0 = mn_major ? (task & 15) * 8 : (task & 7) * 8;
         uint32_t w0[4], w1[4], w2[4];
 #pragma unroll
-        for (int j = 0; j < 4; ++j) split3_pair(s.v[u][2 * j], s.v[u][2 * j + 1], w0[j], w1[j], w2[j]);
+        for (int j = 0; j < 4; ++j) wg::split3_pair(s.v[u][2 * j], s.v[u][2 * j + 1], w0[j], w1[j], w2[j]);
         const uint32_t RS = mn_major ? 2048u : 1024u;
-        uint8_t* p = sm0 + (base + moff((uint32_t)r, (uint32_t)c0, RS));
+        uint8_t* p = sm0 + (base + wg::moff((uint32_t)r, (uint32_t)c0, RS));
         *reinterpret_cast<uint4*>(p) = make_uint4(w0[0], w0[1], w0[2], w0[3]);
         *reinterpret_cast<uint4*>(p + kPartBytes) = make_uint4(w1[0], w1[1], w1[2], w1[3]);
         *reinterpret_cast<uint4*>(p + 2 * kPartBytes) = make_uint4(w2[0], w2[1], w2[2], w2[3]);

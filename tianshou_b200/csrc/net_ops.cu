@@ -12,6 +12,7 @@
 #include <math.h>
 
 #include "common.cuh"
+#include "optim_math.cuh"
 
 namespace {
 
@@ -279,31 +280,23 @@ __global__ void sumsq_kernel(const float* __restrict__ g, int64_t n, double* __r
     if (threadIdx.x == 0) partial[blockIdx.x] = s[0];
 }
 // clip_grad_norm_'s coefficient from sumsq_kernel's `partial` block sums (1 when clipping is off)
-__device__ __forceinline__ float clip_coef(float max_norm, const double* __restrict__ partial, int n_partial) {
+__device__ __forceinline__ float sumsq_clip_coef(float max_norm, const double* __restrict__ partial, int n_partial) {
     float coef = 1.0f;
     if (max_norm > 0.0f && partial) {
         double t = 0.0;
         for (int i = 0; i < n_partial; ++i) t += partial[i];
-        coef = fminf(max_norm / ((float)sqrt(t) + 1e-6f), 1.0f);
+        coef = optim::clip_coef(max_norm, (float)sqrt(t));
     }
     return coef;
 }
-// torch.optim.Adam single-tensor step (lerp / addcmul / addcdiv order), optional clip_grad_norm_ from `partial` block sums.
-// w1 = 1 - beta1 and w2 = 1 - beta2 are formed in double and rounded once, as torch passes them (lerp weight, addcmul
-// value): 1.0f - (float)0.999 would be 1.3e-5 off in relative terms.
+// torch.optim.Adam step (optim_math.cuh), optional clip_grad_norm_ from `partial` block sums; step scalars from the host.
 __global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v, int64_t n,
                             float step_size, float bc2_sqrt, float beta2, float w1, float w2, float eps, float wd, float max_norm,
                             const double* __restrict__ partial, int n_partial) {
-    const float coef = clip_coef(max_norm, partial, n_partial);
+    const float coef = sumsq_clip_coef(max_norm, partial, n_partial);
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-        float gi = g[i] * coef;
-        float pv = p[i];
-        if (wd != 0.0f) gi = fmaf(wd, pv, gi);
-        float mm = m[i], vv = v[i];
-        mm = mm + w1 * (gi - mm);
-        vv = vv * beta2 + w2 * gi * gi;
-        const float denom = sqrtf(vv) / bc2_sqrt + eps;
-        pv = pv - step_size * (mm / denom);
+        float pv = p[i], mm = m[i], vv = v[i];
+        optim::adam_elem(g[i] * coef, pv, mm, vv, step_size, bc2_sqrt, beta2, w1, w2, eps, wd);
         m[i] = mm; v[i] = vv; p[i] = pv;
     }
 }
@@ -312,42 +305,30 @@ __global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, 
 __global__ void adam_dev_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v, int64_t n,
                                 const int64_t* __restrict__ step_dev, double lr, double beta1d, double beta2d, float eps, float wd,
                                 float max_norm, const double* __restrict__ partial, int n_partial) {
-    __shared__ float s_step_size, s_bc2_sqrt, s_coef;
+    __shared__ optim::AdamBias s_bias;
+    __shared__ float s_coef;
     if (threadIdx.x == 0) {
-        const double step = (double)(*step_dev + 1);
-        s_step_size = (float)(lr / (1.0 - pow(beta1d, step)));
-        s_bc2_sqrt = (float)sqrt(1.0 - pow(beta2d, step));
-        s_coef = clip_coef(max_norm, partial, n_partial);
+        s_bias = optim::adam_bias(lr, beta1d, beta2d, *step_dev + 1);
+        s_coef = sumsq_clip_coef(max_norm, partial, n_partial);
     }
     __syncthreads();
-    const float step_size = s_step_size, bc2_sqrt = s_bc2_sqrt, coef = s_coef;
+    const float step_size = s_bias.step_size, bc2_sqrt = s_bias.bc2_sqrt, coef = s_coef;
     const float beta2 = (float)beta2d;
     const float w1 = (float)(1.0 - beta1d), w2 = (float)(1.0 - beta2d);
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-        float gi = g[i] * coef;
-        float pv = p[i];
-        if (wd != 0.0f) gi = fmaf(wd, pv, gi);
-        float mm = m[i], vv = v[i];
-        mm = mm + w1 * (gi - mm);
-        vv = vv * beta2 + w2 * gi * gi;
-        const float denom = sqrtf(vv) / bc2_sqrt + eps;
-        pv = pv - step_size * (mm / denom);
+        float pv = p[i], mm = m[i], vv = v[i];
+        optim::adam_elem(g[i] * coef, pv, mm, vv, step_size, bc2_sqrt, beta2, w1, w2, eps, wd);
         m[i] = mm; v[i] = vv; p[i] = pv;
     }
 }
-// torch.optim.RMSprop single-tensor step without momentum / centering (mul_ / addcmul_ / sqrt / add_ / addcdiv_ order), the
-// clip as adam_kernel.  w_sq = 1 - alpha is formed in double and rounded once, as torch passes addcmul's value.
+// torch.optim.RMSprop step (optim_math.cuh), the clip as adam_kernel
 __global__ void rmsprop_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ sq, int64_t n, float lr,
                                float alpha, float w_sq, float eps, float wd, float max_norm, const double* __restrict__ partial,
                                int n_partial) {
-    const float coef = clip_coef(max_norm, partial, n_partial);
+    const float coef = sumsq_clip_coef(max_norm, partial, n_partial);
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-        float gi = g[i] * coef;
-        float pv = p[i];
-        if (wd != 0.0f) gi = fmaf(wd, pv, gi);
-        float vv = sq[i];
-        vv = vv * alpha + w_sq * gi * gi;
-        pv = pv - lr * (gi / (sqrtf(vv) + eps));
+        float pv = p[i], vv = sq[i];
+        optim::rmsprop_elem(g[i] * coef, pv, vv, lr, alpha, w_sq, eps, wd);
         sq[i] = vv; p[i] = pv;
     }
 }
@@ -456,8 +437,8 @@ extern "C" int ts_adam_step(float* params, const float* grad, float* exp_avg, fl
         sumsq_kernel<<<n_partial, 256, 0, st>>>(grad, n, norm_scratch);
         if (tsb::check_launch("ts_adam_step/norm")) return 1;
     }
-    const double bc1 = 1.0 - pow(beta1, (double)step), bc2 = 1.0 - pow(beta2, (double)step);
-    adam_kernel<<<grid_for(n), 256, 0, st>>>(params, grad, exp_avg, exp_avg_sq, n, (float)(lr / bc1), (float)sqrt(bc2), (float)beta2,
+    const optim::AdamBias bias = optim::adam_bias(lr, beta1, beta2, step);
+    adam_kernel<<<grid_for(n), 256, 0, st>>>(params, grad, exp_avg, exp_avg_sq, n, bias.step_size, bias.bc2_sqrt, (float)beta2,
                                              (float)(1.0 - beta1), (float)(1.0 - beta2), (float)eps, (float)weight_decay, (float)max_grad_norm, norm_scratch, n_partial);
     return tsb::check_launch("ts_adam_step");
 }
@@ -480,9 +461,7 @@ extern "C" int ts_adam_step_dev(float* params, const float* grad, float* exp_avg
     step_inc_kernel<<<1, 1, 0, st>>>(step_dev);
     return tsb::check_launch("ts_adam_step_dev/inc");
 }
-// replaces clip_grad_norm_ + RMSprop.step (algorithm_base.py:496-500; torch/optim/rmsprop.py _single_tensor_rmsprop:
-// square_avg.mul_(alpha).addcmul_(grad, grad, value=1 - alpha); avg = square_avg.sqrt().add_(eps);
-// param.addcdiv_(grad, avg, value=-lr))
+// replaces clip_grad_norm_ + RMSprop.step (algorithm_base.py:496-500)
 extern "C" int ts_rmsprop_step(float* params, const float* grad, float* square_avg, int64_t n, double lr, double alpha, double eps,
                                double weight_decay, double max_grad_norm, double* norm_scratch, ts_stream_t stream) {
     TS_REQUIRE(params && grad && square_avg, "ts_rmsprop_step: null pointer");

@@ -95,13 +95,8 @@ __global__ void npg_rows_kernel(const float* __restrict__ head, const float* __r
         loss_rows[b] = -(ratio_surrogate ? w : lp) * adv[b];
         if (dhead) {
             const float gl = -w * adv[b] * inv_b;
-            for (int a = 0; a < A; ++a) {
-                const float sg = expf(logstd[a]);
-                const float var = sg * sg;
-                const float diff = act[b * A + a] - head[b * A + a];
-                dhead[b * A + a] = gl * diff / var;
-                dlogstd_rows[b * A + a] = gl * (diff * diff / var - 1.0f);
-            }
+            for (int a = 0; a < A; ++a)
+                ppo::normal_backward(act[b * A + a], head[b * A + a], expf(logstd[a]), gl, dhead[b * A + a], dlogstd_rows[b * A + a]);
         }
     }
 }

@@ -1,5 +1,6 @@
-// Per-row PPO loss arithmetic shared by the tensor-core kernels (csrc/mlp_tc.cu).
-// Reference: tianshou/algorithm/modelfree/ppo.py:183-211 with torch's backward tie rules for
+// Per-row PPO / A2C loss arithmetic, the one statement shared by the SIMT kernels (mlp.cu), the tensor-core kernels
+// (mlp_tc.cu), the layer-wise loss rows (ppo_rows.cu) and the NPG / TRPO rows (npg.cu).
+// Reference: tianshou/algorithm/modelfree/ppo.py:183-216 with torch's backward tie rules for
 // minimum / maximum / clamp (derivatives.yaml: equal operands split the gradient in halves).
 #pragma once
 #include <cuda_runtime.h>
@@ -80,20 +81,42 @@ __device__ __forceinline__ void actor_row(const Scalars& s, float logp, float lo
     gl = -s.inv_b * g_ratio * ratio;
 }
 
-// log N(x; mu, sigma) of one action dim, torch.distributions.Normal.log_prob order
+// loss-table entries 0..3 from the loss sums over `rows` rows: loss, actor loss (= -mean objective), value loss, entropy
+// (ppo.py:211-216).  Entries 4.. of the TS_PPO_STATS_STRIDE row are the caller's.
+__device__ __forceinline__ void loss_row(float s_obj, float s_vf, float s_ent, float rows, const ts_ppo_hparams& hp, float* out) {
+    const float clip_loss = -s_obj / rows, vf_loss = s_vf / rows, ent_loss = s_ent / rows;
+    out[0] = clip_loss + (float)hp.vf_coef * vf_loss - (float)hp.ent_coef * ent_loss;
+    out[1] = clip_loss; out[2] = vf_loss; out[3] = ent_loss;
+}
+
+// Diagonal Gaussian head (continuous.py:220-238 + torch.distributions.Normal), one action dim.
+// log N(x; mu, sigma) in Normal.log_prob order: -((x-mu)^2) / (2 var) - log(sigma) - log(sqrt(2 pi))
 __device__ __forceinline__ float normal_logp_term(float x, float mu, float sigma) {
     const float var = sigma * sigma;
     const float diff = x - mu;
     return -(diff * diff) / (2.0f * var) - logf(sigma) - 0.9189385332046727f;
 }
+// d/d mu and d/d log sigma of the log-prob term, given gl = d loss / d log_prob
+__device__ __forceinline__ void normal_backward(float x, float mu, float sigma, float gl, float& dmu, float& dlogstd) {
+    const float var = sigma * sigma;
+    const float diff = x - mu;
+    dmu = gl * diff / var;
+    dlogstd = gl * (diff * diff / var - 1.0f);
+}
+// Normal.entropy: 0.5 + 0.5 log(2 pi) + log sigma
+__device__ __forceinline__ float normal_entropy_term(float sigma) { return 1.4189385332046727f + logf(sigma); }
 
-// Categorical(probs = softmax(z)) of one row (utils/net/discrete.py:69-92 + torch.distributions.Categorical), shared by
-// the PPO loss rows (ppo_rows.cu) and the NPG / TRPO rows (npg.cu).
-constexpr int kCatMaxA = 64;
-struct Cat { float p[kCatMaxA], pn[kCatMaxA], lg[kCatMaxA]; float s2; };
-// p = softmax(z); Categorical renormalises (pn = p / sum p), logits = log(clamp(pn, eps, 1 - eps)); entropy = -sum pn * logits
-__device__ __forceinline__ void cat_forward(const float* z, int A, int action, Cat& c, float& logp, float& ent) {
-    constexpr float eps = 1.1920928955078125e-07f;
+// Categorical(probs = softmax(z)) of one row with at most MaxA actions (utils/net/discrete.py:69-92, reinforce.py:167-192 +
+// torch.distributions.Categorical).
+template <int MaxA>
+struct CatT { float p[MaxA], pn[MaxA], lg[MaxA]; float s2; };
+constexpr int kCatMaxA = 64;       // the layer-wise rows (ppo_rows.cu, npg.cu); the SIMT kernels keep 16-entry rows
+using Cat = CatT<kCatMaxA>;
+// p = softmax(z); Categorical renormalises (pn = p / sum p), logits = log(clamp(pn, eps, 1 - eps)); log_prob gathers,
+// entropy = -sum pn * logits.  Keeps p, pn, lg for the backward.
+template <int MaxA>
+__device__ __forceinline__ void cat_forward(const float* z, int A, int action, CatT<MaxA>& c, float& logp, float& ent) {
+    constexpr float eps = 1.1920928955078125e-07f;     // torch.finfo(float32).eps
     float m = z[0];
     for (int a = 1; a < A; ++a) m = fmaxf(m, z[a]);
     float s = 0.0f;
@@ -109,18 +132,20 @@ __device__ __forceinline__ void cat_forward(const float* z, int A, int action, C
     }
     logp = (action >= 0 && action < A) ? c.lg[action] : 0.0f;
 }
-// autograd's chain: gather + entropy -> log o clamp -> renormalisation -> softmax
-__device__ __forceinline__ void cat_backward(const Cat& c, int A, int action, float gl, float ge, float* dz) {
+// dz[a] = d loss / d z_a given gl = d loss / d log_prob and ge = d loss / d entropy; autograd's chain:
+// gather + entropy -> log o clamp -> renormalisation -> softmax
+template <int MaxA>
+__device__ __forceinline__ void cat_backward(const CatT<MaxA>& c, int A, int action, float gl, float ge, float* dz) {
     constexpr float eps = 1.1920928955078125e-07f;
     float dot = 0.0f;
     for (int a = 0; a < A; ++a) {
         const float dlg = (a == action ? gl : 0.0f) - ge * c.pn[a];
-        const bool pass = c.pn[a] >= eps && c.pn[a] <= 1.0f - eps;
+        const bool pass = c.pn[a] >= eps && c.pn[a] <= 1.0f - eps;        // clamp backward
         dz[a] = -ge * c.lg[a] + (pass ? dlg / c.pn[a] : 0.0f);
         dot += dz[a] * c.pn[a];
     }
     float dot2 = 0.0f;
-    for (int a = 0; a < A; ++a) { dz[a] = (dz[a] - dot) / c.s2; dot2 += dz[a] * c.p[a]; }
+    for (int a = 0; a < A; ++a) { dz[a] = (dz[a] - dot) / c.s2; dot2 += dz[a] * c.p[a]; }   // now d/dp
     for (int a = 0; a < A; ++a) dz[a] = c.p[a] * (dz[a] - dot2);
 }
 

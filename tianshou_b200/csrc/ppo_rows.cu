@@ -45,16 +45,15 @@ __global__ void ppo_rows_kernel(const float* __restrict__ head, const float* __r
         for (int a = 0; a < A; ++a) {
             const float sg = expf(logstd[a]);
             lp += ppo::normal_logp_term(act[b * A + a], head[b * A + a], sg);
-            ent += 1.4189385332046727f + logf(sg);        // 0.5 + 0.5 log(2 pi) + log sigma
+            ent += ppo::normal_entropy_term(sg);
         }
         if (grads) {
             ppo::actor_row(sc, lp, logp_old[b], adv[b], obj, gl);
             for (int a = 0; a < A; ++a) {
-                const float sg = expf(logstd[a]);
-                const float var = sg * sg;
-                const float diff = act[b * A + a] - head[b * A + a];
-                dhead[b * A + a] = gl * diff / var;
-                if (dlogstd_rows) dlogstd_rows[b * A + a] = gl * (diff * diff / var - 1.0f) - sc.ent_coef * sc.inv_b;
+                float dmu, dls;
+                ppo::normal_backward(act[b * A + a], head[b * A + a], expf(logstd[a]), gl, dmu, dls);
+                dhead[b * A + a] = dmu;
+                if (dlogstd_rows) dlogstd_rows[b * A + a] = dls - sc.ent_coef * sc.inv_b;
             }
         }
     }
@@ -62,14 +61,12 @@ __global__ void ppo_rows_kernel(const float* __restrict__ head, const float* __r
     if (grads) {
         float vf_row = 0.0f, dv = 0.0f;
         ppo::critic_row(sc, value[b], ret[b], v_s[b], vf_row, dv);
-        if (sc.a2c) {          // a2c.py:268: plain MSE value loss, no clip (critic_row handles value_clip == 0 the same way)
-        }
         dvalue[b] = dv;
         if (loss_rows) { loss_rows[b * 3] = obj; loss_rows[b * 3 + 1] = vf_row; loss_rows[b * 3 + 2] = ent; }
     }
 }
 
-// (sum obj, sum vf, sum ent) -> stats row: loss, actor loss (= -mean obj), vf loss, entropy        (ppo.py:211-216)
+// (sum obj, sum vf, sum ent) -> stats row entries 0..3 (ppo::loss_row) and 5 (rows)
 __global__ void ppo_stats_kernel(const float* __restrict__ loss_rows, int64_t B, const ts_ppo_hparams hp, float* __restrict__ stats_row) {
     __shared__ float s[3][256];
     float a0 = 0.f, a1 = 0.f, a2 = 0.f;
@@ -85,9 +82,7 @@ __global__ void ppo_stats_kernel(const float* __restrict__ loss_rows, int64_t B,
     }
     if (threadIdx.x == 0) {
         const float rows = (float)B;
-        const float clip_loss = -s[0][0] / rows, vf_loss = s[1][0] / rows, ent_loss = s[2][0] / rows;
-        stats_row[0] = clip_loss + (float)hp.vf_coef * vf_loss - (float)hp.ent_coef * ent_loss;
-        stats_row[1] = clip_loss; stats_row[2] = vf_loss; stats_row[3] = ent_loss;
+        ppo::loss_row(s[0][0], s[1][0], s[2][0], rows, hp, stats_row);
         stats_row[5] = rows;
     }
 }

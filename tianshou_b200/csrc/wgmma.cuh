@@ -33,6 +33,24 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
 __device__ __forceinline__ int frag_row(int e) { return 16 * ((threadIdx.x >> 5) & 3) + ((threadIdx.x & 31) >> 2) + 8 * ((e >> 1) & 1); }
 __device__ __forceinline__ int frag_col(int e) { return 8 * (e >> 2) + 2 * (threadIdx.x & 3) + (e & 1); }
 
+// byte offset of element (r, c) in the blocked layout above (RS = bytes between 8-row groups)
+__device__ __forceinline__ uint32_t moff(uint32_t r, uint32_t c, uint32_t RS) {
+    return (r >> 3) * RS + (c >> 3) * 128u + (r & 7u) * 16u + (c & 7u) * 2u;
+}
+
+// x = b0 + b1 + b2 with three bf16 pieces obtained by TRUNCATION (x & 0xffff0000), each capturing 8
+// more significant bits; the residuals are exact in fp32.  4 ALU ops per element + 3 PRMT per pair.
+// w_p packs piece p of (x0, x1) as two consecutive bf16 columns.
+__device__ __forceinline__ void split3_pair(float x0, float x1, uint32_t& w0, uint32_t& w1, uint32_t& w2) {
+    const uint32_t u0 = __float_as_uint(x0), u1 = __float_as_uint(x1);
+    w0 = __byte_perm(u0, u1, 0x7632);                       // high halves of (x0, x1)
+    const float r0 = x0 - __uint_as_float(u0 & 0xffff0000u), r1 = x1 - __uint_as_float(u1 & 0xffff0000u);
+    const uint32_t v0 = __float_as_uint(r0), v1 = __float_as_uint(r1);
+    w1 = __byte_perm(v0, v1, 0x7632);
+    const float s0 = r0 - __uint_as_float(v0 & 0xffff0000u), s1 = r1 - __uint_as_float(v1 & 0xffff0000u);
+    w2 = __byte_perm(__float_as_uint(s0), __float_as_uint(s1), 0x7632);
+}
+
 // ---- descriptors ------------------------------------------------------------------------------
 // 64-bit shared-memory matrix descriptor, no swizzle: lo32 = (addr >> 4) | (LBO >> 4) << 16 ; hi32 = SBO >> 4
 __device__ __forceinline__ uint32_t desc_lo(uint32_t saddr, uint32_t lbo) { return ((saddr >> 4) & 0x3FFFu) | (((lbo >> 4) & 0x3FFFu) << 16); }
