@@ -11,7 +11,7 @@ import torch
 
 from tianshou_b200.data import Batch, ReplayBuffer, VectorReplayBuffer
 from tianshou_b200.data.batch import minibatch_bounds
-from ts_testutil import ROOT, load_golden, set_buffer_state, synth_rollout
+from ts_testutil import load_golden, set_buffer_state, synth_rollout
 
 
 # ------------------------------------------------------------------------------------- Batch
@@ -137,31 +137,20 @@ def test_device_path_fails_loudly_without_gpu():
 
 
 # ------------------------------------------------------------------------------------ C ABI
-def header_functions(diagnostics: bool = False):
-    text = open(os.path.join(ROOT, "include", "ts_b200.h")).read()
-    text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
-    diag = re.findall(r"#ifdef TS_B200_DIAGNOSTICS(.*?)#endif", text, flags=re.S)
-    text = re.sub(r"#ifdef TS_B200_DIAGNOSTICS.*?#endif", "", text, flags=re.S)
-    if diagnostics:
-        return sorted(set(re.findall(r"\b(ts_[a-z0-9_]+)\s*\(", "".join(diag))))
-    return sorted(set(re.findall(r"\b(ts_[a-z0-9_]+)\s*\(", text)))
-
-
-def test_cabi_library_exports_every_declared_symbol():
+def test_cabi_library_exports_every_parsed_declaration():
     from tianshou_b200 import _cabi
     lib = ctypes.CDLL(_cabi.LIB_PATH)
-    names = header_functions()
+    names = sorted(_cabi.ABI.functions)
     assert len(names) >= 30
     for n in names:
         assert hasattr(lib, n), f"{n} declared in include/ts_b200.h but not exported"
-    bound = set(_cabi.SIGNATURES) | set(_cabi.OTHER_SYMBOLS)
-    assert set(names) == bound, set(names) ^ bound
     # diagnostics (phase timeline, wgmma self-test) live in a separate build and are NOT in the product library
-    diag = header_functions(diagnostics=True)
-    assert set(diag) == set(_cabi.DIAG_SIGNATURES) and len(diag) == 2
+    diag = sorted(_cabi.ABI.diag_functions)
+    assert len(diag) == 2 and not set(diag) & set(names)
     for n in diag:
         assert not hasattr(lib, n), f"diagnostic entry {n} exported by the product library"
     lib2 = _cabi.load_library()
+    assert all(getattr(lib2, n).argtypes is not None for n in names)     # every declaration is bound
     assert lib2.ts_version() == 1
     assert lib2.ts_gae_workspace_bytes(2048 * 3 + 1) > 0
 
@@ -170,6 +159,38 @@ def test_cabi_struct_layouts_match_header():
     from tianshou_b200._cabi import ActorCriticDesc, PPOHParams
     assert ctypes.sizeof(ActorCriticDesc) == 4 * 4 + 14 * 8
     assert ctypes.sizeof(PPOHParams) == 11 * 8 + 3 * 4 + 4      # trailing pad to 8
+    assert ActorCriticDesc.a_w1.offset == 16 and ActorCriticDesc.n_params.offset == 120
+    assert PPOHParams.optimizer.offset == 100
+
+
+def test_cabi_prototypes_follow_the_type_rules():
+    """One declaration per type rule of the header-derived binding, written out by hand."""
+    from tianshou_b200._cabi import ABI, ActorCriticDesc, PPOHParams
+    C = ctypes
+    P, I, I32, I64, D, F = C.c_void_p, C.c_int, C.c_int32, C.c_int64, C.c_double, C.c_float
+    fn = ABI.functions
+    assert fn["ts_gae"] == (I, [P, P, I, P, P, P, P, I, I64, D, D, P, D, P, P, P, I, P, P])
+    assert fn["ts_cql_rows"] == (I, [P, P, P, I64, I32, P, P, F, P, F, F, P, F, F, P, P, P, P, P])
+    assert fn["ts_make_permutation"] == (I, [C.c_uint64, I32, I32, I64, P, P])
+    desc, hp = C.POINTER(ActorCriticDesc), C.POINTER(PPOHParams)
+    assert fn["ts_ppo_update"] == (I, [P, P, P, P, P, P, desc, hp, P, P, P, P, P, P, P, P, P, P, P, P, I64, P, I32, P, I32,
+                                       I32, D, D, P, D, P, P, P, P, P, P])
+    assert fn["ts_peer_open"] == (I, [P, C.POINTER(P)])
+    assert fn["ts_ppo_epoch_multi"] == (I, [P, P, P, P, P, P, desc, hp, P, P, P, P, P, P, P, I64, I64, I64, I32, P, P, P,
+                                            I32, I32, C.POINTER(P), P])
+    assert fn["ts_gae_workspace_bytes"] == (C.c_size_t, [I64])
+    assert fn["ts_last_error"] == (C.c_char_p, [])
+    assert fn["ts_reset_launch_count"] == (None, [])
+
+
+def test_cabi_header_parser_refuses_what_it_cannot_bind():
+    from tianshou_b200._cabi import HeaderError, parse_header
+    ok = parse_header("int ts_ok(int64_t n, const float* x, ts_stream_t s); /* ts_not_a_call( */\n")
+    assert ok.functions == {"ts_ok": (ctypes.c_int, [ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p])}
+    with pytest.raises(HeaderError, match="half h"):
+        parse_header("int ts_ok(void);\nint ts_half(half h, ts_stream_t s);\n")
+    with pytest.raises(HeaderError, match="ts_callback"):
+        parse_header("int ts_ok(void);\nint ts_callback(void (*fn)(int), ts_stream_t s);\n")
 
 
 def test_host_permutation_is_numpy_global_permutation_bit_for_bit():

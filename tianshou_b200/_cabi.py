@@ -8,154 +8,121 @@ from __future__ import annotations
 
 import ctypes as C
 import os
-from typing import Any
+import re
+from typing import Any, NamedTuple
 
 import numpy as np
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libts_b200.so")
-
-TS_F32, TS_F64 = 0, 1
-AC_RELU, AC_CATEGORICAL = 1, 2
-LOSS_PPO, LOSS_A2C = 0, 1
-OPT_ADAM, OPT_RMSPROP = 0, 1
-STATS_STRIDE = 8
-GRAD_EXTRA = 4
+HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ts_b200.h")
 
 
 class ExtensionMissingError(RuntimeError):
     pass
 
 
-class ActorCriticDesc(C.Structure):
-    _fields_ = [
-        ("obs_dim", C.c_int32), ("act_dim", C.c_int32), ("hidden", C.c_int32), ("flags", C.c_int32),
-        ("a_w1", C.c_int64), ("a_b1", C.c_int64), ("a_w2", C.c_int64), ("a_b2", C.c_int64),
-        ("a_w3", C.c_int64), ("a_b3", C.c_int64), ("a_logstd", C.c_int64),
-        ("c_w1", C.c_int64), ("c_b1", C.c_int64), ("c_w2", C.c_int64), ("c_b2", C.c_int64),
-        ("c_w3", C.c_int64), ("c_b3", C.c_int64),
-        ("n_params", C.c_int64),
-    ]
+class HeaderError(ValueError):
+    """A declaration of the C header that the binding has no rule for."""
 
 
-class PPOHParams(C.Structure):
-    _fields_ = [
-        ("eps_clip", C.c_double), ("dual_clip", C.c_double), ("vf_coef", C.c_double),
-        ("ent_coef", C.c_double), ("max_grad_norm", C.c_double), ("adv_eps", C.c_double),
-        ("lr", C.c_double), ("beta1", C.c_double), ("beta2", C.c_double), ("adam_eps", C.c_double),
-        ("weight_decay", C.c_double),
-        ("value_clip", C.c_int32), ("advantage_normalization", C.c_int32), ("loss_kind", C.c_int32),
-        ("optimizer", C.c_int32),
-    ]
+# The header is the only definition of the ABI: every prototype, struct layout and TS_* constant below is parsed from it.
+# Scalars and ts_stream_t bind by name; a pointer to a header struct binds as POINTER(struct), T** and void* const* as
+# POINTER(c_void_p), every other pointer as c_void_p (const char* returns as c_char_p).  Any other type raises, so a
+# header edit never binds silently as something else.
+_SCALARS = {"int": C.c_int, "int32_t": C.c_int32, "int64_t": C.c_int64, "uint64_t": C.c_uint64, "size_t": C.c_size_t,
+            "double": C.c_double, "float": C.c_float, "ts_stream_t": C.c_void_p}
 
 
-_P = C.c_void_p
-_I64 = C.c_int64
-_I32 = C.c_int32
-_D = C.c_double
+class Abi(NamedTuple):
+    functions: dict[str, tuple[Any, list[Any]]]       # name -> (restype, argtypes) of the product library
+    diag_functions: dict[str, tuple[Any, list[Any]]]  # the `#ifdef TS_B200_DIAGNOSTICS` block (libts_b200_diag.so)
+    structs: dict[str, type[C.Structure]]             # typedef name -> layout
+    consts: dict[str, int]                            # every `#define TS_* <int>` and `enum { TS_* = <int> }`
 
-# name -> argtypes (restype is int unless noted); mirrors include/ts_b200.h one to one
-SIGNATURES: dict[str, list[Any]] = {
-    "ts_gae": [_P, _P, C.c_int, _P, _P, _P, _P, C.c_int, _I64, _D, _D, _P, _D, _P, _P, _P, C.c_int, _P, _P],
-    "ts_rms_merge": [_P, _P, _I32, _P],
-    "ts_nstep_return": [_P, _P, _P, _P, _I64, _I64, _I32, _D, _P, C.c_int, _P],
-    "ts_buffer_end_flags": [_P, _P, _P, _P, _I64, _P, _P],
-    "ts_value_mask_rows": [_P, _P, _P, _I64, _I64, _P],
-    "ts_next_index": [_P, _I64, _P, _I64, _P, _P, _P, _P, _P],
-    "ts_prev_index": [_P, _I64, _P, _I64, _P, _P, _P, _P, _P],
-    "ts_stack_next_indices": [_P, _I64, _I32, _P, _I64, _P, _P, _P, _P, _P],
-    "ts_unfinished_index": [_P, _I64, _P, _P, _P, _P, _P, _P, _P],
-    "ts_sample_all_indices": [_P, _I64, _P, _P, _P, _P, _P, _I64, _P, _P],
-    "ts_mark_members": [_P, _I64, _P, _P, _I64, _P, _I64, _P, _P],
-    "ts_gather_rows": [_P, _I64, _P, _I64, _P, _P],
-    "ts_scatter_rows": [_P, _I64, _P, _I64, _P, _P],
-    "ts_segtree_setitem": [_P, _I64, _P, _P, C.c_int, _I64, _P],
-    "ts_segtree_reduce": [_P, _I64, _I64, _I64, _P, _P],
-    "ts_segtree_prefix_sum_idx": [_P, _I64, _P, _I64, _P, _P],
-    "ts_segtree_sample": [_P, _I64, _P, _I64, _P, _P],
-    "ts_prio_update_weight": [_P, _I64, _P, _P, C.c_int, _I64, _D, _D, _P, _P],
-    "ts_prio_get_weight": [_P, _I64, _P, _I64, _P, _D, C.c_int, _P, _P],
-    "ts_critic_forward": [_P, C.POINTER(ActorCriticDesc), _P, _P, _P, _P, _I64, _P],
-    "ts_actor_logp": [_P, C.POINTER(ActorCriticDesc), _P, _P, _I64, _P, _P, _P],
-    "ts_ppo_grad": [_P, C.POINTER(ActorCriticDesc), C.POINTER(PPOHParams), _P, _P, _P, _P, _P, _P, _P,
-                    _I64, _I64, _I64, _P, _P, C.POINTER(_I32), _P],
-    "ts_grad_reduce": [_P, _I32, C.POINTER(ActorCriticDesc), _P, _P],
-    "ts_minibatch_adv_sums": [_P, _P, _I64, _I64, _P, _P],
-    "ts_adv_moments_finalize": [_P, _I64, _P, _P],
-    "ts_clip_adam_step": [_P, _P, _P, _I32, _P, _P, _P, C.POINTER(ActorCriticDesc), C.POINTER(PPOHParams), _P, _P],
-    "ts_ppo_update": [_P, _P, _P, _P, _P, _P, C.POINTER(ActorCriticDesc), C.POINTER(PPOHParams),
-                      _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I64, _P, _I32,
-                      C.POINTER(_I64), _I32, _I32, _D, _D, _P, _D, _P, _P, _P, _P, _P, _P],
-    "ts_peer_alloc": [_I64, C.POINTER(C.c_void_p), _P],
-    "ts_peer_open": [_P, C.POINTER(C.c_void_p)],
-    "ts_peer_close": [_P],
-    "ts_peer_free": [_P],
-    "ts_epoch_adv_sums": [_P, _P, _I64, _I64, _I64, _I32, _P, _P],
-    "ts_epoch_adv_finalize": [_P, _I64, _I64, _I64, _I32, _I32, _P, _P],
-    "ts_ppo_epoch_multi": [_P, _P, _P, _P, _P, _P, C.POINTER(ActorCriticDesc), C.POINTER(PPOHParams),
-                           _P, _P, _P, _P, _P, _P, _P, _I64, _I64, _I64, _I32, _P, _P, _P, _I32, _I32,
-                           C.POINTER(C.c_void_p), _P],
-    "ts_host_mt19937_permutation": [_P, C.POINTER(_I32), _I64, _P],
-    "ts_host_perm_job_start": [_P, _I32, _I64, _I32, _P, _I32, C.POINTER(C.c_void_p)],
-    "ts_host_perm_job_wait": [_P, _I32],
-    "ts_host_perm_job_finish": [_P, _P, C.POINTER(_I32)],
-    "ts_host_perm_feed_start": [_P, _P, _P, _I64, _I32, C.POINTER(C.c_void_p)],
-    "ts_host_perm_feed_wait_row": [_P, _I32, _P],
-    "ts_host_perm_feed_finish": [_P],
-    "ts_make_permutation": [C.c_uint64, _I32, _I32, _I64, _P, _P],
-    "ts_narrow_i64_i32": [_P, _I64, _P, _P],
-    # layered networks of the off-policy algorithms (net_gemm.cu / net_ops.cu)
-    "ts_net_gemm": [_P, _I64, _I32, _P, _I64, _I32, _P, _I64, _I32, _I32, _I32, _P, _I32, _P, _I64, _I32, _I32, _P, _I64, _P],
-    "ts_ppo_rows": [_P, _P, _P, _P, _P, _P, _P, _P, _I64, _I32, _I32, _P, _I64, _P, _P, _P, _P, _P, _P, _P],
-    "ts_ppo_rows_stats": [_P, _I64, _P, _P, _P],
-    "ts_net_colsum": [_P, _I64, _I32, _I32, _P, _I32, _P],
-    # NPG / TRPO (npg.cu)
-    "ts_npg_fvp_rows": [_P, _P, _P, _P, _I64, _I32, _I32, _P, _P, _P],
-    "ts_npg_rows": [_P, _P, _P, _P, _P, _I64, _I32, _I32, _I32, _P, _P, _P, _P],
-    "ts_npg_kl_rows": [_P, _P, _P, _P, _I64, _I32, _I32, _P, _P],
-    "ts_npg_mean_rows": [_P, _I64, _P, _P],
-    "ts_cg_init": [_P, _P, _P, _P, _I64, _P, _P],
-    "ts_cg_step": [_P, _P, _P, _P, _I64, _D, _D, _P, _P, _P],
-    "ts_trpo_step_size": [_P, _P, _I64, _D, _D, _P, _P, _P],
-    "ts_npg_axpy": [_P, _P, _P, _D, _P, _I64, _P],
-    "ts_trpo_decide": [_P, _P, _I64, _I32, _I32, _D, _D, _P, _P, _P, _P],
-    "ts_npg_normalize_adv": [_P, _I64, _P],
-    # GAIL (gail.cu)
-    "ts_gail_reward_rows": [_P, _I64, _P, _P],
-    "ts_gail_disc_rows": [_P, _I64, _I64, _P, _P, _P],
-    # discrete SAC (discrete_sac.cu)
-    "ts_discrete_sac_rows": [_P, _P, _P, C.c_float, _I64, _I32, _P, _P, _P, _P, C.c_float, _P],
-    # CQL (cql.cu)
-    "ts_cql_rows": [_P, _P, _P, _I64, _I32, _P, _P, C.c_float, _P, C.c_float, C.c_float, _P, C.c_float, C.c_float, _P, _P, _P, _P, _P],
-    "ts_cql_losses": [_P, _P, _P, _P, _I64, _I64, C.c_float, C.c_float, _P, C.c_float, C.c_float, C.c_float, _P, _P, _P],
-    "ts_cql_target": [_P, _P, _P, C.c_float, _P, _P, C.c_float, _I64, _P, _P],
-    "ts_stack_prev_indices": [_P, _I64, _I32, _P, _I64, _P, _P, _P, _P, _P],
-    "ts_im2col_u8": [_P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _D, _P, _P],
-    "ts_im2col_f32": [_P, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P],
-    "ts_col2im_f32": [_P, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P, _P],
-    "ts_nhwc_to_nchw_flat": [_P, _I32, _I32, _I32, _P, _P],
-    "ts_nchw_flat_to_nhwc": [_P, _I32, _I32, _I32, _P, _P, _P],
-    "ts_concat2": [_P, _I32, _P, _I32, _I64, _P, _P],
-    "ts_squashed_gaussian": [_P, _I64, _P, _I64, _I32, C.c_float, C.c_float, C.c_float, _P, _P, _P, _P],
-    "ts_squashed_gaussian_bwd": [_P, _I64, _P, _P, _P, _P, _I64, _I32, C.c_float, C.c_float, C.c_float, C.c_float, _P, _P],
-    "ts_critic_mse": [_P, _P, _P, _I64, _P, _P, _P, _P],
-    "ts_dqn_loss": [_P, _P, _P, _P, _I64, _I32, C.c_float, _P, _P, _P, _P],
-    "ts_dqn_target": [_P, _P, _I64, _I32, _I32, _P, _P],
-    "ts_sac_target": [_P, _P, _P, C.c_float, _I64, _P, _P],
-    "ts_sac_actor_q_grad": [_P, _P, _P, C.c_float, _I64, _P, _P, _P, _P],
-    "ts_mean": [_P, _I64, _P, _P],
-    "ts_adam_step": [_P, _P, _P, _P, _I64, _I64, _D, _D, _D, _D, _D, _D, _P, _P],
-    "ts_adam_step_dev": [_P, _P, _P, _P, _I64, _P, _D, _D, _D, _D, _D, _D, _P, _P],
-    "ts_rmsprop_step": [_P, _P, _P, _I64, _D, _D, _D, _D, _D, _P, _P],
-    "ts_polyak_update": [_P, _P, _I64, _D, _P],
-}
-# diagnostics build only (libts_b200_diag.so, tools/): not part of the product library
-DIAG_SIGNATURES: dict[str, list[Any]] = {
-    "ts_tc_timeline": [_I32, _P],
-    "ts_umma_selftest": [_P, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P],
-}
-DIAG_LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "libts_b200_diag.so")
+
+def _ctype(decl: str, structs: dict[str, type[C.Structure]], where: str, ret: bool = False) -> Any:
+    """ctypes type of one parameter or struct member (type and name) or, with ``ret``, of a return type."""
+    tokens = [t for t in re.findall(r"\w+|\*", decl) if t != "const"]
+    names, stars = [t for t in tokens if t != "*"], tokens.count("*")
+    if not ret and len(names) > 1:
+        names.pop()                                   # the parameter's name
+    if len(names) == 1:
+        base = names[0]
+        if stars == 0 and base in _SCALARS:
+            return _SCALARS[base]
+        if stars == 0 and ret and base == "void":
+            return None
+        if stars == 1 and base in structs:
+            return C.POINTER(structs[base])
+        if stars == 1 and ret and base == "char":
+            return C.c_char_p
+        if stars == 1:
+            return C.c_void_p
+        if stars == 2:
+            return C.POINTER(C.c_void_p)
+    raise HeaderError(f"no ctypes rule for {decl.strip()!r} in: {' '.join(where.split())}")
+
+
+def _functions(text: str, structs: dict[str, type[C.Structure]]) -> dict[str, tuple[Any, list[Any]]]:
+    text = re.sub(r"^\s*#.*$", "", text, flags=re.M)      # preprocessor lines
+    decl = re.compile(r"([A-Za-z_][\w\s*]*?)\b(ts_\w+)\s*\(([^()]*)\)\s*;")
+    out = {}
+    for m in decl.finditer(text):
+        ret, name, params = m.groups()
+        args = [] if params.strip() in ("", "void") else [_ctype(p, structs, m[0]) for p in params.split(",")]
+        out[name] = (_ctype(ret, structs, m[0], ret=True), args)
+    unread = re.search(r"[^;{}]*\bts_\w+\s*\([^;]*;?", decl.sub("", text))
+    if unread:
+        raise HeaderError(f"cannot read the declaration {' '.join(unread[0].split())!r}")
+    return out
+
+
+def parse_header(text: str) -> Abi:
+    """The ABI declared by C header text in the dialect of include/ts_b200.h (no library needed)."""
+    text = re.sub(r"/\*.*?\*/|//[^\n]*", " ", text, flags=re.S)
+    consts = {k: int(v) for k, v in re.findall(r"^\s*#define\s+(TS_\w+)\s+(-?\d+)\s*$", text, flags=re.M)}
+    for body in re.findall(r"\benum\s*\{(.*?)\}", text, flags=re.S):
+        consts.update((k, int(v)) for k, v in re.findall(r"\b(TS_\w+)\s*=\s*(-?\d+)", body))
+    structs: dict[str, type[C.Structure]] = {}
+    for body, name in re.findall(r"typedef\s+struct\s*\w*\s*\{(.*?)\}\s*(\w+)\s*;", text, flags=re.S):
+        fields = []
+        for member in filter(str.strip, body.split(";")):
+            first, *more = member.split(",")          # `int64_t a_w1, a_b1, ...;`
+            ctype = _ctype(first, structs, member)
+            names = [re.findall(r"\w+", first)[-1], *(n.strip() for n in more)]
+            if not all(re.fullmatch(r"\w+", n) for n in names):
+                raise HeaderError(f"cannot read the member {' '.join(member.split())!r} of {name}")
+            fields += [(n, ctype) for n in names]
+        structs[name] = type(name, (C.Structure,), {"_fields_": fields})
+    diag = re.search(r"#ifdef\s+TS_B200_DIAGNOSTICS\b(.*?)#endif", text, flags=re.S)
+    product = text.replace(diag[0], "") if diag else text
+    return Abi(_functions(product, structs), _functions(diag[1] if diag else "", structs), structs, consts)
+
+
+with open(HEADER_PATH) as _f:
+    ABI = parse_header(_f.read())
+
+TS_F32, TS_F64 = ABI.consts["TS_F32"], ABI.consts["TS_F64"]
+AC_RELU, AC_CATEGORICAL = ABI.consts["TS_AC_RELU"], ABI.consts["TS_AC_CATEGORICAL"]
+LOSS_PPO, LOSS_A2C = ABI.consts["TS_LOSS_PPO"], ABI.consts["TS_LOSS_A2C"]
+OPT_ADAM, OPT_RMSPROP = ABI.consts["TS_OPT_ADAM"], ABI.consts["TS_OPT_RMSPROP"]
+STATS_STRIDE = ABI.consts["TS_PPO_STATS_STRIDE"]
+GRAD_EXTRA = ABI.consts["TS_PPO_GRAD_EXTRA"]
+TS_PEER_HANDLE_BYTES = ABI.consts["TS_PEER_HANDLE_BYTES"]
+ActorCriticDesc = ABI.structs["ts_actor_critic_desc"]
+PPOHParams = ABI.structs["ts_ppo_hparams"]
+
+DIAG_LIB_PATH = os.path.join(_HERE, "libts_b200_diag.so")
+_lib: C.CDLL | None = None
+
+
+def _bind(lib: C.CDLL, functions: dict[str, tuple[Any, list[Any]]]) -> C.CDLL:
+    for name, (restype, argtypes) in functions.items():
+        fn = getattr(lib, name)
+        fn.restype, fn.argtypes = restype, argtypes
+    return lib
 
 
 def use_diagnostics_library() -> C.CDLL:
@@ -164,23 +131,12 @@ def use_diagnostics_library() -> C.CDLL:
     if not os.path.exists(DIAG_LIB_PATH):
         raise ExtensionMissingError(f"{DIAG_LIB_PATH} not found: build it with `python -m tianshou_b200.csrc.build --diag`")
     _lib = None
-    lib = load_library(DIAG_LIB_PATH)
-    for name, argtypes in DIAG_SIGNATURES.items():
-        fn = getattr(lib, name)
-        fn.argtypes = argtypes
-        fn.restype = C.c_int
-    _lib = lib
-    return lib
-
-OTHER_SYMBOLS = ["ts_version", "ts_last_error", "ts_launch_count", "ts_reset_launch_count",
-                 "ts_gae_workspace_bytes", "ts_ppo_partial_rows", "ts_ppo_weight_image_bytes",
-                 "ts_ppo_peer_buffer_bytes", "ts_net_gemm_workspace_floats"]
-
-_lib: C.CDLL | None = None
+    _lib = _bind(load_library(DIAG_LIB_PATH), ABI.diag_functions)
+    return _lib
 
 
 def load_library(path: str | None = None) -> C.CDLL:
-    """dlopen the C-ABI library and attach prototypes.  Raises ExtensionMissingError loudly."""
+    """dlopen the C-ABI library and attach the header's prototypes.  Raises ExtensionMissingError loudly."""
     global _lib
     if _lib is not None and path is None:
         return _lib
@@ -190,24 +146,7 @@ def load_library(path: str | None = None) -> C.CDLL:
             f"{p} not found: build it with `python -m tianshou_b200.csrc.build` "
             "(nvcc, sm_90a).  tianshou_b200 has no CPU fallback."
         )
-    lib = C.CDLL(p)
-    for name, argtypes in SIGNATURES.items():
-        fn = getattr(lib, name)
-        fn.argtypes = argtypes
-        fn.restype = C.c_int
-    lib.ts_version.restype = C.c_int
-    lib.ts_last_error.restype = C.c_char_p
-    lib.ts_launch_count.restype = C.c_int64
-    lib.ts_reset_launch_count.restype = None
-    lib.ts_gae_workspace_bytes.argtypes = [_I64]
-    lib.ts_gae_workspace_bytes.restype = C.c_size_t
-    lib.ts_ppo_partial_rows.restype = C.c_int32
-    lib.ts_ppo_weight_image_bytes.argtypes = [C.POINTER(ActorCriticDesc)]
-    lib.ts_ppo_weight_image_bytes.restype = C.c_int64
-    lib.ts_ppo_peer_buffer_bytes.argtypes = [C.POINTER(ActorCriticDesc), _I32]
-    lib.ts_ppo_peer_buffer_bytes.restype = C.c_int64
-    lib.ts_net_gemm_workspace_floats.argtypes = [_I32, _I32, _I32]
-    lib.ts_net_gemm_workspace_floats.restype = C.c_int64
+    lib = _bind(C.CDLL(p), ABI.functions)
     if path is None:
         _lib = lib
     return lib

@@ -17,10 +17,10 @@ from typing import Any
 import torch
 from torch import nn
 
-from .._cabi import call, load_library, ptr, stream_ptr
+from .._cabi import ABI, call, load_library, ptr, stream_ptr
 from .flat_params import FlatGroup, UnsupportedModelError
 
-ACT_NONE, ACT_RELU, ACT_TANH = 0, 1, 2
+ACT_NONE, ACT_RELU, ACT_TANH = ABI.consts["TS_ACT_NONE"], ABI.consts["TS_ACT_RELU"], ABI.consts["TS_ACT_TANH"]
 
 
 def polyak_update(target: FlatGroup, source: FlatGroup, tau: float) -> None:

@@ -54,8 +54,8 @@ def broadcast_params_(flat: torch.Tensor, src: int = 0) -> torch.Tensor:
 class PeerExchange:
     """Exchange buffers of the in-kernel gradient all-reduce (``ts_ppo_epoch_multi``).
 
-    Every rank allocates one IPC-shareable buffer (``ts_peer_alloc``), the 64-byte handles travel
-    through ``all_gather`` and every rank maps its peers' buffers (``ts_peer_open``).  After that the
+    Every rank allocates one IPC-shareable buffer (``ts_peer_alloc``), the handles (``TS_PEER_HANDLE_BYTES``
+    each) travel through ``all_gather`` and every rank maps its peers' buffers (``ts_peer_open``).  After that the
     data path is kernel-only: 8-byte (value, sequence) packets over NVLink.  ``create`` is collective
     (every rank must call it) and returns None on EVERY rank when any rank cannot allocate or map
     (no P2P between the devices, IPC blocked); the caller then keeps the NCCL path.
@@ -77,9 +77,9 @@ class PeerExchange:
     def create(cls, desc, device: torch.device) -> "PeerExchange | None":
         import ctypes as C
 
-        from ._cabi import call, load_library
+        from ._cabi import TS_PEER_HANDLE_BYTES, call, load_library
         ex = cls()
-        handle = (C.c_uint8 * 64)()
+        handle = (C.c_uint8 * TS_PEER_HANDLE_BYTES)()
         ok = True
         try:   # phase 1 (local): allocate + export
             nbytes = int(load_library().ts_ppo_peer_buffer_bytes(C.byref(desc), ex.world))
@@ -94,8 +94,8 @@ class PeerExchange:
             ex.close()
             return None
         mine = torch.tensor(list(handle), dtype=torch.uint8, device=device)
-        allh = torch.empty((ex.world, 64), dtype=torch.uint8, device=device)
-        dist.all_gather_into_tensor(allh, mine.reshape(1, 64))
+        allh = torch.empty((ex.world, TS_PEER_HANDLE_BYTES), dtype=torch.uint8, device=device)
+        dist.all_gather_into_tensor(allh, mine.reshape(1, TS_PEER_HANDLE_BYTES))
         allh = allh.cpu()
         ex.ptrs = (C.c_void_p * ex.world)()
         try:   # phase 2 (local): map the peers
@@ -103,7 +103,7 @@ class PeerExchange:
                 if r == ex.rank:
                     ex.ptrs[r] = ex._own.value
                 else:
-                    h = (C.c_uint8 * 64)(*allh[r].tolist())
+                    h = (C.c_uint8 * TS_PEER_HANDLE_BYTES)(*allh[r].tolist())
                     p = C.c_void_p()
                     call("ts_peer_open", h, C.byref(p))
                     ex._opened.append(p)
