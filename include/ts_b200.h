@@ -596,6 +596,28 @@ int ts_cql_losses(const float* q1, const float* q2, const float* sq_rows, const 
 int ts_cql_target(const float* q1, const float* q2, const float* logp, float alpha, const float* rew, const float* done,
                   float gamma, int64_t B, float* out, ts_stream_t stream);
 
+/* ---- TD3 / TD3+BC (td3.cu) ---- */
+/* The deterministic actor's action rows written straight into a critic input x [B][O + A] = [obs | a]
+ * (utils/net/continuous.py:84, modelfree/td3.py:190-202): a = max_action * tanh(z) from the actor's last-layer output z [B][A];
+ * with noise [B][A] (nullable: the actor step) a += clamp(noise * policy_noise, -noise_clip, noise_clip), the clamp skipped when
+ * noise_clip <= 0 and the sum NOT clipped back to the action bounds.  Any B (grid-stride). */
+int ts_td3_act_rows(const float* z, const float* noise, int64_t B, int32_t A, float max_action, float policy_noise,
+                    float noise_clip, const float* obs, int32_t O, float* x, ts_stream_t stream);
+/* out = torch.min(q1, q2) of the two lagged critics (modelfree/td3.py:94-102); NaN propagates.  Any B (grid-stride). */
+int ts_td3_target_min(const float* q1, const float* q2, int64_t B, float* out, ts_stream_t stream);
+/* The actor loss on q = Q1(s, pi(s)) [B] (modelfree/td3.py:214-219, imitation/td3_bc.py:113-120), one block, fixed-order sums
+ * (bit-identical from run to run).  act (nullable) [B][A]: the batch actions of TD3+BC, with pi = max_action * tanh(z):
+ *   act == NULL : *loss = -mean(q);                                              dq[b] = -1 / B
+ *   act != NULL : lmbda = alpha / mean|q| (detached); *loss = -lmbda mean(q) + mean((pi - act)^2);  dq[b] = -lmbda / B
+ * Every row of dq [B] is written. */
+int ts_td3_actor_rows(const float* q, const float* z, const float* act, int64_t B, int32_t A, float max_action, float alpha,
+                      float* dq, float* loss, ts_stream_t stream);
+/* Backward of pi = max_action * tanh(z) (and of TD3+BC's F.mse_loss(pi, act) when act is given):
+ * dz = (dact + [act] 2 (pi - act) / (B A)) * max_action * (1 - tanh(z)^2); dact [B][A] = d loss / d pi through critic 1.
+ * Any B (grid-stride). */
+int ts_td3_actor_head_bwd(const float* z, const float* dact, const float* act, int64_t B, int32_t A, float max_action, float* dz,
+                          ts_stream_t stream);
+
 #ifdef TS_B200_DIAGNOSTICS
 /* Diagnostics build only (libts_b200_diag.so, `python -m tianshou_b200.csrc.build --diag`): not part of the product library. */
 /* Hardware self-test of the wgmma building blocks (csrc/wgmma.cuh), one CTA:

@@ -1,18 +1,19 @@
 from .base import Algorithm, OfflineAlgorithm, OffPolicyAlgorithm, OnPolicyAlgorithm, Policy, TrainingStats
 from .flat_params import UnsupportedModelError
-from .imitation import CQL, GAIL, CQLTrainingStats, GailTrainingStats
+from .imitation import CQL, GAIL, TD3BC, CQLTrainingStats, GailTrainingStats
 from .modelfree.a2c import A2CTrainingStats, ActorCriticOnPolicyAlgorithm
 from .modelfree.discrete_sac import DiscreteSAC
 from .modelfree.npg import NPG, NPGTrainingStats
 from .modelfree.ppo import A2C, PPO
 from .modelfree.reinforce import DiscreteActorPolicy, ProbabilisticActorPolicy
+from .modelfree.td3 import TD3, TD3TrainingStats
 from .modelfree.trpo import TRPO, TRPOTrainingStats
 from .optim import AdamOptimizerFactory, LRSchedulerFactoryLinear, OptimizerFactory, RMSpropOptimizerFactory
 
 __all__ = [
     "Algorithm", "OfflineAlgorithm", "OffPolicyAlgorithm", "OnPolicyAlgorithm", "Policy", "TrainingStats",
     "UnsupportedModelError", "A2CTrainingStats", "ActorCriticOnPolicyAlgorithm", "PPO", "A2C", "NPG", "TRPO", "NPGTrainingStats", "TRPOTrainingStats",
-    "GAIL", "GailTrainingStats", "DiscreteSAC", "CQL", "CQLTrainingStats",
+    "GAIL", "GailTrainingStats", "DiscreteSAC", "CQL", "CQLTrainingStats", "TD3", "TD3TrainingStats", "TD3BC",
     "ProbabilisticActorPolicy", "DiscreteActorPolicy", "AdamOptimizerFactory", "LRSchedulerFactoryLinear", "OptimizerFactory",
     "RMSpropOptimizerFactory",
 ]

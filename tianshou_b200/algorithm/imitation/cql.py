@@ -29,8 +29,9 @@ from ..._cabi import call, ptr, stream_ptr
 from ...data import Batch, ReplayBuffer
 from ..base import OfflineAlgorithm
 from ..flat_params import FlatGroup
-from ..modelfree.sac import Alpha, ContinuousTwinCritic, SACPolicy, SACTrainingStats
+from ..modelfree.sac import Alpha, SACPolicy, SACTrainingStats, SquashedGaussianTwinCritic
 from ..optim import OptimizerFactory
+from ..twin_critic import _EvalModeModule
 
 
 @dataclass(kw_only=True)
@@ -41,23 +42,7 @@ class CQLTrainingStats(SACTrainingStats):
     cql_alpha_loss: float | None = None
 
 
-class _EvalModeModule(nn.Module):
-    """A lagged network as the reference holds it (utils/lagged_network.py:21-41): the copy under ``.module``, always in eval
-    mode, so ``state_dict()`` has the reference's ``critic_old.module.*`` keys."""
-
-    def __init__(self, module: nn.Module) -> None:
-        super().__init__()
-        self.module = module.eval()
-
-    def train(self, mode: bool = True) -> "_EvalModeModule":
-        super().train(False)
-        return self
-
-    def forward(self, *args: Any, **kwargs: Any) -> Any:
-        return self.module(*args, **kwargs)
-
-
-class CQL(ContinuousTwinCritic, OfflineAlgorithm):
+class CQL(SquashedGaussianTwinCritic, OfflineAlgorithm):
     """Conservative Q-learning (arXiv:2006.04779), reference API and semantics (cql.py:32-400).
 
     The update reproduces what ``CQL._update_with_batch`` computes:
@@ -152,6 +137,10 @@ class CQL(ContinuousTwinCritic, OfflineAlgorithm):
             buffer._meta = Batch(**buffer._meta.__dict__, calibration_returns=returns)
             buffer.__dict__.get("_dev_cache", {}).pop("calibration_returns", None)     # device_array() uploads the new key
         return buffer
+
+    def _preprocess_batch(self, batch: Batch, buffer: ReplayBuffer, indices: np.ndarray) -> Batch:
+        """Nothing: CQL's one-step target is part of its update (cql.py:282-292), there is no n-step return."""
+        return batch
 
     def _sample(self, buffer: ReplayBuffer, sample_size: int | None) -> tuple[Batch, Any]:
         """Indices from the buffer's host RNG streams (identical to the reference's draws); rows stay on the device."""

@@ -11,9 +11,10 @@ Per ``update(buffer, sample_size)``:
          forward -> ``ts_sac_target`` -> ``ts_nstep_return``; per critic forward / loss / backward (``ts_net_gemm``) + Adam;
          actor forward, critics' input-gradient GEMMs (the second accumulating into the first), tanh-Gaussian head backward,
          actor backward + Adam; Polyak axpy.
-Every Linear layer's forward / input gradient / weight gradient is one wgmma GEMM launch (csrc/net_gemm.cu).  The networks,
-the actor forward, the critic pair and the actor step are ``ContinuousTwinCritic``'s, shared with CQL (imitation/cql.py); it
-stands on the twin-critic core of twin_critic.py.
+Every Linear layer's forward / input gradient / weight gradient is one wgmma GEMM launch (csrc/net_gemm.cu).  The critic pair,
+the row reads, the critic step and the n-step target are ``ContinuousTwinCritic``'s, shared with CQL and TD3; the actor forward
+and the actor step are ``SquashedGaussianTwinCritic``'s, shared with CQL (imitation/cql.py); both stand on the twin-critic core
+of twin_critic.py.
 """
 from __future__ import annotations
 
@@ -185,31 +186,58 @@ def describe_gaussian_actor(actor: Any, obs_dim: int) -> tuple[list[_Layer], lis
 
 
 class ContinuousTwinCritic(TwinCriticAlgorithm):
-    """The tanh-squashed Gaussian actor and the two Q(s, a) critics SAC and CQL share: building them, the actor forward,
-    both critics on concat(obs, act), and SAC's actor step."""
+    """What the continuous twin-critic algorithms (SAC, CQL, TD3, TD3+BC) share: two Q(s, a) critics on concat(obs, act), the
+    row reads, the critics' squared-loss step and the n-step target.  The subclass supplies ``_describe_actor(actor, obs_dim)``
+    (layer chain, parameters in flat order, action width) and, for the n-step target, ``_target_q``."""
+
+    _cols_override: Any = None          # the mirror's columns while a graphed body runs (no cross-stream wait inside a capture)
+
+    def _describe_actor(self, actor: nn.Module, obs_dim: int) -> tuple[list[_Layer], list[nn.Parameter], int]:
+        raise NotImplementedError
 
     def _build_networks(self, *, lagged: tuple[nn.Module, nn.Module], policy_optim: OptimizerFactory,
                         critic_optim: OptimizerFactory, critic2_optim: OptimizerFactory | None,
-                        max_grad_norm: float | None = None) -> None:
+                        max_grad_norm: float | None = None, lagged_actor: nn.Module | None = None) -> None:
         def describe_actor(actor: nn.Module) -> tuple[list[_Layer], list[nn.Parameter]]:
             self.obs_dim = int(module_layers(actor.preprocess)[0].in_features)
-            layers, params, self.act_dim = describe_gaussian_actor(actor, self.obs_dim)
+            layers, params, self.act_dim = self._describe_actor(actor, self.obs_dim)
             return layers, params
 
         self._build_twin_critic(describe_actor=describe_actor,
                                 describe_critic=lambda net, _: describe_q_critic(net, self.obs_dim, self.act_dim), lagged=lagged,
                                 policy_optim=policy_optim, critic_optim=critic_optim, critic2_optim=critic2_optim,
-                                max_grad_norm=max_grad_norm)
+                                max_grad_norm=max_grad_norm, lagged_actor=lagged_actor)
 
-    def _actor_forward(self, obs: torch.Tensor, tag: str) -> tuple[list[torch.Tensor], torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
-        """policy(batch) on the device (sac.py:108-131): returns (activations, act, log_prob, sigma, noise)."""
-        B, A = obs.shape[0], self.act_dim
-        acts = self._actor.forward(obs, B, tag)
-        noise = self._noise_fn((B, A)).to(self._dev, torch.float32).contiguous()
-        act, logp, sigma = self._buf(tag + "_act", (B, A)), self._buf(tag + "_logp", B), self._buf(tag + "_sigma", (B, A))
-        call("ts_squashed_gaussian", ptr(acts[-1]), 2 * A, ptr(noise), B, A, SIGMA_MIN, SIGMA_MAX, _F32_EPS, ptr(act), ptr(logp),
-             ptr(sigma), stream_ptr(self._dev))
-        return acts, act, logp, sigma, noise
+    def _rows(self, buffer: ReplayBuffer, key: str, indices: np.ndarray | torch.Tensor) -> torch.Tensor:
+        """buffer[key][indices] as a dense fp32 [I, width] device tensor: gathered from the device mirror when the
+        buffer keeps one (no host traffic), else a host gather of the sampled rows + one upload."""
+        from ... import ops
+        return ops.buffer_rows(buffer, key, indices, self._dev, cols=self._cols_override)
+
+    def _obs_next_rows(self, buffer: ReplayBuffer, indices: np.ndarray | torch.Tensor) -> torch.Tensor:
+        """``buffer[indices].obs_next``: the stored column, or ``obs`` at ``buffer.next(indices)``."""
+        if buffer._save_obs_next:
+            obs_next = self._rows(buffer, "obs_next", indices)
+        else:
+            obs_next = self._rows(buffer, "obs", buffer.next(indices))
+        return obs_next.contiguous()
+
+    def _sample(self, buffer: ReplayBuffer, sample_size: int | None) -> tuple[Batch, Any]:
+        """Indices from the buffer's host RNG streams (identical to the reference's draws); rows stay on the device."""
+        indices = buffer.sample_indices(sample_size)
+        batch = Batch()
+        batch.__dict__["obs"] = self._rows(buffer, "obs", indices).contiguous()
+        batch.__dict__["act"] = self._rows(buffer, "act", indices).contiguous()
+        weight = per_weight(buffer, indices, self._dev)
+        if weight is not None:
+            batch.__dict__["weight"] = weight
+        batch.__dict__["info"] = Batch()
+        return batch, indices
+
+    def _preprocess_batch(self, batch: Batch, buffer: ReplayBuffer, indices: np.ndarray) -> Batch:
+        """The n-step return of ``_target_q`` into ``batch.returns`` (ddpg.py:287-302)."""
+        return self.compute_nstep_return(batch=batch, buffer=buffer, indices=indices, target_q_fn=self._target_q,
+                                         gamma=self.gamma, n_step=self.n_step_return_horizon)
 
     def _concat(self, obs: torch.Tensor, act: torch.Tensor, out: torch.Tensor) -> None:
         call("ts_concat2", ptr(obs), self.obs_dim, ptr(act), self.act_dim, obs.shape[0], ptr(out), stream_ptr(self._dev))
@@ -220,6 +248,39 @@ class ContinuousTwinCritic(TwinCriticAlgorithm):
         x = self._buf(f"{tag}_x", (B, self.obs_dim + self.act_dim))
         self._concat(obs, act, x)
         return [self._lagged_forward(k, x, B, tag) if target else self._c[k].forward(x, B, tag) for k in range(2)]
+
+    def _critic_step(self, k: int, x: torch.Tensor, returns: torch.Tensor, weight: torch.Tensor | None, optim: Any,
+                     out_loss: torch.Tensor) -> torch.Tensor:
+        """``_minimize_critic_squared_loss`` (ddpg.py:267-285) on the critic input x = concat(obs, act): forward, weighted
+        MSE, backward, Adam."""
+        B = x.shape[0]
+        st = stream_ptr(self._dev)
+        acts = self._c[k].forward(x, B, "cu")
+        td = self._buf(f"td{k}", B)
+        dq = self._buf("dq", (B, 1))
+        rows = self._buf("loss_rows", B)
+        call("ts_critic_mse", ptr(acts[-1]), ptr(returns), ptr(weight), B, ptr(td), ptr(dq), ptr(rows), st)
+        call("ts_mean", ptr(rows), B, ptr(out_loss), st)
+        self._c[k].backward(acts, dq, B, "cu")
+        self._adam(self._g_c[k], optim._optim, optim._max_grad_norm)
+        return td
+
+
+class SquashedGaussianTwinCritic(ContinuousTwinCritic):
+    """The tanh-squashed Gaussian actor SAC and CQL share: its description, its forward and SAC's actor step."""
+
+    def _describe_actor(self, actor: nn.Module, obs_dim: int) -> tuple[list[_Layer], list[nn.Parameter], int]:
+        return describe_gaussian_actor(actor, obs_dim)
+
+    def _actor_forward(self, obs: torch.Tensor, tag: str) -> tuple[list[torch.Tensor], torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
+        """policy(batch) on the device (sac.py:108-131): returns (activations, act, log_prob, sigma, noise)."""
+        B, A = obs.shape[0], self.act_dim
+        acts = self._actor.forward(obs, B, tag)
+        noise = self._noise_fn((B, A)).to(self._dev, torch.float32).contiguous()
+        act, logp, sigma = self._buf(tag + "_act", (B, A)), self._buf(tag + "_logp", B), self._buf(tag + "_sigma", (B, A))
+        call("ts_squashed_gaussian", ptr(acts[-1]), 2 * A, ptr(noise), B, A, SIGMA_MIN, SIGMA_MAX, _F32_EPS, ptr(act), ptr(logp),
+             ptr(sigma), stream_ptr(self._dev))
+        return acts, act, logp, sigma, noise
 
     def _actor_step(self, obs: torch.Tensor, alpha: float, out_loss: torch.Tensor) -> torch.Tensor:
         """SAC's actor step against the current critics: L = mean(alpha * log pi(a|s) - min(Q1, Q2)(s, a)) with
@@ -245,7 +306,7 @@ class ContinuousTwinCritic(TwinCriticAlgorithm):
         return logp
 
 
-class SAC(ContinuousTwinCritic, OffPolicyAlgorithm):
+class SAC(SquashedGaussianTwinCritic, OffPolicyAlgorithm):
     """Soft Actor-Critic (arXiv:1801.01290 / 1812.05905), reference API (sac.py:218-336)."""
 
     def __init__(self, *, policy: SACPolicy, policy_optim: OptimizerFactory, critic: nn.Module, critic_optim: OptimizerFactory,
@@ -276,21 +337,10 @@ class SAC(ContinuousTwinCritic, OffPolicyAlgorithm):
         dev = self._dev
         self._noise_fn = lambda shape: torch.normal(torch.zeros(shape, device=dev), torch.ones(shape, device=dev))
 
-    # ------------------------------------------------------------------ helpers
-    def _rows(self, buffer: ReplayBuffer, key: str, indices: np.ndarray | torch.Tensor) -> torch.Tensor:
-        """buffer[key][indices] as a dense fp32 [I, width] device tensor: gathered from the device mirror when the
-        buffer keeps one (no host traffic), else a host gather of the sampled rows + one upload."""
-        from ... import ops
-        return ops.buffer_rows(buffer, key, indices, self._dev, cols=self._cols_override)
-
     # ------------------------------------------------------------------ target
     def _target_q(self, buffer: ReplayBuffer, indices: np.ndarray) -> torch.Tensor:
         """min(Q1', Q2')(s', a') - alpha * log pi(a'|s') with a' ~ pi(.|s')   (ddpg.py:327-339, td3.py:94-102, sac.py:298-302)"""
-        if buffer._save_obs_next:
-            obs_next = self._rows(buffer, "obs_next", indices)
-        else:
-            obs_next = self._rows(buffer, "obs", buffer.next(indices))
-        obs_next = obs_next.contiguous()
+        obs_next = self._obs_next_rows(buffer, indices)
         B = obs_next.shape[0]
         _, act, logp, _, _ = self._actor_forward(obs_next, "tq")
         t_acts = self._q_pair(obs_next, act, "tq", target=True)
@@ -298,39 +348,6 @@ class SAC(ContinuousTwinCritic, OffPolicyAlgorithm):
         call("ts_sac_target", ptr(t_acts[0][-1]), ptr(t_acts[1][-1]), ptr(logp), float(self.alpha.value), B, ptr(out),
              stream_ptr(self._dev))
         return out
-
-    def _preprocess_batch(self, batch: Batch, buffer: ReplayBuffer, indices: np.ndarray) -> Batch:
-        return self.compute_nstep_return(batch=batch, buffer=buffer, indices=indices, target_q_fn=self._target_q,
-                                         gamma=self.gamma, n_step=self.n_step_return_horizon)
-
-    def _sample(self, buffer: ReplayBuffer, sample_size: int | None) -> tuple[Batch, Any]:
-        """Indices from the buffer's host RNG streams (identical to the reference's draws); rows stay on the device."""
-        indices = buffer.sample_indices(sample_size)
-        batch = Batch()
-        batch.__dict__["obs"] = self._rows(buffer, "obs", indices).contiguous()
-        batch.__dict__["act"] = self._rows(buffer, "act", indices).contiguous()
-        weight = per_weight(buffer, indices, self._dev)
-        if weight is not None:
-            batch.__dict__["weight"] = weight
-        batch.__dict__["info"] = Batch()
-        return batch, indices
-
-    # ------------------------------------------------------------------ update
-    def _critic_step(self, k: int, x: torch.Tensor, returns: torch.Tensor, weight: torch.Tensor | None, optim: Any,
-                     out_loss: torch.Tensor) -> torch.Tensor:
-        """``_minimize_critic_squared_loss`` (ddpg.py:267-285) on the critic input x = concat(obs, act): forward, weighted
-        MSE, backward, Adam."""
-        B = x.shape[0]
-        st = stream_ptr(self._dev)
-        acts = self._c[k].forward(x, B, "cu")
-        td = self._buf(f"td{k}", B)
-        dq = self._buf("dq", (B, 1))
-        rows = self._buf("loss_rows", B)
-        call("ts_critic_mse", ptr(acts[-1]), ptr(returns), ptr(weight), B, ptr(td), ptr(dq), ptr(rows), st)
-        call("ts_mean", ptr(rows), B, ptr(out_loss), st)
-        self._c[k].backward(acts, dq, B, "cu")
-        self._adam(self._g_c[k], optim._optim, optim._max_grad_norm)
-        return td
 
     def _update_with_batch(self, batch: Batch) -> SACTrainingStats:
         dev = self._dev
@@ -356,7 +373,6 @@ class SAC(ContinuousTwinCritic, OffPolicyAlgorithm):
 
     # ------------------------------------------------------------------ CUDA-graph mode
     _in_graph_body = False
-    _cols_override: Any = None          # the mirror's columns while the graphed body runs (no cross-stream wait inside a capture)
 
     def _graph_usable(self, buffer: ReplayBuffer) -> bool:
         cols = buffer.device_columns() if hasattr(buffer, "device_columns") else None

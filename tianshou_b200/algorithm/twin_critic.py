@@ -1,9 +1,10 @@
-"""What the twin-critic algorithms (SAC, discrete SAC, CQL) share: one actor and two (critic, lagged critic) pairs as flat
-groups on one CUDA device, their three optimisers, the scratch, the one Adam seam, the lagged forward and Polyak; plus the
-sampling helpers the off-policy algorithms share with DQN.
+"""What the twin-critic algorithms (SAC, discrete SAC, CQL, TD3, TD3+BC) share: one actor (with an optional lagged copy) and
+two (critic, lagged critic) pairs as flat groups on one CUDA device, their three optimisers, the scratch, the one Adam seam,
+the lagged forwards and Polyak; plus the sampling helpers the off-policy algorithms share with DQN.
 
-Reference: modelfree/td3.py:40-92 (dual critics, ``critic2=None`` deep-copies the critic), utils/lagged_network.py:8-80
-(Polyak), data/buffer/prio.py:104-106 (the importance weight of a prioritised sample).
+Reference: modelfree/td3.py:40-92 (dual critics, ``critic2=None`` deep-copies the critic), :183 (TD3's lagged actor),
+utils/lagged_network.py:8-80 (Polyak, the lagged copy under ``.module``), data/buffer/prio.py:104-106 (the importance weight of
+a prioritised sample).
 """
 from __future__ import annotations
 
@@ -70,6 +71,22 @@ def sample_discrete(buffer: ReplayBuffer, sample_size: int | None, obs_source: C
     return batch, indices
 
 
+class _EvalModeModule(nn.Module):
+    """A lagged network as the reference holds it (utils/lagged_network.py:21-41): the copy under ``.module``, always in eval
+    mode, so ``state_dict()`` has the reference's ``critic_old.module.*`` keys."""
+
+    def __init__(self, module: nn.Module) -> None:
+        super().__init__()
+        self.module = module.eval()
+
+    def train(self, mode: bool = True) -> "_EvalModeModule":
+        super().train(False)
+        return self
+
+    def forward(self, *args: Any, **kwargs: Any) -> Any:
+        return self.module(*args, **kwargs)
+
+
 def _group_adam_step(group: FlatGroup, optimizer: torch.optim.Optimizer, max_grad_norm: float | None) -> None:
     """The default Adam seam: the group's own ``adam_step``, looked up on the instance, so a step replaced on one group (to
     record its gradient, say) is the one the update takes."""
@@ -77,19 +94,23 @@ def _group_adam_step(group: FlatGroup, optimizer: torch.optim.Optimizer, max_gra
 
 
 class TwinCriticAlgorithm(Algorithm):
-    """An actor and two critics with a lagged copy each, stepped on the device.  The subclass assigns ``critic``,
-    ``critic2``, their lagged modules ``critic_old`` / ``critic2_old`` and ``tau``, then calls ``_build_twin_critic``."""
+    """An actor and two critics with a lagged copy each (and optionally a lagged actor), stepped on the device.  The subclass
+    assigns ``critic``, ``critic2``, their lagged modules ``critic_old`` / ``critic2_old`` and ``tau``, then calls
+    ``_build_twin_critic``."""
 
     def _build_twin_critic(self, *, describe_actor: Describe, describe_critic: Describe, lagged: tuple[nn.Module, nn.Module],
                            policy_optim: OptimizerFactory, critic_optim: OptimizerFactory,
-                           critic2_optim: OptimizerFactory | None, max_grad_norm: float | None = None) -> None:
+                           critic2_optim: OptimizerFactory | None, max_grad_norm: float | None = None,
+                           lagged_actor: nn.Module | None = None) -> None:
         """``describe_actor(actor)`` and ``describe_critic(net, role)`` return (layer chain, parameters in flat order);
-        ``lagged`` are the lagged critics as ``describe_critic`` reads them.  ``critic2_optim`` defaults to ``critic_optim``;
-        ``max_grad_norm`` clips both critics' steps."""
+        ``lagged`` are the lagged critics as ``describe_critic`` reads them, ``lagged_actor`` (None: there is none) the lagged
+        actor as ``describe_actor`` reads it.  ``critic2_optim`` defaults to ``critic_optim``; ``max_grad_norm`` clips both
+        critics' steps."""
         dev = self._dev = cuda_device_of(self.policy.actor, self.critic, self.critic2)
         a_layers, a_params = describe_actor(self.policy.actor)
         self._g_actor = FlatGroup(a_params, dev)
         self._actor = FusedStack(a_layers, self._g_actor, "actor")
+        self._g_at = None if lagged_actor is None else FlatGroup(describe_actor(lagged_actor)[1], dev)
         self._g_c, self._c, self._g_ct = [], [], []
         for name, src, tgt in (("critic", self.critic, lagged[0]), ("critic2", self.critic2, lagged[1])):
             layers, params = describe_critic(src, name)
@@ -112,7 +133,15 @@ class TwinCriticAlgorithm(Algorithm):
         self._g_ct[k].ensure_adopted()
         return self._c[k].forward(x, rows, tag, frames=frames, params=self._g_ct[k].flat)
 
+    def _lagged_actor_forward(self, x: torch.Tensor, rows: int, tag: str) -> list[torch.Tensor]:
+        """The lagged actor on ``x``: its activation list."""
+        self._g_at.ensure_adopted()
+        return self._actor.forward(x, rows, tag, params=self._g_at.flat)
+
     def _polyak(self) -> None:
-        """``_update_lagged_network_weights``: both lagged critics toward their critics by ``tau``."""
+        """``_update_lagged_network_weights``: both lagged critics (and the lagged actor, when there is one) toward their
+        networks by ``tau``."""
         for k in range(2):
             polyak_update(self._g_ct[k], self._g_c[k], self.tau)
+        if self._g_at is not None:
+            polyak_update(self._g_at, self._g_actor, self.tau)

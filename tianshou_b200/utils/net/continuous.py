@@ -1,4 +1,4 @@
-"""Gaussian actor / state-value critic heads (API of tianshou/utils/net/continuous.py:96-238)."""
+"""Deterministic and Gaussian actors / critic heads (API of tianshou/utils/net/continuous.py:28-238)."""
 from __future__ import annotations
 
 import warnings
@@ -14,6 +14,34 @@ from .common import MLP, ModuleWithVectorOutput, TLinearLayer
 
 SIGMA_MIN = -20
 SIGMA_MAX = 2
+
+
+class AbstractContinuousActorDeterministic(ModuleWithVectorOutput):
+    """Marker interface for continuous deterministic actors (DDPG like), continuous.py:28-29."""
+
+
+class ContinuousActorDeterministic(AbstractContinuousActorDeterministic):
+    """s -> ``max_action * tanh(last(preprocess(s)))`` (continuous.py:32-85): the actor of DDPG / TD3 / TD3+BC.  The submodules
+    and their order are the reference's, so ``state_dict()`` keys and seeded initial weights match."""
+
+    def __init__(self, *, preprocess_net: ModuleWithVectorOutput, action_shape: Any, hidden_sizes: Sequence[int] = (),
+                 max_action: float = 1.0) -> None:
+        output_dim = int(np.prod(action_shape))
+        super().__init__(output_dim)
+        self.preprocess = preprocess_net
+        self.last = MLP(input_dim=preprocess_net.get_output_dim(), output_dim=self.output_dim, hidden_sizes=hidden_sizes)
+        self.max_action = max_action
+
+    def get_preprocess_net(self) -> ModuleWithVectorOutput:
+        return self.preprocess
+
+    def get_output_dim(self) -> int:
+        return self.output_dim
+
+    def forward(self, obs: Any, state: Any = None, info: dict[str, Any] | None = None) -> tuple[torch.Tensor, Any]:
+        action_BA, hidden_BH = self.preprocess(obs, state)
+        action_BA = self.max_action * torch.tanh(self.last(action_BA))
+        return action_BA, hidden_BH
 
 
 class ContinuousCritic(ModuleWithVectorOutput):
