@@ -618,6 +618,48 @@ int ts_td3_actor_rows(const float* q, const float* z, const float* act, int64_t 
 int ts_td3_actor_head_bwd(const float* z, const float* dact, const float* act, int64_t B, int32_t A, float max_action, float* dz,
                           ts_stream_t stream);
 
+/* ---- BCQ (bcq.cu) ---- */
+/* The VAE's reparameterisation (utils/net/continuous.py:464-470): from head = [mean | log_std_raw] [B][2L] and eps [B][L],
+ * std = exp(clamp(log_std_raw, -4, 15)) into std_out [B][L] and z = mean + std * eps straight into the decoder input
+ * x [B][O + L] = [s | z].  Any B (grid-stride). */
+int ts_bcq_vae_reparam(const float* head, const float* eps, int64_t B, int32_t L, const float* s, int32_t O, float* std_out,
+                       float* x, ts_stream_t stream);
+/* The VAE loss (imitation/bcq.py:202-206) on the decoder output y [B][A], one block, fixed-order sums (bit-identical from run to
+ * run): *loss = mean((act - recon)^2) + mean(-log std + (std^2 + mean^2 - 1) / 2) / 2 with recon = max_action * tanh(y);
+ * dy [B][A] = d loss / d y (the KL term does not reach y). */
+int ts_bcq_vae_loss(const float* y, const float* act, const float* head, const float* std_in, int64_t B, int32_t A, int32_t L,
+                    float max_action, float* dy, float* loss, ts_stream_t stream);
+/* The backward of the VAE head: from dz [B][L] (the decoder's input gradient over the z columns) and the KL term,
+ * dhead [B][2L] = d loss / d [mean | log_std_raw]; the log_std clamp passes the gradient at its bounds (torch's clamp).  Any B. */
+int ts_bcq_vae_head_bwd(const float* head, const float* std_in, const float* eps, const float* dz, int64_t B, int32_t L,
+                        float* dhead, ts_stream_t stream);
+/* The decoder input of VAE.decode with a drawn latent (continuous.py:481-490, bcq.py:213-217): x [B N][O + L] =
+ * [s[r / N] | clamp(z[r], -clip, clip)], the repeat_interleave of s fused in.  Any B. */
+int ts_bcq_decode_input(const float* s, int64_t B, int32_t N, int32_t O, const float* z, int32_t L, float clip, float* x,
+                        ts_stream_t stream);
+/* Decoded actions beside their states: x [rows][O + A] = [s[r step] | max_action * tanh(y[r step])], s with row stride lds,
+ * y [.][A] the decoder output.  step > 1 picks one row per group of step rows.  Any rows. */
+int ts_bcq_act_rows(const float* s, int64_t lds, const float* y, int64_t step, int64_t rows, int32_t O, int32_t A,
+                    float max_action, float* x, ts_stream_t stream);
+/* Perturbation.forward (continuous.py:407-412) into a critic input x [rows][O + A] = [s[r] | clamp(a + phi_m tanh(logits[r / S]),
+ * -max_action, max_action)] with the decoded action a = vae_max * tanh(y[r]), phi_m = phi * max_action and max_action the
+ * perturbation's; S = 1 gives every row its own logits (a Net preprocess), S = the group size broadcasts one logits row over
+ * the group (an MLP preprocess's row 0).  Any rows. */
+int ts_bcq_perturb(const float* logits, int64_t S, const float* y, int64_t rows, int32_t A, float vae_max, float max_action,
+                   float phi_m, const float* s, int64_t lds, int32_t O, float* x, ts_stream_t stream);
+/* Backward of ts_bcq_perturb to dlogits [G][A] from dact [G S][A] = d loss / d perturbed action: per group a fixed-order sum of
+ * dact where the clamp passed (inclusive bounds), times phi_m * (1 - tanh(logits)^2).  Any G. */
+int ts_bcq_perturb_bwd(const float* logits, int64_t S, int64_t G, const float* y, const float* dact, int32_t A, float vae_max,
+                       float max_action, float phi_m, float* dlogits, ts_stream_t stream);
+/* BCQ's one-step target (bcq.py:222-237): out[b] = rew[b] + logical_not(done[b]) * gamma * max over the N rows of group b of
+ * lmbda * min(q1, q2) + one_minus_lmbda * max(q1, q2), fp32 in torch's order; NaN propagates.  rew / done fp32 [B]. */
+int ts_bcq_target(const float* q1, const float* q2, int64_t B, int32_t N, float lmbda, float one_minus_lmbda, const float* rew,
+                  const float* done, float gamma, float* out, ts_stream_t stream);
+/* BCQPolicy's choice (bcq.py:111-114): per group g of S rows of q, the first index of the maximum (a NaN is the maximum, as in
+ * torch.argmax); act [G][A] = that row's columns col0 .. col0 + A of x (row stride ldx), idx [G] (nullable) = the index. */
+int ts_bcq_select(const float* q, int64_t G, int64_t S, const float* x, int64_t ldx, int32_t col0, int32_t A, float* act,
+                  int64_t* idx, ts_stream_t stream);
+
 #ifdef TS_B200_DIAGNOSTICS
 /* Diagnostics build only (libts_b200_diag.so, `python -m tianshou_b200.csrc.build --diag`): not part of the product library. */
 /* Hardware self-test of the wgmma building blocks (csrc/wgmma.cuh), one CTA:

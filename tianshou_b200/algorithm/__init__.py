@@ -1,6 +1,6 @@
 from .base import Algorithm, OfflineAlgorithm, OffPolicyAlgorithm, OnPolicyAlgorithm, Policy, TrainingStats
 from .flat_params import UnsupportedModelError
-from .imitation import CQL, GAIL, TD3BC, CQLTrainingStats, GailTrainingStats
+from .imitation import BCQ, CQL, GAIL, TD3BC, BCQPolicy, BCQTrainingStats, CQLTrainingStats, GailTrainingStats
 from .modelfree.a2c import A2CTrainingStats, ActorCriticOnPolicyAlgorithm
 from .modelfree.discrete_sac import DiscreteSAC
 from .modelfree.npg import NPG, NPGTrainingStats
@@ -13,7 +13,7 @@ from .optim import AdamOptimizerFactory, LRSchedulerFactoryLinear, OptimizerFact
 __all__ = [
     "Algorithm", "OfflineAlgorithm", "OffPolicyAlgorithm", "OnPolicyAlgorithm", "Policy", "TrainingStats",
     "UnsupportedModelError", "A2CTrainingStats", "ActorCriticOnPolicyAlgorithm", "PPO", "A2C", "NPG", "TRPO", "NPGTrainingStats", "TRPOTrainingStats",
-    "GAIL", "GailTrainingStats", "DiscreteSAC", "CQL", "CQLTrainingStats", "TD3", "TD3TrainingStats", "TD3BC",
+    "GAIL", "GailTrainingStats", "DiscreteSAC", "BCQ", "BCQPolicy", "BCQTrainingStats", "CQL", "CQLTrainingStats", "TD3", "TD3TrainingStats", "TD3BC",
     "ProbabilisticActorPolicy", "DiscreteActorPolicy", "AdamOptimizerFactory", "LRSchedulerFactoryLinear", "OptimizerFactory",
     "RMSpropOptimizerFactory",
 ]

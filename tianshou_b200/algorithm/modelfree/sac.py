@@ -197,16 +197,19 @@ class ContinuousTwinCritic(TwinCriticAlgorithm):
 
     def _build_networks(self, *, lagged: tuple[nn.Module, nn.Module], policy_optim: OptimizerFactory,
                         critic_optim: OptimizerFactory, critic2_optim: OptimizerFactory | None,
-                        max_grad_norm: float | None = None, lagged_actor: nn.Module | None = None) -> None:
+                        max_grad_norm: float | None = None, lagged_actor: nn.Module | None = None,
+                        actor: nn.Module | None = None, obs_dim: int | None = None) -> None:
+        """``actor`` / ``obs_dim``: an actor other than ``policy.actor`` and the observation width, for an actor without a
+        ``preprocess`` net on the observations alone (BCQ's perturbation network reads [s | a])."""
         def describe_actor(actor: nn.Module) -> tuple[list[_Layer], list[nn.Parameter]]:
-            self.obs_dim = int(module_layers(actor.preprocess)[0].in_features)
+            self.obs_dim = int(module_layers(actor.preprocess)[0].in_features) if obs_dim is None else obs_dim
             layers, params, self.act_dim = self._describe_actor(actor, self.obs_dim)
             return layers, params
 
         self._build_twin_critic(describe_actor=describe_actor,
                                 describe_critic=lambda net, _: describe_q_critic(net, self.obs_dim, self.act_dim), lagged=lagged,
                                 policy_optim=policy_optim, critic_optim=critic_optim, critic2_optim=critic2_optim,
-                                max_grad_norm=max_grad_norm, lagged_actor=lagged_actor)
+                                max_grad_norm=max_grad_norm, lagged_actor=lagged_actor, actor=actor)
 
     def _rows(self, buffer: ReplayBuffer, key: str, indices: np.ndarray | torch.Tensor) -> torch.Tensor:
         """buffer[key][indices] as a dense fp32 [I, width] device tensor: gathered from the device mirror when the

@@ -1,4 +1,4 @@
-"""What the twin-critic algorithms (SAC, discrete SAC, CQL, TD3, TD3+BC) share: one actor (with an optional lagged copy) and
+"""What the twin-critic algorithms (SAC, discrete SAC, CQL, TD3, TD3+BC, BCQ) share: one actor (with an optional lagged copy) and
 two (critic, lagged critic) pairs as flat groups on one CUDA device, their three optimisers, the scratch, the one Adam seam,
 the lagged forwards and Polyak; plus the sampling helpers the off-policy algorithms share with DQN.
 
@@ -101,13 +101,15 @@ class TwinCriticAlgorithm(Algorithm):
     def _build_twin_critic(self, *, describe_actor: Describe, describe_critic: Describe, lagged: tuple[nn.Module, nn.Module],
                            policy_optim: OptimizerFactory, critic_optim: OptimizerFactory,
                            critic2_optim: OptimizerFactory | None, max_grad_norm: float | None = None,
-                           lagged_actor: nn.Module | None = None) -> None:
+                           lagged_actor: nn.Module | None = None, actor: nn.Module | None = None) -> None:
         """``describe_actor(actor)`` and ``describe_critic(net, role)`` return (layer chain, parameters in flat order);
         ``lagged`` are the lagged critics as ``describe_critic`` reads them, ``lagged_actor`` (None: there is none) the lagged
         actor as ``describe_actor`` reads it.  ``critic2_optim`` defaults to ``critic_optim``; ``max_grad_norm`` clips both
-        critics' steps."""
-        dev = self._dev = cuda_device_of(self.policy.actor, self.critic, self.critic2)
-        a_layers, a_params = describe_actor(self.policy.actor)
+        critics' steps.  ``actor``: the actor network when it is not ``policy.actor`` (BCQ's perturbation network); then
+        ``policy_optim`` covers that network alone instead of the whole policy."""
+        actor_net = self.policy.actor if actor is None else actor
+        dev = self._dev = cuda_device_of(actor_net, self.critic, self.critic2)
+        a_layers, a_params = describe_actor(actor_net)
         self._g_actor = FlatGroup(a_params, dev)
         self._actor = FusedStack(a_layers, self._g_actor, "actor")
         self._g_at = None if lagged_actor is None else FlatGroup(describe_actor(lagged_actor)[1], dev)
@@ -119,7 +121,7 @@ class TwinCriticAlgorithm(Algorithm):
             self._g_c.append(g)
             self._c.append(FusedStack(layers, g, name))
             self._g_ct.append(FlatGroup(tparams, dev))
-        self.policy_optim = self._create_optimizer(self.policy, policy_optim)
+        self.policy_optim = self._create_optimizer(self.policy if actor is None else actor, policy_optim)
         self.critic_optim = self._create_optimizer(self.critic, critic_optim, max_grad_norm=max_grad_norm)
         self.critic2_optim = self._create_optimizer(self.critic2, critic2_optim or critic_optim, max_grad_norm=max_grad_norm)
         for o, g in ((self.policy_optim, self._g_actor), (self.critic_optim, self._g_c[0]), (self.critic2_optim, self._g_c[1])):

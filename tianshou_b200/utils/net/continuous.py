@@ -110,3 +110,50 @@ class ContinuousActorProbabilistic(ModuleWithVectorOutput):
             shape[1] = -1
             sigma = (self.sigma_param.view(shape) + torch.zeros_like(mu)).exp()
         return (mu, sigma), state
+
+
+class Perturbation(nn.Module):
+    """BCQ's perturbation network (continuous.py:378-412): ``clamp(a + phi * max_action * tanh(logits), +-max_action)`` with
+    ``logits = preprocess_net(cat([s, a], -1))[0]``.  As in the reference, that ``[0]`` is the logits of a ``Net`` (which
+    returns ``(logits, state)``) but ROW 0 of the output of an ``MLP``, whose perturbation then applies to every row."""
+
+    def __init__(self, *, preprocess_net: nn.Module, max_action: float, phi: float = 0.05):
+        super().__init__()
+        self.preprocess_net = preprocess_net
+        self.max_action = max_action
+        self.phi = phi
+
+    def forward(self, state: torch.Tensor, action: torch.Tensor) -> torch.Tensor:
+        logits = self.preprocess_net(torch.cat([state, action], -1))[0]
+        noise = self.phi * self.max_action * torch.tanh(logits)
+        return (noise + action).clamp(-self.max_action, self.max_action)
+
+
+class VAE(nn.Module):
+    """The VAE over actions of BCQ (continuous.py:415-490): the encoder on [s | a] (output width ``hidden_dim``), the ``mean`` and
+    ``log_std`` heads (``log_std`` clamped to [-4, 15]), the decoder on [s | z] (output width A) under ``max_action * tanh``.
+    ``decode(state)`` without a latent draws it with ``torch.randn`` on torch's CPU generator, clamped to [-0.5, 0.5]."""
+
+    def __init__(self, *, encoder: nn.Module, decoder: nn.Module, hidden_dim: int, latent_dim: int, max_action: float):
+        super().__init__()
+        self.encoder = encoder
+        self.mean = nn.Linear(hidden_dim, latent_dim)
+        self.log_std = nn.Linear(hidden_dim, latent_dim)
+        self.decoder = decoder
+        self.max_action = max_action
+        self.latent_dim = latent_dim
+
+    def forward(self, state: torch.Tensor, action: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        latent_z = self.encoder(torch.cat([state, action], -1))
+        mean = self.mean(latent_z)
+        log_std = self.log_std(latent_z).clamp(-4, 15)
+        std = torch.exp(log_std)
+        latent_z = mean + std * torch.randn_like(std)
+        reconstruction = self.decode(state, latent_z)
+        return reconstruction, mean, std
+
+    def decode(self, state: torch.Tensor, latent_z: torch.Tensor | None = None) -> torch.Tensor:
+        if latent_z is None:
+            device = torch_device(self)
+            latent_z = torch.randn(state.shape[:-1] + (self.latent_dim,)).to(device).clamp(-0.5, 0.5)
+        return self.max_action * torch.tanh(self.decoder(torch.cat([state, latent_z], -1)))
