@@ -209,6 +209,22 @@ typedef struct ts_actor_critic_desc {
 int ts_critic_forward(const float* params, const ts_actor_critic_desc* desc /* host */,
                       const float* obs0, float* v_out0, const float* obs1, float* v_out1,
                       int64_t n, ts_stream_t stream);
+/* Which rows of obs_next repeat the following row of obs (a rollout: all but the episode / segment ends), so that the
+ * critic need not be evaluated on them.  alias[i] (n bytes) = 1 iff i + 1 < n and the obs_dim 32-bit words of obs_next[i]
+ * equal those of obs[i + 1] (bitwise: -0.0 vs 0.0 or two NaN payloads count as different); extra[0 .. *n_extra) (capacity n,
+ * ascending) lists the rows with alias == 0; n_extra: device int32[1].  Deterministic (no atomics), no host sync.
+ * workspace: ts_next_alias_workspace_bytes(n) bytes of scratch.  n < 2^31. */
+int64_t ts_next_alias_workspace_bytes(int64_t n);
+int ts_next_alias_map(const float* obs, const float* obs_next, int64_t n, int32_t obs_dim, uint8_t* alias,
+                      int32_t* extra, int32_t* n_extra, void* workspace, ts_stream_t stream);
+/* ts_critic_forward(obs, v_s, obs_next, v_next) with one critic evaluation per distinct row, given the map of
+ * ts_next_alias_map(obs, obs_next): v_s[j] = critic(obs[j]); v_next[i] = v_s[i + 1] where alias[i];
+ * v_next[extra[k]] = critic(obs_next[extra[k]]) for k < *n_extra.  A row's value does not depend on where it sits in a
+ * tile, so v_s and v_next are bit for bit those of ts_critic_forward.  The tensor-core path does this in one launch whose
+ * tile count follows *n_extra on the device; networks outside its envelope evaluate both inputs in full. */
+int ts_critic_forward_dedup(const float* params, const ts_actor_critic_desc* desc /* host */, const float* obs,
+                            const float* obs_next, const uint8_t* alias, const int32_t* extra,
+                            const int32_t* n_extra, float* v_s, float* v_next, int64_t n, ts_stream_t stream);
 /* logp_out[r] = Independent(Normal(mu(obs[r]), exp(logstd)), 1).log_prob(act[r])
  * (ppo.py:157-161 with reinforce.py:167-192).  mu_out (n*act_dim, nullable) receives mu.
  * TS_AC_CATEGORICAL: logp_out[r] = Categorical(probs = softmax(logits(obs[r]))).log_prob(act[r]) with act one f32
@@ -319,6 +335,20 @@ int ts_ppo_update(float* params, float* grad, float* partials, float* exp_avg, f
                   const int64_t* bounds /* host */, int32_t n_minibatch, int32_t recompute_adv,
                   double gamma, double lam, double* rms_state, double rms_eps, void* gae_ws,
                   void* adv_tmp, void* weight_image, float* stats, void* row_feed, ts_stream_t stream);
+/* ts_ppo_update whose value recompute evaluates the critic once per distinct observation: next_alias / next_extra /
+ * n_next_extra are the map of ts_next_alias_map(obs, obs_next) (see ts_critic_forward_dedup; same results).  All three
+ * NULL: exactly ts_ppo_update. */
+int ts_ppo_update_dedup(float* params, float* grad, float* partials, float* exp_avg, float* exp_avg_sq,
+                        int64_t* step_count, const ts_actor_critic_desc* desc, const ts_ppo_hparams* hp,
+                        const float* obs, const float* obs_next, const float* act, const double* rew,
+                        const uint8_t* terminated, const uint8_t* truncated, const uint8_t* extra_end,
+                        float* v_s, float* returns, float* adv, const float* logp_old,
+                        float* v_next_tmp, int64_t N, const int32_t* perm, int32_t repeat,
+                        const int64_t* bounds /* host */, int32_t n_minibatch, int32_t recompute_adv,
+                        double gamma, double lam, double* rms_state, double rms_eps, void* gae_ws,
+                        void* adv_tmp, void* weight_image, float* stats, void* row_feed,
+                        const uint8_t* next_alias, const int32_t* next_extra, const int32_t* n_next_extra,
+                        ts_stream_t stream);
 
 /* ---- multi-GPU fused update: gradient all-reduce INSIDE the epoch kernel over NVLink peer memory -------------
  * Replaces, for one process per GPU (data-parallel replicas, each rank owns its own rollout shard), the

@@ -17,6 +17,7 @@ from __future__ import annotations
 import contextlib
 import ctypes as C
 import os
+import weakref
 from abc import ABC
 from dataclasses import dataclass
 from typing import Any
@@ -85,6 +86,7 @@ class ActorCriticOnPolicyAlgorithm(OnPolicyAlgorithm, ABC):
         self.rollout_partition = rollout_partition
         self.data_parallel = bool(data_parallel)
         self._active_order: MinibatchOrder | None = None
+        self._next_alias: tuple[Any, Any, ops.NextAliasMap] | None = None
         self.critic = critic
         assert 0.0 <= gae_lambda <= 1.0, f"GAE lambda should be in [0, 1] but got: {gae_lambda}"
         assert 0.0 <= gamma <= 1.0, f"discount factor gamma should be in [0, 1] but got: {gamma}"
@@ -267,7 +269,11 @@ class ActorCriticOnPolicyAlgorithm(OnPolicyAlgorithm, ABC):
             v_s.view(w, n // w).copy_(full[:, 0])
             v_next.view(w, n // w).copy_(full[:, 1])
         else:
-            ops.critic_forward(self._flat.flat, self._desc, batch.obs, batch.obs_next, out=v_s, out2=v_next)
+            amap = self._next_alias_map(batch, build=buffer is not None)
+            if amap is not None:
+                ops.critic_forward_dedup(self._flat.flat, self._desc, batch.obs, batch.obs_next, amap, out=v_s, out2=v_next)
+            else:
+                ops.critic_forward(self._flat.flat, self._desc, batch.obs, batch.obs_next, out=v_s, out2=v_next)
         rms = self._rms_device() if self.return_scaling else None
         adv = self._buf("adv", n, torch.float32)
         ret = self._buf("returns", n, torch.float32)
@@ -283,6 +289,24 @@ class ActorCriticOnPolicyAlgorithm(OnPolicyAlgorithm, ABC):
             self._merge_rms_across_ranks(rms, moments)
         batch.__dict__["v_s"], batch.__dict__["returns"], batch.__dict__["adv"] = v_s, ret, adv
         return batch
+
+    def _next_alias_map(self, batch: Batch, build: bool = False) -> ops.NextAliasMap | None:
+        """The map of the rows of ``batch.obs_next`` that repeat the next row of ``batch.obs``, so that the value pass
+        evaluates the critic once per distinct observation.  Built from the data once per update (``build``: the
+        preprocess call); the recompute calls get it back as long as the batch still holds the very tensors it was
+        built from, and None (= evaluate both inputs in full) otherwise."""
+        obs, obs_next = batch.obs, batch.obs_next
+        if build:
+            n = obs.shape[0]
+            amap = ops.NextAliasMap(self._buf("next_alias", n, torch.uint8), self._buf("next_extra", n, torch.int32),
+                                    self._buf("next_extra_count", 1, torch.int32))
+            need = int(load_library().ts_next_alias_workspace_bytes(n))
+            ops.next_alias_map(obs, obs_next, out=amap, workspace=self._buf("next_alias_ws", max(need, 4), torch.uint8))
+            self._next_alias = (weakref.ref(obs), weakref.ref(obs_next), amap)
+        if self._next_alias is None:
+            return None
+        ref_obs, ref_next, amap = self._next_alias
+        return amap if ref_obs() is obs and ref_next() is obs_next else None
 
     def _gae_workspace(self, n: int) -> torch.Tensor:
         from ..._cabi import load_library

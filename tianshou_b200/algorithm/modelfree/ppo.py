@@ -95,21 +95,24 @@ class FusedActorCriticUpdate(ActorCriticOnPolicyAlgorithm):
 
     def _device_passes(self, batch: Batch, perm_rows: torch.Tensor | None, bounds: list[tuple[int, int]], hp: Any,
                        stats: torch.Tensor, nrep: int, recompute: bool, feed: Any = None) -> None:
-        """``nrep`` passes over the minibatches as ONE asynchronous C call (``ts_ppo_update``): per pass an
-        optional critic + GAE recompute and one persistent launch covering every optimiser step."""
+        """``nrep`` passes over the minibatches as ONE asynchronous C call (``ts_ppo_update_dedup``): per pass an
+        optional critic + GAE recompute (with the alias map of the preprocess call, when the batch is still the one it was
+        built from) and one persistent launch covering every optimiser step."""
         f, dev = self._flat, self.device
         N, n_mb = batch.obs.shape[0], len(bounds)
         adv_tmp = self._buf("adv_tmp", 32 + 8 * n_mb, torch.uint8)
         adv_tmp.zero_()
         bounds_c = (C.c_int64 * (2 * n_mb))(*[x for b in bounds for x in b])
-        call("ts_ppo_update", ptr(f.flat), ptr(f.grad), ptr(f.partials), ptr(f.exp_avg), ptr(f.exp_avg_sq), ptr(f.step_dev),
+        amap = self._next_alias_map(batch) if recompute else None
+        call("ts_ppo_update_dedup", ptr(f.flat), ptr(f.grad), ptr(f.partials), ptr(f.exp_avg), ptr(f.exp_avg_sq), ptr(f.step_dev),
              C.byref(self._desc), C.byref(hp), ptr(batch.obs), ptr(batch.obs_next), ptr(batch.act),
              ptr(batch.rew), ptr(batch.terminated), ptr(batch.truncated), ptr(batch.get("_unfinished")),
              ptr(batch.v_s), ptr(batch.returns), ptr(batch.adv), ptr(batch.logp_old),
              ptr(self._buf("v_next", N, torch.float32)), N, ptr(perm_rows), nrep, bounds_c, n_mb,
              int(recompute), float(self.gamma), float(self.gae_lambda),
              ptr(self._rms_device()) if self.return_scaling else None, float(self._eps),
-             ptr(self._gae_workspace(N)), ptr(adv_tmp), ptr(f.weight_image), ptr(stats), feed, stream_ptr(dev))
+             ptr(self._gae_workspace(N)), ptr(adv_tmp), ptr(f.weight_image), ptr(stats), feed,
+             *((ptr(amap.alias), ptr(amap.extra), ptr(amap.count)) if amap is not None else (None, None, None)), stream_ptr(dev))
 
     # ------------------------------------------------------------------ multi-GPU, fused (NVLink peer memory)
     def _peer_exchange(self, bounds: list[tuple[int, int]]):

@@ -248,9 +248,95 @@ __global__ void narrow_kernel(const int64_t* __restrict__ src, int64_t n, int32_
     if (t < n) dst[t] = (int32_t)src[t];
 }
 
+// ---- next-observation alias map ---------------------------------------------------------------------
+// In a rollout obs_next[i] is obs[i + 1] except where an episode or an env's segment ends, so critic(obs_next[i]) is
+// the value already computed for row i + 1.  alias[i] = 1 iff the two rows hold the same 32-bit words (a bitwise test:
+// -0.0 vs 0.0 and different NaN payloads count as different, which only costs an evaluation); the rows with alias == 0
+// are listed in ascending order in `extra`.  Nothing is assumed about the buffer layout: a shuffled batch lists every row.
+constexpr int kAliasThreads = 256;      // rows per block: one warp compares 32 consecutive rows, coalesced over their words
+
+__global__ void __launch_bounds__(kAliasThreads) next_alias_mark_kernel(
+    const uint32_t* __restrict__ obs, const uint32_t* __restrict__ obs_next, int64_t n, int width,
+    uint8_t* __restrict__ alias, int32_t* __restrict__ block_extra) {
+    const int lane = threadIdx.x & 31;
+    const int64_t i0 = (int64_t)blockIdx.x * kAliasThreads + (threadIdx.x & ~31);     // first row of the warp
+    const int64_t rows = tsb::imin(32, n - 1 - i0);          // rows of the warp that have a successor (may be <= 0)
+    const uint32_t* a = obs_next + i0 * width;
+    const uint32_t* b = obs + (i0 + 1) * width;
+    unsigned differs = 0u;                                   // bit r: row i0 + r differs in a word this lane compared
+    for (int64_t w = lane; w < rows * width; w += 32) {
+        if (a[w] != b[w]) differs |= 1u << (unsigned)(w / width);
+    }
+    differs = __reduce_or_sync(0xffffffffu, differs);
+    const int64_t i = i0 + lane;
+    const bool same = lane < rows && !((differs >> lane) & 1u);
+    if (i < n) alias[i] = same ? 1 : 0;
+    const int cnt = __syncthreads_count(i < n && !same);
+    if (threadIdx.x == 0) block_extra[blockIdx.x] = cnt;
+}
+
+// Ordered compaction of the rows with alias == 0: a block's first slot is the sum of the earlier blocks' counts, the
+// order inside a block comes from a ballot scan -- no atomics, so `extra` is the same list on every run.
+__global__ void __launch_bounds__(kAliasThreads) next_alias_compact_kernel(
+    const uint8_t* __restrict__ alias, int64_t n, const int32_t* __restrict__ block_extra,
+    int32_t* __restrict__ extra, int32_t* __restrict__ n_extra) {
+    __shared__ int s_warp[kAliasThreads / 32];
+    __shared__ int s_base;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    int before_blocks = 0;
+    for (int b = tid; b < (int)blockIdx.x; b += kAliasThreads) before_blocks += block_extra[b];
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) before_blocks += __shfl_xor_sync(0xffffffffu, before_blocks, off);
+    if (lane == 0) s_warp[warp] = before_blocks;
+    __syncthreads();
+    if (tid == 0) {
+        int base = 0;
+        for (int w = 0; w < kAliasThreads / 32; ++w) base += s_warp[w];
+        s_base = base;
+    }
+    __syncthreads();
+    const int64_t i = (int64_t)blockIdx.x * kAliasThreads + tid;
+    const bool keep = i < n && alias[i] == 0;
+    const unsigned bal = __ballot_sync(0xffffffffu, keep);
+    const int base = s_base;
+    __syncthreads();                                          // s_warp is reused
+    if (lane == 0) s_warp[warp] = __popc(bal);
+    __syncthreads();
+    int before = 0, total = 0;
+    for (int w = 0; w < kAliasThreads / 32; ++w) {
+        if (w < warp) before += s_warp[w];
+        total += s_warp[w];
+    }
+    if (keep) extra[base + before + __popc(bal & ((1u << lane) - 1u))] = (int32_t)i;
+    if (blockIdx.x == gridDim.x - 1 && tid == 0) *n_extra = base + total;
+}
+
 inline unsigned blocks_for(int64_t n, int threads) { return (unsigned)((n + threads - 1) / threads); }
 
 }  // namespace
+
+extern "C" int64_t ts_next_alias_workspace_bytes(int64_t n) {
+    return n > 0 ? 4 * (int64_t)blocks_for(n, kAliasThreads) : 0;
+}
+
+extern "C" int ts_next_alias_map(const float* obs, const float* obs_next, int64_t n, int32_t obs_dim, uint8_t* alias,
+                                 int32_t* extra, int32_t* n_extra, void* workspace, ts_stream_t stream) {
+    TS_REQUIRE(n >= 0 && n < (1ll << 31) && obs_dim >= 1, "ts_next_alias_map: bad shape");
+    TS_REQUIRE(n_extra, "ts_next_alias_map: null n_extra");
+    cudaStream_t st = tsb::as_stream(stream);
+    if (n == 0) {
+        TS_CUDA(cudaMemsetAsync(n_extra, 0, sizeof(int32_t), st));
+        return 0;
+    }
+    TS_REQUIRE(obs && obs_next && alias && extra && workspace, "ts_next_alias_map: null pointer");
+    int32_t* block_extra = static_cast<int32_t*>(workspace);
+    const unsigned grid = blocks_for(n, kAliasThreads);
+    next_alias_mark_kernel<<<grid, kAliasThreads, 0, st>>>(reinterpret_cast<const uint32_t*>(obs),
+                                                           reinterpret_cast<const uint32_t*>(obs_next), n, obs_dim, alias, block_extra);
+    if (tsb::check_launch("ts_next_alias_map/mark")) return 1;
+    next_alias_compact_kernel<<<grid, kAliasThreads, 0, st>>>(alias, n, block_extra, extra, n_extra);
+    return tsb::check_launch("ts_next_alias_map");
+}
 
 #define META_ARGS_OK(fn) \
     TS_REQUIRE(offset && done && last_index && lengths && E > 0, fn ": null buffer metadata")

@@ -759,7 +759,8 @@ int launch_ppo_grad_tc(const float* params, const ts_actor_critic_desc& d, const
                        const int32_t* perm, int64_t lo, int64_t hi, int64_t global_rows, const float* adv_moments,
                        float* grad, cudaStream_t st);
 int launch_forward_tc(int mode, const float* params, const ts_actor_critic_desc& d, const float* in0, float* out0,
-                      const float* in1, float* out1, int64_t n, cudaStream_t st);
+                      const float* in1, float* out1, int64_t n, const uint8_t* alias, const int32_t* extra,
+                      const int32_t* n_extra, cudaStream_t st);
 int launch_ppo_epoch_tc(float* params, const ts_actor_critic_desc& d, const ts_ppo_hparams& hp, const float* obs,
                         const float* act, const float* adv, const float* ret, const float* logp_old, const float* v_s,
                         const int32_t* perm, int64_t lo0, int64_t mb_size, int64_t end, int n_mb, const float* adv_moments,
@@ -779,13 +780,25 @@ extern "C" int ts_critic_forward(const float* params, const ts_actor_critic_desc
     if (n == 0) return 0;
     TS_REQUIRE(params && obs0 && v_out0 && (!obs1 || v_out1), "ts_critic_forward: null pointer");
     if (tsb::tc_supported(*desc) && !tsb::simt_forced())
-        return tsb::launch_forward_tc(0, params, *desc, obs0, v_out0, obs1, v_out1, n, tsb::as_stream(stream));
+        return tsb::launch_forward_tc(0, params, *desc, obs0, v_out0, obs1, v_out1, n, nullptr, nullptr, nullptr, tsb::as_stream(stream));
     const size_t smem = smem_bytes(*desc, 0);
     if (set_smem(critic_forward_kernel, smem, "ts_critic_forward")) return 1;
     const int64_t tiles = ((n + kRows - 1) / kRows) * (obs1 ? 2 : 1);
     const unsigned grid = (unsigned)tsb::imin((int64_t)tiles, tsb::num_sms());
     critic_forward_kernel<<<grid, kThreads, smem, tsb::as_stream(stream)>>>(params, *desc, obs0, v_out0, obs1, v_out1, n);
     return tsb::check_launch("ts_critic_forward");
+}
+
+extern "C" int ts_critic_forward_dedup(const float* params, const ts_actor_critic_desc* desc, const float* obs,
+                                       const float* obs_next, const uint8_t* alias, const int32_t* extra,
+                                       const int32_t* n_extra, float* v_s, float* v_next, int64_t n, ts_stream_t stream) {
+    if (check_desc(desc, "ts_critic_forward_dedup")) return 2;
+    if (n == 0) return 0;
+    TS_REQUIRE(params && obs && obs_next && alias && extra && n_extra && v_s && v_next, "ts_critic_forward_dedup: null pointer");
+    if (tsb::tc_supported(*desc) && !tsb::simt_forced())
+        return tsb::launch_forward_tc(0, params, *desc, obs, v_s, obs_next, v_next, n, alias, extra, n_extra, tsb::as_stream(stream));
+    // fp32 SIMT kernel (obs_dim > 32): both inputs in full -- the same values, without the saving
+    return ts_critic_forward(params, desc, obs, v_s, obs_next, v_next, n, stream);
 }
 
 extern "C" int ts_actor_logp(const float* params, const ts_actor_critic_desc* desc, const float* obs,
@@ -795,7 +808,7 @@ extern "C" int ts_actor_logp(const float* params, const ts_actor_critic_desc* de
     if (n == 0) return 0;
     TS_REQUIRE(params && obs && act && logp_out, "ts_actor_logp: null pointer");
     if (tsb::tc_supported(*desc) && !tsb::simt_forced())
-        return tsb::launch_forward_tc(1, params, *desc, obs, logp_out, act, mu_out, n, tsb::as_stream(stream));
+        return tsb::launch_forward_tc(1, params, *desc, obs, logp_out, act, mu_out, n, nullptr, nullptr, nullptr, tsb::as_stream(stream));
     const size_t smem = smem_bytes(*desc, 1);
     if (set_smem(actor_logp_kernel, smem, "ts_actor_logp")) return 1;
     const int64_t tiles = (n + kRows - 1) / kRows;
@@ -906,8 +919,27 @@ extern "C" int ts_ppo_update(float* params, float* grad, float* partials, float*
                              int32_t n_minibatch, int32_t recompute_adv, double gamma, double lam,
                              double* rms_state, double rms_eps, void* gae_ws, void* adv_tmp,
                              void* weight_image, float* stats, void* row_feed, ts_stream_t stream) {
+    return ts_ppo_update_dedup(params, grad, partials, exp_avg, exp_avg_sq, step_count, desc, hp, obs, obs_next, act, rew,
+                               terminated, truncated, extra_end, v_s, returns, adv, logp_old, v_next_tmp, N, perm, repeat,
+                               bounds, n_minibatch, recompute_adv, gamma, lam, rms_state, rms_eps, gae_ws, adv_tmp,
+                               weight_image, stats, row_feed, nullptr, nullptr, nullptr, stream);
+}
+
+extern "C" int ts_ppo_update_dedup(float* params, float* grad, float* partials, float* exp_avg, float* exp_avg_sq,
+                                   int64_t* step_count, const ts_actor_critic_desc* desc,
+                                   const ts_ppo_hparams* hp, const float* obs, const float* obs_next,
+                                   const float* act, const double* rew, const uint8_t* terminated,
+                                   const uint8_t* truncated, const uint8_t* extra_end, float* v_s,
+                                   float* returns, float* adv, const float* logp_old, float* v_next_tmp,
+                                   int64_t N, const int32_t* perm, int32_t repeat, const int64_t* bounds,
+                                   int32_t n_minibatch, int32_t recompute_adv, double gamma, double lam,
+                                   double* rms_state, double rms_eps, void* gae_ws, void* adv_tmp,
+                                   void* weight_image, float* stats, void* row_feed, const uint8_t* next_alias,
+                                   const int32_t* next_extra, const int32_t* n_next_extra, ts_stream_t stream) {
     if (check_desc(desc, "ts_ppo_update")) return 2;
     TS_REQUIRE(hp && bounds && stats && partials && grad && repeat >= 0 && n_minibatch >= 0, "ts_ppo_update: bad arguments");
+    TS_REQUIRE((next_alias != nullptr) == (next_extra != nullptr) && (next_alias != nullptr) == (n_next_extra != nullptr),
+               "ts_ppo_update: the next-observation alias map is three pointers, all or none");
     TS_REQUIRE(!hp->advantage_normalization || adv_tmp, "ts_ppo_update: adv_tmp required");
     static const bool no_fuse = [] { const char* e = getenv("TS_B200_NO_FUSED_STEP"); return e && e[0] == '1'; }();
     const bool fused = tsb::tc_supported(*desc) && !tsb::simt_forced() && !no_fuse;
@@ -924,7 +956,9 @@ extern "C" int ts_ppo_update(float* params, float* grad, float* partials, float*
     for (int r = 0; r < repeat; ++r) {
         if (recompute_adv && r > 0) {    // ppo.py:174-178 -> a2c.py:115-153
             TS_REQUIRE(obs_next && rew && v_next_tmp && gae_ws, "ts_ppo_update: recompute needs obs_next/rew/scratch");
-            if (int e = ts_critic_forward(params, desc, obs, v_s, obs_next, v_next_tmp, N, stream)) return e;
+            if (int e = next_alias ? ts_critic_forward_dedup(params, desc, obs, obs_next, next_alias, next_extra, n_next_extra,
+                                                             v_s, v_next_tmp, N, stream)
+                                   : ts_critic_forward(params, desc, obs, v_s, obs_next, v_next_tmp, N, stream)) return e;
             if (int e = ts_gae(v_s, v_next_tmp, TS_F32, rew, terminated, truncated, extra_end, 1, N, gamma,
                                lam, rms_state, rms_eps, nullptr, adv, returns, TS_F32, gae_ws, stream)) return e;
         }

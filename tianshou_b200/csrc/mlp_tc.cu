@@ -1029,11 +1029,15 @@ __host__ __device__ constexpr SmemF make_smem_f(int kxp, uint32_t sbase) {
 }
 
 // MODE 0: out0[r] = critic(in0[r]) and (if in1) out1[r] = critic(in1[r])      (a2c.py:123-126)
+//         With the alias map of ts_next_alias_map(in0, in1) the second range holds only the *n_extra rows of in1 that do
+//         not repeat the following row of in0 (gathered through `extra`, scattered to out1); the thread that writes
+//         out0[j] also writes out1[j - 1] where alias[j - 1].  n_extra is read on the device: the persistent loop follows it.
 // MODE 1: out0[r] = log N(in1[r] | mu(in0[r]), exp(logstd)), out1 = mu (nullable)   (ppo.py:157-161)
 template <int MODE, int KXP>
 __global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(
     const float* __restrict__ params, const ts_actor_critic_desc d, const float* __restrict__ in0,
-    float* __restrict__ out0, const float* __restrict__ in1, float* __restrict__ out1, int64_t n) {
+    float* __restrict__ out0, const float* __restrict__ in1, float* __restrict__ out1, int64_t n,
+    const uint8_t* __restrict__ alias /* nullable */, const int32_t* __restrict__ extra, const int32_t* __restrict__ n_extra) {
     extern __shared__ __align__(1024) uint8_t sm[];
     const int tid = threadIdx.x, lane = tid & 31;
     const uint32_t sbase = wg::smem_u32(sm);
@@ -1059,21 +1063,25 @@ __global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(
         ls[tid] = (MODE == 1 && tid < out_dim) ? expf(__ldg(params + g.ls + tid)) : 1.0f;
     }
 
+    const bool dedup = MODE == 0 && alias != nullptr;
     const int64_t tiles_per = (n + kRows - 1) / kRows;
-    const int64_t tiles = tiles_per * ((MODE == 0 && in1) ? 2 : 1);
+    const int64_t n2 = (MODE == 0 && in1) ? (dedup ? (int64_t)__ldg(n_extra) : n) : 0;      // rows of the second range
+    const int64_t tiles = tiles_per + (n2 + kRows - 1) / kRows;
     const int64_t my_n = tiles > (int64_t)blockIdx.x ? (tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;   // tiles of this CTA
     auto tile_of = [&](int64_t k) { return (int64_t)blockIdx.x + k * gridDim.x; };
     auto tile_src = [&](int64_t t, const float*& src, int64_t& row0, int& nrows, bool& second) {
         second = t >= tiles_per;
         row0 = (second ? t - tiles_per : t) * kRows;
-        nrows = (int)tsb::imin((int64_t)kRows, n - row0);
+        nrows = (int)tsb::imin((int64_t)kRows, (second ? n2 : n) - row0);
         src = (MODE == 0 && second) ? in1 : in0;
     };
     auto x_load = [&](int64_t k, float (&xv)[8]) {     // one (row, 8-column chunk) per thread
         const float* src; int64_t row0; int nrows; bool second;
         tile_src(tile_of(k), src, row0, nrows, second);
         chunk_load(kRows, d.obs_dim, S.KXP, [&](int r) {
-            return r < nrows ? src + (row0 + r) * d.obs_dim : (const float*)nullptr;
+            if (r >= nrows) return (const float*)nullptr;
+            const int64_t row = (dedup && second) ? (int64_t)__ldg(extra + row0 + r) : row0 + r;
+            return src + row * d.obs_dim;
         }, xv);
     };
     const int half = tid >> 8;                 // column half of the thread's layer elements
@@ -1116,7 +1124,14 @@ __global__ void __launch_bounds__(kThreads, 1) forward_tc_kernel(
         if (tid < nrows) {
             const int r = tid;
             if (MODE == 0) {
-                (second ? out1 : out0)[row0 + r] = (part[r] + part[kMaxAct * kRows + r]) + b3[0];
+                const float v = (part[r] + part[kMaxAct * kRows + r]) + b3[0];
+                const int64_t row = row0 + r;
+                if (!second) {
+                    out0[row] = v;
+                    if (dedup && row > 0 && __ldg(alias + row - 1)) out1[row - 1] = v;
+                } else {
+                    out1[dedup ? (int64_t)__ldg(extra + row) : row] = v;
+                }
             } else {
                 float lp = 0.0f;
                 for (int a = 0; a < out_dim; ++a) {
@@ -1224,18 +1239,20 @@ int64_t weight_image_bytes(const ts_actor_critic_desc& d) {
 }
 
 int launch_forward_tc(int mode, const float* params, const ts_actor_critic_desc& d, const float* in0, float* out0,
-                      const float* in1, float* out1, int64_t n, cudaStream_t st) {
+                      const float* in1, float* out1, int64_t n, const uint8_t* alias, const int32_t* extra,
+                      const int32_t* n_extra, cudaStream_t st) {
     return with_kxp(d.obs_dim, [&](auto kxp) {
         constexpr int KXP = decltype(kxp)::value;
         constexpr size_t smem = make_smem_f(KXP, 0).total;
-        const int64_t tiles = ((n + kRows - 1) / kRows) * ((mode == 0 && in1) ? 2 : 1);
+        // with an alias map the second range's length is known on the device only: the first range alone sizes the grid
+        const int64_t tiles = ((n + kRows - 1) / kRows) * ((mode == 0 && in1 && !alias) ? 2 : 1);
         const unsigned grid = (unsigned)imin(tiles, num_sms());
         if (mode == 0) {
             if (int e = opt_in_smem<forward_tc_kernel<0, KXP>>(smem)) return e;
-            forward_tc_kernel<0, KXP><<<grid, kThreads, smem, st>>>(params, d, in0, out0, in1, out1, n);
+            forward_tc_kernel<0, KXP><<<grid, kThreads, smem, st>>>(params, d, in0, out0, in1, out1, n, alias, extra, n_extra);
         } else {
             if (int e = opt_in_smem<forward_tc_kernel<1, KXP>>(smem)) return e;
-            forward_tc_kernel<1, KXP><<<grid, kThreads, smem, st>>>(params, d, in0, out0, in1, out1, n);
+            forward_tc_kernel<1, KXP><<<grid, kThreads, smem, st>>>(params, d, in0, out0, in1, out1, n, nullptr, nullptr, nullptr);
         }
         return check_launch(mode == 0 ? "ts_critic_forward(tc)" : "ts_actor_logp(tc)");
     });

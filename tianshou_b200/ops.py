@@ -278,6 +278,45 @@ def critic_forward(params: torch.Tensor, desc: ActorCriticDesc, obs: torch.Tenso
     return (out, out2) if obs2 is not None else out
 
 
+@dataclass
+class NextAliasMap:
+    """Which rows of ``obs_next`` repeat the following row of ``obs`` (``ts_next_alias_map``): ``alias`` uint8[n],
+    ``extra`` int32[n] of which the first ``count[0]`` entries list the rows with ``alias == 0`` in ascending order."""
+
+    alias: torch.Tensor
+    extra: torch.Tensor
+    count: torch.Tensor       # int32[1] on the device: reading it is a host sync, the kernels never need one
+
+
+def next_alias_map(obs: torch.Tensor, obs_next: torch.Tensor, out: NextAliasMap | None = None,
+                   workspace: torch.Tensor | None = None) -> NextAliasMap:
+    n, dev = obs.shape[0], obs.device
+    assert obs.dtype == torch.float32 and obs_next.dtype == torch.float32 and obs.shape == obs_next.shape
+    if out is None:
+        out = NextAliasMap(torch.empty(n, dtype=torch.uint8, device=dev), torch.empty(n, dtype=torch.int32, device=dev),
+                           torch.empty(1, dtype=torch.int32, device=dev))
+    need = int(_cabi.load_library().ts_next_alias_workspace_bytes(n))
+    if workspace is None or workspace.numel() < need:
+        workspace = torch.empty(max(need, 4), dtype=torch.uint8, device=dev)
+    call("ts_next_alias_map", ptr(obs), ptr(obs_next), n, obs[0].numel() if n else 1, ptr(out.alias), ptr(out.extra),
+         ptr(out.count), ptr(workspace), stream_ptr(dev))
+    return out
+
+
+def critic_forward_dedup(params: torch.Tensor, desc: ActorCriticDesc, obs: torch.Tensor, obs_next: torch.Tensor,
+                         amap: NextAliasMap, out: torch.Tensor | None = None, out2: torch.Tensor | None = None):
+    """``critic_forward(params, desc, obs, obs_next)`` with one evaluation per distinct row; ``amap`` must be
+    ``next_alias_map(obs, obs_next)`` of these very tensors.  Same bits as ``critic_forward``."""
+    n = obs.shape[0]
+    if out is None:
+        out = torch.empty(n, dtype=torch.float32, device=obs.device)
+    if out2 is None:
+        out2 = torch.empty(n, dtype=torch.float32, device=obs.device)
+    call("ts_critic_forward_dedup", ptr(params), C.byref(desc), ptr(obs), ptr(obs_next), ptr(amap.alias), ptr(amap.extra),
+         ptr(amap.count), ptr(out), ptr(out2), n, stream_ptr(obs.device))
+    return out, out2
+
+
 def actor_logp(params: torch.Tensor, desc: ActorCriticDesc, obs: torch.Tensor, act: torch.Tensor,
                want_mu: bool = False, out: torch.Tensor | None = None):
     n = obs.shape[0]
