@@ -690,6 +690,42 @@ int ts_bcq_target(const float* q1, const float* q2, int64_t B, int32_t N, float 
 int ts_bcq_select(const float* q, int64_t G, int64_t S, const float* x, int64_t ldx, int32_t col0, int32_t A, float* act,
                   int64_t* idx, ts_stream_t stream);
 
+/* ---- discrete BCQ (discrete_bcq.cu) ---- */
+/* Discrete BCQ's bootstrap value (imitation/discrete_bcq.py:115-118 the policy's masked arg-max, :228-234 the target):
+ * per row b, mask_a = (logits[b][a] - max_a logits[b]) < log_tau (log_tau = -inf masks nothing),
+ * a* = argmax_a (q_online[b][a] - FLT_MAX * mask_a) evaluated in fp32 with torch.argmax's rule (lowest index among ties, a NaN
+ * is the maximum), out[b] = q_old[b][a*]; act_out [B] (nullable) = a*.  [B, A] row-major, one warp per row, any A >= 1, any B. */
+int ts_discrete_bcq_target(const float* q_online, const float* logits, const float* q_old, float log_tau, int64_t B, int32_t A,
+                           float* out, int64_t* act_out, ts_stream_t stream);
+/* Discrete BCQ's loss (discrete_bcq.py:244-252) on the Q head's q [B][A] and the imitator head's logits [B][A]:
+ * losses[4] = (loss, q_loss, i_loss, reg_loss) with q_loss = smooth_l1_loss(q[b][act[b]], returns[b]) (beta 1, mean),
+ * i_loss = nll_loss(log_softmax(logits), act) (mean), reg_loss = mean(logits^2) over B * A, loss = q_loss + i_loss +
+ * penalty * reg_loss; dq, dlogits [B][A] = d loss / d q, d loss / d logits (every element written).  act must lie in [0, A):
+ * the caller checks it.  rows [3][B] is scratch (the per-row terms).  One warp per row, then one block summing the rows in a
+ * fixed order: two calls on the same input are bit-identical.  Any A >= 1, any B >= 1. */
+int ts_discrete_bcq_rows(const float* q, const float* logits, const int64_t* act, const float* returns, int64_t B, int32_t A,
+                         float penalty, float* dq, float* dlogits, float* rows, float* losses, ts_stream_t stream);
+
+/* ---- discrete CRR (discrete_crr.cu) ---- */
+enum { TS_CRR_EXP = 0, TS_CRR_BINARY = 1, TS_CRR_ALL = 2 };
+/* Discrete CRR's loss (imitation/discrete_crr.py:131-158) on the critic head's q [B][A] and the actor head's logits [B][A]
+ * at s, and the lagged heads' q_old, logits_old [B][A] at s' (the same pointers as q / logits are allowed).  Per row, with
+ * p = softmax(logits), qa = q[b][act[b]]: target = rew + gamma * (done > 0 ? 0 : sum_a softmax(logits_old)_a q_old_a);
+ * adv = qa - sum_a p_a q_a; coef = clamp(exp(adv / beta), 0, ratio_upper_bound) | 1[adv > 0] | 1 by mode;
+ * losses[4] = (loss, actor_loss, critic_loss, cql_loss): critic_loss = mean_b 0.5 (qa - target)^2, cql_loss = mean_b
+ * (logsumexp(q[b]) - qa), and actor_loss = mean_b(-log p[act]) * mean_b(coef): the reference multiplies -log_prob [B] by the
+ * coefficient [B, 1] (discrete_crr.py:155), which broadcasts to [B, B], so its mean is the product of the two means, not the mean
+ * of the per-row products.  loss = actor_loss + critic_loss + min_q_weight * cql_loss.
+ * dq, dlogits [B][A] = d loss / d q, d loss / d logits as the reference's autograd takes it: the advantage is not detached, so
+ * in TS_CRR_EXP mode the coefficient carries gradient into q (through qa and sum p q) and into the logits (through p) wherever
+ * the clamp passes; the other modes carry none through the coefficient.  rew, done fp32 [B]; act in [0, A), checked by the
+ * caller; rows [4 B + 2] scratch (the per-row terms and the two means).  Three launches (rows, their sums in one block, the
+ * gradient, which needs the two batch means), fixed-order sums, bit-identical from run to run.  Any A >= 1, any B >= 1. */
+int ts_discrete_crr_rows(const float* q, const float* logits, const int64_t* act, const float* q_old, const float* logits_old,
+                         const float* rew, const float* done, int64_t B, int32_t A, float gamma, int32_t mode, float beta,
+                         float ratio_upper_bound, float min_q_weight, float* dq, float* dlogits, float* rows, float* losses,
+                         ts_stream_t stream);
+
 #ifdef TS_B200_DIAGNOSTICS
 /* Diagnostics build only (libts_b200_diag.so, `python -m tianshou_b200.csrc.build --diag`): not part of the product library. */
 /* Hardware self-test of the wgmma building blocks (csrc/wgmma.cuh), one CTA:

@@ -1,6 +1,7 @@
 from .base import Algorithm, OfflineAlgorithm, OffPolicyAlgorithm, OnPolicyAlgorithm, Policy, TrainingStats
 from .flat_params import UnsupportedModelError
-from .imitation import BCQ, CQL, GAIL, TD3BC, BCQPolicy, BCQTrainingStats, CQLTrainingStats, GailTrainingStats
+from .imitation import (BCQ, CQL, GAIL, TD3BC, BCQPolicy, BCQTrainingStats, CQLTrainingStats, DiscreteBCQ, DiscreteBCQPolicy,
+                        DiscreteBCQTrainingStats, DiscreteCRR, DiscreteCRRTrainingStats, GailTrainingStats)
 from .modelfree.a2c import A2CTrainingStats, ActorCriticOnPolicyAlgorithm
 from .modelfree.discrete_sac import DiscreteSAC
 from .modelfree.npg import NPG, NPGTrainingStats
@@ -15,5 +16,6 @@ __all__ = [
     "UnsupportedModelError", "A2CTrainingStats", "ActorCriticOnPolicyAlgorithm", "PPO", "A2C", "NPG", "TRPO", "NPGTrainingStats", "TRPOTrainingStats",
     "GAIL", "GailTrainingStats", "DiscreteSAC", "BCQ", "BCQPolicy", "BCQTrainingStats", "CQL", "CQLTrainingStats", "TD3", "TD3TrainingStats", "TD3BC",
     "ProbabilisticActorPolicy", "DiscreteActorPolicy", "AdamOptimizerFactory", "LRSchedulerFactoryLinear", "OptimizerFactory",
-    "RMSpropOptimizerFactory",
+    "RMSpropOptimizerFactory", "DiscreteBCQ", "DiscreteBCQPolicy", "DiscreteBCQTrainingStats", "DiscreteCRR",
+    "DiscreteCRRTrainingStats",
 ]
