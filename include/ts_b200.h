@@ -726,6 +726,28 @@ int ts_discrete_crr_rows(const float* q, const float* logits, const int64_t* act
                          float ratio_upper_bound, float min_q_weight, float* dq, float* dlogits, float* rows, float* losses,
                          ts_stream_t stream);
 
+/* ---- QR-DQN and discrete CQL (qrdqn.cu) ---- */
+/* QR-DQN's target distribution (modelfree/qrdqn.py:94-106 with compute_q_value = logits.mean(2), :18-20): q_online, q_next
+ * [B][A][N] at s_{t+n} (q_next the lagged network's output, or q_online itself); per row b, m_a = mean_k q_online[b][a][k] in
+ * fp32, a* = argmax_a m_a with torch.argmax's rule (lowest index among ties, a NaN is the maximum), out [B][N] = q_next[b][a*];
+ * act_out [B] (nullable) = a*.  The arg-max always comes from q_online (the reference has no is_double switch).  One warp per
+ * row, any A >= 1, N >= 1, B. */
+int ts_qrdqn_target(const float* q_online, const float* q_next, int64_t B, int32_t A, int32_t N, float* out, int64_t* act_out,
+                    ts_stream_t stream);
+/* The quantile-Huber loss of QR-DQN (qrdqn.py:108-131) and, with min_q_weight > 0, discrete CQL (imitation/discrete_cql.py:80-113)
+ * on q [B][A][N] at s, the n-step returns [B][N], tau_hat [N] (the reference's midpoints, built by the caller) and the importance
+ * weight [B] (nullable: 1).  With c_i = q[b][act[b]][i], u_ij = returns[b][j] - c_i, h_ij = smooth_l1(u_ij) (beta 1):
+ * qr_b = (1/N) sum_i sum_j h_ij |tau_i - 1[u_ij <= 0]|, prio [B] = (1/N) sum_i sum_j h_ij;
+ * losses[4] = (loss, qr_loss, cql_loss, mean_b prio) with qr_loss = mean_b(weight_b qr_b), cql_loss = mean_b(logsumexp_a m_a -
+ * m_act) over the quantile means m_a = mean_k q[b][a][k] (0 when min_q_weight == 0), loss = qr_loss + min_q_weight * cql_loss.
+ * dq [B][A][N] = d loss / d q, every element written: the indicator is detached, as in the reference, and the weight scales the
+ * quantile term only.  act must lie in [0, A): the caller checks it.  rows [3][B] is scratch.  One block per row (threads over
+ * the current quantiles, the row's targets and taus in shared memory), then one block summing the rows in a fixed order: two
+ * calls on the same input are bit-identical.  Any B >= 1, A >= 1, N >= 2 with 2 N (+ A when min_q_weight > 0) <= 12288;
+ * larger shapes are refused. */
+int ts_qrdqn_rows(const float* q, const int64_t* act, const float* returns, const float* tau_hat, const float* weight, int64_t B,
+                  int32_t A, int32_t N, float min_q_weight, float* dq, float* prio, float* rows, float* losses, ts_stream_t stream);
+
 #ifdef TS_B200_DIAGNOSTICS
 /* Diagnostics build only (libts_b200_diag.so, `python -m tianshou_b200.csrc.build --diag`): not part of the product library. */
 /* Hardware self-test of the wgmma building blocks (csrc/wgmma.cuh), one CTA:

@@ -1,11 +1,13 @@
 from .base import Algorithm, OfflineAlgorithm, OffPolicyAlgorithm, OnPolicyAlgorithm, Policy, TrainingStats
 from .flat_params import UnsupportedModelError
 from .imitation import (BCQ, CQL, GAIL, TD3BC, BCQPolicy, BCQTrainingStats, CQLTrainingStats, DiscreteBCQ, DiscreteBCQPolicy,
-                        DiscreteBCQTrainingStats, DiscreteCRR, DiscreteCRRTrainingStats, GailTrainingStats)
+                        DiscreteBCQTrainingStats, DiscreteCQL, DiscreteCQLTrainingStats, DiscreteCRR, DiscreteCRRTrainingStats,
+                        GailTrainingStats)
 from .modelfree.a2c import A2CTrainingStats, ActorCriticOnPolicyAlgorithm
 from .modelfree.discrete_sac import DiscreteSAC
 from .modelfree.npg import NPG, NPGTrainingStats
 from .modelfree.ppo import A2C, PPO
+from .modelfree.qrdqn import QRDQN, QRDQNPolicy
 from .modelfree.reinforce import DiscreteActorPolicy, ProbabilisticActorPolicy
 from .modelfree.td3 import TD3, TD3TrainingStats
 from .modelfree.trpo import TRPO, TRPOTrainingStats
@@ -17,5 +19,5 @@ __all__ = [
     "GAIL", "GailTrainingStats", "DiscreteSAC", "BCQ", "BCQPolicy", "BCQTrainingStats", "CQL", "CQLTrainingStats", "TD3", "TD3TrainingStats", "TD3BC",
     "ProbabilisticActorPolicy", "DiscreteActorPolicy", "AdamOptimizerFactory", "LRSchedulerFactoryLinear", "OptimizerFactory",
     "RMSpropOptimizerFactory", "DiscreteBCQ", "DiscreteBCQPolicy", "DiscreteBCQTrainingStats", "DiscreteCRR",
-    "DiscreteCRRTrainingStats",
+    "DiscreteCRRTrainingStats", "QRDQN", "QRDQNPolicy", "DiscreteCQL", "DiscreteCQLTrainingStats",
 ]

@@ -1,3 +1,3 @@
-from .atari_network import DQNet, ScaledObsInputActionReprNet, scale_obs
+from .atari_network import DQNet, QRDQNet, ScaledObsInputActionReprNet, scale_obs
 
-__all__ = ["DQNet", "ScaledObsInputActionReprNet", "scale_obs"]
+__all__ = ["DQNet", "QRDQNet", "ScaledObsInputActionReprNet", "scale_obs"]

@@ -1,4 +1,4 @@
-"""NatureCNN Q-network (API of tianshou/env/atari/atari_network.py:26-122).
+"""NatureCNN Q-networks (API of tianshou/env/atari/atari_network.py:26-122, :211-235).
 
 Ordinary ``nn.Module``s: the Collector runs them for action selection; ``DQN.update`` reads the same parameter
 storage through a flat view and runs the conv stack as implicit GEMM on the tensor cores (algorithm/netgraph.py).
@@ -69,3 +69,17 @@ class DQNet(ModuleWithVectorOutput):
     def forward(self, obs: Any, state: Any = None, info: dict | None = None) -> tuple[torch.Tensor, Any]:
         obs = torch.as_tensor(obs, device=torch_device(self), dtype=torch.float32)
         return self.net(obs), state
+
+
+class QRDQNet(DQNet):
+    """Distributional Reinforcement Learning with Quantile Regression (atari_network.py:211-235): a ``DQNet`` whose last Linear
+    has ``actions * num_quantiles`` outputs, returned as ``[B, actions, num_quantiles]``."""
+
+    def __init__(self, *, c: int, h: int, w: int, action_shape: Sequence[int] | int, num_quantiles: int = 200) -> None:
+        self.action_num = int(np.prod(action_shape))
+        super().__init__(c=c, h=h, w=w, action_shape=[self.action_num * num_quantiles])
+        self.num_quantiles = num_quantiles
+
+    def forward(self, obs: Any, state: Any = None, info: dict | None = None) -> tuple[torch.Tensor, Any]:
+        obs, state = super().forward(obs)
+        return obs.view(-1, self.action_num, self.num_quantiles), state

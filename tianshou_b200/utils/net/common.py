@@ -89,14 +89,15 @@ class MLP(ModuleWithVectorOutput):
 
 class Net(ModuleWithVectorOutput):
     """obs -> MLP features (``(logits, state)`` tuple like the reference, common.py:223-369).
-    Only the plain (non-dueling, non-atom) configuration is provided."""
+    ``num_atoms > 1`` widens the last layer to ``prod(action_shape) * num_atoms`` outputs and returns them as
+    ``[B, actions, num_atoms]`` (the distributional heads of QR-DQN, common.py:298-369); the dueling head is not provided."""
 
     def __init__(self, *, state_shape: int | Sequence[int], action_shape: Any = 0,
                  hidden_sizes: Sequence[int] = (), norm_layer: Any = None, norm_args: Any = None,
                  activation: Any = nn.ReLU, act_args: Any = None, softmax: bool = False,
-                 concat: bool = False, linear_layer: TLinearLayer = nn.Linear) -> None:
+                 concat: bool = False, num_atoms: int = 1, linear_layer: TLinearLayer = nn.Linear) -> None:
         input_dim = int(np.prod(state_shape))
-        action_dim = int(np.prod(action_shape))
+        action_dim = int(np.prod(action_shape)) * num_atoms
         if concat:
             input_dim += action_dim
         model = MLP(input_dim=input_dim, output_dim=action_dim if not concat else 0,
@@ -104,10 +105,13 @@ class Net(ModuleWithVectorOutput):
                     activation=activation, act_args=act_args, linear_layer=linear_layer)
         super().__init__(model.output_dim)
         self.softmax = softmax
+        self.num_atoms = num_atoms
         self.model = model
 
     def forward(self, obs: Any, state: Any = None, info: dict | None = None) -> tuple[torch.Tensor, Any]:
         logits = self.model(obs)
+        if self.num_atoms > 1:
+            logits = logits.view(logits.shape[0], -1, self.num_atoms)
         if self.softmax:
             logits = torch.softmax(logits, dim=-1)
         return logits, state
