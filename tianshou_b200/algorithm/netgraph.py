@@ -55,16 +55,19 @@ def _activation_code(m: nn.Module) -> int:
     raise UnsupportedModelError(f"fused layered networks support ReLU / Tanh activations only, got {m}")
 
 
+def _flat_chain(mods: list[nn.Module]) -> list[nn.Module]:
+    out: list[nn.Module] = []
+    for m in mods:
+        out += _flat_chain(list(m)) if isinstance(m, nn.Sequential) else [m]
+    return out
+
+
 def compile_sequential(mods: list[nn.Module], input_shape: tuple[int, ...]) -> list[_Layer]:
-    """Linear / Conv2d / ReLU / Flatten chain -> layer list.  ``input_shape`` = (features,) or (C, H, W)."""
+    """Linear / Conv2d / ReLU / Flatten chain -> layer list.  ``input_shape`` = (features,) or (C, H, W).  Nested
+    ``nn.Sequential`` containers are read as the flat chain they run."""
     layers: list[_Layer] = []
     shape = tuple(int(x) for x in input_shape)
-    for m in mods:
-        if isinstance(m, nn.Sequential):
-            sub = compile_sequential(list(m), shape)
-            layers += sub
-            shape = _out_shape(sub, shape)
-            continue
+    for m in _flat_chain(mods):
         if isinstance(m, nn.Linear):
             if len(shape) != 1 or shape[0] != m.in_features:
                 raise UnsupportedModelError(f"Linear({m.in_features}) after shape {shape}")
@@ -88,6 +91,11 @@ def compile_sequential(mods: list[nn.Module], input_shape: tuple[int, ...]) -> l
             shape = (m.out_channels, Ho, Wo)
         elif isinstance(m, nn.Flatten):
             if len(shape) == 3:
+                # the stack flattens a convolution's NHWC rows into torch's NCHW order; a network input has no such rows
+                # (the frame source feeds the first convolution only, dense rows are NCHW already)
+                if not layers:
+                    raise UnsupportedModelError(f"Flatten of the {shape} network input: flatten the observation before the "
+                                                "network, or start the network with a convolution")
                 layers.append(_Layer("flatten", C=shape[0], H=shape[1], W=shape[2], in_dim=shape[0] * shape[1] * shape[2],
                                      out_dim=shape[0] * shape[1] * shape[2]))
                 shape = (shape[0] * shape[1] * shape[2],)
@@ -219,13 +227,13 @@ class FusedStack:
     def backward(self, acts: list[torch.Tensor], dy: torch.Tensor, rows: int, tag: str = "a", *, param_grads: bool = True,
                  input_grad: bool = False, input_cols: tuple[int, int] | None = None, dy_preact: bool = False,
                  input_act: tuple[int, torch.Tensor] | None = None, dx_out: torch.Tensor | None = None,
-                 dx_accumulate: bool = False, grad_accumulate: bool = False) -> torch.Tensor | None:
+                 dx_accumulate: bool = False) -> torch.Tensor | None:
         """Back-propagate ``dy`` = gradient w.r.t. the LAST layer's output (its activation must be none, or ``dy_preact``: the
         caller already folded the last activation's derivative in).  Weight / bias gradients are STORED into the group's
-        gradient buffer (``zero_grad`` + ``backward`` of algorithm_base.py:497-498) or added with ``grad_accumulate`` (a trunk
-        shared by two losses).  With ``input_grad`` returns d loss / d input (columns ``input_cols`` of the first Linear's
-        input), multiplied by the derivative of the activation ``input_act = (kind, y)`` that produced this stack's input (a
-        head on top of a trunk), written to / accumulated into ``dx_out`` when given."""
+        gradient buffer (``zero_grad`` + ``backward`` of algorithm_base.py:497-498).  With ``input_grad`` returns d loss /
+        d input (columns ``input_cols`` of the first Linear's input), multiplied by the derivative of the activation
+        ``input_act = (kind, y)`` that produced this stack's input (a head on top of a trunk; ``y`` holds all of the first
+        Linear's input columns, the same columns of it are read), written to / accumulated into ``dx_out`` when given."""
         g = self.group
         st = stream_ptr(self.device)
         n = len(self.layers)
@@ -238,15 +246,13 @@ class FusedStack:
             prev_act = self._producer_act(i) if i > 0 else (input_act[0] if input_act is not None else ACT_NONE)
             act_src = x_in if i > 0 else (input_act[1] if input_act is not None else None)
             need_dx = i > 0 or input_grad
-            acc = int(grad_accumulate)
             if L.kind == "linear":
                 M_rows = rows
                 if param_grads:
                     gw = g.grad.data_ptr() + 4 * g.offset(L.weight)
                     gb = g.grad.data_ptr() + 4 * g.offset(L.bias)
-                    self._gemm(ptr(dz), L.out_dim, 1, ptr(x_in), L.in_dim, 1, gw, L.in_dim, L.out_dim, L.in_dim, M_rows,
-                               accumulate=grad_accumulate)
-                    call("ts_net_colsum", ptr(dz), L.out_dim, M_rows, L.out_dim, gb, acc, st)
+                    self._gemm(ptr(dz), L.out_dim, 1, ptr(x_in), L.in_dim, 1, gw, L.in_dim, L.out_dim, L.in_dim, M_rows)
+                    call("ts_net_colsum", ptr(dz), L.out_dim, M_rows, L.out_dim, gb, 0, st)
                 if need_dx:
                     lo, hi = (0, L.in_dim) if (i > 0 or input_cols is None) else input_cols
                     width = hi - lo
@@ -254,7 +260,7 @@ class FusedStack:
                         dx = dx_out
                     else:
                         dx = self._buf((tag, "dx", i), M_rows * width)[: M_rows * width].view(M_rows, width)
-                    mask = ptr(act_src) if prev_act != ACT_NONE else None
+                    mask = ptr(act_src) + 4 * lo if prev_act != ACT_NONE else None
                     self._gemm(ptr(dz), L.out_dim, 0, self._w(L) + 4 * lo, L.in_dim, 1, ptr(dx), width, M_rows, width, L.out_dim,
                                mask=mask, ld_mask=L.in_dim, mask_kind=prev_act if prev_act != ACT_NONE else ACT_RELU,
                                accumulate=(i == 0 and dx_accumulate))
@@ -267,9 +273,8 @@ class FusedStack:
                 if param_grads:
                     gw = g.grad.data_ptr() + 4 * g.offset(L.weight)
                     gb = g.grad.data_ptr() + 4 * g.offset(L.bias)
-                    self._gemm(ptr(dz), L.out_dim, 1, ptr(col), L.in_dim, 1, gw, L.in_dim, L.out_dim, L.in_dim, R,
-                               accumulate=grad_accumulate)
-                    call("ts_net_colsum", ptr(dz), L.out_dim, R, L.out_dim, gb, acc, st)
+                    self._gemm(ptr(dz), L.out_dim, 1, ptr(col), L.in_dim, 1, gw, L.in_dim, L.out_dim, L.in_dim, R)
+                    call("ts_net_colsum", ptr(dz), L.out_dim, R, L.out_dim, gb, 0, st)
                 if i > 0:
                     dcol = self._buf((tag, "dcol", i), R * L.in_dim)[: R * L.in_dim].view(R, L.in_dim)
                     self._gemm(ptr(dz), L.out_dim, 0, self._w(L), L.in_dim, 1, ptr(dcol), L.in_dim, R, L.in_dim, L.out_dim)
