@@ -93,8 +93,8 @@ def build_crr(g, **over):
 @gpu
 @pytest.mark.parametrize("variant,mirror", [("mlp", False), ("mlp", True), ("cnn", False), ("cnn", True), ("sep", False)])
 def test_update_matches_reference(variant, mirror):
-    """All three modes, ``target_update_freq`` 0 (cnn) and several lagged copies (mlp, sep); ``_iter`` advances AFTER the step, so
-    the golden's lagged parameters are one copy later than discrete BCQ's schedule would leave them."""
+    """All three modes, ``target_update_freq`` 0 (cnn) and several lagged copies (mlp, sep), which must fall on the updates the
+    reference copies on: the golden's lagged parameters are the last copy's."""
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden(f"dcrr_ref_{variant}.npz")
     algo, buf = build_crr(g), buffer_from_golden(g, mirror)

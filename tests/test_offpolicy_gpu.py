@@ -634,3 +634,83 @@ def test_dqn_stored_stacks_bit_identical_to_single_frame_storage():
     assert all(torch.equal(x, y) for x, y in zip(a["returns"], b["returns"], strict=True))
     assert all(torch.equal(x, y) for x, y in zip(a["grad"], b["grad"], strict=True))
     assert a["loss"] == b["loss"] and torch.equal(a["flat"], b["flat"])
+
+
+def test_dqn_state_dict_keys():
+    """The reference's keys (test_oracle_offpolicy.py checks them against the reference): the lagged copy under ``.module``."""
+    from test_oracle_offpolicy import DQN_MLP_STATE_DICT_KEYS
+
+    from tianshou_b200.algorithm import AdamOptimizerFactory
+    from tianshou_b200.algorithm.modelfree.dqn import DQN, DiscreteQLearningPolicy
+    from tianshou_b200.utils.net.common import Net
+    policy = DiscreteQLearningPolicy(model=Net(state_shape=(4,), action_shape=3, hidden_sizes=(16,)).to(DEV), action_space=_Discrete(3))
+    algo = DQN(policy=policy, optim=AdamOptimizerFactory(lr=1e-3), target_update_freq=10)
+    assert list(algo.state_dict().keys()) == DQN_MLP_STATE_DICT_KEYS
+
+
+def test_dqn_state_dict_round_trip_continues_identically():
+    """A fresh DQN with other initial weights, loaded from another's ``state_dict()``, continues bit for bit: online, lagged
+    and optimiser state.  With ``target_update_freq`` 10 the six updates copy the lagged network once, in the first, so
+    the loaded algorithm's targets come from the lagged network the load restored.  ``_iter`` is a plain attribute, as in
+    the reference: whoever restores a run restores it too."""
+    import copy
+
+    from tianshou_b200.algorithm import AdamOptimizerFactory
+    from tianshou_b200.algorithm.modelfree.dqn import DQN, DiscreteQLearningPolicy
+    from tianshou_b200.utils import policy_within_training_step
+    A = 6
+
+    def build(seed):
+        net, buf = _dqn_grad_setup("mlp", A, seed=seed, per=False)
+        return DQN(policy=DiscreteQLearningPolicy(model=net, action_space=_Discrete(A)), optim=AdamOptimizerFactory(lr=1e-3),
+                   gamma=0.9, n_step_return_horizon=2, target_update_freq=10), buf
+
+    a, buf_a = build(5)
+    for u in range(3):
+        np.random.seed(u)
+        with policy_within_training_step(a.policy):
+            a.update(buffer=buf_a, sample_size=64)
+    b, _ = build(6)
+    b.load_state_dict(copy.deepcopy(a.state_dict()))
+    b._iter = a._iter
+    for algo in (a, b):
+        buf = _dqn_grad_setup("mlp", A, seed=5, per=False)[1]
+        for u in range(3):
+            np.random.seed(10 + u)
+            with policy_within_training_step(algo.policy):
+                algo.update(buffer=buf, sample_size=64)
+    for ga, gb in ((a._group, b._group), (a._g_old, b._g_old)):
+        assert torch.equal(ga.flat, gb.flat) and torch.equal(ga.exp_avg, gb.exp_avg) and torch.equal(ga.exp_avg_sq, gb.exp_avg_sq)
+    assert a._group.step == b._group.step
+
+
+@pytest.mark.parametrize("algo_name", ["dqn", "discrete_sac"])
+@pytest.mark.parametrize("bad", ["A", "-1"])
+def test_drawn_actions_outside_the_network_outputs_are_refused(algo_name, bad):
+    """The loss kernels index a row of A values with each drawn action: a buffer holding A or -1 is refused on the host
+    while the batch is drawn, before anything is launched."""
+    from tianshou_b200.algorithm import AdamOptimizerFactory, DiscreteSAC
+    from tianshou_b200.algorithm.modelfree.discrete_sac import DiscreteSACPolicy
+    from tianshou_b200.algorithm.modelfree.dqn import DQN, DiscreteQLearningPolicy
+    from tianshou_b200.data import Batch, VectorReplayBuffer
+    from tianshou_b200.utils import policy_within_training_step
+    from tianshou_b200.utils.net.common import Net
+    from tianshou_b200.utils.net.discrete import DiscreteActor, DiscreteCritic
+    A = 3
+    net = lambda **kw: Net(state_shape=(4,), hidden_sizes=(16,), **kw).to(DEV)
+    if algo_name == "dqn":
+        algo = DQN(policy=DiscreteQLearningPolicy(model=net(action_shape=A), action_space=_Discrete(A)),
+                   optim=AdamOptimizerFactory(lr=1e-3), target_update_freq=2)
+    else:
+        actor = DiscreteActor(preprocess_net=net(), action_shape=A, softmax_output=False).to(DEV)
+        algo = DiscreteSAC(policy=DiscreteSACPolicy(actor=actor, action_space=_Discrete(A)), policy_optim=AdamOptimizerFactory(lr=1e-3),
+                           critic=DiscreteCritic(preprocess_net=net(), last_size=A).to(DEV), critic_optim=AdamOptimizerFactory(lr=1e-3))
+    buf = VectorReplayBuffer(40, 4, device=DEV)
+    rng = np.random.default_rng(0)
+    for _ in range(8):
+        buf.add(Batch(obs=rng.standard_normal((4, 4)).astype(np.float32), act=np.array([0, 1, A if bad == "A" else -1, 2]),
+                      rew=np.zeros(4), terminated=np.zeros(4, bool), truncated=np.zeros(4, bool),
+                      obs_next=rng.standard_normal((4, 4)).astype(np.float32)), buffer_ids=np.arange(4))
+    np.random.seed(0)
+    with pytest.raises(ValueError, match="actions in"), policy_within_training_step(algo.policy):
+        algo.update(buffer=buf, sample_size=32)

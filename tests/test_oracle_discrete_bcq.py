@@ -181,3 +181,32 @@ def test_two_head_network_detects_sharing_and_refuses():
     b.last.model[-1] = torch.nn.Linear(8, 3, bias=False)
     with pytest.raises(UnsupportedModelError, match="bias"):
         build(a, b)
+
+
+def test_lagged_group_is_a_prefix_of_the_online_layout():
+    """A lagged copy's flat buffer is the online layout cut short: a copy of the network whose parameters lead the group,
+    or of the whole group, is accepted and ``refresh_lagged`` copies that prefix into the lagged modules; parameters whose
+    shapes differ from the online ones at any position are refused."""
+    import copy
+
+    from tianshou_b200.algorithm import UnsupportedModelError
+    from tianshou_b200.algorithm.discrete_q import lagged_group, refresh_lagged
+    from tianshou_b200.algorithm.flat_params import FlatGroup
+    from tianshou_b200.algorithm.shared_trunk import two_head_parameters
+    from tianshou_b200.utils.net.common import Net
+    model, imitator = _heads(False)
+    online = FlatGroup(two_head_parameters(model, imitator), torch.device("cpu"))
+    model_old = copy.deepcopy(model)
+    lagged = lagged_group(online, list(model_old.parameters()))
+    assert lagged.n == sum(p.numel() for p in model.parameters()) < online.n
+    with torch.no_grad():
+        online.flat.add_(1.0)
+    refresh_lagged(online, lagged)
+    assert torch.equal(lagged.flat, online.flat[: lagged.n])
+    assert all(torch.equal(p, q) for p, q in zip(model_old.parameters(), model.parameters(), strict=True))
+    assert lagged_group(online, list(copy.deepcopy(torch.nn.ModuleList([model, imitator])).parameters())).n == online.n
+    wide, _ = _heads(False, trunk=lambda: Net(state_shape=(4,), hidden_sizes=(32,)))
+    extra = torch.nn.Parameter(torch.zeros(3))
+    for params in (list(wide.parameters()), list(model.parameters())[::-1], [*copy.deepcopy(online.params), extra]):
+        with pytest.raises(UnsupportedModelError, match="not a prefix"):
+            lagged_group(online, params)

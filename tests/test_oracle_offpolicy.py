@@ -83,3 +83,28 @@ def test_dqn_oracle_matches_reference_run(variant):
     _close(list(net.parameters()), g, f"u{n_up - 1}_q_", lr, "q")
     if freq > 0:
         _close(list(net_old.parameters()), g, f"u{n_up - 1}_qold_", lr, "lagged q")
+
+
+# the state_dict() keys of DQN with a target network on Net(state_shape=(4,), action_shape=3, hidden_sizes=(16,)): the policy's
+# network, the lagged copy under ``.module`` (utils/lagged_network.py:21-41), the optimisers
+DQN_MLP_STATE_DICT_KEYS = [
+    "policy.model.model.model.0.weight", "policy.model.model.model.0.bias", "policy.model.model.model.2.weight",
+    "policy.model.model.model.2.bias", "model_old.module.model.model.0.weight", "model_old.module.model.model.0.bias",
+    "model_old.module.model.model.2.weight", "model_old.module.model.model.2.bias", "_optimizers",
+]
+
+
+def test_reference_dqn_state_dict_keys():
+    """The reference's keys for the net whose keys test_offpolicy_gpu.py checks on the device DQN."""
+    from oracle.ref_shim import import_reference, reference_available
+    if not reference_available():
+        pytest.skip("reference tree not present")
+    import_reference()
+    import gymnasium as gym
+    from tianshou.algorithm.modelfree.dqn import DQN, DiscreteQLearningPolicy
+    from tianshou.algorithm.optim import AdamOptimizerFactory
+    from tianshou.utils.net.common import Net
+    policy = DiscreteQLearningPolicy(model=Net(state_shape=(4,), action_shape=3, hidden_sizes=(16,)),
+                                     action_space=gym.spaces.Discrete(3))
+    algo = DQN(policy=policy, optim=AdamOptimizerFactory(lr=1e-3), target_update_freq=10)
+    assert list(algo.state_dict().keys()) == DQN_MLP_STATE_DICT_KEYS

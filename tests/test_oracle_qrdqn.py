@@ -139,7 +139,7 @@ def test_qrdqnet_matches_reference():
 def test_layer_chain_of_quantile_networks():
     """The device path reads either network as a plain chain ending in Linear(., A * N): what describe_q_network and
     compile_sequential see."""
-    from tianshou_b200.algorithm.modelfree.dqn import describe_q_network
+    from tianshou_b200.algorithm.discrete_q import describe_q_network
     from tianshou_b200.algorithm.netgraph import ACT_NONE, compile_sequential, module_layers
     from tianshou_b200.env.atari import QRDQNet, ScaledObsInputActionReprNet
     from tianshou_b200.utils.net.common import Net

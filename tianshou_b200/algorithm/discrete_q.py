@@ -1,0 +1,127 @@
+"""What the discrete-action value-based updates share: DQN, QR-DQN, discrete CQL, discrete BCQ and discrete CRR stand on
+``DiscreteQCore``; discrete SAC reads its networks and draws its batches with the same functions.
+
+Reference: modelfree/dqn.py:170-283 (QLearningOffPolicyAlgorithm: the n-step return, the lagged network refreshed when
+``_iter % target_update_freq == 0``), :384-401 (``q[np.arange(len(q)), batch.act]``: an action outside the network's outputs
+raises), utils/lagged_network.py:21-41 and :81-103 (the lagged copy under ``.module``, its full copy), utils/net/discrete.py:29-123
+(``DiscreteActor`` / ``DiscreteCritic``: a preprocess net, then the ``last`` MLP).
+"""
+from __future__ import annotations
+
+from collections.abc import Callable
+from typing import Any
+
+import numpy as np
+import torch
+from torch import nn
+
+from .._cabi import to_device
+from ..data import Batch, ReplayBuffer
+from .base import Algorithm
+from .flat_params import DeviceScratch, FlatGroup, UnsupportedModelError
+from .netgraph import module_layers
+from .obs_source import DeviceObsSource, device_obs_source
+from .twin_critic import per_weight
+
+
+def describe_q_network(model: Any) -> tuple[Any, tuple[int, ...], float]:
+    """(inner module with the layer chain, input shape, input denominator) of a Q-network: ``DQNet`` (optionally behind
+    ``ScaledObsInputActionReprNet``) or an MLP ``Net`` on flat observations."""
+    scale = 1.0          # the DENOMINATOR the observation is divided by before the network
+    inner = model
+    if hasattr(model, "denom") and hasattr(model, "module"):
+        scale = float(model.denom)
+        inner = model.module
+    if hasattr(inner, "input_shape"):
+        return inner, tuple(inner.input_shape), scale
+    first = module_layers(inner)[0]
+    if isinstance(first, nn.Linear):
+        return inner, (int(first.in_features),), scale
+    raise UnsupportedModelError(f"cannot infer the input shape of {type(inner).__name__}")
+
+
+def describe_discrete_head(net: Any, role: str) -> tuple[Any, Any, tuple[int, ...], float]:
+    """``DiscreteActor`` / ``DiscreteCritic`` -> (the preprocess net's inner module, the ``last`` MLP, input shape, input
+    denominator).  The preprocess net is anything ``describe_q_network`` reads; a softmax output of it is refused."""
+    pre, last = getattr(net, "preprocess", None), getattr(net, "last", None)
+    if pre is None or last is None:
+        raise UnsupportedModelError(f"{role}: expected a DiscreteActor / DiscreteCritic (preprocess net + last MLP), got "
+                                    f"{type(net).__name__}")
+    try:
+        inner, shape, scale = describe_q_network(pre)
+    except UnsupportedModelError as e:
+        raise UnsupportedModelError(f"{role}: {e}") from e
+    if getattr(pre, "softmax", False) or getattr(inner, "softmax", False):
+        raise UnsupportedModelError(f"{role}: a softmax preprocess output is not supported")
+    return inner, last, shape, scale
+
+
+def sample_discrete(buffer: ReplayBuffer, sample_size: int | None, obs_source: Callable[..., DeviceObsSource],
+                    device: torch.device, n_actions: int) -> tuple[Batch, Any]:
+    """Indices from the buffer's host RNG streams (identical to the reference's draws); the observations as
+    ``obs_source(buffer, indices, "obs")`` reads them on the device, the actions as int64 device rows, the importance weight
+    of a prioritised buffer.  The loss kernels index a row of ``n_actions`` values with each drawn action: an action outside
+    ``[0, n_actions)`` is refused here, before anything is launched."""
+    indices = buffer.sample_indices(sample_size)
+    act = np.asarray(buffer.act)[indices]
+    if act.size and (act.min() < 0 or act.max() >= n_actions):
+        raise ValueError(f"the buffer holds actions in [{act.min()}, {act.max()}], the networks have {n_actions} outputs")
+    batch = Batch()
+    batch.__dict__["obs"] = obs_source(buffer, indices, "obs")
+    batch.__dict__["act"] = to_device(np.ascontiguousarray(act.reshape(-1)).astype(np.int64), device)
+    weight = per_weight(buffer, indices, device)
+    if weight is not None:
+        batch.__dict__["weight"] = weight
+    batch.__dict__["info"] = Batch()
+    return batch, indices
+
+
+def lagged_group(online: FlatGroup, lagged_params: list[nn.Parameter]) -> FlatGroup:
+    """The flat group of a lagged copy whose parameters match the first ``len(lagged_params)`` of ``online``'s, shape by
+    shape: its flat buffer is a prefix of the online layout, so the online chains run on it as ``params=`` and one copy
+    refreshes it.  A copy of the whole network is the trivial prefix.  The lagged modules' parameters become views of it."""
+    shapes = [tuple(p.shape) for p in lagged_params]
+    if shapes != [tuple(p.shape) for p in online.params[: len(shapes)]]:
+        raise UnsupportedModelError(f"the lagged network's parameter shapes {shapes} are not a prefix of the online network's "
+                                    f"{[tuple(p.shape) for p in online.params]}")
+    return FlatGroup(lagged_params, online.device)
+
+
+def refresh_lagged(online: FlatGroup, lagged: FlatGroup) -> None:
+    """The full copy of the lagged network (lagged_network.py:81-103): one device copy of the online prefix."""
+    online.ensure_adopted()
+    lagged.ensure_adopted()
+    lagged.flat.copy_(online.flat[: lagged.n])
+
+
+class DiscreteQCore(Algorithm):
+    """A discrete-action value-based update on one CUDA device.  The subclass builds its networks, calls ``_init_discrete``
+    and sets ``gamma``, ``n_step``, ``_target_q``, ``_group`` and (with a lagged network) ``_g_old``; the core reads the
+    observations, draws the batch (refusing actions outside ``[0, n_actions)``), computes the n-step return and refreshes
+    the lagged copy on its tick."""
+
+    def _init_discrete(self, dev: torch.device, in_shape: tuple[int, ...], in_scale: float, n_actions: int) -> None:
+        self._dev, self._in_shape, self._in_scale, self.n_actions = dev, in_shape, in_scale, n_actions
+        self._iter = 0
+        self._scratch = DeviceScratch(dev)
+        self._buf = self._scratch.tensor
+
+    def _obs_source(self, buffer: ReplayBuffer, indices: np.ndarray | torch.Tensor, key: str = "obs") -> DeviceObsSource:
+        """How the network reads ``buffer[indices].<key>`` without materialising it on the host (obs_source.py)."""
+        return device_obs_source(buffer, indices, key, self._in_shape, self._in_scale, self._dev, self._buf)
+
+    def _sample(self, buffer: ReplayBuffer, sample_size: int | None) -> tuple[Batch, Any]:
+        return sample_discrete(buffer, sample_size, self._obs_source, self._dev, self.n_actions)
+
+    def _preprocess_batch(self, batch: Batch, buffer: ReplayBuffer, indices: np.ndarray) -> Batch:
+        return self.compute_nstep_return(batch=batch, buffer=buffer, indices=indices, target_q_fn=self._target_q,
+                                         gamma=self.gamma, n_step=self.n_step)
+
+    def _tick_lagged(self, freq: int) -> None:
+        """Before the step: the lagged copy is refreshed when ``freq > 0 and _iter % freq == 0``, then ``_iter`` advances."""
+        if freq > 0 and self._iter % freq == 0:
+            self._refresh_lagged()
+        self._iter += 1
+
+    def _refresh_lagged(self) -> None:
+        refresh_lagged(self._group, self._g_old)

@@ -27,12 +27,12 @@ from torch import nn
 from ..._cabi import call, ptr, stream_ptr
 from ...data import Batch, ReplayBuffer
 from ..base import OfflineAlgorithm
-from ..flat_params import DeviceScratch, FlatGroup, UnsupportedModelError, bind_optimizer
+from ..discrete_q import DiscreteQCore, lagged_group
+from ..flat_params import FlatGroup, UnsupportedModelError, bind_optimizer
 from ..modelfree.dqn import DiscreteQLearningPolicy, SimpleLossTrainingStats
-from ..obs_source import DeviceObsSource, device_obs_source
 from ..optim import OptimizerFactory
 from ..shared_trunk import TwoHeadNetwork, two_head_parameters
-from ..twin_critic import _EvalModeModule, cuda_device_of, sample_discrete
+from ..twin_critic import _EvalModeModule, cuda_device_of
 
 INF = torch.finfo(torch.float32).max
 
@@ -42,13 +42,6 @@ class DiscreteBCQTrainingStats(SimpleLossTrainingStats):
     q_loss: float
     i_loss: float
     reg_loss: float
-
-
-def check_actions_in_range(buffer: ReplayBuffer, indices: np.ndarray, n_actions: int) -> None:
-    """The loss kernels index a row of ``n_actions`` values with the stored action: refuse anything else on the host."""
-    act = np.asarray(buffer.act)[indices]
-    if act.size and (act.min() < 0 or act.max() >= n_actions):
-        raise ValueError(f"the buffer holds actions in [{act.min()}, {act.max()}], the networks have {n_actions} outputs")
 
 
 class DiscreteBCQPolicy(DiscreteQLearningPolicy):
@@ -78,7 +71,7 @@ class DiscreteBCQPolicy(DiscreteQLearningPolicy):
         return Batch(act=act, state=state, q_value=q_value, imitation_logits=imitation_logits, logits=imitation_logits)
 
 
-class DiscreteBCQ(OfflineAlgorithm):
+class DiscreteBCQ(DiscreteQCore, OfflineAlgorithm):
     """Discrete BCQ, reference API and semantics (discrete_bcq.py:130-261).
 
     ``policy.model`` and ``policy.imitator`` are ``DiscreteActor(softmax_output=False)`` / ``DiscreteCritic``-shaped networks
@@ -98,38 +91,27 @@ class DiscreteBCQ(OfflineAlgorithm):
         self.n_step = n_step_return_horizon
         self._target = True
         self.freq = target_update_freq
-        self._iter = 0
         self._weight_reg = imitation_logits_penalty
         model, imitator = policy.model, policy.imitator
         for name, net in (("model", model), ("imitator", imitator)):
             if getattr(net, "softmax_output", False):
                 raise UnsupportedModelError(f"{name}: DiscreteActor(softmax_output=True) is not supported: the update reads the "
                                             "output as Q-values / logits; build it with softmax_output=False")
-        dev = self._dev = cuda_device_of(model, imitator)
+        dev = cuda_device_of(model, imitator)
         self._group = FlatGroup(two_head_parameters(model, imitator), dev)
         self._net = TwoHeadNetwork(model, imitator, self._group, roles=("model", "imitator"))
-        self._in_shape, self._in_scale = self._net.in_shape, self._net.in_scale
-        self.n_actions = int(policy.action_space.n)
+        n_actions = int(policy.action_space.n)
         for name, n in zip(("model", "imitator"), self._net.n_out):
-            if n != self.n_actions:
-                raise UnsupportedModelError(f"{name} has {n} outputs for {self.n_actions} actions")
+            if n != n_actions:
+                raise UnsupportedModelError(f"{name} has {n} outputs for {n_actions} actions")
+        self._init_discrete(dev, self._net.in_shape, self._net.in_scale, n_actions)
         self.optim = self._create_optimizer(policy, optim)
         bind_optimizer(self.optim, self._group)
         # the model's parameters lead the flat order, so the lagged model's flat buffer is a prefix of the same layout
         self.model_old = _EvalModeModule(deepcopy(model))
-        self._g_old = FlatGroup(list(self.model_old.module.parameters()), dev)
-        self._scratch = DeviceScratch(dev)
-        self._buf = self._scratch.tensor
+        self._g_old = lagged_group(self._group, list(self.model_old.module.parameters()))
 
-    # ------------------------------------------------------------------ sampling / target
-    def _obs_source(self, buffer: ReplayBuffer, indices: np.ndarray | torch.Tensor, key: str = "obs") -> DeviceObsSource:
-        return device_obs_source(buffer, indices, key, self._in_shape, self._in_scale, self._dev, self._buf)
-
-    def _sample(self, buffer: ReplayBuffer, sample_size: int | None) -> tuple[Batch, Any]:
-        batch, indices = sample_discrete(buffer, sample_size, self._obs_source, self._dev)
-        check_actions_in_range(buffer, indices, self.n_actions)
-        return batch, indices
-
+    # ------------------------------------------------------------------ target
     def _target_q(self, buffer: ReplayBuffer, indices: np.ndarray) -> torch.Tensor:
         """Q_old(s', argmax_a Q(s', a) over the actions the imitator keeps)   (discrete_bcq.py:228-234)."""
         src = self._obs_source(buffer, indices, "obs_next")
@@ -141,20 +123,9 @@ class DiscreteBCQ(OfflineAlgorithm):
              self.n_actions, ptr(out), None, stream_ptr(self._dev))
         return out
 
-    def _preprocess_batch(self, batch: Batch, buffer: ReplayBuffer, indices: np.ndarray) -> Batch:
-        return self.compute_nstep_return(batch=batch, buffer=buffer, indices=indices, target_q_fn=self._target_q,
-                                         gamma=self.gamma, n_step=self.n_step)
-
     # ------------------------------------------------------------------ update
-    def _update_lagged_network_weights(self) -> None:
-        self._group.ensure_adopted()
-        self._g_old.ensure_adopted()
-        self._g_old.flat.copy_(self._group.flat[: self._g_old.n])         # full copy (lagged_network.py:81-87)
-
     def _update_with_batch(self, batch: Batch) -> DiscreteBCQTrainingStats:
-        if self._iter % self.freq == 0:
-            self._update_lagged_network_weights()
-        self._iter += 1
+        self._tick_lagged(self.freq)
         src = batch.obs
         B, A = src.rows, self.n_actions
         acts = self._net.forward(src, "up")

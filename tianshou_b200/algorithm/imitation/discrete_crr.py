@@ -25,14 +25,13 @@ from torch import nn
 from ..._cabi import ABI, call, ptr, stream_ptr, to_device
 from ...data import Batch, ReplayBuffer
 from ..base import OfflineAlgorithm
-from ..flat_params import DeviceScratch, FlatGroup, UnsupportedModelError, bind_optimizer
+from ..discrete_q import DiscreteQCore, lagged_group
+from ..flat_params import FlatGroup, UnsupportedModelError, bind_optimizer
 from ..modelfree.dqn import SimpleLossTrainingStats
 from ..modelfree.reinforce import DiscreteActorPolicy
-from ..obs_source import DeviceObsSource, device_obs_source
 from ..optim import OptimizerFactory
 from ..shared_trunk import TwoHeadNetwork, two_head_parameters
-from ..twin_critic import _EvalModeModule, cuda_device_of, sample_discrete
-from .discrete_bcq import check_actions_in_range
+from ..twin_critic import _EvalModeModule, cuda_device_of
 
 _MODES = {"exp": ABI.consts["TS_CRR_EXP"], "binary": ABI.consts["TS_CRR_BINARY"], "all": ABI.consts["TS_CRR_ALL"]}
 
@@ -56,7 +55,7 @@ class DiscountedReturnComputation:
         assert 0.0 <= self.gamma <= 1.0, "discount factor gamma should be in [0, 1]"
 
 
-class DiscreteCRR(OfflineAlgorithm):
+class DiscreteCRR(DiscreteQCore, OfflineAlgorithm):
     """Discrete CRR, reference API and semantics (discrete_crr.py:33-167).
 
     The policy's actor (``DiscreteActor(softmax_output=False)``) and ``critic`` (``DiscreteCritic(last_size=n_actions)``) sit on
@@ -66,10 +65,11 @@ class DiscreteCRR(OfflineAlgorithm):
     of ``-log_prob`` ``[B]`` with the coefficient ``[B, 1]`` broadcasts to ``[B, B]``, so ``actor_loss`` is
     ``mean(-log_prob) * mean(coefficient)``.  The target is one-step, on ``batch.done``.
 
-    ``target_update_freq > 0``: the lagged actor and critic are copied when ``_iter % target_update_freq == 0``, ``_iter``
-    advancing AFTER the step; both copies are taken at the same moment, so on the device they are one lagged flat buffer of
-    the whole group, and ``critic_old``'s own copy of a shared trunk is kept equal to ``actor_old``'s.  ``0``: the lagged
-    networks are the online ones.
+    ``target_update_freq > 0``: the lagged actor and critic are copied when ``_iter % target_update_freq == 0``, before the
+    step; both copies are taken at the same moment, so on the device they are one lagged flat buffer of the whole group, and
+    ``critic_old``'s own copy of a shared trunk is kept equal to ``actor_old``'s.  ``0``: the lagged networks are the online
+    ones.  ``_iter`` advances in the copy's tick, before the step, where the reference advances it after the step: after every
+    completed update it holds the same count, and the copies fall on the same updates.
 
     ``batch.returns`` is not produced: the reference computes Monte-Carlo returns in ``_preprocess_batch`` and its loss never
     reads them, so parameters and statistics are the same with ``return_standardization`` on and off; the running return
@@ -89,19 +89,18 @@ class DiscreteCRR(OfflineAlgorithm):
         if getattr(actor, "softmax_output", False):
             raise UnsupportedModelError("DiscreteActor(softmax_output=True): discrete CRR reads the actor output as logits, "
                                         "probabilities would be treated as logits; build the actor with softmax_output=False")
-        dev = self._dev = cuda_device_of(actor, critic)
+        dev = cuda_device_of(actor, critic)
         self._group = FlatGroup(two_head_parameters(actor, critic), dev)
         self._net = TwoHeadNetwork(actor, critic, self._group, roles=("actor", "critic"))
-        self._in_shape, self._in_scale = self._net.in_shape, self._net.in_scale
-        self.n_actions = int(policy.action_space.n)
+        n_actions = int(policy.action_space.n)
         for name, n in zip(("actor", "critic"), self._net.n_out):
-            if n != self.n_actions:
-                raise UnsupportedModelError(f"{name} has {n} outputs for {self.n_actions} actions")
+            if n != n_actions:
+                raise UnsupportedModelError(f"{name} has {n} outputs for {n_actions} actions")
+        self._init_discrete(dev, self._net.in_shape, self._net.in_scale, n_actions)
         self.optim = self._create_optimizer(nn.ModuleList([policy, critic]), optim)
         bind_optimizer(self.optim, self._group)
         self._target = target_update_freq > 0
         self._freq = target_update_freq
-        self._iter = 0
         self._g_old: FlatGroup | None = None
         if self._target:
             self.actor_old = _EvalModeModule(deepcopy(actor))
@@ -109,7 +108,7 @@ class DiscreteCRR(OfflineAlgorithm):
             a_old, c_old = self.actor_old.module, self.critic_old.module
             # the online flat order with the lagged modules' parameters; of a shared trunk actor_old's copy is the one in it
             tail = c_old.last.parameters() if self._net.shared else c_old.parameters()
-            self._g_old = FlatGroup([*a_old.parameters(), *tail], dev)
+            self._g_old = lagged_group(self._group, [*a_old.parameters(), *tail])
         else:
             self.actor_old = actor
             self.critic_old = critic
@@ -117,28 +116,23 @@ class DiscreteCRR(OfflineAlgorithm):
         self._ratio_upper_bound = ratio_upper_bound
         self._beta = beta
         self._min_q_weight = min_q_weight
-        self._scratch = DeviceScratch(dev)
-        self._buf = self._scratch.tensor
 
     # ------------------------------------------------------------------ sampling
-    def _obs_source(self, buffer: ReplayBuffer, indices: np.ndarray | torch.Tensor, key: str = "obs") -> DeviceObsSource:
-        return device_obs_source(buffer, indices, key, self._in_shape, self._in_scale, self._dev, self._buf)
-
     def _sample(self, buffer: ReplayBuffer, sample_size: int | None) -> tuple[Batch, Any]:
-        """``sample_discrete`` plus what the one-step target needs of the drawn rows: ``obs_next`` as a device observation
+        """The core's sample plus what the one-step target needs of the drawn rows: ``obs_next`` as a device observation
         source, ``rew`` and ``done`` as fp32 rows (``to_torch_as(batch.rew, q)``, ``batch.done > 0``)."""
-        batch, indices = sample_discrete(buffer, sample_size, self._obs_source, self._dev)
-        check_actions_in_range(buffer, indices, self.n_actions)
+        batch, indices = super()._sample(buffer, sample_size)
         batch.__dict__["obs_next"] = self._obs_source(buffer, indices, "obs_next")
         batch.__dict__["rew"] = to_device(np.asarray(buffer.rew)[indices].astype(np.float32).reshape(-1), self._dev)
         batch.__dict__["done"] = to_device(np.asarray(buffer.done)[indices].astype(np.float32).reshape(-1), self._dev)
         return batch, indices
 
+    def _preprocess_batch(self, batch: Batch, buffer: ReplayBuffer, indices: np.ndarray) -> Batch:
+        return batch
+
     # ------------------------------------------------------------------ update
-    def _update_lagged_network_weights(self) -> None:
-        self._group.ensure_adopted()
-        self._g_old.ensure_adopted()
-        self._g_old.flat.copy_(self._group.flat)                           # full copy (lagged_network.py:81-87)
+    def _refresh_lagged(self) -> None:
+        super()._refresh_lagged()
         if self._net.shared:
             with torch.no_grad():
                 for tp, sp in zip(self.critic_old.module.preprocess.parameters(), self.actor_old.module.preprocess.parameters(),
@@ -146,8 +140,7 @@ class DiscreteCRR(OfflineAlgorithm):
                     tp.copy_(sp)
 
     def _update_with_batch(self, batch: Batch) -> DiscreteCRRTrainingStats:
-        if self._target and self._iter % self._freq == 0:
-            self._update_lagged_network_weights()
+        self._tick_lagged(self._freq)
         src, src_next = batch.obs, batch.obs_next
         B, A = src.rows, self.n_actions
         on = self._net.forward(src, "up")
@@ -162,6 +155,5 @@ class DiscreteCRR(OfflineAlgorithm):
              ptr(losses), stream_ptr(self._dev))
         self._net.backward(on, dlogits, dq, "up")
         self._group.adam_step(self.optim._optim, self.optim._max_grad_norm)
-        self._iter += 1
         l = losses.cpu().numpy()                # the only host read of the losses
         return DiscreteCRRTrainingStats(loss=float(l[0]), actor_loss=float(l[1]), critic_loss=float(l[2]), cql_loss=float(l[3]))

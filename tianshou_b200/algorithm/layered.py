@@ -24,7 +24,7 @@ from torch import nn
 from .. import ops
 from .._cabi import AC_CATEGORICAL, AC_RELU, STATS_STRIDE, ActorCriticDesc, call, ptr, stream_ptr
 from .flat_params import DeviceScratch, FlatGroup, UnsupportedModelError
-from .netgraph import ACT_NONE, ACT_RELU, FusedStack, _Layer, compile_sequential, module_layers
+from .netgraph import ACT_NONE, ACT_RELU, FusedStack, _Layer, compile_sequential, layer_params, module_layers
 
 _CHUNK = 131072          # rows per forward chunk of the whole-rollout passes (bounds the activation scratch)
 
@@ -44,10 +44,6 @@ class ActorCriticSpec:
     c_trunk: list[_Layer]
     c_head: list[_Layer]
     group_params: list[list[nn.Parameter]]
-
-
-def _layer_params(layers: list[_Layer]) -> list[nn.Parameter]:
-    return [p for L in layers if L.weight is not None for p in (L.weight, L.bias)]
 
 
 def parse_actor_critic(actor: Any, critic: Any, *, split: bool) -> ActorCriticSpec:
@@ -84,8 +80,8 @@ def parse_actor_critic(actor: Any, critic: Any, *, split: bool) -> ActorCriticSp
     if act_dim > 64:
         raise UnsupportedModelError("action width > 64 unsupported")
     a_ids, c_ids = set(map(id, actor.parameters())), set(map(id, critic.parameters()))
-    trunk_ids = [id(p) for p in _layer_params(a_trunk)]
-    shared = trunk_ids == [id(p) for p in _layer_params(c_trunk)] and [L.act for L in a_trunk] == [L.act for L in c_trunk]
+    trunk_ids = [id(p) for p in layer_params(a_trunk)]
+    shared = trunk_ids == [id(p) for p in layer_params(c_trunk)] and [L.act for L in a_trunk] == [L.act for L in c_trunk]
     if (a_ids & c_ids) != (set(trunk_ids) if shared else set()):
         raise UnsupportedModelError("partially shared trunks are unsupported")
     if split and shared:
@@ -93,7 +89,7 @@ def parse_actor_critic(actor: Any, critic: Any, *, split: bool) -> ActorCriticSp
                                     "shared trunks are unsupported")
     params = list({id(p): p for p in [*actor.parameters(), *critic.parameters()]}.values())   # ActorCritic order, shared once
     sigma_param = None if categorical else actor.sigma_param
-    covered = {id(p) for p in _layer_params([*a_trunk, *c_trunk, *a_head, *c_head])}
+    covered = {id(p) for p in layer_params([*a_trunk, *c_trunk, *a_head, *c_head])}
     if [id(p) for p in params if id(p) not in covered] != ([] if categorical else [id(sigma_param)]):
         raise UnsupportedModelError("actor / critic hold parameters outside the Linear layers")
     return ActorCriticSpec(obs_dim, act_dim, categorical, shared, sigma_param, a_trunk, a_head, c_trunk, c_head,

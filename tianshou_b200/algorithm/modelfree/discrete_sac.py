@@ -29,12 +29,12 @@ from torch.distributions import Categorical
 from ..._cabi import call, ptr, stream_ptr
 from ...data import Batch, ReplayBuffer
 from ..base import OffPolicyAlgorithm, Policy
+from ..discrete_q import describe_discrete_head, sample_discrete
 from ..flat_params import UnsupportedModelError
-from ..netgraph import ACT_NONE, _Layer, compile_sequential, module_layers
+from ..netgraph import ACT_NONE, _Layer, compile_sequential, layer_params, module_layers
 from ..obs_source import DeviceObsSource, device_obs_source
 from ..optim import OptimizerFactory
-from ..twin_critic import TwinCriticAlgorithm, pop_batch_weight, sample_discrete
-from .dqn import describe_q_network
+from ..twin_critic import TwinCriticAlgorithm, pop_batch_weight
 from .sac import Alpha, SACTrainingStats
 
 
@@ -65,25 +65,17 @@ class DiscreteSACPolicy(Policy):
         return Batch(logits=logits, act=act, state=hidden, dist=dist)
 
 
-def describe_discrete_head_network(net: Any, role: str) -> tuple[list[_Layer], list[nn.Parameter], tuple[int, ...], float]:
-    """``DiscreteActor`` / ``DiscreteCritic`` -> (layer chain ``module_layers(preprocess) + module_layers(last)``, its
-    parameters, input shape, input denominator).  The preprocess net is anything DQN reads: an MLP ``Net`` on flat
-    observations or ``DQNet``, optionally behind ``ScaledObsInputActionReprNet``."""
-    pre, last = getattr(net, "preprocess", None), getattr(net, "last", None)
-    if pre is None or last is None:
-        raise UnsupportedModelError(f"{role}: expected a DiscreteActor / DiscreteCritic (preprocess net + last MLP), got "
-                                    f"{type(net).__name__}")
-    if getattr(pre, "softmax", False):
-        raise UnsupportedModelError(f"{role}: a softmax preprocess output is not supported")
+def _head_chain(net: Any, role: str) -> tuple[list[_Layer], tuple[int, ...], float]:
+    """(layer chain ``module_layers(preprocess) + module_layers(last)``, input shape, input denominator) of a
+    ``DiscreteActor`` / ``DiscreteCritic`` over the actions."""
+    inner, last, shape, scale = describe_discrete_head(net, role)
     try:
-        inner, shape, scale = describe_q_network(pre)
         layers = compile_sequential(module_layers(inner) + module_layers(last), shape)
     except UnsupportedModelError as e:
         raise UnsupportedModelError(f"{role}: {e}") from e
     if layers[-1].kind != "linear" or layers[-1].act != ACT_NONE:
         raise UnsupportedModelError(f"{role}: must end in a linear layer over the actions")
-    params = [p for L in layers if L.weight is not None for p in (L.weight, L.bias)]
-    return layers, params, shape, scale
+    return layers, shape, scale
 
 
 class DiscreteSAC(TwinCriticAlgorithm, OffPolicyAlgorithm):
@@ -122,21 +114,21 @@ class DiscreteSAC(TwinCriticAlgorithm, OffPolicyAlgorithm):
                                 critic2_optim=critic2_optim)
 
     def _describe_actor(self, actor: nn.Module) -> tuple[list[_Layer], list[nn.Parameter]]:
-        layers, params, self._in_shape, self._in_scale = describe_discrete_head_network(actor, "actor")
+        layers, self._in_shape, self._in_scale = _head_chain(actor, "actor")
         self.n_actions = layers[-1].out_dim
         if self.n_actions != int(self.policy.action_space.n):
             raise UnsupportedModelError(f"actor has {self.n_actions} outputs for {int(self.policy.action_space.n)} actions")
-        return layers, params
+        return layers, layer_params(layers)
 
     def _describe_critic(self, net: nn.Module, name: str) -> tuple[list[_Layer], list[nn.Parameter]]:
         """A critic read as the actor reads the observation, one output per action."""
-        layers, params, shape, scale = describe_discrete_head_network(net, name)
+        layers, shape, scale = _head_chain(net, name)
         if (shape, scale) != (self._in_shape, self._in_scale):
             raise UnsupportedModelError(f"{name} reads the observation as shape {shape} / denominator {scale}, the actor as "
                                         f"{self._in_shape} / {self._in_scale}: the networks must read it the same way")
         if layers[-1].out_dim != self.n_actions:
             raise UnsupportedModelError(f"{name} has {layers[-1].out_dim} outputs for {self.n_actions} actions")
-        return layers, params
+        return layers, layer_params(layers)
 
     # ------------------------------------------------------------------ helpers
     def _obs_source(self, buffer: ReplayBuffer, indices: np.ndarray | torch.Tensor, key: str = "obs") -> DeviceObsSource:
@@ -169,7 +161,7 @@ class DiscreteSAC(TwinCriticAlgorithm, OffPolicyAlgorithm):
                                          gamma=self.gamma, n_step=self.n_step_return_horizon)
 
     def _sample(self, buffer: ReplayBuffer, sample_size: int | None) -> tuple[Batch, Any]:
-        return sample_discrete(buffer, sample_size, self._obs_source, self._dev)
+        return sample_discrete(buffer, sample_size, self._obs_source, self._dev, self.n_actions)
 
     # ------------------------------------------------------------------ update
     def _critic_step(self, k: int, src: DeviceObsSource, act: torch.Tensor, returns: torch.Tensor, weight: torch.Tensor | None,

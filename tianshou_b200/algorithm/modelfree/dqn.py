@@ -26,11 +26,12 @@ from torch import nn
 from ..._cabi import call, ptr, stream_ptr
 from ...data import Batch, ReplayBuffer, to_numpy
 from ..base import OffPolicyAlgorithm, Policy, TrainingStats
-from ..flat_params import DeviceScratch, FlatGroup, UnsupportedModelError, bind_optimizer
-from ..netgraph import ACT_NONE, FusedStack, compile_sequential, module_layers
-from ..obs_source import DeviceObsSource, device_obs_source
+from ..discrete_q import DiscreteQCore, describe_q_network, lagged_group
+from ..flat_params import FlatGroup, UnsupportedModelError, bind_optimizer
+from ..netgraph import ACT_NONE, FusedStack, compile_sequential, layer_params, module_layers
+from ..obs_source import DeviceObsSource
 from ..optim import OptimizerFactory
-from ..twin_critic import cuda_device_of, pop_batch_weight, sample_discrete
+from ..twin_critic import _EvalModeModule, cuda_device_of, pop_batch_weight
 
 
 @dataclass(kw_only=True)
@@ -88,23 +89,7 @@ class DiscreteQLearningPolicy(Policy):
         raise NotImplementedError(f"Currently only numpy array is supported for action, but got {type(act)}")
 
 
-def describe_q_network(model: Any) -> tuple[Any, tuple[int, ...], float]:
-    """(inner module with the layer chain, input shape, input denominator) of a Q-network: ``DQNet`` (optionally behind
-    ``ScaledObsInputActionReprNet``) or an MLP ``Net`` on flat observations."""
-    scale = 1.0          # the DENOMINATOR the observation is divided by before the network
-    inner = model
-    if hasattr(model, "denom") and hasattr(model, "module"):
-        scale = float(model.denom)
-        inner = model.module
-    if hasattr(inner, "input_shape"):
-        return inner, tuple(inner.input_shape), scale
-    first = module_layers(inner)[0]
-    if isinstance(first, nn.Linear):
-        return inner, (int(first.in_features),), scale
-    raise UnsupportedModelError(f"cannot infer the input shape of {type(inner).__name__}")
-
-
-class DQN(OffPolicyAlgorithm):
+class DQN(DiscreteQCore, OffPolicyAlgorithm):
     """DQN / double DQN with a periodically copied target network (dqn.py:286-404)."""
 
     def __init__(self, *, policy: DiscreteQLearningPolicy, optim: OptimizerFactory, gamma: float = 0.99,
@@ -118,37 +103,35 @@ class DQN(OffPolicyAlgorithm):
         self.target_update_freq = target_update_freq
         self.is_double = is_double
         self.huber_loss_delta = huber_loss_delta
-        self._iter = 0
-        dev = self._dev = cuda_device_of(policy.model)
-        inner, self._in_shape, self._in_scale = describe_q_network(policy.model)
-        layers = compile_sequential(module_layers(inner), self._in_shape)
+        dev = cuda_device_of(policy.model)
+        inner, in_shape, in_scale = describe_q_network(policy.model)
+        layers = compile_sequential(module_layers(inner), in_shape)
         if layers[-1].kind != "linear" or layers[-1].act != ACT_NONE:
             raise UnsupportedModelError("Q-network must end in a linear layer over the actions")
-        self.n_actions = layers[-1].out_dim
-        params = [p for L in layers if L.weight is not None for p in (L.weight, L.bias)]
-        self._group = FlatGroup(params, dev)
+        self._init_discrete(dev, in_shape, in_scale, layers[-1].out_dim)
+        self._group = FlatGroup(layer_params(layers), dev)
         self._net = FusedStack(layers, self._group, "q")
         self.optim = self._create_optimizer(policy, optim)
         bind_optimizer(self.optim, self._group)
-        self.model_old = deepcopy(policy.model).eval() if self.use_target_network else None
-        self._target_flat = self._group.flat.clone() if self.use_target_network else None
-        self._scratch = DeviceScratch(dev)
-        self._buf = self._scratch.tensor
+        self.model_old: _EvalModeModule | None = None
+        self._g_old: FlatGroup | None = None
+        if self.use_target_network:
+            self.model_old = _EvalModeModule(deepcopy(policy.model))
+            self._g_old = lagged_group(self._group, list(self.model_old.parameters()))
 
     @property
     def use_target_network(self) -> bool:
         return self.target_update_freq > 0
 
-    # ------------------------------------------------------------------ observations -> first-layer input
-    def _obs_source(self, buffer: ReplayBuffer, indices: np.ndarray | torch.Tensor, key: str = "obs") -> DeviceObsSource:
-        """How the network reads ``buffer[indices].<key>`` without materialising it on the host (obs_source.py)."""
-        return device_obs_source(buffer, indices, key, self._in_shape, self._in_scale, self._dev, self._buf)
-
     def _q_values(self, src: DeviceObsSource, tag: str, target: bool = False) -> tuple[list[torch.Tensor], torch.Tensor]:
-        acts = self._net.forward(src.x, src.rows, tag, frames=src.frames, params=self._target_flat if target else None)
+        params = None
+        if target:
+            self._g_old.ensure_adopted()
+            params = self._g_old.flat
+        acts = self._net.forward(src.x, src.rows, tag, frames=src.frames, params=params)
         return acts, acts[-1]
 
-    # ------------------------------------------------------------------ target / n-step
+    # ------------------------------------------------------------------ target
     def _target_q(self, buffer: ReplayBuffer, indices: np.ndarray) -> torch.Tensor:
         """Q_old(s', argmax_a Q(s', a)) (double) or max_a Q_old(s', a)   (dqn.py:365-380)."""
         src = self._obs_source(buffer, indices, "obs_next")
@@ -159,25 +142,9 @@ class DQN(OffPolicyAlgorithm):
         call("ts_dqn_target", ptr(q_online), ptr(q_tgt), B, self.n_actions, int(self.is_double), ptr(out), stream_ptr(self._dev))
         return out
 
-    def _preprocess_batch(self, batch: Batch, buffer: ReplayBuffer, indices: np.ndarray) -> Batch:
-        return self.compute_nstep_return(batch=batch, buffer=buffer, indices=indices, target_q_fn=self._target_q,
-                                         gamma=self.gamma, n_step=self.n_step)
-
-    def _sample(self, buffer: ReplayBuffer, sample_size: int | None) -> tuple[Batch, Any]:
-        return sample_discrete(buffer, sample_size, self._obs_source, self._dev)
-
     # ------------------------------------------------------------------ update
-    def _periodically_update_lagged_network_weights(self) -> None:
-        if self.use_target_network and self._iter % self.target_update_freq == 0:
-            self._group.ensure_adopted()
-            self._target_flat.copy_(self._group.flat)                       # full copy (lagged_network.py:98-103)
-            with torch.no_grad():
-                for tp, sp in zip(self.model_old.parameters(), self.policy.model.parameters(), strict=True):
-                    tp.copy_(sp)
-        self._iter += 1
-
     def _update_with_batch(self, batch: Batch) -> SimpleLossTrainingStats:
-        self._periodically_update_lagged_network_weights()
+        self._tick_lagged(self.target_update_freq)
         st = stream_ptr(self._dev)
         src = batch.obs
         B = src.rows

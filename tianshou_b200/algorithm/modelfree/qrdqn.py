@@ -17,7 +17,6 @@ only view that output as ``[B, actions, N]``, which is the kernels' row layout.
 from __future__ import annotations
 
 from copy import deepcopy
-from typing import Any
 
 import numpy as np
 import torch
@@ -26,13 +25,12 @@ from torch import nn
 from ..._cabi import call, ptr, stream_ptr
 from ...data import Batch, ReplayBuffer
 from ..base import OffPolicyAlgorithm
-from ..flat_params import DeviceScratch, FlatGroup, UnsupportedModelError, bind_optimizer
-from ..imitation.discrete_bcq import check_actions_in_range
-from ..netgraph import ACT_NONE, FusedStack, compile_sequential, module_layers
-from ..obs_source import DeviceObsSource, device_obs_source
+from ..discrete_q import DiscreteQCore, describe_q_network, lagged_group
+from ..flat_params import FlatGroup, UnsupportedModelError, bind_optimizer
+from ..netgraph import ACT_NONE, FusedStack, compile_sequential, layer_params, module_layers
 from ..optim import OptimizerFactory
-from ..twin_critic import _EvalModeModule, cuda_device_of, pop_batch_weight, sample_discrete
-from .dqn import DiscreteQLearningPolicy, SimpleLossTrainingStats, describe_q_network
+from ..twin_critic import _EvalModeModule, cuda_device_of, pop_batch_weight
+from .dqn import DiscreteQLearningPolicy, SimpleLossTrainingStats
 
 
 class QRDQNPolicy(DiscreteQLearningPolicy):
@@ -42,7 +40,7 @@ class QRDQNPolicy(DiscreteQLearningPolicy):
         return super().compute_q_value(logits.mean(2), mask)
 
 
-class QRDQN(OffPolicyAlgorithm):
+class QRDQN(DiscreteQCore, OffPolicyAlgorithm):
     """QR-DQN, reference API and semantics (qrdqn.py:26-131).
 
     ``policy.model`` is a ``Net(num_atoms=num_quantiles)`` on flat observations or a ``QRDQNet`` (optionally behind
@@ -62,21 +60,21 @@ class QRDQN(OffPolicyAlgorithm):
         self.gamma = gamma
         self.n_step = n_step_return_horizon
         self.target_update_freq = target_update_freq
-        self._iter = 0
         self.num_quantiles = num_quantiles
-        dev = self._dev = cuda_device_of(policy.model)
-        inner, self._in_shape, self._in_scale = describe_q_network(policy.model)
+        dev = cuda_device_of(policy.model)
+        inner, in_shape, in_scale = describe_q_network(policy.model)
         if getattr(inner, "softmax", False):
             raise UnsupportedModelError("Net(softmax=True): QR-DQN reads the network output as quantiles; build it with "
                                         "softmax=False")
-        layers = compile_sequential(module_layers(inner), self._in_shape)
+        layers = compile_sequential(module_layers(inner), in_shape)
         if layers[-1].kind != "linear" or layers[-1].act != ACT_NONE:
             raise UnsupportedModelError("the quantile network must end in a linear layer over actions * num_quantiles")
-        self.n_actions = int(policy.action_space.n)
-        if layers[-1].out_dim != self.n_actions * num_quantiles:
-            raise UnsupportedModelError(f"the network has {layers[-1].out_dim} outputs, not {self.n_actions} actions x "
+        n_actions = int(policy.action_space.n)
+        if layers[-1].out_dim != n_actions * num_quantiles:
+            raise UnsupportedModelError(f"the network has {layers[-1].out_dim} outputs, not {n_actions} actions x "
                                         f"{num_quantiles} quantiles")
-        self._group = FlatGroup([p for L in layers if L.weight is not None for p in (L.weight, L.bias)], dev)
+        self._init_discrete(dev, in_shape, in_scale, n_actions)
+        self._group = FlatGroup(layer_params(layers), dev)
         self._net = FusedStack(layers, self._group, "qr")
         self.optim = self._create_optimizer(policy, optim)
         bind_optimizer(self.optim, self._group)
@@ -87,25 +85,13 @@ class QRDQN(OffPolicyAlgorithm):
         self._g_old: FlatGroup | None = None
         if self.use_target_network:
             self.model_old = _EvalModeModule(deepcopy(policy.model))
-            old_inner = describe_q_network(self.model_old.module)[0]
-            old_layers = compile_sequential(module_layers(old_inner), self._in_shape)
-            self._g_old = FlatGroup([p for L in old_layers if L.weight is not None for p in (L.weight, L.bias)], dev)
-        self._scratch = DeviceScratch(dev)
-        self._buf = self._scratch.tensor
+            self._g_old = lagged_group(self._group, list(self.model_old.parameters()))
 
     @property
     def use_target_network(self) -> bool:
         return self.target_update_freq > 0
 
-    # ------------------------------------------------------------------ sampling / target
-    def _obs_source(self, buffer: ReplayBuffer, indices: np.ndarray | torch.Tensor, key: str = "obs") -> DeviceObsSource:
-        return device_obs_source(buffer, indices, key, self._in_shape, self._in_scale, self._dev, self._buf)
-
-    def _sample(self, buffer: ReplayBuffer, sample_size: int | None) -> tuple[Batch, Any]:
-        batch, indices = sample_discrete(buffer, sample_size, self._obs_source, self._dev)
-        check_actions_in_range(buffer, indices, self.n_actions)
-        return batch, indices
-
+    # ------------------------------------------------------------------ target
     def _target_q(self, buffer: ReplayBuffer, indices: np.ndarray) -> torch.Tensor:
         """The quantiles of Q_old(s', argmax_a mean_k Q(s', a, k))   (qrdqn.py:94-106)."""
         src = self._obs_source(buffer, indices, "obs_next")
@@ -120,21 +106,10 @@ class QRDQN(OffPolicyAlgorithm):
              stream_ptr(self._dev))
         return out
 
-    def _preprocess_batch(self, batch: Batch, buffer: ReplayBuffer, indices: np.ndarray) -> Batch:
-        return self.compute_nstep_return(batch=batch, buffer=buffer, indices=indices, target_q_fn=self._target_q,
-                                         gamma=self.gamma, n_step=self.n_step)
-
     # ------------------------------------------------------------------ update
-    def _periodically_update_lagged_network_weights(self) -> None:
-        if self.use_target_network and self._iter % self.target_update_freq == 0:
-            self._group.ensure_adopted()
-            self._g_old.ensure_adopted()
-            self._g_old.flat.copy_(self._group.flat)                        # full copy (lagged_network.py:98-103)
-        self._iter += 1
-
     def _quantile_step(self, batch: Batch, min_q_weight: float) -> np.ndarray:
         """One step on the quantile-Huber loss (+ ``min_q_weight`` times the CQL penalty): (loss, qr_loss, cql_loss)."""
-        self._periodically_update_lagged_network_weights()
+        self._tick_lagged(self.target_update_freq)
         src = batch.obs
         B, A, N = src.rows, self.n_actions, self.num_quantiles
         weight = pop_batch_weight(batch, self._dev)

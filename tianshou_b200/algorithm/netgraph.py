@@ -47,6 +47,11 @@ class _Layer:
     Wo: int = 0
 
 
+def layer_params(layers: list[_Layer]) -> list[nn.Parameter]:
+    """Every weight and bias of ``layers``, in layer order: the flat order of a ``FlatGroup`` over the chain."""
+    return [p for L in layers if L.weight is not None for p in (L.weight, L.bias)]
+
+
 def _activation_code(m: nn.Module) -> int:
     if type(m) is nn.ReLU:
         return ACT_RELU

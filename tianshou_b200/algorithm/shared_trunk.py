@@ -8,14 +8,14 @@ thing without a trunk: two full chains in the same flat group.
 """
 from __future__ import annotations
 
-from typing import Any, NamedTuple
+from typing import NamedTuple
 
 import torch
 from torch import nn
 
+from .discrete_q import describe_discrete_head
 from .flat_params import FlatGroup, UnsupportedModelError
-from .modelfree.dqn import describe_q_network
-from .netgraph import ACT_NONE, FusedStack, _Layer, compile_sequential, module_layers, _out_shape
+from .netgraph import ACT_NONE, FusedStack, _out_shape, compile_sequential, layer_params, module_layers
 from .obs_source import DeviceObsSource
 
 
@@ -40,24 +40,6 @@ def two_head_parameters(a: nn.Module, b: nn.Module) -> list[nn.Parameter]:
     return out
 
 
-def _parts(net: Any, role: str) -> tuple[Any, Any, tuple[int, ...], float]:
-    pre, last = getattr(net, "preprocess", None), getattr(net, "last", None)
-    if pre is None or last is None:
-        raise UnsupportedModelError(f"{role}: expected a DiscreteActor / DiscreteCritic (preprocess net + last MLP), got "
-                                    f"{type(net).__name__}")
-    try:
-        inner, shape, scale = describe_q_network(pre)
-    except UnsupportedModelError as e:
-        raise UnsupportedModelError(f"{role}: {e}") from e
-    if getattr(pre, "softmax", False) or getattr(inner, "softmax", False):
-        raise UnsupportedModelError(f"{role}: a softmax preprocess output is not supported")
-    return inner, last, shape, scale
-
-
-def _layer_params(layers: list[_Layer]) -> list[nn.Parameter]:
-    return [p for L in layers if L.weight is not None for p in (L.weight, L.bias)]
-
-
 class TwoHeadNetwork:
     """Heads ``a`` and ``b`` (each ``preprocess`` + ``last``) in one ``FlatGroup`` built over ``two_head_parameters(a, b)``.
     ``shared``: both hold the same preprocess parameters, so the trunk is compiled and evaluated once."""
@@ -65,8 +47,8 @@ class TwoHeadNetwork:
     def __init__(self, a: nn.Module, b: nn.Module, group: FlatGroup, roles: tuple[str, str] = ("a", "b")) -> None:
         self.group = group
         self.device = group.device
-        pre_a, last_a, shape, scale = _parts(a, roles[0])
-        pre_b, last_b, shape_b, scale_b = _parts(b, roles[1])
+        pre_a, last_a, shape, scale = describe_discrete_head(a, roles[0])
+        pre_b, last_b, shape_b, scale_b = describe_discrete_head(b, roles[1])
         ids_a, ids_b = {id(p) for p in a.preprocess.parameters()}, {id(p) for p in b.preprocess.parameters()}
         own_a, own_b = {id(p) for p in a.parameters()}, {id(p) for p in b.parameters()}
         self.shared = bool(ids_a) and ids_a == ids_b
@@ -95,7 +77,7 @@ class TwoHeadNetwork:
                 raise UnsupportedModelError(f"{role}: must end in a linear layer (with a bias, without activation) over its outputs")
             if chain[0].kind != "linear" and self.shared:
                 raise UnsupportedModelError(f"{role}: the head on a shared trunk must start with a linear layer")
-        covered = {id(p) for p in _layer_params(trunk + chains[0] + chains[1])}
+        covered = {id(p) for p in layer_params(trunk + chains[0] + chains[1])}
         if covered != {id(p) for p in group.params}:
             raise UnsupportedModelError("the flat group's parameters differ from the parameters of the compiled layers")
         self.n_out = (chains[0][-1].out_dim, chains[1][-1].out_dim)

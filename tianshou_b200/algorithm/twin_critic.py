@@ -1,6 +1,7 @@
 """What the twin-critic algorithms (SAC, discrete SAC, CQL, TD3, TD3+BC, BCQ) share: one actor (with an optional lagged copy) and
 two (critic, lagged critic) pairs as flat groups on one CUDA device, their three optimisers, the scratch, the one Adam seam,
-the lagged forwards and Polyak; plus the sampling helpers the off-policy algorithms share with DQN.
+the lagged forwards and Polyak; plus the importance weight of a prioritised sample, the ``batch.weight`` coercion and the
+reference's ``.module`` wrapper of a lagged network, which the discrete Q-learning core (discrete_q.py) uses too.
 
 Reference: modelfree/td3.py:40-92 (dual critics, ``critic2=None`` deep-copies the critic), :183 (TD3's lagged actor),
 utils/lagged_network.py:8-80 (Polyak, the lagged copy under ``.module``), data/buffer/prio.py:104-106 (the importance weight of
@@ -20,7 +21,6 @@ from ..data import Batch, ReplayBuffer
 from .base import Algorithm
 from .flat_params import DeviceScratch, FlatGroup, UnsupportedModelError, bind_optimizer
 from .netgraph import FusedStack, _Layer, polyak_update
-from .obs_source import DeviceObsSource
 from .optim import OptimizerFactory
 
 Describe = Callable[..., tuple[list[_Layer], list[nn.Parameter]]]
@@ -52,23 +52,6 @@ def pop_batch_weight(batch: Batch, device: torch.device) -> torch.Tensor | None:
     if not isinstance(weight, torch.Tensor):
         weight = to_device(np.asarray(weight, dtype=np.float32), device)
     return weight.reshape(-1).to(device, torch.float32).contiguous()
-
-
-def sample_discrete(buffer: ReplayBuffer, sample_size: int | None, obs_source: Callable[..., DeviceObsSource],
-                    device: torch.device) -> tuple[Batch, Any]:
-    """Indices from the buffer's host RNG streams (identical to the reference's draws); the observations as
-    ``obs_source(buffer, indices, "obs")`` reads them on the device, the actions as int64 device rows, the importance weight
-    of a prioritised buffer."""
-    indices = buffer.sample_indices(sample_size)
-    batch = Batch()
-    batch.__dict__["obs"] = obs_source(buffer, indices, "obs")
-    act = np.asarray(buffer.act)[indices]
-    batch.__dict__["act"] = to_device(np.ascontiguousarray(act.reshape(-1)).astype(np.int64), device)
-    weight = per_weight(buffer, indices, device)
-    if weight is not None:
-        batch.__dict__["weight"] = weight
-    batch.__dict__["info"] = Batch()
-    return batch, indices
 
 
 class _EvalModeModule(nn.Module):
