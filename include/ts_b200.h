@@ -164,7 +164,13 @@ int ts_segtree_prefix_sum_idx(const double* tree, int64_t bound, const double* v
 int ts_segtree_sample(const double* tree, int64_t bound, const double* u, int64_t n, int64_t* out,
                       ts_stream_t stream);
 /* PrioritizedReplayBuffer.update_weight (prio.py:81-90): w = |td|+eps; tree[idx] = w^alpha;
- * prio_minmax (device double[2] = {max_prio, min_prio}) updated with max/min of w. */
+ * prio_minmax (device double[2] = {max_prio, min_prio}) updated with max/min of every w, duplicates
+ * included (the tree keeps the last duplicate's w^alpha).  The arithmetic follows numpy's dtypes:
+ * TS_F32 td: w = fl32(|td| + fl32(eps)), leaf = (double)powf(w, (float)alpha), minmax with (double)w;
+ * TS_F64 td: w, w^alpha and minmax in double.  Device powf / pow are not correctly rounded (CUDA
+ * documents 4 / 2 ulp), so leaves can differ from numpy's in the last bits and so can sampled
+ * indices: for bit-exact indices compute w^alpha with the host pow (as data/buffer/prio.py does)
+ * and write it with ts_segtree_setitem. */
 int ts_prio_update_weight(double* tree, int64_t bound, const int64_t* index, const void* td,
                           int td_dtype, int64_t n, double alpha, double eps, double* prio_minmax,
                           ts_stream_t stream);

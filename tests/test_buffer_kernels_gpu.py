@@ -9,7 +9,9 @@ Bars:
   on the longest composition chain (in-thread, warp, CTA and the look-back over every tile to the right); f32 outputs
   add one rounding;
 - bit-identical between the 128-bit and the scalar GAE path, between calls that reuse one workspace, and between the
-  minibatch and epoch advantage sums.
+  minibatch and epoch advantage sums;
+- the prioritized-replay kernels against numpy's expressions in the TD errors' dtype: the running min / max and the
+  tree's parents bit-exact, every power within the documented error of CUDA's powf / pow plus the host's.
 """
 import math
 import warnings
@@ -515,6 +517,126 @@ def test_segtree_prefix_queries_ties_and_edges(size):
     u = np.concatenate([[0.0, np.nextafter(1.0, 0.0)], rng.random(4096)])
     got = tree.sample_device(on_dev(u)).cpu().numpy()
     assert np.array_equal(got, onp.segtree_prefix_sum_idx(ref, tree.bound, u * total))
+
+
+# ------------------------------------------------------------------------------------------ prioritized replay
+# The CUDA C++ Programming Guide (appendix "Mathematical Functions") documents a maximum error of 4 ulp for powf and of
+# 2 ulp for pow over their full range; numpy's float32 / float64 power calls the host libm, which is within 1 ulp.  So a
+# device power lies within 5 (float32) or 3 (float64) ulp of numpy's, and one ulp of x is at most eps(type) * |x|.
+POW_ULP = {"f32": 4 + 1, "f64": 2 + 1}
+EPS = {"f32": 2.0 ** -23, "f64": 2.0 ** -52}
+PRIO_EPS = np.finfo(np.float32).eps.item()          # prio.py: self._eps, a Python float
+
+
+def prio_update(tree, minmax, idx, td, alpha, eps=PRIO_EPS):
+    c = _cabi()
+    dt = c.TS_F32 if td.dtype == np.float32 else c.TS_F64
+    d_idx, d_td = on_dev(idx), on_dev(td)       # held: a freed temporary's block would be handed to the next one
+    call("ts_prio_update_weight", ptr(tree.tree), tree.bound, ptr(d_idx), ptr(d_td), dt, len(idx), alpha, eps,
+         ptr(minmax), stream())
+
+
+def prio_update_reference(td, alpha, eps=PRIO_EPS):
+    """The reference's own expressions (prio.py update_weight): numpy keeps a float32 array combined with a Python float in
+    float32, so w and w ** alpha are float32 for float32 TD errors."""
+    w = np.abs(td) + eps
+    leaf = w ** alpha
+    assert w.dtype == leaf.dtype == td.dtype
+    return w, leaf
+
+
+@pytest.mark.parametrize("tdt", ["f32", "f64"])
+@pytest.mark.parametrize("n", [1, 1000, 1025, 32768])
+def test_prio_update_weight_matches_numpy_expressions(n, tdt):
+    """``ts_prio_update_weight`` against numpy's ``|td| + eps`` and ``w ** alpha`` in the TD errors' own dtype, twice on one
+    tree.  Each batch draws its indices from a small pool (duplicates everywhere) and starts with two items that lose to a
+    later duplicate of their index: one carries the batch's largest w, the other the smallest (td = 0).  ``prio_minmax`` is
+    bit-exact (the losers count, as ``weight.max()`` / ``min()`` see every item); each leaf holds the last duplicate's value
+    within POW_ULP; float32 leaves are float32 numbers; untouched leaves keep their bits; every parent is exactly
+    ``left + right`` of the device's own children."""
+    rng = np.random.default_rng(n + (0 if tdt == "f32" else 7))
+    size = 5000
+    tree, _ = make_tree(size)
+    bound = tree.bound
+    init = rng.random(size)
+    ops().segtree_setitem(tree.tree, bound, on_dev(np.arange(size, dtype=np.int64)), on_dev(init))
+    minmax = torch.tensor([1.0, 1.0], dtype=torch.float64, device=DEV)
+    ref_max, ref_min = 1.0, 1.0
+    alpha = 0.6
+    pool = rng.choice(size, max(1, min(size, n // 3)), replace=False)
+    for call_no in range(2):
+        idx = pool[rng.integers(0, len(pool), n)].astype(np.int64)
+        td = (rng.standard_normal(n) * (3.0 if call_no else 0.2)).astype(NDT[tdt])
+        td[rng.random(n) < 0.05] = 0
+        if n >= 3:
+            idx[0] = idx[1] = idx[-1]
+            td[0] = NDT[tdt](50.0 + call_no)
+            td[1] = 0
+        before = tree.tree.cpu().numpy()
+        prio_update(tree, minmax, idx, td, alpha)
+        got = tree.tree.cpu().numpy()
+        w, leaf = prio_update_reference(td, alpha)
+        ref_max, ref_min = max(ref_max, w.max()), min(ref_min, w.min())           # prio.py: max(self._max_prio, weight.max())
+        mm = minmax.cpu().numpy()
+        assert mm[0] == float(ref_max) and mm[1] == float(ref_min), (call_no, mm, ref_max, ref_min)
+        last = {}
+        for k, i in enumerate(idx):
+            last[int(i)] = k                      # last write wins
+        slots = np.array(sorted(last), dtype=np.int64)
+        winners = np.array([last[int(i)] for i in slots])
+        g_leaf = got[bound + slots]
+        r_leaf = leaf[winners].astype(np.float64)
+        tol = POW_ULP[tdt] * EPS[tdt] * np.abs(r_leaf)
+        assert_within(f"ts_prio_update_weight {tdt} leaves vs numpy w ** alpha", g_leaf, r_leaf, tol)
+        if tdt == "f32":
+            assert np.array_equal(g_leaf, g_leaf.astype(np.float32).astype(np.float64)), "f32 leaves must be float32 numbers"
+        if n >= 3:                                # the losers' values are 50 ** 0.6 and eps ** 0.6, far from the winner's
+            assert abs(got[bound + idx[-1]] - leaf[-1]) <= POW_ULP[tdt] * EPS[tdt] * abs(float(leaf[-1]))
+        untouched = np.ones(bound, dtype=bool)
+        untouched[slots] = False
+        assert np.array_equal(got[bound:][untouched], before[bound:][untouched])
+        parents = np.arange(1, bound)
+        assert np.array_equal(got[parents], got[2 * parents] + got[2 * parents + 1])
+
+
+def test_prio_update_weight_batch_limit():
+    """One CTA resolves duplicates with a 32-bit win mask per thread: 32 x 1024 items per call, more are refused."""
+    tree, _ = make_tree(100)
+    minmax = torch.tensor([1.0, 1.0], dtype=torch.float64, device=DEV)
+    idx = np.zeros(32 * 1024 + 1, dtype=np.int64)
+    with pytest.raises(RuntimeError, match="at most 32768 items"):
+        prio_update(tree, minmax, idx, np.ones(len(idx), dtype=np.float32), 0.6)
+
+
+@pytest.mark.parametrize("weight_norm", [0, 1], ids=["raw", "weight_norm"])
+@pytest.mark.parametrize("n", [1, 1000, 1025, 5000])
+def test_prio_get_weight_matches_numpy_expressions(n, weight_norm):
+    """``ts_prio_get_weight`` against ``(weight[index] / min_prio) ** (-beta)`` and ``weight / weight.max()`` in float64.  The
+    quotient is one correctly rounded division on both sides, so the power's error is all there is: POW_ULP of the result;
+    dividing by the batch maximum (itself a power) doubles that and adds one rounding on each side.  With weight_norm the batch's largest entry is exactly 1.
+    n > 1024 makes the kernel's single block loop."""
+    rng = np.random.default_rng(n + 10 * weight_norm)
+    size = 3000
+    tree, _ = make_tree(size)
+    leaves = rng.uniform(1e-4, 3.0, size) ** 0.6
+    ops().segtree_setitem(tree.tree, tree.bound, on_dev(np.arange(size, dtype=np.int64)), on_dev(leaves))
+    min_prio = float(np.float32(1.2e-4))
+    minmax = torch.tensor([3.0, min_prio], dtype=torch.float64, device=DEV)
+    for beta in (0.4, 1.0, 0.0):
+        idx = rng.integers(0, size, n).astype(np.int64)
+        out = torch.full((n,), float("nan"), dtype=torch.float64, device=DEV)
+        d_idx = on_dev(idx)
+        call("ts_prio_get_weight", ptr(tree.tree), tree.bound, ptr(d_idx), n, ptr(minmax), beta, weight_norm, ptr(out),
+             stream())
+        got = out.cpu().numpy()
+        ref = (leaves[idx] / min_prio) ** (-beta)
+        if weight_norm:
+            ref = ref / np.max(ref)
+            assert got.max() == 1.0
+        tol = (2 * POW_ULP["f64"] + 1 if weight_norm else POW_ULP["f64"]) * EPS["f64"] * np.abs(ref)
+        assert_within(f"ts_prio_get_weight beta {beta} weight_norm {weight_norm}", got, ref, tol)
+        if beta == 0.0:
+            assert np.all(got == 1.0)
 
 
 # ------------------------------------------------------------------------------------------------- row movement

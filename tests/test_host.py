@@ -193,6 +193,60 @@ def test_cabi_header_parser_refuses_what_it_cannot_bind():
         parse_header("int ts_ok(void);\nint ts_callback(void (*fn)(int), ts_stream_t s);\n")
 
 
+# Exported functions that the suite reaches only through a Python wrapper, and the test that does: (file, test name).
+ABI_REACHED_THROUGH = {
+    "ts_npg_fvp_rows": ("test_npg_gpu.py", "test_fvp_vs_fp64_double_backward"),            # NPG._fvp
+    "ts_segtree_setitem": ("test_buffer_kernels_gpu.py", "test_segtree_setitem_batches_with_duplicates"),
+    "ts_segtree_reduce": ("test_buffer_kernels_gpu.py", "test_segtree_reduce_ranges"),
+    "ts_segtree_prefix_sum_idx": ("test_buffer_kernels_gpu.py", "test_segtree_prefix_queries_ties_and_edges"),
+    "ts_segtree_sample": ("test_kernels_gpu.py", "test_segtree_vs_reference_outputs"),    # SegmentTree.sample_device
+    "ts_gather_rows": ("test_buffer_kernels_gpu.py", "test_gather_scatter_rows_alignment"),
+    "ts_mark_members": ("test_buffer_kernels_gpu.py", "test_mark_members_edges"),
+    "ts_narrow_i64_i32": ("test_buffer_kernels_gpu.py", "test_narrow_i64_i32_near_int32_limits"),
+    "ts_next_index": ("test_buffer_kernels_gpu.py", "test_index_kernels_unequal_subbuffers"),
+    "ts_prev_index": ("test_buffer_kernels_gpu.py", "test_index_kernels_unequal_subbuffers"),
+    "ts_unfinished_index": ("test_buffer_kernels_gpu.py", "test_index_kernels_unequal_subbuffers"),
+    "ts_stack_next_indices": ("test_buffer_kernels_gpu.py", "test_index_kernels_unequal_subbuffers"),
+    "ts_nstep_return": ("test_buffer_kernels_gpu.py", "test_nstep_end_flag_at_every_window_position"),
+    "ts_value_mask_rows": ("test_buffer_kernels_gpu.py", "test_value_mask_rows_special_values"),
+    "ts_host_mt19937_permutation": ("test_host.py", "test_host_permutation_is_numpy_global_permutation_bit_for_bit"),
+    "ts_host_perm_job_start": ("test_host.py", "test_permutation_job_matches_numpy_stream"),
+    "ts_host_perm_job_wait": ("test_host.py", "test_permutation_job_matches_numpy_stream"),
+    "ts_host_perm_job_finish": ("test_host.py", "test_permutation_job_matches_numpy_stream"),
+    "ts_host_perm_feed_start": ("test_minibatch_order_gpu.py", "test_rows_and_numpy_state_per_source"),
+    "ts_host_perm_feed_wait_row": ("test_minibatch_order_gpu.py", "test_rows_and_numpy_state_per_source"),
+    "ts_host_perm_feed_finish": ("test_minibatch_order_gpu.py", "test_rows_and_numpy_state_per_source"),
+}
+# Exported functions that compute nothing a reference could check, with the reason.
+ABI_PLUMBING = {
+    "ts_launch_count": "a counter of kernel launches, read by _cabi.launch_count for the launch-budget tests",
+    "ts_next_alias_workspace_bytes": "a workspace size for the caller's allocation",
+    "ts_ppo_partial_rows": "the row count of the PPO gradient-partials workspace",
+    "ts_ppo_weight_image_bytes": "a workspace size for the caller's allocation",
+    "ts_ppo_peer_buffer_bytes": "the size of the peer-exchange buffer of multi-GPU PPO",
+    "ts_peer_alloc": "IPC buffer lifecycle of multi-GPU PPO, driven by parallel.py in the two-rank tests",
+    "ts_peer_close": "IPC buffer lifecycle of multi-GPU PPO, driven by parallel.py in the two-rank tests",
+    "ts_peer_free": "IPC buffer lifecycle of multi-GPU PPO, driven by parallel.py in the two-rank tests",
+}
+
+
+def test_every_exported_function_is_tested():
+    """Every function of the C ABI is named in some test, reached by a named test through a wrapper, or is plumbing that
+    computes nothing checkable.  A new export without a test fails here; so does a stale entry in either table."""
+    from tianshou_b200._cabi import ABI
+    here = os.path.dirname(os.path.abspath(__file__))
+    sources = {f: open(os.path.join(here, f)).read() for f in sorted(os.listdir(here)) if f.endswith(".py")}
+    text = "\n".join(sources.values())
+    exported = set(ABI.functions)
+    assert set(ABI_REACHED_THROUGH) <= exported and set(ABI_PLUMBING) <= exported
+    assert not set(ABI_REACHED_THROUGH) & set(ABI_PLUMBING)
+    for name, (f, test) in ABI_REACHED_THROUGH.items():
+        assert re.search(rf"^def {test}\(", sources.get(f, ""), flags=re.M), f"{name}: {f}::{test} does not exist"
+    tables = set(ABI_REACHED_THROUGH) | set(ABI_PLUMBING)
+    untested = sorted(n for n in exported - tables if not re.search(rf"\b{n}\b", text))
+    assert not untested, f"exported but called by no test: {untested}"
+
+
 def test_host_permutation_is_numpy_global_permutation_bit_for_bit():
     """The product path's minibatch order == np.random.permutation on the global stream (batch.py:1209),
     including the RNG state it leaves behind."""

@@ -13,6 +13,8 @@
 // update, #envs per add) over a 2^20..2^22-leaf tree, so the work is latency- not bandwidth-bound.
 // The prefix-sum descent is one thread per query: log2(bound) dependent 8-byte loads; the top
 // ~15 levels of the tree stay L2-resident.
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace {
@@ -51,10 +53,19 @@ __global__ void __launch_bounds__(kSetThreads) setitem_kernel(
         for (int64_t k = tid; k < n; k += kSetThreads, ++j) {
             double v = (double)value[k];
             if (prio_mode) {          // prio.py:82-85: w = |td| + eps ; tree = w ** alpha
-                v = fabs(v) + eps;
-                lmax = fmax(lmax, v);
-                lmin = fmin(lmin, v);
-                v = pow(v, alpha);
+                if constexpr (std::is_same_v<TV, float>) {
+                    // numpy keeps a float32 array combined with a Python float in float32: eps and alpha are
+                    // rounded to float32, |td| + eps and the power are float32 operations, the tree widens after
+                    const float w = fabsf(value[k]) + (float)eps;
+                    lmax = fmax(lmax, (double)w);
+                    lmin = fmin(lmin, (double)w);
+                    v = (double)powf(w, (float)alpha);
+                } else {
+                    v = fabs(v) + eps;
+                    lmax = fmax(lmax, v);
+                    lmin = fmin(lmin, v);
+                    v = pow(v, alpha);
+                }
             }
             if ((win_mask >> j) & 1u) tree[bound + index[k]] = v;
         }
