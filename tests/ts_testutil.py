@@ -178,13 +178,15 @@ def ac_named_params(actor, critic) -> dict:
     return d
 
 
-def actor_critic_reference_fp64(actor, critic, mb: dict, hp: dict) -> dict:
+def actor_critic_reference_fp64(actor, critic, mb: dict, hp: dict, group_order: bool = False) -> dict:
     """``ppo_reference_fp64`` for the whole fused family: Tanh or ReLU trunks, a shared trunk (actor and critic copied
     together, so autograd adds both losses' gradients into the same leaves) and the categorical head as
     ``Categorical(probs=softmax(z))`` computes it -- renormalise, clamp with the FLOAT32 eps the reference's fp32 run
     uses (torch's own ``clamp_probs`` would take the float64 eps here), log.  Runs the modules' own Linear layers in
     float64 on CPU.  Returns v, mu (Gaussian: the mean; categorical: softmax(z) before renormalisation), pn (categorical:
-    the renormalised probabilities), logp, the loss parts and ``grads`` keyed like ``ac_named_params``."""
+    the renormalised probabilities), logp, the loss parts and ``grads`` keyed like ``ac_named_params``, or with
+    ``group_order`` (networks of any depth) one flat float64 vector in ``ActorCritic(actor, critic).parameters()`` order,
+    a shared trunk once -- the layout of the layer-wise path's ``FlatGroup``."""
     import copy
 
     import torch
@@ -231,7 +233,11 @@ def actor_critic_reference_fp64(actor, critic, mb: dict, hp: dict) -> dict:
     ent = ent.mean()
     loss = clip_loss + hp["vf_coef"] * vf_loss - hp["ent_coef"] * ent
     loss.backward()
-    grads = {k: p.grad.numpy().copy() for k, p in ac_named_params(a, c).items()}
+    if group_order:
+        from tianshou_b200.utils.net.common import ActorCritic
+        grads = np.concatenate([p.grad.numpy().reshape(-1) for p in ActorCritic(a, c).parameters()])
+    else:
+        grads = {k: p.grad.numpy().copy() for k, p in ac_named_params(a, c).items()}
     d = lambda x: None if x is None else x.detach().numpy().copy()
     return dict(v=d(value), mu=d(mu), pn=d(pn), logp=d(logp), loss=loss.item(), clip=clip_loss.item(), vf=vf_loss.item(),
                 ent=ent.item(), grads=grads)
