@@ -754,6 +754,38 @@ int ts_qrdqn_target(const float* q_online, const float* q_next, int64_t B, int32
 int ts_qrdqn_rows(const float* q, const int64_t* act, const float* returns, const float* tau_hat, const float* weight, int64_t B,
                   int32_t A, int32_t N, float min_q_weight, float* dq, float* prio, float* rows, float* losses, ts_stream_t stream);
 
+/* ---- IQN (iqn.cu) ---- */
+/* The network of IQN (utils/net/discrete.py:163-216) is a trunk on B rows (feat [B][D]), the cosine embedding of S fractions per
+ * row and a head on the B * S rows h[b * S + s] = feat[b] * e[b * S + s], sample-major, so the head's output is q [B][S][A].  The
+ * GEMMs (the embedding's Linear(C, D) + ReLU included) are ts_net_gemm launches; these are the pieces between them.
+ * ts_iqn_cos: out [R][C] = cos(taus[r] * (fl32(pi) * (c + 1))) with both products rounded in fp32, bit for bit the argument the
+ * reference's CosineEmbeddingNetwork forms (discrete.py:144-160: np.pi times an fp32 arange, times the fractions), and cosf at
+ * full accuracy.  Any R >= 0, C >= 1. */
+int ts_iqn_cos(const float* taus, int64_t R, int32_t C, float* out, ts_stream_t stream);
+/* ts_iqn_mix: h [B * S][D] = feat [B][D] (row b repeated over its S samples) * e [B * S][D]   (discrete.py:211-214). */
+int ts_iqn_mix(const float* feat, const float* e, int64_t B, int32_t S, int32_t D, float* h, ts_stream_t stream);
+/* ts_iqn_mix_backward: from dh [B * S][D] = d loss / d h, dfeat [B][D] = (sum_s dh[b * S + s] * e[b * S + s], s in order) times the
+ * derivative of the trunk's last activation trunk_act (TS_ACT_NONE / RELU / TANH, at its output trunk_out [B][D], the rule of
+ * ts_net_gemm's mask; nullable with TS_ACT_NONE), and de_pre [B * S][D] = dh * feat[b] * 1[e > 0], the gradient at the embedding's
+ * pre-activation (e is its ReLU output).  Bit-identical from run to run. */
+int ts_iqn_mix_backward(const float* dh, const float* feat, const float* e, int64_t B, int32_t S, int32_t D, int32_t trunk_act,
+                        const float* trunk_out, float* dfeat, float* de_pre, ts_stream_t stream);
+/* IQN's target distribution (modelfree/qrdqn.py:94-106 through IQNPolicy, iqn.py:72-100): q_online [B][S_on][A] and q_next
+ * [B][S_next][A] at s_{t+n} (q_next the lagged network's output on its own fractions, or q_online itself); per row b,
+ * m_a = mean_s q_online[b][s][a] in fp32, a* = argmax_a m_a with torch.argmax's rule (lowest index among ties, a NaN is the
+ * maximum), out [B][S_next] = q_next[b][.][a*]; act_out [B] (nullable) = a*.  One warp per row, any A, S_on, S_next >= 1, B. */
+int ts_iqn_target(const float* q_online, const float* q_next, int64_t B, int32_t A, int32_t S_on, int32_t S_next, float* out,
+                  int64_t* act_out, ts_stream_t stream);
+/* The quantile-Huber loss of IQN (iqn.py:156-183) on q [B][S_on][A] at s, the fractions taus [B][S_on] of that forward, the n-step
+ * returns [B][S_t] and the importance weight [B] (nullable: 1).  With c_i = q[b][i][act[b]], u_ij = returns[b][j] - c_i,
+ * h_ij = smooth_l1(u_ij) (beta 1): qr_b = (1/S_on) sum_i sum_j h_ij |taus[b][i] - 1[u_ij <= 0]|, prio [B] = (1/S_on) sum_i sum_j
+ * h_ij; losses[4] = (loss, loss, 0, mean_b prio) with loss = mean_b(weight_b qr_b).  dq [B][S_on][A] = d loss / d q, every element
+ * written (the indicator detached, as in the reference).  act must lie in [0, A): the caller checks it.  rows [3][B] is scratch.
+ * One block per row (threads over the current quantiles, the row's targets in shared memory), then one block summing the rows in
+ * a fixed order: two calls on the same input are bit-identical.  Any B, A, S_on >= 1 and S_t <= 12288; larger S_t is refused. */
+int ts_iqn_rows(const float* q, const int64_t* act, const float* returns, const float* taus, const float* weight, int64_t B,
+                int32_t A, int32_t S_on, int32_t S_t, float* dq, float* prio, float* rows, float* losses, ts_stream_t stream);
+
 #ifdef TS_B200_DIAGNOSTICS
 /* Diagnostics build only (libts_b200_diag.so, `python -m tianshou_b200.csrc.build --diag`): not part of the product library. */
 /* Hardware self-test of the wgmma building blocks (csrc/wgmma.cuh), one CTA:

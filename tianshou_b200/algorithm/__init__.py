@@ -5,6 +5,7 @@ from .imitation import (BCQ, CQL, GAIL, TD3BC, BCQPolicy, BCQTrainingStats, CQLT
                         GailTrainingStats)
 from .modelfree.a2c import A2CTrainingStats, ActorCriticOnPolicyAlgorithm
 from .modelfree.discrete_sac import DiscreteSAC
+from .modelfree.iqn import IQN, IQNPolicy
 from .modelfree.npg import NPG, NPGTrainingStats
 from .modelfree.ppo import A2C, PPO
 from .modelfree.qrdqn import QRDQN, QRDQNPolicy
@@ -19,5 +20,5 @@ __all__ = [
     "GAIL", "GailTrainingStats", "DiscreteSAC", "BCQ", "BCQPolicy", "BCQTrainingStats", "CQL", "CQLTrainingStats", "TD3", "TD3TrainingStats", "TD3BC",
     "ProbabilisticActorPolicy", "DiscreteActorPolicy", "AdamOptimizerFactory", "LRSchedulerFactoryLinear", "OptimizerFactory",
     "RMSpropOptimizerFactory", "DiscreteBCQ", "DiscreteBCQPolicy", "DiscreteBCQTrainingStats", "DiscreteCRR",
-    "DiscreteCRRTrainingStats", "QRDQN", "QRDQNPolicy", "DiscreteCQL", "DiscreteCQLTrainingStats",
+    "DiscreteCRRTrainingStats", "QRDQN", "QRDQNPolicy", "DiscreteCQL", "DiscreteCQLTrainingStats", "IQN", "IQNPolicy",
 ]

@@ -62,20 +62,7 @@ class QRDQN(DiscreteQCore, OffPolicyAlgorithm):
         self.target_update_freq = target_update_freq
         self.num_quantiles = num_quantiles
         dev = cuda_device_of(policy.model)
-        inner, in_shape, in_scale = describe_q_network(policy.model)
-        if getattr(inner, "softmax", False):
-            raise UnsupportedModelError("Net(softmax=True): QR-DQN reads the network output as quantiles; build it with "
-                                        "softmax=False")
-        layers = compile_sequential(module_layers(inner), in_shape)
-        if layers[-1].kind != "linear" or layers[-1].act != ACT_NONE:
-            raise UnsupportedModelError("the quantile network must end in a linear layer over actions * num_quantiles")
-        n_actions = int(policy.action_space.n)
-        if layers[-1].out_dim != n_actions * num_quantiles:
-            raise UnsupportedModelError(f"the network has {layers[-1].out_dim} outputs, not {n_actions} actions x "
-                                        f"{num_quantiles} quantiles")
-        self._init_discrete(dev, in_shape, in_scale, n_actions)
-        self._group = FlatGroup(layer_params(layers), dev)
-        self._net = FusedStack(layers, self._group, "qr")
+        self._build_network(policy, dev)
         self.optim = self._create_optimizer(policy, optim)
         bind_optimizer(self.optim, self._group)
         # the midpoints exactly as the reference forms them in fp32 on the CPU (not (k + 0.5) / N, which differs in the last bit)
@@ -86,6 +73,24 @@ class QRDQN(DiscreteQCore, OffPolicyAlgorithm):
         if self.use_target_network:
             self.model_old = _EvalModeModule(deepcopy(policy.model))
             self._g_old = lagged_group(self._group, list(self.model_old.parameters()))
+
+    def _build_network(self, policy: QRDQNPolicy, dev: torch.device) -> None:
+        """Read ``policy.model`` as a plain layer chain ending in ``Linear(., actions * num_quantiles)``, refuse anything else,
+        and set up the core (``_init_discrete``), the flat group over the model's parameters and the device network."""
+        inner, in_shape, in_scale = describe_q_network(policy.model)
+        if getattr(inner, "softmax", False):
+            raise UnsupportedModelError("Net(softmax=True): QR-DQN reads the network output as quantiles; build it with "
+                                        "softmax=False")
+        layers = compile_sequential(module_layers(inner), in_shape)
+        if layers[-1].kind != "linear" or layers[-1].act != ACT_NONE:
+            raise UnsupportedModelError("the quantile network must end in a linear layer over actions * num_quantiles")
+        n_actions = int(policy.action_space.n)
+        if layers[-1].out_dim != n_actions * self.num_quantiles:
+            raise UnsupportedModelError(f"the network has {layers[-1].out_dim} outputs, not {n_actions} actions x "
+                                        f"{self.num_quantiles} quantiles")
+        self._init_discrete(dev, in_shape, in_scale, n_actions)
+        self._group = FlatGroup(layer_params(layers), dev)
+        self._net = FusedStack(layers, self._group, "qr")
 
     @property
     def use_target_network(self) -> bool:

@@ -7,20 +7,14 @@
 #include <math.h>
 
 #include "common.cuh"
+#include "quantile.cuh"
 #include "row_sums.cuh"
 
 namespace {
 
+using tsb::argmax_before;
 using tsb::kRowsPerBlock;
 using tsb::kRowThreads;
-
-// torch.argmax's order on (value, index): a NaN is the maximum, ties go to the lowest index
-__device__ __forceinline__ bool argmax_before(float v, int i, float bv, int bi) {
-    if (bi < 0) return true;
-    const bool vn = isnan(v), bn = isnan(bv);
-    if (vn || bn) return vn && (!bn || i < bi);
-    return v > bv || (v == bv && i < bi);
-}
 
 // Per row b: mask_a = (logits[b][a] - max_a logits[b]) < log_tau, a* = first argmax_a (q_online[b][a] - FLT_MAX * mask_a) in fp32
 // as torch evaluates it, out[b] = q_old[b][a*].  The arg-max-logit action is never masked (log_tau < 0), so a* always exists.

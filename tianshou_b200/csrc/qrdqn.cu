@@ -9,32 +9,18 @@
 #include <math.h>
 
 #include "common.cuh"
+#include "quantile.cuh"
 #include "row_sums.cuh"
 
 namespace {
 
+using tsb::argmax_before;
 using tsb::kRowsPerBlock;
 using tsb::kRowThreads;
 
 constexpr int kQrThreads = 256;
 constexpr int kQrWarps = kQrThreads / 32;
 constexpr int kQrSmemFloats = 48 * 1024 / 4;     // the default dynamic shared-memory limit: N targets, N taus, A means
-
-// torch.argmax's order on (value, index): a NaN is the maximum, ties go to the lowest index (as in discrete_bcq.cu)
-__device__ __forceinline__ bool argmax_before(float v, int i, float bv, int bi) {
-    if (bi < 0) return true;
-    const bool vn = isnan(v), bn = isnan(bv);
-    if (vn || bn) return vn && (!bn || i < bi);
-    return v > bv || (v == bv && i < bi);
-}
-
-// mean of x[0 .. N) over one warp: every lane adds its stride in order, then the butterfly; every lane returns the same value,
-// and two equal rows give equal means
-__device__ __forceinline__ float quantile_mean(const float* __restrict__ x, int N, int lane) {
-    float s = 0.0f;
-    for (int k = lane; k < N; k += 32) s += x[k];
-    return tsb::warp_sum(s) / (float)N;
-}
 
 // Per row b: m_a = mean_k q_online[b][a][k], a* = the first arg-max of m (NaN the maximum), out[b][k] = q_next[b][a*][k].
 // One warp per row.
@@ -47,25 +33,13 @@ __global__ void __launch_bounds__(kRowThreads) qrdqn_target_kernel(const float* 
         float bv = 0.0f;
         int bi = -1;
         for (int a = 0; a < A; ++a) {
-            const float m = quantile_mean(q_online + b * AN + (int64_t)a * N, N, lane);
+            const float m = tsb::quantile_mean(q_online + b * AN + (int64_t)a * N, N, 1, lane);
             if (argmax_before(m, a, bv, bi)) { bv = m; bi = a; }
         }
         const float* src = q_next + b * AN + (int64_t)bi * N;
         for (int k = lane; k < N; k += 32) out[b * N + k] = src[k];
         if (lane == 0 && act_out) act_out[b] = bi;
     }
-}
-
-// fixed-order sum over the CTA: the warp butterfly, then warp 0 adds the per-warp values in order.  Every thread returns it.
-__device__ __forceinline__ float block_sum(float v, float* __restrict__ red) {
-    v = tsb::warp_sum(v);
-    __syncthreads();                         // red may still be read by the previous call
-    if (tsb::lane_id() == 0) red[tsb::warp_id()] = v;
-    __syncthreads();
-    float s = 0.0f;
-#pragma unroll
-    for (int w = 0; w < kQrWarps; ++w) s += red[w];
-    return s;
 }
 
 // One CTA per row b (grid-stride), threads over the current quantiles i.  With c_i = q[b][act][i], t = returns[b],
@@ -98,7 +72,7 @@ __global__ void __launch_bounds__(kQrThreads) qrdqn_rows_kernel(
         float cql_row = 0.0f, p_act = 0.0f;
         if (cql) {
             for (int a = warp; a < A; a += kQrWarps) {
-                const float ma = quantile_mean(qb + (int64_t)a * N, N, lane);
+                const float ma = tsb::quantile_mean(qb + (int64_t)a * N, N, 1, lane);
                 if (lane == 0) m[a] = ma;
             }
             __syncthreads();
@@ -131,22 +105,14 @@ __global__ void __launch_bounds__(kQrThreads) qrdqn_rows_kernel(
             const float c = qb[(int64_t)ab * N + i];
             const float ti = tau[i];
             float sq = 0.0f, sp = 0.0f, sg = 0.0f;
-            for (int j = 0; j < N; ++j) {
-                const float u = t[j] - c;
-                const float au = fabsf(u);
-                const float h = au < 1.0f ? 0.5f * au * au : au - 0.5f;
-                const float w = fabsf(ti - (u <= 0.0f ? 1.0f : 0.0f));
-                sq += h * w;
-                sp += h;
-                sg += w * fminf(fmaxf(u, -1.0f), 1.0f);
-            }
+            for (int j = 0; j < N; ++j) tsb::quantile_huber_pair(t[j], c, ti, sq, sp, sg);
             acc_qr += sq;
             acc_p += sp;
             db[(int64_t)ab * N + i] = g_scale * sg + cql_act;
         }
         const float inv_n = 1.0f / (float)N;
-        const float qr = block_sum(acc_qr, red) * inv_n;
-        const float pr = block_sum(acc_p, red) * inv_n;
+        const float qr = tsb::block_sum<kQrWarps>(acc_qr, red) * inv_n;
+        const float pr = tsb::block_sum<kQrWarps>(acc_p, red) * inv_n;
         if (tid == 0) {
             rows[b] = wb * qr;
             rows[B + b] = cql_row;
