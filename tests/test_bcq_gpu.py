@@ -337,7 +337,12 @@ GRAD_CASES = [(17, 6, (256, 256), (512, 512), 12, False), (17, 6, (256, 256), (5
 @gpu
 @pytest.mark.parametrize("O,A,H,VH,L,per_row", GRAD_CASES, ids=[f"O{c[0]}-A{c[1]}-{'net' if c[5] else 'mlp'}" for c in GRAD_CASES])
 def test_update_gradients_vs_fp64_autograd(O, A, H, VH, L, per_row):
-    """One update at batch 256 with N = 10, max_action 2 and phi 0.5: the VAE's and both critics' gradients, taken before their
+    grad_case(O, A, H, VH, L, per_row)
+
+
+def grad_case(O, A, H, VH, L, per_row, B=256, edge=""):
+    """One update at batch ``B`` (256 in the suite's own cases) with N = 10, max_action 2 and phi 0.5: the VAE's and both
+    critics' gradients, taken before their
     Adam steps, against float64 autograd of the eager restatement on copies of the modules with the same eps and latents; the
     perturbation step's against float64 autograd of the actor loss on the pre-update perturbation network with the VAE and
     critic 1 the update stepped (an Adam step is about lr * sign(g), so a float64 re-run of those steps could move a weight by
@@ -345,7 +350,7 @@ def test_update_gradients_vs_fp64_autograd(O, A, H, VH, L, per_row):
     from oracle.oracle_bcq import BcqNets, bcq_update
     from tianshou_b200.algorithm.flat_params import FlatGroup
     from tianshou_b200.utils import policy_within_training_step
-    m, B, N, phi = 2.0, 256, 10, 0.5
+    m, N, phi = 2.0, 10, 0.5
     cfg = dict(obs=O, act=A, hidden=H, vae_hidden=VH, latent=L, max_action=m, phi=phi, per_row=per_row, critic2=True, actor_lr=1e-3,
                critic_lr=1e-3, critic2_lr=3e-4, vae_lr=1e-3, gamma=0.99, tau=0.005, lmbda=0.75, N=N, S=10, init_seed=O + A)
     algo = _build(cfg)
@@ -379,7 +384,7 @@ def test_update_gradients_vs_fp64_autograd(O, A, H, VH, L, per_row):
                        *nets.dec.parameters()], lr=1e-3)]           # the VAE group's flat order: the two heads' rows adjacent
     torch.manual_seed(31)
     ref = bcq_update(nets, opts, batch, lambda shape: eps_seen[0].double().cpu(), gamma=0.99, tau=0.005, lmbda=0.75, N=N)
-    tag = f"bcq_grad/O{O}_A{A}_{'net' if per_row else 'mlp'}"
+    tag = f"bcq_grad{edge}/O{O}_A{A}_{'net' if per_row else 'mlp'}"
     for name, opt in (("vae", opts[3]), ("c1", opts[1]), ("c2", opts[2])):
         want = torch.cat([x.reshape(-1) for x in opt.seen]).numpy()
         record_parity(f"{tag}/grad_{name}", cap[name].numpy(), want, rtol=2e-4, atol=1e-4 * float(np.abs(want).max()) + 1e-12)
@@ -404,6 +409,8 @@ def test_update_gradients_vs_fp64_autograd(O, A, H, VH, L, per_row):
     scale = (1e-3 if not per_row else 1e-4) * float(np.abs(want).max())
     record_parity(f"{tag}/grad_pert", cap["pert"].numpy(), want, rtol=2e-4, atol=scale + 1e-12)
     record_parity(f"{tag}/actor_loss", np.array([stats.actor_loss]), np.array([loss.item()]), rtol=2e-5, atol=1e-5)
+    assert len(cap["indices"]) == B and eps_seen[0].shape[0] == B, "the update must run on the B sampled rows"
+    assert algo._scratch["t_xc"].shape[0] == B * N, "the target's sampled-action rows must be B x N"
 
 
 # ------------------------------------------------------------------------------------------------------------ host sync

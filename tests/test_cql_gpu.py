@@ -276,7 +276,12 @@ GRAD_CASES = [(11, 3, (256, 256), 10), (376, 17, (64, 64), 3)]
 @gpu
 @pytest.mark.parametrize("O,A,H,R", GRAD_CASES, ids=["hopper", "obs376-act17"])
 def test_update_gradients_vs_fp64_autograd(O, A, H, R):
-    """One update: the gradient of each of the four optimiser steps (actor, Lagrange multiplier, critic 1, critic 2), taken
+    grad_case(O, A, H, R)
+
+
+def grad_case(O, A, H, R, B=128, edge=""):
+    """One update at batch ``B`` (128 in the suite's own cases): the gradient of each of the four optimiser steps (actor,
+    Lagrange multiplier, critic 1, critic 2), taken
     before its Adam step, against float64 autograd of the eager restatement on copies of the modules with the same batch,
     noise and random actions.  Adam's first step is lr * sign(g); this is the check that sees a gradient off by a factor."""
     from oracle.oracle_cql import cql_nets, cql_update
@@ -302,7 +307,6 @@ def test_update_gradients_vs_fp64_autograd(O, A, H, R):
     for m in (nets.a_trunk, nets.a_mu, nets.a_sigma, *nets.c, *nets.c_old):
         m.double()
     buf = algo.process_buffer(_random_buffer(O, A, 600, seed=O))
-    B = 128
     noises = []
 
     def noise(shape):
@@ -337,7 +341,7 @@ def test_update_gradients_vs_fp64_autograd(O, A, H, R):
     ref = cql_update(nets, opts, 0.2, (la, la_opt), batch, lambda shape: next(it).double().cpu(), gamma=0.99, tau=0.005, temperature=1.0,
                      cql_weight=1.0, num_repeat_actions=R, lagrange_threshold=10.0, min_action=-0.5, max_action=1.0, alpha_min=0.0,
                      alpha_max=1e6, max_grad_norm=1e9)
-    tag = f"cql_grad/O{O}_A{A}"
+    tag = f"cql_grad{edge}/O{O}_A{A}"
     for name, opt in (("actor", opts[0]), ("c1", opts[1]), ("c2", opts[2]), ("la", la_opt)):
         want = torch.cat([g.reshape(-1) for g in opt.seen]).numpy()
         got = cap[name].numpy()
@@ -347,6 +351,7 @@ def test_update_gradients_vs_fp64_autograd(O, A, H, R):
         record_parity(f"{tag}/grad_{name}", got, want, rtol=2e-4, atol=1e-4 * float(np.abs(want).max()) + 1e-12)
     record_parity(f"{tag}/losses", np.array([stats.actor_loss, stats.critic1_loss, stats.critic2_loss, stats.cql_alpha_loss]),
                   np.array([ref["actor_loss"], ref["critic1_loss"], ref["critic2_loss"], ref["cql_alpha_loss"]]), rtol=2e-5, atol=1e-5)
+    assert len(idx) == B and algo._scratch["rep_idx"].numel() == B * R, "the repeated-action rows must be B x R"
 
 
 # ------------------------------------------------------------------------------------------------------------ host sync

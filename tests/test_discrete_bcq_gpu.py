@@ -312,7 +312,12 @@ def test_update_matches_reference(variant, mirror):
 @gpu
 @pytest.mark.parametrize("name,kind,shared,kw", TRUNK_CASES[:4], ids=[c[0] for c in TRUNK_CASES[:4]])
 def test_update_gradient_vs_fp64_autograd(name, kind, shared, kw):
-    """One update: the flat gradient, snapshotted before its Adam step, against float64 autograd of the reference loss
+    grad_case(name, kind, shared, kw)
+
+
+def grad_case(name, kind, shared, kw, B=64, edge=""):
+    """One update at batch ``B`` (64 in the suite's own cases): the flat gradient, snapshotted before its Adam step, against
+    float64 autograd of the reference loss
     (discrete_bcq.py:244-252) on copies of the modules with the same weights, batch and returns.  Adam's first step is
     lr * sign(g), so a gradient off by a constant factor leaves the parameters unchanged; this is the check that sees it."""
     from tianshou_b200.algorithm import AdamOptimizerFactory, DiscreteBCQ, DiscreteBCQPolicy
@@ -321,7 +326,7 @@ def test_update_gradient_vs_fp64_autograd(name, kind, shared, kw):
     from tianshou_b200.utils import policy_within_training_step
     torch.manual_seed(5 + len(name))
     rng = np.random.default_rng(len(name))
-    A, E, T, B, penalty = 6, 4, 48, 64, 0.2
+    A, E, T, penalty = 6, 4, 48, 0.2
     model, imitator = make_heads(kind, shared, A, (24,), **kw)
     algo = DiscreteBCQ(policy=DiscreteBCQPolicy(model=model, imitator=imitator, action_space=_Discrete(A), target_update_freq=3,
                                                 unlikely_action_threshold=0.4),
@@ -367,9 +372,10 @@ def test_update_gradient_vs_fp64_autograd(name, kind, shared, kw):
     loss = ql + il + penalty * reg
     loss.backward()
     from tianshou_b200.algorithm.shared_trunk import two_head_parameters
-    check_flat_grads(f"dbcq_grad/{name}", grp.params, grp, cap["grad"], two_head_parameters(ref[0], ref[1]))
-    record_parity(f"dbcq_grad/{name}/losses", np.array([stats.loss, stats.q_loss, stats.i_loss, stats.reg_loss]),
+    check_flat_grads(f"dbcq_grad{edge}/{name}", grp.params, grp, cap["grad"], two_head_parameters(ref[0], ref[1]))
+    record_parity(f"dbcq_grad{edge}/{name}/losses", np.array([stats.loss, stats.q_loss, stats.i_loss, stats.reg_loss]),
                   np.array([loss.item(), ql.item(), il.item(), reg.item()]), rtol=2e-5, atol=2e-6)
+    assert len(idx) == B, "the update must run on the B sampled rows"
 
 
 # ------------------------------------------------------------------------------------------------------------ state_dict

@@ -125,7 +125,12 @@ def test_update_matches_reference(variant, mirror):
 @pytest.mark.parametrize("mode", ["exp", "binary", "all"])
 @pytest.mark.parametrize("name,kind,shared,kw", TRUNK_CASES[:4], ids=[c[0] for c in TRUNK_CASES[:4]])
 def test_update_gradient_vs_fp64_autograd(name, kind, shared, kw, mode):
-    """One update with a lagged copy: the flat gradient before its Adam step against float64 autograd of the reference loss
+    grad_case(name, kind, shared, kw, mode)
+
+
+def grad_case(name, kind, shared, kw, mode, B=64, edge=""):
+    """One update at batch ``B`` (64 in the suite's own cases) with a lagged copy: the flat gradient before its Adam step
+    against float64 autograd of the reference loss
     (discrete_crr.py:131-158, its [B] x [B, 1] broadcast included) on copies of the modules."""
     from tianshou_b200.algorithm import AdamOptimizerFactory, DiscreteActorPolicy, DiscreteCRR
     from tianshou_b200.algorithm.flat_params import FlatGroup
@@ -134,7 +139,7 @@ def test_update_gradient_vs_fp64_autograd(name, kind, shared, kw, mode):
     from tianshou_b200.utils import policy_within_training_step
     torch.manual_seed(9 + len(name))
     rng = np.random.default_rng(len(name) + len(mode))
-    A, E, T, B, gamma, beta, bound, w = 6, 4, 48, 64, 0.9, 0.5, 1.1, 3.0
+    A, E, T, gamma, beta, bound, w = 6, 4, 48, 0.9, 0.5, 1.1, 3.0
     actor, critic = make_heads(kind, shared, A, (24,), critic_b=True, **kw)
     algo = DiscreteCRR(policy=DiscreteActorPolicy(actor=actor, action_space=_Discrete(A)), critic=critic, optim=AdamOptimizerFactory(lr=1e-3),
                        gamma=gamma, policy_improvement_mode=mode, ratio_upper_bound=bound, beta=beta, min_q_weight=w, target_update_freq=2)
@@ -190,9 +195,10 @@ def test_update_gradient_vs_fp64_autograd(name, kind, shared, kw, mode):
     cql = (q.logsumexp(1) - qa.squeeze(-1)).mean()
     loss = actor_loss + critic_loss + w * cql
     loss.backward()
-    check_flat_grads(f"dcrr_grad/{name}_{mode}", grp.params, grp, cap["grad"], two_head_parameters(ref[0], ref[1]))
-    record_parity(f"dcrr_grad/{name}_{mode}/losses", np.array([stats.loss, stats.actor_loss, stats.critic_loss, stats.cql_loss]),
+    check_flat_grads(f"dcrr_grad{edge}/{name}_{mode}", grp.params, grp, cap["grad"], two_head_parameters(ref[0], ref[1]))
+    record_parity(f"dcrr_grad{edge}/{name}_{mode}/losses", np.array([stats.loss, stats.actor_loss, stats.critic_loss, stats.cql_loss]),
                   np.array([loss.item(), actor_loss.item(), critic_loss.item(), cql.item()]), rtol=5e-5, atol=5e-6)
+    assert len(idx) == B, "the update must run on the B sampled rows"
 
 
 @gpu

@@ -265,17 +265,20 @@ def _copy64(mod, group, flat):
     return c
 
 
-def _check_grads(tag, mod, group, grad, ref_mod):
+def _check_grads(tag, mod, group, grad, ref_mod, rows=0):
     """Every parameter's gradient read through ``group.view``.  The GEMMs are fp32-faithful (bf16x3), the weight
     gradients sum B products per element: 2e-4 relative plus 1e-4 of the tensor's largest value (the three-product
-    weight-gradient bound of test_tc_shapes_gpu)."""
+    weight-gradient bound of test_tc_shapes_gpu), or the documented sum-length term of ``rows`` rows where that is larger."""
+    from ts_testutil import sum_length_rel
+    rel = max(1e-4, sum_length_rel(rows))
     for (name, p), (_, q) in zip(mod.named_parameters(), ref_mod.named_parameters(), strict=True):
         ref = q.grad.numpy()
         got = group.view(grad, p).view(p.shape).cpu().numpy()
-        record_parity(f"{tag}/grad_{name}", got, ref, rtol=2e-4, atol=1e-4 * float(np.abs(ref).max()) + 1e-12)
+        record_parity(f"{tag}/grad_{name}", got, ref, rtol=2e-4, atol=rel * float(np.abs(ref).max()) + 1e-12)
 
 
-def _sac_grad_case(O, A, H, separate_critic2, per, auto_alpha, seed):
+def _sac_grad_case(O, A, H, separate_critic2, per, auto_alpha, seed, B=256, edge=""):
+    """One SAC update at batch ``B`` checked against float64 autograd; returns the captured batch and the update's stats."""
     from tianshou_b200.algorithm import AdamOptimizerFactory
     from tianshou_b200.algorithm.modelfree.sac import SAC, AutoAlpha, SACPolicy
     from tianshou_b200.algorithm.flat_params import FlatGroup
@@ -337,12 +340,11 @@ def _sac_grad_case(O, A, H, separate_critic2, per, auto_alpha, seed):
 
     algo._noise_fn, algo._adam, algo._preprocess_batch, algo._postprocess_batch = noise, adam, pre, post
     log_alpha0 = float(alpha._log_alpha.item()) if auto_alpha else None
-    B = 256
     np.random.seed(seed)
     with policy_within_training_step(algo.policy):
         stats = algo.update(buffer=buf, sample_size=B)
     torch.cuda.synchronize()
-    tag = f"sac_grad/{O}x{A}_c2{int(separate_critic2)}_per{int(per)}_auto{int(auto_alpha)}"
+    tag = f"sac_grad{edge}/{O}x{A}_c2{int(separate_critic2)}_per{int(per)}_auto{int(auto_alpha)}"
     assert [g for g, *_ in cap["adam"]] == groups and len(cap["noise"]) == 2
     obs, act, R = (cap[k].cpu().to(torch.float64) for k in ("obs", "act", "returns"))
     w = cap["weight"].cpu().to(torch.float64) if per else torch.ones(B, dtype=torch.float64)
@@ -356,7 +358,7 @@ def _sac_grad_case(O, A, H, separate_critic2, per, auto_alpha, seed):
         loss = (td.pow(2) * w).mean()
         loss.backward()
         tds.append(td.detach())
-        _check_grads(f"{tag}/critic{k + 1}", mod, group, grad, ref)
+        _check_grads(f"{tag}/critic{k + 1}", mod, group, grad, ref, rows=B)
         record_parity(f"{tag}/{losskey}", np.array([getattr(stats, losskey)]), np.array([loss.item()]), rtol=2e-5, atol=1e-7)
     if per:          # the priority update (td1 + td2) / 2 (sac.py:318)
         record_parity(f"{tag}/prio_td", cap["prio_td"].cpu().numpy(), ((tds[0] + tds[1]) / 2).numpy(), rtol=1e-5,
@@ -375,10 +377,11 @@ def _sac_grad_case(O, A, H, separate_critic2, per, auto_alpha, seed):
     qs = [m.last.model(m.preprocess.model.model(torch.cat([obs, t], 1))).view(-1) for m in rc]
     alpha0 = float(np.exp(log_alpha0)) if auto_alpha else 0.2
     (alpha0 * logp - torch.min(qs[0], qs[1])).mean().backward()
-    _check_grads(f"{tag}/actor", actor, group, grad, ra)
+    _check_grads(f"{tag}/actor", actor, group, grad, ra, rows=B)
     sat = float((algo._scratch["au_act"].abs() == 1.0).float().mean())
     clamped = float(((raw < -20.0) | (raw > 2.0)).double().mean())
-    assert sat > 0.05 and clamped > 0.2, "the head biases must saturate some actions and clamp some log-sigmas"
+    if B >= 64:      # a handful of rows need not hit every head bias
+        assert sat > 0.05 and clamped > 0.2, "the head biases must saturate some actions and clamp some log-sigmas"
     ties = float((qs[0] == qs[1]).double().mean())
     assert ties == (0.0 if separate_critic2 else 1.0), "critic2=None deep-copies the critic: every row ties"
     lp_k = algo._scratch["au_logp"].cpu().to(torch.float64)
@@ -404,6 +407,7 @@ def _sac_grad_case(O, A, H, separate_critic2, per, auto_alpha, seed):
         record_parity(f"{tag}/log_alpha", np.array([alpha._log_alpha.item()]), np.array([ref_la]), rtol=0.0, atol=1e-6)
     else:
         assert stats.alpha_loss is None
+    return cap, stats
 
 
 SAC_GRAD_CASES = [
@@ -485,6 +489,10 @@ DQN_GRAD_CASES = [
 @pytest.mark.parametrize("kind,loss,per,is_double,tuf", DQN_GRAD_CASES,
                          ids=[f"{c[0]}-{c[1]}-per{int(c[2])}-double{int(c[3])}-tuf{c[4]}" for c in DQN_GRAD_CASES])
 def test_dqn_update_gradients_vs_fp64_autograd(kind, loss, per, is_double, tuf):
+    _dqn_grad_case(kind, loss, per, is_double, tuf)
+
+
+def _dqn_grad_case(kind, loss, per, is_double, tuf, B=None, edge=""):
     """Two DQN updates: the flat gradient snapshotted at FlatGroup.adam_step against float64 autograd of the reference loss
     (dqn.py:384-401: MSE weighted by the PER importance weights, or the unweighted Huber loss with delta 0.5, which puts
     rows on both sides) on a copy of the same module with the same parameters and batch; the TD errors handed to the
@@ -526,14 +534,15 @@ def test_dqn_update_gradients_vs_fp64_autograd(kind, loss, per, is_double, tuf):
         return orig_post(batch, buffer, indices)
 
     algo._preprocess_batch, algo._postprocess_batch = pre, post
-    B = 64 if kind == "cnn_stacked" else 256
+    if B is None:
+        B = 64 if kind == "cnn_stacked" else 256
     sides = set()
     for u in range(2):
         np.random.seed(700 + u)
         with policy_within_training_step(algo.policy):
             stats = algo.update(buffer=buf, sample_size=B)
         c = cap[u]
-        tag = f"dqn_grad/{kind}_{loss}_per{int(per)}_d{int(is_double)}_tuf{tuf}_u{u}"
+        tag = f"dqn_grad{edge}/{kind}_{loss}_per{int(per)}_d{int(is_double)}_tuf{tuf}_u{u}"
         idx = c["indices"]
         ref = _copy64(net, group, c["flat"])
         obs = np.asarray(buf.obs)[idx]
@@ -559,10 +568,11 @@ def test_dqn_update_gradients_vs_fp64_autograd(kind, loss, per, is_double, tuf):
             w = c["weight"].to(torch.float64) if per else 1.0
             L = ((R - q_sel).pow(2) * w).mean()
         L.backward()
-        _check_grads(tag, net, group, c["grad"], ref)
+        _check_grads(tag, net, group, c["grad"], ref, rows=B)
         record_parity(f"{tag}/loss", np.array([stats.loss]), np.array([L.item()]), rtol=2e-5, atol=1e-7)
         record_parity(f"{tag}/td", c["td"].numpy(), (R - q_sel).detach().numpy(), rtol=1e-5, atol=1e-5 * float(R.abs().max()))
-    if loss == "huber":
+        assert len(idx) == B and c["td"].numel() == B, "the update must run on the B sampled rows"
+    if loss == "huber" and B >= 64:
         assert sides == {"inside", "outside"}, "the Huber rows must lie on both sides of delta"
 
 

@@ -307,7 +307,12 @@ def make_buffer(kind, A, rng, E=4, T=48):
 @gpu
 @pytest.mark.parametrize("kind,mqw", [("mlp", 0.0), ("mlp", 10.0), ("cnn", 10.0)])
 def test_update_gradient_vs_fp64_autograd(kind, mqw):
-    """One update: the flat gradient, snapshotted before its Adam step, against float64 autograd of the reference's loss
+    grad_case(kind, mqw)
+
+
+def grad_case(kind, mqw, B=64, edge=""):
+    """One update at batch ``B`` (64 in the suite's own cases): the flat gradient, snapshotted before its Adam step, against
+    float64 autograd of the reference's loss
     (qrdqn.py:114-128, discrete_cql.py:86-106) on a copy of the module with the same weights, batch and returns.  Adam's first
     step is lr * sign(g), so a gradient off by a constant factor leaves the parameters unchanged; this is the check that sees it.
     The GEMMs are fp32-faithful (bf16x3) and a weight gradient sums B products per element: 2e-4 relative plus 1e-4 of the
@@ -317,7 +322,7 @@ def test_update_gradient_vs_fp64_autograd(kind, mqw):
     from tianshou_b200.utils import policy_within_training_step
     torch.manual_seed(3)
     rng = np.random.default_rng(4)
-    A, N, B = 5, 33, 64
+    A, N = 5, 33
     model = model_from_cfg(kind, A, N, hidden=(48, 40))
     policy = QRDQNPolicy(model=model, action_space=_Discrete(A))
     kw = dict(policy=policy, optim=AdamOptimizerFactory(lr=1e-3), gamma=0.9, num_quantiles=N, n_step_return_horizon=2,
@@ -357,10 +362,11 @@ def test_update_gradient_vs_fp64_autograd(kind, mqw):
     for i, (p, r) in enumerate(zip(grp.params, ref_params, strict=True)):
         want = r.grad.numpy()
         got = grp.view(cap["grad"], p).view(p.shape).cpu().numpy()
-        record_parity(f"qrdqn_grad/{kind}_m{int(mqw)}/grad_{i}", got, want, rtol=2e-4, atol=1e-4 * float(np.abs(want).max()) + 1e-12)
+        record_parity(f"qrdqn_grad{edge}/{kind}_m{int(mqw)}/grad_{i}", got, want, rtol=2e-4, atol=1e-4 * float(np.abs(want).max()) + 1e-12)
     got = [stats.loss, stats.qr_loss, stats.cql_loss] if mqw else [stats.loss]
     want = [loss.item(), qr.item(), cql.item()] if mqw else [loss.item()]
-    record_parity(f"qrdqn_grad/{kind}_m{int(mqw)}/losses", np.array(got), np.array(want), rtol=2e-5, atol=2e-6)
+    record_parity(f"qrdqn_grad{edge}/{kind}_m{int(mqw)}/losses", np.array(got), np.array(want), rtol=2e-5, atol=2e-6)
+    assert len(idx) == B and cap["returns"].shape[0] == B, "the update must run on the B sampled rows"
 
 
 # ------------------------------------------------------------------------------------------------------------ state_dict

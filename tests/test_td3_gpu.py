@@ -283,7 +283,12 @@ GRAD_CASES = [(17, 6, (256, 256), "td3"), (17, 6, (256, 256), "bc"), (376, 17, (
 @gpu
 @pytest.mark.parametrize("O,A,H,algo_kind", GRAD_CASES, ids=[f"O{c[0]}-A{c[1]}-{c[3]}" for c in GRAD_CASES])
 def test_update_gradients_vs_fp64_autograd(O, A, H, algo_kind):
-    """Two updates at batch 256 with n = 3 and max_action 2: an actor step, then a critic-only step.  Each critic step's
+    grad_case(O, A, H, algo_kind)
+
+
+def grad_case(O, A, H, algo_kind, B=256, edge=""):
+    """Two updates at batch ``B`` (256 in the suite's own cases) with n = 3 and max_action 2: an actor step, then a critic-only
+    step.  Each critic step's
     gradient, taken before its Adam step, against float64 autograd of the eager restatement on copies of the modules with the same
     batch and target noise; the actor step's against float64 autograd of the actor loss on the pre-update actor and the critic 1
     the update stepped (the actor step runs against the updated critic, whose Adam step is lr * sign(g) and so moves a weight by
@@ -291,7 +296,7 @@ def test_update_gradients_vs_fp64_autograd(O, A, H, algo_kind):
     from oracle.oracle_td3 import Td3Nets, actor_objective, td3_update
     from tianshou_b200.algorithm.flat_params import FlatGroup
     from tianshou_b200.utils import policy_within_training_step
-    m, B = 2.0, 256
+    m = 2.0
     cfg = dict(obs=O, act=A, hidden=H, max_action=m, critic2=True, critic2_lr=1e-3, action_scaling=False, actor_lr=1e-4,
                critic_lr=3e-4, tau=0.005, gamma=0.99, policy_noise=0.2, freq=2, noise_clip=0.5, n_step=3, algo=algo_kind, alpha=2.5)
     torch.manual_seed(3)
@@ -343,21 +348,22 @@ def test_update_gradients_vs_fp64_autograd(O, A, H, algo_kind):
             loss = actor_objective(anets, f64("obs"), f64("act"), 2.5 if algo_kind == "bc" else None)
             grads = torch.autograd.grad(loss, list(anets.a.parameters()))
             want = torch.cat([x.reshape(-1) for x in grads]).numpy()
-            record_parity(f"td3_grad/O{O}_A{A}_{algo_kind}_u{u}/grad_actor", cap["actor"].numpy(), want, rtol=2e-4,
+            record_parity(f"td3_grad{edge}/O{O}_A{A}_{algo_kind}_u{u}/grad_actor", cap["actor"].numpy(), want, rtol=2e-4,
                           atol=1e-4 * float(np.abs(want).max()) + 1e-12)
-            record_parity(f"td3_grad/O{O}_A{A}_{algo_kind}_u{u}/actor_loss", np.array([stats.actor_loss]), np.array([loss.item()]),
+            record_parity(f"td3_grad{edge}/O{O}_A{A}_{algo_kind}_u{u}/actor_loss", np.array([stats.actor_loss]), np.array([loss.item()]),
                           rtol=2e-5, atol=1e-5)
         assert set(cap) == ({"indices", "actor", "c1", "c2"} if actor_step else {"indices", "c1", "c2"})
         it = iter(noises)
         opts = [_Recorder(nets.a.parameters(), lr=1e-4), _Recorder(nets.c[0].parameters(), lr=3e-4), _Recorder(nets.c[1].parameters(), lr=1e-3)]
         ref = td3_update(nets, opts, d, cap["indices"], lambda shape: next(it).double().cpu(), gamma=0.99, n_step=3, tau=0.005,
                          policy_noise=0.2, noise_clip=0.5, actor_step=actor_step, bc_alpha=2.5 if algo_kind == "bc" else None)
-        tag = f"td3_grad/O{O}_A{A}_{algo_kind}_u{u}"
+        tag = f"td3_grad{edge}/O{O}_A{A}_{algo_kind}_u{u}"
         for name, opt in (("c1", opts[1]), ("c2", opts[2])):
             want = torch.cat([x.reshape(-1) for x in opt.seen]).numpy()
             record_parity(f"{tag}/grad_{name}", cap[name].numpy(), want, rtol=2e-4, atol=1e-4 * float(np.abs(want).max()) + 1e-12)
         record_parity(f"{tag}/losses", np.array([stats.critic1_loss, stats.critic2_loss]),
                       np.array([ref["critic1_loss"], ref["critic2_loss"]]), rtol=2e-5, atol=1e-5)
+        assert len(cap["indices"]) == B and all(x.shape[0] == B for x in noises), "the update must run on the B sampled rows"
 
 
 # ------------------------------------------------------------------------------------------------------------ host sync

@@ -159,6 +159,13 @@ def ppo_reference_fp64(actor, critic, mb: dict, hp: dict) -> dict:
 F32_EPS = float(np.finfo(np.float32).eps)
 
 
+def sum_length_rel(rows: int) -> float:
+    """The accumulation term of a sum over ``rows`` rows, as a fraction of the result's largest value.  It is the bound
+    test_net_gpu documents for ``ts_net_gemm``: one fp32 accumulator takes (rows / 16) x 6 MMA additions, each rounding by up to
+    2^-24.  It passes the 1e-4 of the gradient bars only beyond about 4,400 rows."""
+    return (int(rows) + 15) // 16 * 6 * 2.0 ** -24
+
+
 def ac_named_params(actor, critic) -> dict:
     """``named_params`` for every actor-critic the fused kernels accept: Gaussian (``mu`` head + ``a_logstd``) or
     categorical (DiscreteActor, ``last`` head, no log-std) and separate or shared trunks.  A shared trunk has one set of
