@@ -786,6 +786,35 @@ int ts_iqn_target(const float* q_online, const float* q_next, int64_t B, int32_t
 int ts_iqn_rows(const float* q, const int64_t* act, const float* returns, const float* taus, const float* weight, int64_t B,
                 int32_t A, int32_t S_on, int32_t S_t, float* dq, float* prio, float* rows, float* losses, ts_stream_t stream);
 
+/* ---- FQF (fqf.cu) ---- */
+/* FQF's network is IQN's, evaluated at fractions that a one-layer fraction net proposes from the trunk's features; the quantile
+ * passes are the IQN launches above, the quantile loss is ts_iqn_rows with tau_hats as the per-row fractions.
+ * ts_fqf_fractions: the fraction proposal (utils/net/discrete.py:219-252) from the fraction net's output z [B][N]: per row,
+ * p [B][N] = softmax(z), logp [B][N] = max(z - logsumexp(z), -FLT_MAX) (Categorical's normalised logits with its entropy's clamp),
+ * H [B] = -sum_j logp * p, taus [B][N + 1] = (0, cumsum p) with the cumsum in order in double, rounded to fp32 at each step (as
+ * torch's CPU cumsum), tau_hats [B][N] = (taus[:, :-1] + taus[:, 1:]) / 2 and inner [B][N - 1] = taus[:, 1:-1], contiguous, to
+ * feed ts_iqn_cos.  One block per row.  Any B >= 0, 2 <= N <= 12288; larger N is refused. */
+int ts_fqf_fractions(const float* z, int64_t B, int32_t N, float* taus, float* tau_hats, float* inner, float* p, float* logp,
+                     float* H, ts_stream_t stream);
+/* FQF's target distribution (fqf.py:94-98, :178-193): q_online [B][N][A] at s_{t+n} on its tau_hats, its fractions taus [B][N + 1],
+ * q_next [B][N][A] (the lagged network on the online tau_hats, or q_online itself).  Per row, m_a = sum_n (taus[n + 1] - taus[n]) *
+ * q_online[b][n][a] with the widths and products rounded in fp32, a* = argmax_a m_a with torch.argmax's rule (lowest index among
+ * ties, a NaN is the maximum), out [B][N] = q_next[b][.][a*]; act_out [B] (nullable) = a*.  One warp per row, any A, N >= 1, B. */
+int ts_fqf_target(const float* q_online, const float* taus, const float* q_next, int64_t B, int32_t A, int32_t N, float* out,
+                  int64_t* act_out, ts_stream_t stream);
+/* FQF's fraction loss (fqf.py:221-247) and its gradient at the fraction net's output.  q_hat [B][N][A] are the quantiles at
+ * tau_hats, q_tau [B][N - 1][A] those at taus[:, 1:-1]; taus, p, logp, H are ts_fqf_fractions' outputs.  With the chosen action's
+ * quantiles, g_i (i = 1 .. N - 1) is the reference's gradient_of_taus with its strict > / < sign tests; per row
+ * fraction_b = sum_i g_i taus[b][i].  dz [B][N] = (1/B) p_j ((G_j - sum_k p_k G_k) + ent_coef (logp_j + H_b)), G_j = sum_{i > j} g_i
+ * (0 where p_j is 0): the gradient of fraction_loss - ent_coef * mean_b H.  losses[4] = (fraction_loss - ent_coef * entropy_loss,
+ * fraction_loss, entropy_loss, 0) with fraction_loss = mean_b fraction_b and entropy_loss = mean_b H_b; placed after ts_iqn_rows'
+ * four, one read returns all of an update's statistics.  act must lie in [0, A): the caller checks it.  rows [3][B] is scratch.
+ * One block per row, then one block summing the rows in a fixed order: two calls on the same input are bit-identical.  Any
+ * B, A >= 1, 2 <= N <= 12288 and finite ent_coef; anything else is refused. */
+int ts_fqf_fraction_rows(const float* q_hat, const float* q_tau, const int64_t* act, const float* taus, const float* p,
+                         const float* logp, const float* H, int64_t B, int32_t A, int32_t N, float ent_coef, float* dz, float* rows,
+                         float* losses, ts_stream_t stream);
+
 #ifdef TS_B200_DIAGNOSTICS
 /* Diagnostics build only (libts_b200_diag.so, `python -m tianshou_b200.csrc.build --diag`): not part of the product library. */
 /* Hardware self-test of the wgmma building blocks (csrc/wgmma.cuh), one CTA:

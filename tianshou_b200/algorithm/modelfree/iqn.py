@@ -80,25 +80,13 @@ class _IqnActs(NamedTuple):
     head: list[torch.Tensor]
 
 
-class IQN(QRDQN):
-    """IQN, reference API and semantics (iqn.py:103-183): QR-DQN's target rule and loss shape with sampled fractions.
+class QuantileNetworkCore:
+    """The device network of an ``ImplicitQuantileNetwork`` (IQN's, and FQF's ``FullQuantileFunction``): the trunk, the
+    one-layer embedding and the head as ``FusedStack``s in one flat group, in the model's parameter order (``preprocess.*``,
+    ``last.*``, ``embed_model.net.0.*``), its forward at given fractions and its backward.  The algorithm mixing it in is a
+    ``DiscreteQCore``."""
 
-    ``policy.model`` is an ``ImplicitQuantileNetwork`` whose preprocess net is a ``Net`` or a ``DQNet(features_only=True)``
-    (optionally behind ``ScaledObsInputActionReprNet``) and whose ``last`` MLP ends in ``Linear(., actions)``.  The target takes
-    the arg-max of the online network's sample means at s_{t+n} and the lagged network's ``target_sample_size`` quantiles of
-    that action, on fractions of its own; with ``target_update_freq == 0`` both come from one online forward, and the returns
-    have ``online_sample_size`` columns.  The loss pairs each of the step's ``online_sample_size`` quantiles, with its own
-    fraction, against every return column.  ``num_quantiles`` only becomes ``tau_hat`` in ``state_dict()``, as in the reference.
-    """
-
-    def __init__(self, *, policy: IQNPolicy, optim: OptimizerFactory, gamma: float = 0.99, num_quantiles: int = 200,
-                 n_step_return_horizon: int = 1, target_update_freq: int = 0) -> None:
-        super().__init__(policy=policy, optim=optim, gamma=gamma, num_quantiles=num_quantiles,
-                         n_step_return_horizon=n_step_return_horizon, target_update_freq=target_update_freq)
-
-    def _build_network(self, policy: QRDQNPolicy, dev: torch.device) -> None:
-        """The trunk, the embedding and the head of an ``ImplicitQuantileNetwork`` in one flat group, in the model's parameter
-        order (``preprocess.*``, ``last.*``, ``embed_model.net.0.*``)."""
+    def _build_quantile_network(self, policy: QRDQNPolicy, dev: torch.device) -> None:
         model = policy.model
         inner, last, in_shape, in_scale = describe_discrete_head(model, "model")
         embed_model = getattr(model, "embed_model", None)
@@ -132,6 +120,57 @@ class IQN(QRDQN):
         # in Flatten applies its producer's ReLU mask in its own backward
         self._trunk_act = trunk[-1].act if trunk[-1].kind != "flatten" else ACT_NONE
 
+    def _quantiles_at(self, feat: torch.Tensor, taus: torch.Tensor | None, S: int, tag: str, params: torch.Tensor | None = None,
+                      cos: torch.Tensor | None = None) -> tuple[torch.Tensor, list[torch.Tensor], list[torch.Tensor]]:
+        """(cos, embed, head) of the network (``params``: the lagged flat buffer) on the trunk output ``feat [B, D]`` at the
+        fractions ``taus [B, S]``, or at the cosine features ``cos [B * S, C]`` of fractions already embedded."""
+        B, C, D = feat.shape[0], self.num_cosines, self._feat_dim
+        R = B * S
+        st = stream_ptr(self._dev)
+        if cos is None:
+            cos = self._buf(f"{tag}_cos", (R, C))
+            call("ts_iqn_cos", ptr(taus), R, C, ptr(cos), st)
+        embed = self._embed.forward(cos, R, tag, params=params)
+        h = self._buf(f"{tag}_h", (R, D))
+        call("ts_iqn_mix", ptr(feat), ptr(embed[-1]), B, S, D, ptr(h), st)
+        head = self._head.forward(h, R, tag, params=params)
+        return cos, embed, head
+
+    def _quantile_backward(self, trunk: list[torch.Tensor], embed: list[torch.Tensor], head: list[torch.Tensor], dq: torch.Tensor,
+                           S: int, tag: str) -> None:
+        """Every parameter's gradient of the loss whose gradient w.r.t. q is ``dq [B * S, A]``, stored into the group's gradient
+        buffer: head (with its input gradient dh), ``ts_iqn_mix_backward`` (dfeat and the embedding's pre-activation gradient),
+        the embedding's weight and bias gradients, then the trunk."""
+        feat = trunk[-1]
+        B, D = feat.shape[0], self._feat_dim
+        R = B * S
+        dh = self._head.backward(head, dq, R, tag, input_grad=True)
+        dfeat, de_pre = self._buf(f"{tag}_dfeat", (B, D)), self._buf(f"{tag}_de_pre", (R, D))
+        call("ts_iqn_mix_backward", ptr(dh), ptr(feat), ptr(embed[-1]), B, S, D, int(self._trunk_act),
+             ptr(feat) if self._trunk_act != ACT_NONE else None, ptr(dfeat), ptr(de_pre), stream_ptr(self._dev))
+        self._embed.backward(embed, de_pre, R, tag, dy_preact=True)
+        self._trunk.backward(trunk, dfeat, B, tag, dy_preact=True)
+
+
+class IQN(QuantileNetworkCore, QRDQN):
+    """IQN, reference API and semantics (iqn.py:103-183): QR-DQN's target rule and loss shape with sampled fractions.
+
+    ``policy.model`` is an ``ImplicitQuantileNetwork`` whose preprocess net is a ``Net`` or a ``DQNet(features_only=True)``
+    (optionally behind ``ScaledObsInputActionReprNet``) and whose ``last`` MLP ends in ``Linear(., actions)``.  The target takes
+    the arg-max of the online network's sample means at s_{t+n} and the lagged network's ``target_sample_size`` quantiles of
+    that action, on fractions of its own; with ``target_update_freq == 0`` both come from one online forward, and the returns
+    have ``online_sample_size`` columns.  The loss pairs each of the step's ``online_sample_size`` quantiles, with its own
+    fraction, against every return column.  ``num_quantiles`` only becomes ``tau_hat`` in ``state_dict()``, as in the reference.
+    """
+
+    def __init__(self, *, policy: IQNPolicy, optim: OptimizerFactory, gamma: float = 0.99, num_quantiles: int = 200,
+                 n_step_return_horizon: int = 1, target_update_freq: int = 0) -> None:
+        super().__init__(policy=policy, optim=optim, gamma=gamma, num_quantiles=num_quantiles,
+                         n_step_return_horizon=n_step_return_horizon, target_update_freq=target_update_freq)
+
+    def _build_network(self, policy: QRDQNPolicy, dev: torch.device) -> None:
+        self._build_quantile_network(policy, dev)
+
     # ------------------------------------------------------------------ network
     def _draw_taus(self, rows: int, sample_size: int) -> torch.Tensor:
         """The fractions of one forward: ``torch.rand(rows, sample_size)`` in fp32 on the device, the call the reference's
@@ -141,32 +180,15 @@ class IQN(QRDQN):
 
     def _quantiles(self, src: DeviceObsSource, S: int, tag: str, params: torch.Tensor | None = None) -> _IqnActs:
         """q[B][S][A] of the network (``params``: the lagged flat buffer) on ``S`` fresh fractions per row."""
-        B, R, C, D = src.rows, src.rows * S, self.num_cosines, self._feat_dim
-        st = stream_ptr(self._dev)
+        B = src.rows
         trunk = self._trunk.forward(src.x, B, tag, frames=src.frames, params=params)
         taus = self._draw_taus(B, S)
         assert taus.shape == (B, S) and taus.dtype == torch.float32 and taus.is_contiguous() and taus.device == self._dev
-        cos = self._buf(f"{tag}_cos", (R, C))
-        call("ts_iqn_cos", ptr(taus), R, C, ptr(cos), st)
-        embed = self._embed.forward(cos, R, tag, params=params)
-        h = self._buf(f"{tag}_h", (R, D))
-        call("ts_iqn_mix", ptr(trunk[-1]), ptr(embed[-1]), B, S, D, ptr(h), st)
-        head = self._head.forward(h, R, tag, params=params)
+        _, embed, head = self._quantiles_at(trunk[-1], taus, S, tag, params)
         return _IqnActs(trunk, taus, embed, head)
 
     def _backward(self, f: _IqnActs, dq: torch.Tensor, S: int, tag: str) -> None:
-        """Every parameter's gradient of the loss whose gradient w.r.t. q is ``dq [B * S, A]``, stored into the group's gradient
-        buffer: head (with its input gradient dh), ``ts_iqn_mix_backward`` (dfeat and the embedding's pre-activation gradient),
-        the embedding's weight and bias gradients, then the trunk."""
-        feat = f.trunk[-1]
-        B, D = feat.shape[0], self._feat_dim
-        R = B * S
-        dh = self._head.backward(f.head, dq, R, tag, input_grad=True)
-        dfeat, de_pre = self._buf(f"{tag}_dfeat", (B, D)), self._buf(f"{tag}_de_pre", (R, D))
-        call("ts_iqn_mix_backward", ptr(dh), ptr(feat), ptr(f.embed[-1]), B, S, D, int(self._trunk_act),
-             ptr(feat) if self._trunk_act != ACT_NONE else None, ptr(dfeat), ptr(de_pre), stream_ptr(self._dev))
-        self._embed.backward(f.embed, de_pre, R, tag, dy_preact=True)
-        self._trunk.backward(f.trunk, dfeat, B, tag, dy_preact=True)
+        self._quantile_backward(f.trunk, f.embed, f.head, dq, S, tag)
 
     # ------------------------------------------------------------------ target
     def _target_q(self, buffer: ReplayBuffer, indices: np.ndarray) -> torch.Tensor:

@@ -63,7 +63,7 @@ class QRDQN(DiscreteQCore, OffPolicyAlgorithm):
         self.num_quantiles = num_quantiles
         dev = cuda_device_of(policy.model)
         self._build_network(policy, dev)
-        self.optim = self._create_optimizer(policy, optim)
+        self.optim = self._create_policy_optimizer(policy, optim)
         bind_optimizer(self.optim, self._group)
         # the midpoints exactly as the reference forms them in fp32 on the CPU (not (k + 0.5) / N, which differs in the last bit)
         tau = torch.linspace(0, 1, num_quantiles + 1)
@@ -91,6 +91,10 @@ class QRDQN(DiscreteQCore, OffPolicyAlgorithm):
         self._init_discrete(dev, in_shape, in_scale, n_actions)
         self._group = FlatGroup(layer_params(layers), dev)
         self._net = FusedStack(layers, self._group, "qr")
+
+    def _create_policy_optimizer(self, policy: QRDQNPolicy, optim: OptimizerFactory) -> OffPolicyAlgorithm.Optimizer:
+        """The optimiser of ``_group``: over the whole policy here; FQF leaves its fraction model to an optimiser of its own."""
+        return self._create_optimizer(policy, optim)
 
     @property
     def use_target_network(self) -> bool:

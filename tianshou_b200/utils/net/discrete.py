@@ -1,4 +1,5 @@
-"""Discrete-action actor / critic heads and IQN's quantile network (API of tianshou/utils/net/discrete.py:22-216)."""
+"""Discrete-action actor / critic heads, IQN's quantile network and FQF's fraction proposal and full quantile function (API of
+tianshou/utils/net/discrete.py:22-314)."""
 from __future__ import annotations
 
 from collections.abc import Sequence
@@ -9,6 +10,7 @@ import torch
 import torch.nn.functional as F
 from torch import nn
 
+from ...data import Batch
 from .common import MLP, ModuleWithVectorOutput
 
 
@@ -92,3 +94,56 @@ class ImplicitQuantileNetwork(DiscreteCritic):
         h = (feat.unsqueeze(1) * self.embed_model(taus)).view(B * sample_size, -1)
         q = self.last(h).view(B, sample_size, -1).transpose(1, 2)
         return (q, taus), hidden
+
+
+class FractionProposalNetwork(nn.Module):
+    """FQF's fraction proposal (discrete.py:219-252): ``Linear(embedding_dim, num_fractions)`` (Xavier-uniform weight at gain
+    0.01, zero bias) on the trunk's features, read as the logits of a ``Categorical``.  ``forward`` returns ``taus [B, N + 1]``
+    (0, then the cumulative sum of the probabilities), ``tau_hats [B, N]`` (the midpoints, detached) and the entropies ``[B]``."""
+
+    def __init__(self, num_fractions: int, embedding_dim: int) -> None:
+        super().__init__()
+        self.net = nn.Linear(embedding_dim, num_fractions)
+        torch.nn.init.xavier_uniform_(self.net.weight, gain=0.01)
+        torch.nn.init.constant_(self.net.bias, 0)
+        self.num_fractions = num_fractions
+        self.embedding_dim = embedding_dim
+
+    def forward(self, obs_embeddings: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        dist = torch.distributions.Categorical(logits=self.net(obs_embeddings))
+        taus = F.pad(torch.cumsum(dist.probs, dim=1), (1, 0))
+        tau_hats = (taus[:, :-1] + taus[:, 1:]).detach() / 2.0
+        return taus, tau_hats, dist.entropy()
+
+
+class FullQuantileFunction(ImplicitQuantileNetwork):
+    """FQF's quantile network (discrete.py:255-314): IQN's network evaluated at the fractions a ``FractionProposalNetwork``
+    proposes from the trunk's detached features.  ``forward`` returns ``((quantiles [B, actions, N] at tau_hats, fractions,
+    quantiles_tau), hidden)`` with ``fractions = Batch(taus, tau_hats, entropies)`` (or the ``fractions`` passed in, whose
+    ``tau_hats`` are then used); in training mode ``quantiles_tau [B, actions, N - 1]`` are the quantiles at ``taus[:, 1:-1]``,
+    computed without gradient, else None."""
+
+    def __init__(self, *, preprocess_net: ModuleWithVectorOutput, action_shape: Any, hidden_sizes: Sequence[int] = (),
+                 num_cosines: int = 64) -> None:
+        super().__init__(preprocess_net=preprocess_net, action_shape=action_shape, hidden_sizes=hidden_sizes,
+                         num_cosines=num_cosines)
+
+    def _compute_quantiles(self, obs: torch.Tensor, taus: torch.Tensor) -> torch.Tensor:
+        B, S = taus.shape
+        h = (obs.unsqueeze(1) * self.embed_model(taus)).view(B * S, -1)
+        return self.last(h).view(B, S, -1).transpose(1, 2)
+
+    def forward(self, obs: Any, propose_model: FractionProposalNetwork, fractions: Batch | None = None,  # type: ignore[override]
+                **kwargs: Any) -> tuple[Any, Any]:
+        feat, hidden = self.preprocess(obs, state=kwargs.get("state"))
+        if fractions is None:
+            taus, tau_hats, entropies = propose_model(feat.detach())
+            fractions = Batch(taus=taus, tau_hats=tau_hats, entropies=entropies)
+        else:
+            taus, tau_hats = fractions.taus, fractions.tau_hats
+        quantiles = self._compute_quantiles(feat, tau_hats)
+        quantiles_tau = None
+        if self.training:
+            with torch.no_grad():
+                quantiles_tau = self._compute_quantiles(feat, taus[:, 1:-1])
+        return (quantiles, fractions, quantiles_tau), hidden
