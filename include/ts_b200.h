@@ -463,6 +463,26 @@ int ts_net_gemm(const float* a, int64_t lda, int32_t a_mn_major, const float* b,
 int64_t ts_net_gemm_workspace_floats(int32_t M, int32_t N, int32_t K);
 /* out[n] (+)= sum_m x[m * ld + n]  (bias gradients) */
 int ts_net_colsum(const float* x, int64_t ld, int32_t M, int32_t N, float* out, int32_t accumulate, ts_stream_t stream);
+/* `batch` GEMMs of ts_net_gemm's contract in one launch (the members of an EnsembleLinear layer, utils/net/common.py:518-550):
+ * member e reads a + e * stride_a, b + e * stride_b, bias + e * stride_bias, act_grad_src + e * stride_mask and writes
+ * c + e * stride_c (element strides; 0 = the operand is shared by every member).  Split-K counts the output tiles of all
+ * members; workspace: ts_net_gemm_batched_workspace_floats(batch, M, N, K) floats ([members][splits][M][N]).  With one member
+ * the result is bitwise ts_net_gemm's (ts_net_gemm is that case).  With W_e[k * out + n] ([E][in][out]):
+ *   forward      Y_e  = act(X W_e + b_e) : A = X  (lda = in, 0),  B = W_e (ldb = out, 1)
+ *   input grad   dX_e = dZ_e W_e^T       : A = dZ_e (lda = out, 0), B = W_e (ldb = out, 0)
+ *   weight grad  dW_e = X^T dZ_e         : A = X (lda = in, 1), B = dZ_e (ldb = out, 1), C [in][out] */
+int ts_net_gemm_batched(int32_t batch, const float* a, int64_t lda, int32_t a_mn_major, int64_t stride_a, const float* b,
+                        int64_t ldb, int32_t b_mn_major, int64_t stride_b, float* c, int64_t ldc, int64_t stride_c, int32_t M,
+                        int32_t N, int32_t K, const float* bias, int64_t stride_bias, int32_t act, const float* act_grad_src,
+                        int64_t ld_mask, int64_t stride_mask, int32_t act_grad_kind, int32_t accumulate, float* workspace,
+                        int64_t workspace_floats, ts_stream_t stream);
+int64_t ts_net_gemm_batched_workspace_floats(int32_t batch, int32_t M, int32_t N, int32_t K);
+/* out[e * stride_out + n] (+)= sum_m x[e * stride_x + m * ld + n] for e < batch (per-member bias gradients) */
+int ts_net_colsum_batched(int32_t batch, const float* x, int64_t ld, int64_t stride_x, int32_t M, int32_t N, float* out,
+                          int64_t stride_out, int32_t accumulate, ts_stream_t stream);
+/* out[i] (+)= sum_{e < batch} x[e * stride + i], i < n, members added in index order (no atomics) */
+int ts_net_member_sum(const float* x, int32_t batch, int64_t stride, int64_t n, float* out, int32_t accumulate,
+                      ts_stream_t stream);
 
 /* PPO / A2C loss rows between the forward and backward GEMMs of a layered actor-critic (ppo.py:179-216, a2c.py:262-270):
  * head [B][A] = mu (Gaussian, sigma = exp(logstd[A])) or logits (categorical: Categorical(probs = softmax(logits)),
@@ -653,6 +673,25 @@ int ts_td3_actor_rows(const float* q, const float* z, const float* act, int64_t 
  * Any B (grid-stride). */
 int ts_td3_actor_head_bwd(const float* z, const float* dact, const float* act, int64_t B, int32_t A, float max_action, float* dz,
                           ts_stream_t stream);
+
+/* ---- REDQ (redq.cu) ---- */
+/* The target of REDQ (modelfree/redq.py:254-269) from the lagged ensemble's q [E][B] on (s', a'): over the members whose bit is
+ * set in `subset` (at most 64 members), target_mode TS_REDQ_MIN: min (NaN propagates), TS_REDQ_MEAN: their sum in member order
+ * / count; out[b] = that - alpha * logp[b].  Any B (grid-stride). */
+#define TS_REDQ_MIN 0
+#define TS_REDQ_MEAN 1
+int ts_redq_target(const float* q, int32_t E, int64_t B, uint64_t subset, int32_t target_mode, float alpha, const float* logp,
+                   float* out, ts_stream_t stream);
+/* The ensemble's critic loss (redq.py:273-279) on q [E][B], target [B] and weight [B] (nullable: 1): td [E][B] = q - target,
+ * dq [E][B] = 2 w td / (E B), row_mean [B] = mean_e td (signed: the prioritised buffer's batch.weight), rows [B] = sum_e td^2 w
+ * (scratch) and *loss = mean(td^2 w) over E * B, summed in a fixed order (bit-identical from run to run). */
+int ts_redq_critic_rows(const float* q, const float* target, const float* weight, int32_t E, int64_t B, float* td, float* dq,
+                        float* row_mean, float* rows, float* loss, ts_stream_t stream);
+/* The actor loss (redq.py:285-289) on q [E][B] = Q_e(s, pi(s)) and logp [B]: rows [B] = alpha logp - mean_e q (scratch),
+ * *loss = mean(rows) in a fixed order, dq [E][B] = -1 / (E B).  The loss's gradient at logp is alpha / B at every row: the
+ * alpha_over_b of ts_squashed_gaussian_bwd. */
+int ts_redq_actor_rows(const float* q, const float* logp, int32_t E, int64_t B, float alpha, float* dq, float* rows, float* loss,
+                       ts_stream_t stream);
 
 /* ---- BCQ (bcq.cu) ---- */
 /* The VAE's reparameterisation (utils/net/continuous.py:464-470): from head = [mean | log_std_raw] [B][2L] and eps [B][L],

@@ -10,6 +10,7 @@ from .modelfree.iqn import IQN, IQNPolicy
 from .modelfree.npg import NPG, NPGTrainingStats
 from .modelfree.ppo import A2C, PPO
 from .modelfree.qrdqn import QRDQN, QRDQNPolicy
+from .modelfree.redq import REDQ, REDQPolicy, REDQTrainingStats
 from .modelfree.reinforce import DiscreteActorPolicy, ProbabilisticActorPolicy
 from .modelfree.td3 import TD3, TD3TrainingStats
 from .modelfree.trpo import TRPO, TRPOTrainingStats
@@ -22,5 +23,5 @@ __all__ = [
     "ProbabilisticActorPolicy", "DiscreteActorPolicy", "AdamOptimizerFactory", "LRSchedulerFactoryLinear", "OptimizerFactory",
     "RMSpropOptimizerFactory", "DiscreteBCQ", "DiscreteBCQPolicy", "DiscreteBCQTrainingStats", "DiscreteCRR",
     "DiscreteCRRTrainingStats", "QRDQN", "QRDQNPolicy", "DiscreteCQL", "DiscreteCQLTrainingStats", "IQN", "IQNPolicy",
-    "FQF", "FQFPolicy", "FQFTrainingStats",
+    "FQF", "FQFPolicy", "FQFTrainingStats", "REDQ", "REDQPolicy", "REDQTrainingStats",
 ]

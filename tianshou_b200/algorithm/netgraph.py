@@ -4,7 +4,8 @@ A ``FusedStack`` is the kernel-side view of a torch module stack made of ``nn.Li
 ``nn.ReLU`` / ``nn.Flatten`` (the reference's ``MLP`` / ``Net`` / ``ContinuousCritic`` / ``DQNet``,
 utils/net/common.py:76-369, utils/net/continuous.py:96-238, env/atari/atari_network.py:60-122): every layer's
 forward, input gradient and weight gradient is ONE ``ts_net_gemm`` launch (wgmma, fp32-faithful), convolutions
-run as implicit GEMM over im2col rows.  Parameters live in a ``FlatGroup`` (flat_params.py: one flat fp32 buffer per optimiser,
+run as implicit GEMM over im2col rows.  A chain of ``EnsembleLinear`` layers (utils/net/common.py, REDQ's critic ensemble)
+runs every member of a layer in one batched launch (``ts_net_gemm_batched``) on ``[E, rows, features]`` activations.  Parameters live in a ``FlatGroup`` (flat_params.py: one flat fp32 buffer per optimiser,
 ``nn.Parameter``s are views of it) so Adam and the Polyak update are single kernels and ``state_dict()`` keeps
 working.  There is no autograd graph and no eager-PyTorch path: unsupported layers raise ``UnsupportedModelError``.
 """
@@ -31,7 +32,7 @@ def polyak_update(target: FlatGroup, source: FlatGroup, tau: float) -> None:
 
 @dataclass
 class _Layer:
-    kind: str                      # "linear" | "conv" | "flatten"
+    kind: str                      # "linear" | "conv" | "flatten" | "ensemble"
     weight: nn.Parameter | None = None
     bias: nn.Parameter | None = None
     act: int = ACT_NONE
@@ -45,6 +46,8 @@ class _Layer:
     s: int = 0
     Ho: int = 0
     Wo: int = 0
+    # ensemble: members E; weight [E, in, out] (W_e[k * out + n]), bias [E, 1, out]
+    E: int = 0
 
 
 def layer_params(layers: list[_Layer]) -> list[nn.Parameter]:
@@ -67,13 +70,24 @@ def _flat_chain(mods: list[nn.Module]) -> list[nn.Module]:
     return out
 
 
-def compile_sequential(mods: list[nn.Module], input_shape: tuple[int, ...]) -> list[_Layer]:
+def compile_sequential(mods: list[nn.Module], input_shape: tuple[int, ...], ensemble: bool = False) -> list[_Layer]:
     """Linear / Conv2d / ReLU / Flatten chain -> layer list.  ``input_shape`` = (features,) or (C, H, W).  Nested
-    ``nn.Sequential`` containers are read as the flat chain they run."""
+    ``nn.Sequential`` containers are read as the flat chain they run.  With ``ensemble`` a chain of ``EnsembleLinear`` layers
+    (with ReLU / Tanh between them) is an ensemble chain: every layer has the same member count and a bias, and no other layer
+    kind joins it."""
+    from ..utils.net.common import EnsembleLinear
     layers: list[_Layer] = []
     shape = tuple(int(x) for x in input_shape)
     for m in _flat_chain(mods):
-        if isinstance(m, nn.Linear):
+        if ensemble and isinstance(m, EnsembleLinear):
+            E, d_in, d_out = (int(x) for x in m.weight.shape)
+            if len(shape) != 1 or shape[0] != d_in:
+                raise UnsupportedModelError(f"EnsembleLinear({d_in}) after shape {shape}")
+            if m.bias_weights is None:
+                raise UnsupportedModelError("EnsembleLinear layers need a bias")
+            layers.append(_Layer("ensemble", m.weight, m.bias_weights, ACT_NONE, d_in, d_out, E=E))
+            shape = (d_out,)
+        elif isinstance(m, nn.Linear):
             if len(shape) != 1 or shape[0] != m.in_features:
                 raise UnsupportedModelError(f"Linear({m.in_features}) after shape {shape}")
             if m.bias is None:
@@ -113,6 +127,12 @@ def compile_sequential(mods: list[nn.Module], input_shape: tuple[int, ...]) -> l
             continue
         else:
             raise UnsupportedModelError(f"layer {m} is outside the fused layered-network family")
+    ens = {L.E for L in layers if L.kind == "ensemble"}
+    if ens and any(L.kind != "ensemble" for L in layers):
+        raise UnsupportedModelError("a chain mixes EnsembleLinear with other layers: an ensemble chain is EnsembleLinear + "
+                                    "ReLU / Tanh only")
+    if len(ens) > 1:
+        raise UnsupportedModelError(f"EnsembleLinear layers of different ensemble sizes {sorted(ens)} in one chain")
     # FusedStack.backward masks a convolution's or a flatten's input gradient with ReLU only: refuse a Tanh there now
     # rather than in the middle of the first update
     for prev, L in zip(layers, layers[1:]):
@@ -160,6 +180,16 @@ class FusedStack:
         call("ts_net_gemm", a, lda, a_mn, b, ldb, b_mn, c, ldc, M, N, K, bias, act, mask, ld_mask, int(mask_kind), int(accumulate),
              ptr(ws) if ws is not None else None, ws_n, stream_ptr(self.device))
 
+    def _gemm_batched(self, E, a, lda, a_mn, sa, b, ldb, b_mn, sb, c, ldc, sc, M, N, K, bias=None, s_bias=0, act=ACT_NONE,
+                      mask=None, ld_mask=0, s_mask=0, mask_kind=ACT_RELU, accumulate=False) -> None:
+        key = (E, M, N, K)
+        ws_n = self._ws_sizes.get(key)
+        if ws_n is None:
+            ws_n = self._ws_sizes[key] = int(self._lib.ts_net_gemm_batched_workspace_floats(E, M, N, K))
+        ws = self._buf(("ws",), ws_n) if ws_n > 0 else None
+        call("ts_net_gemm_batched", E, a, lda, a_mn, sa, b, ldb, b_mn, sb, c, ldc, sc, M, N, K, bias, s_bias, act, mask, ld_mask,
+             s_mask, int(mask_kind), int(accumulate), ptr(ws) if ws is not None else None, ws_n, stream_ptr(self.device))
+
     def _w(self, L: _Layer, flat: torch.Tensor | None = None) -> int:
         g = self.group
         base = (flat if flat is not None else g.flat).data_ptr()
@@ -186,6 +216,12 @@ class FusedStack:
                 y = self._buf((tag, "y", i), rows * L.out_dim)[: rows * L.out_dim].view(rows, L.out_dim)
                 self._gemm(ptr(cur), L.in_dim, 0, self._w(L, params), L.in_dim, 0, ptr(y), L.out_dim, rows, L.out_dim, L.in_dim,
                            bias=self._b(L, params), act=L.act)
+            elif L.kind == "ensemble":      # [E, rows, out]; the first layer reads the shared [rows, in] input
+                n_out = L.E * rows * L.out_dim
+                y = self._buf((tag, "y", i), n_out)[:n_out].view(L.E, rows, L.out_dim)
+                self._gemm_batched(L.E, ptr(cur), L.in_dim, 0, 0 if i == 0 else rows * L.in_dim, self._w(L, params), L.out_dim, 1,
+                                   L.in_dim * L.out_dim, ptr(y), L.out_dim, rows * L.out_dim, rows, L.out_dim, L.in_dim,
+                                   bias=self._b(L, params), s_bias=L.out_dim, act=L.act)
             elif L.kind == "conv":
                 R = rows * L.Ho * L.Wo
                 col = self._buf((tag, "col", i), R * L.in_dim)[: R * L.in_dim].view(R, L.in_dim)
@@ -215,7 +251,7 @@ class FusedStack:
         cur = x_dot
         for i, L in enumerate(self.layers):
             if L.kind != "linear":
-                raise UnsupportedModelError("tangent passes support Linear layers only")
+                raise UnsupportedModelError(f"tangent passes support Linear layers only, not {L.kind} layers")
             yd = self._buf((tag, "t", i), rows * L.out_dim)[: rows * L.out_dim].view(rows, L.out_dim)
             mask = ptr(acts[i + 1]) if L.act != ACT_NONE else None
             kind = L.act if L.act != ACT_NONE else ACT_RELU
@@ -269,6 +305,29 @@ class FusedStack:
                     self._gemm(ptr(dz), L.out_dim, 0, self._w(L) + 4 * lo, L.in_dim, 1, ptr(dx), width, M_rows, width, L.out_dim,
                                mask=mask, ld_mask=L.in_dim, mask_kind=prev_act if prev_act != ACT_NONE else ACT_RELU,
                                accumulate=(i == 0 and dx_accumulate))
+                    dz = dx
+            elif L.kind == "ensemble":
+                s_x = 0 if i == 0 else rows * L.in_dim          # the first layer's input is shared by every member
+                s_z = rows * L.out_dim
+                if param_grads:
+                    gw = g.grad.data_ptr() + 4 * g.offset(L.weight)
+                    gb = g.grad.data_ptr() + 4 * g.offset(L.bias)
+                    self._gemm_batched(L.E, ptr(x_in), L.in_dim, 1, s_x, ptr(dz), L.out_dim, 1, s_z, gw, L.out_dim,
+                                       L.in_dim * L.out_dim, L.in_dim, L.out_dim, rows)
+                    call("ts_net_colsum_batched", L.E, ptr(dz), L.out_dim, s_z, rows, L.out_dim, gb, L.out_dim, 0, st)
+                if need_dx:
+                    lo, hi = (0, L.in_dim) if (i > 0 or input_cols is None) else input_cols
+                    width = hi - lo
+                    n_dx = L.E * rows * width
+                    dx = self._buf((tag, "dx", i), n_dx)[:n_dx].view(L.E, rows, width)
+                    mask = ptr(act_src) + 4 * lo if prev_act != ACT_NONE else None
+                    self._gemm_batched(L.E, ptr(dz), L.out_dim, 0, s_z, self._w(L) + 4 * lo * L.out_dim, L.out_dim, 0,
+                                       L.in_dim * L.out_dim, ptr(dx), width, rows * width, rows, width, L.out_dim, mask=mask,
+                                       ld_mask=L.in_dim, s_mask=s_x, mask_kind=prev_act if prev_act != ACT_NONE else ACT_RELU)
+                    if i == 0:      # d loss / d input of the shared input: the members' gradients summed in member order
+                        out = dx_out if dx_out is not None else self._buf((tag, "dxsum"), rows * width)[: rows * width].view(rows, width)
+                        call("ts_net_member_sum", ptr(dx), L.E, rows * width, rows * width, ptr(out), int(dx_accumulate), st)
+                        dx = out
                     dz = dx
             elif L.kind == "conv":
                 if prev_act == ACT_TANH:

@@ -14,6 +14,11 @@
 // partial-product wgmma.mma_async per K = 16 step for its 64 rows into an fp32 register accumulator (64 x 128);
 // staging of chunk i + 1 overlaps the MMAs of chunk i.  Epilogue: registers -> bias -> activation -> optional
 // ReLU-derivative mask -> fp32 stores (or split-K partial).
+//
+// Batched form (the members of an ensemble layer, tianshou/utils/net/common.py:518-550): `batch` independent GEMMs of one
+// shape, member e reading A + e * stride_a, B + e * stride_b, bias + e * stride_bias, mask + e * stride_mask and writing
+// C + e * stride_c (a stride of 0 shares the operand).  grid.z = members x splits; the single GEMM is the one-member case, with
+// the same tiles, split choice and reduction order.
 #include "common.cuh"
 #include "wgmma.cuh"
 
@@ -43,8 +48,9 @@ struct GemmParams {
     int64_t ld_mask;     //   mask_kind TS_ACT_RELU: x * (y > 0) ;  TS_ACT_TANH: x * (1 - y^2)
     int mask_kind;
     int accumulate;      // C += result
-    int splits;          // split-K factor (grid.z); partials are reduced by splitk_reduce_kernel
+    int splits;          // split-K factor; partials are reduced by splitk_reduce_kernel
     int k_per_split;     // multiple of BK
+    int64_t stride_a, stride_b, stride_c, stride_bias, stride_mask;   // per-member element strides (0: shared)
 };
 
 // Stage one 128 (mn) x 64 (k) chunk of an operand.  Shared-memory matrix = [rows = non-contiguous dim][cols =
@@ -106,7 +112,11 @@ __global__ void __launch_bounds__(kThreads, 1) net_gemm_kernel(const GemmParams 
     extern __shared__ __align__(1024) uint8_t sm[];
     const int tid = threadIdx.x, wgi = tid >> 7;
     const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
-    const int kb = blockIdx.z * P.k_per_split;
+    const int member = (int)blockIdx.z / P.splits, split = (int)blockIdx.z - member * P.splits;
+    const int kb = split * P.k_per_split;
+    Operand opa = P.a, opb = P.b;
+    opa.p += member * P.stride_a;
+    opb.p += member * P.stride_b;
     const int ke = P.splits > 1 ? (int)tsb::imin((int64_t)P.K, (int64_t)kb + P.k_per_split) : P.K;
     const uint32_t sbase = wg::smem_u32(sm);
     uint8_t* sm0 = sm - sbase;
@@ -122,8 +132,8 @@ __global__ void __launch_bounds__(kThreads, 1) net_gemm_kernel(const GemmParams 
         const int st = i & 1;
         const int k0 = kb + i * BK;
         Staged sa, sb;
-        load_operand(sa, P.a, m0, k0, ke);
-        load_operand(sb, P.b, n0, k0, ke);
+        load_operand(sa, opa, m0, k0, ke);
+        load_operand(sb, opb, n0, k0, ke);
         if (i >= 2) {            // both warpgroups' MMAs of chunk i - 2 are done with this stage
             wg::wait<1>();
             __syncthreads();
@@ -142,9 +152,11 @@ __global__ void __launch_bounds__(kThreads, 1) net_gemm_kernel(const GemmParams 
     wg::wait<0>();
 
     // ---- epilogue: the thread's accumulator elements, two consecutive columns per store ------------------------
-    float* cbase = P.c + (P.splits > 1 ? (int64_t)blockIdx.z * P.M * P.N : 0);
+    float* cbase = P.splits > 1 ? P.c + (int64_t)blockIdx.z * P.M * P.N : P.c + member * P.stride_c;
     const int64_t ldc = P.splits > 1 ? P.N : P.ldc;
     const bool plain = P.splits > 1;         // partials: raw accumulator, epilogue ops happen in the reduce kernel
+    const float* bias = P.bias ? P.bias + member * P.stride_bias : nullptr;
+    const float* mask = P.mask ? P.mask + member * P.stride_mask : nullptr;
 #pragma unroll
     for (int e = 0; e < BN / 2; e += 2) {
         const int m = m0 + 64 * wgi + wg::frag_row(e), n = n0 + wg::frag_col(e);
@@ -157,9 +169,9 @@ __global__ void __launch_bounds__(kThreads, 1) net_gemm_kernel(const GemmParams 
             for (int j = 0; j < 2; ++j) {
                 if (j == 1 && !pair) break;
                 float x = v[j];
-                if (P.bias) x += __ldg(P.bias + n + j);
+                if (bias) x += __ldg(bias + n + j);
                 x = apply_act(x, P.act);
-                if (P.mask) x = apply_act_grad(x, __ldg(P.mask + (int64_t)m * P.ld_mask + n + j), P.mask_kind);
+                if (mask) x = apply_act_grad(x, __ldg(mask + (int64_t)m * P.ld_mask + n + j), P.mask_kind);
                 if (P.accumulate) x += dst[j];
                 v[j] = x;
             }
@@ -172,29 +184,36 @@ __global__ void __launch_bounds__(kThreads, 1) net_gemm_kernel(const GemmParams 
     }
 }
 
-// C (+)= epilogue( sum_z partial[z] ), fixed summation order (deterministic)
-__global__ void splitk_reduce_kernel(const float* __restrict__ part, int splits, float* __restrict__ c, int64_t ldc, int M, int N,
-                                     const float* __restrict__ bias, int act, const float* __restrict__ mask, int64_t ld_mask,
-                                     int mask_kind, int accumulate) {
-    const int64_t total = (int64_t)M * N;
-    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
+// C (+)= epilogue( sum_z partial[z] ) for every member, fixed summation order (deterministic).  partial = [members][splits][M][N].
+__global__ void splitk_reduce_kernel(const float* __restrict__ part, int splits, int batch, float* __restrict__ c, int64_t ldc,
+                                     int64_t stride_c, int M, int N, const float* __restrict__ bias, int64_t stride_bias, int act,
+                                     const float* __restrict__ mask, int64_t ld_mask, int64_t stride_mask, int mask_kind,
+                                     int accumulate) {
+    const int64_t per = (int64_t)M * N, total = per * batch;
+    for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t member = t / per, e = t - member * per;
         const int m = (int)(e / N), n = (int)(e - (int64_t)m * N);
+        const float* pm = part + member * splits * per;
         float x = 0.0f;
-        for (int z = 0; z < splits; ++z) x += part[(int64_t)z * total + e];
-        if (bias) x += __ldg(bias + n);
+        for (int z = 0; z < splits; ++z) x += pm[(int64_t)z * per + e];
+        if (bias) x += __ldg(bias + member * stride_bias + n);
         x = apply_act(x, act);
-        if (mask) x = apply_act_grad(x, __ldg(mask + (int64_t)m * ld_mask + n), mask_kind);
-        float* dst = c + (int64_t)m * ldc + n;
+        if (mask) x = apply_act_grad(x, __ldg(mask + member * stride_mask + (int64_t)m * ld_mask + n), mask_kind);
+        float* dst = c + member * stride_c + (int64_t)m * ldc + n;
         if (accumulate) x += *dst;
         *dst = x;
     }
 }
 
-// out[n] (+)= sum_m x[m * ld + n]   (bias gradients): block = 32 columns x 8 row lanes, fixed order
-__global__ void colsum_kernel(const float* __restrict__ x, int64_t ld, int M, int N, float* __restrict__ out, int accumulate) {
+// out[e * stride_out + n] (+)= sum_m x[e * stride_x + m * ld + n]   (bias gradients; blockIdx.y = member e): block = 32 columns
+// x 8 row lanes, fixed order
+__global__ void colsum_kernel(const float* __restrict__ x, int64_t ld, int64_t stride_x, int M, int N, float* __restrict__ out,
+                              int64_t stride_out, int accumulate) {
     __shared__ float s[8][33];
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
     const int n = blockIdx.x * 32 + lane;
+    x += (int64_t)blockIdx.y * stride_x;
+    out += (int64_t)blockIdx.y * stride_out;
     float acc = 0.0f;
     if (n < N) {
         for (int m = w; m < M; m += 8) acc += __ldg(x + (int64_t)m * ld + n);
@@ -209,15 +228,25 @@ __global__ void colsum_kernel(const float* __restrict__ x, int64_t ld, int M, in
     }
 }
 
+// out[i] (+)= sum_e x[e * stride + i], members in index order (the summed input gradient of an ensemble's first layer)
+__global__ void member_sum_kernel(const float* __restrict__ x, int batch, int64_t stride, int64_t n, float* __restrict__ out,
+                                  int accumulate) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        float t = x[i];
+        for (int e = 1; e < batch; ++e) t += x[(int64_t)e * stride + i];
+        out[i] = accumulate ? out[i] + t : t;
+    }
+}
+
 }  // namespace
 
 namespace tsb {
 
-size_t net_gemm_workspace_floats(int M, int N, int K, int* splits_out) {
+size_t net_gemm_workspace_floats(int batch, int M, int N, int K, int* splits_out) {
     // split-K whenever the output tiles alone leave most SMs idle: weight gradients over im2col rows (K = tens of thousands),
     // and every layer of a batch-256 MLP (4 output tiles, 4 .. 7 chunks: a lone CTA per tile would walk them one round trip
-    // after the other while the other SMs idle)
-    const int tiles = ((M + BM - 1) / BM) * ((N + BN - 1) / BN);
+    // after the other while the other SMs idle).  The tiles of all members count.
+    const int tiles = ((M + BM - 1) / BM) * ((N + BN - 1) / BN) * batch;
     const int chunks = (K + BK - 1) / BK;
     int splits = 1;
     if (chunks >= 2 && tiles < 64) {
@@ -225,12 +254,13 @@ size_t net_gemm_workspace_floats(int M, int N, int K, int* splits_out) {
         if (splits < 1) splits = 1;
     }
     if (splits_out) *splits_out = splits;
-    return splits > 1 ? (size_t)splits * M * N : 0;
+    return splits > 1 ? (size_t)batch * splits * M * N : 0;
 }
 
-int net_gemm(const float* a, int64_t lda, int a_mn, const float* b, int64_t ldb, int b_mn, float* c, int64_t ldc, int M, int N,
-             int K, const float* bias, int act, const float* mask, int64_t ld_mask, int mask_kind, int accumulate, float* workspace,
-             size_t workspace_floats, cudaStream_t st) {
+int net_gemm_batched(int batch, const float* a, int64_t lda, int a_mn, int64_t stride_a, const float* b, int64_t ldb, int b_mn,
+                     int64_t stride_b, float* c, int64_t ldc, int64_t stride_c, int M, int N, int K, const float* bias,
+                     int64_t stride_bias, int act, const float* mask, int64_t ld_mask, int64_t stride_mask, int mask_kind,
+                     int accumulate, float* workspace, size_t workspace_floats, cudaStream_t st) {
     static bool configured[kMaxDevices] = {};
     const int dev = device_ordinal();
     if (!configured[dev]) {
@@ -240,15 +270,17 @@ int net_gemm(const float* a, int64_t lda, int a_mn, const float* b, int64_t ldb,
         TS_CUDA(cudaFuncSetAttribute(net_gemm_kernel<1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
         configured[dev] = true;
     }
-    if (M <= 0 || N <= 0) return 0;
+    if (M <= 0 || N <= 0 || batch <= 0) return 0;
     GemmParams P;
     P.a = Operand{a, lda, a_mn, M};
     P.b = Operand{b, ldb, b_mn, N};
     P.c = c; P.ldc = ldc; P.M = M; P.N = N; P.K = K;
     P.bias = bias; P.act = act; P.mask = mask; P.ld_mask = ld_mask; P.mask_kind = mask_kind; P.accumulate = accumulate;
+    P.stride_a = stride_a; P.stride_b = stride_b; P.stride_c = stride_c; P.stride_bias = stride_bias; P.stride_mask = stride_mask;
     int splits = 1;
-    const size_t need = net_gemm_workspace_floats(M, N, K, &splits);
+    const size_t need = net_gemm_workspace_floats(batch, M, N, K, &splits);
     if (splits > 1 && (workspace == nullptr || workspace_floats < need)) splits = 1;     // no room: run unsplit
+    if ((int64_t)splits * batch > 65535) splits = 1;                                     // grid.z limit
     const int chunks = (K + BK - 1) / BK;
     P.splits = splits;
     P.k_per_split = splits > 1 ? ((chunks + splits - 1) / splits) * BK : K;
@@ -257,24 +289,31 @@ int net_gemm(const float* a, int64_t lda, int a_mn, const float* b, int64_t ldb,
         P.splits = splits;
         P.c = workspace;
     }
-    const dim3 grid((M + BM - 1) / BM, (N + BN - 1) / BN, splits);
+    const dim3 grid((M + BM - 1) / BM, (N + BN - 1) / BN, (unsigned)(splits * batch));
     if (a_mn && b_mn) net_gemm_kernel<1, 1><<<grid, kThreads, kSmemBytes, st>>>(P);
     else if (a_mn) net_gemm_kernel<1, 0><<<grid, kThreads, kSmemBytes, st>>>(P);
     else if (b_mn) net_gemm_kernel<0, 1><<<grid, kThreads, kSmemBytes, st>>>(P);
     else net_gemm_kernel<0, 0><<<grid, kThreads, kSmemBytes, st>>>(P);
     if (check_launch("ts_net_gemm")) return 1;
     if (splits > 1) {
-        const int64_t total = (int64_t)M * N;
-        splitk_reduce_kernel<<<(unsigned)imin((total + 255) / 256, num_sms() * 8), 256, 0, st>>>(workspace, splits, c, ldc, M, N, bias, act,
-                                                                                           mask, ld_mask, mask_kind, accumulate);
+        const int64_t total = (int64_t)M * N * batch;
+        splitk_reduce_kernel<<<(unsigned)imin((total + 255) / 256, num_sms() * 8), 256, 0, st>>>(
+            workspace, splits, batch, c, ldc, stride_c, M, N, bias, stride_bias, act, mask, ld_mask, stride_mask, mask_kind, accumulate);
         if (check_launch("ts_net_gemm/splitk")) return 1;
     }
     return 0;
 }
 
+int net_gemm(const float* a, int64_t lda, int a_mn, const float* b, int64_t ldb, int b_mn, float* c, int64_t ldc, int M, int N,
+             int K, const float* bias, int act, const float* mask, int64_t ld_mask, int mask_kind, int accumulate, float* workspace,
+             size_t workspace_floats, cudaStream_t st) {
+    return net_gemm_batched(1, a, lda, a_mn, 0, b, ldb, b_mn, 0, c, ldc, 0, M, N, K, bias, 0, act, mask, ld_mask, 0, mask_kind,
+                            accumulate, workspace, workspace_floats, st);
+}
+
 int net_colsum(const float* x, int64_t ld, int M, int N, float* out, int accumulate, cudaStream_t st) {
     if (N <= 0) return 0;
-    colsum_kernel<<<(N + 31) / 32, 256, 0, st>>>(x, ld, M, N, out, accumulate);
+    colsum_kernel<<<(N + 31) / 32, 256, 0, st>>>(x, ld, 0, M, N, out, 0, accumulate);
     return check_launch("ts_net_colsum");
 }
 
@@ -292,10 +331,48 @@ extern "C" int ts_net_gemm(const float* a, int64_t lda, int32_t a_mn_major, cons
 }
 
 extern "C" int64_t ts_net_gemm_workspace_floats(int32_t M, int32_t N, int32_t K) {
-    return (int64_t)tsb::net_gemm_workspace_floats(M, N, K, nullptr);
+    return (int64_t)tsb::net_gemm_workspace_floats(1, M, N, K, nullptr);
+}
+
+extern "C" int ts_net_gemm_batched(int32_t batch, const float* a, int64_t lda, int32_t a_mn_major, int64_t stride_a, const float* b,
+                                   int64_t ldb, int32_t b_mn_major, int64_t stride_b, float* c, int64_t ldc, int64_t stride_c,
+                                   int32_t M, int32_t N, int32_t K, const float* bias, int64_t stride_bias, int32_t act,
+                                   const float* act_grad_src, int64_t ld_mask, int64_t stride_mask, int32_t act_grad_kind,
+                                   int32_t accumulate, float* workspace, int64_t workspace_floats, ts_stream_t stream) {
+    TS_REQUIRE(a && b && c && batch >= 0 && M >= 0 && N >= 0 && K >= 0, "ts_net_gemm_batched: null pointer / negative size");
+    TS_REQUIRE(stride_a >= 0 && stride_b >= 0 && stride_c >= 0 && stride_bias >= 0 && stride_mask >= 0,
+               "ts_net_gemm_batched: negative member stride");
+    TS_REQUIRE(batch <= 65535, "ts_net_gemm_batched: %d members exceed the grid", batch);
+    TS_REQUIRE(act >= TS_ACT_NONE && act <= TS_ACT_TANH, "ts_net_gemm_batched: unknown activation %d", act);
+    TS_REQUIRE(!act_grad_src || act_grad_kind == TS_ACT_RELU || act_grad_kind == TS_ACT_TANH,
+               "ts_net_gemm_batched: unknown act_grad_kind %d", act_grad_kind);
+    return tsb::net_gemm_batched(batch, a, lda, a_mn_major, stride_a, b, ldb, b_mn_major, stride_b, c, ldc, stride_c, M, N, K, bias,
+                                 stride_bias, act, act_grad_src, ld_mask, stride_mask, act_grad_kind, accumulate, workspace,
+                                 (size_t)(workspace_floats > 0 ? workspace_floats : 0), tsb::as_stream(stream));
+}
+
+extern "C" int64_t ts_net_gemm_batched_workspace_floats(int32_t batch, int32_t M, int32_t N, int32_t K) {
+    return batch > 0 ? (int64_t)tsb::net_gemm_workspace_floats(batch, M, N, K, nullptr) : 0;
 }
 
 extern "C" int ts_net_colsum(const float* x, int64_t ld, int32_t M, int32_t N, float* out, int32_t accumulate, ts_stream_t stream) {
     TS_REQUIRE(x && out, "ts_net_colsum: null pointer");
     return tsb::net_colsum(x, ld, M, N, out, accumulate, tsb::as_stream(stream));
+}
+
+extern "C" int ts_net_colsum_batched(int32_t batch, const float* x, int64_t ld, int64_t stride_x, int32_t M, int32_t N, float* out,
+                                     int64_t stride_out, int32_t accumulate, ts_stream_t stream) {
+    TS_REQUIRE(x && out && batch >= 0 && batch <= 65535, "ts_net_colsum_batched: bad argument");
+    if (N <= 0 || batch == 0) return 0;
+    colsum_kernel<<<dim3((N + 31) / 32, batch), 256, 0, tsb::as_stream(stream)>>>(x, ld, stride_x, M, N, out, stride_out, accumulate);
+    return tsb::check_launch("ts_net_colsum_batched");
+}
+
+extern "C" int ts_net_member_sum(const float* x, int32_t batch, int64_t stride, int64_t n, float* out, int32_t accumulate,
+                                 ts_stream_t stream) {
+    TS_REQUIRE(x && out && batch >= 1 && n >= 0 && stride >= 0, "ts_net_member_sum: bad argument");
+    if (n == 0) return 0;
+    member_sum_kernel<<<(unsigned)tsb::imin((n + 255) / 256, (int64_t)tsb::num_sms() * 8), 256, 0, tsb::as_stream(stream)>>>(
+        x, batch, stride, n, out, accumulate);
+    return tsb::check_launch("ts_net_member_sum");
 }

@@ -117,6 +117,28 @@ class Net(ModuleWithVectorOutput):
         return logits, state
 
 
+class EnsembleLinear(nn.Module):
+    """``ensemble_size`` Linear layers applied side by side (common.py:518-550): ``x @ weight + bias_weights`` with
+    ``weight [E, in, out]`` and ``bias_weights [E, 1, out]``, so a ``[B, in]`` input gives ``[E, B, out]`` and an
+    ``[E, B, in]`` input maps member by member.  Initialised like the reference, uniform in +-sqrt(1 / in)."""
+
+    def __init__(self, ensemble_size: int, in_feature: int, out_feature: int, bias: bool = True) -> None:
+        super().__init__()
+        k = np.sqrt(1.0 / in_feature)
+        weight_data = torch.rand((ensemble_size, in_feature, out_feature)) * 2 * k - k
+        self.weight = nn.Parameter(weight_data, requires_grad=True)
+        self.bias_weights: nn.Parameter | None = None
+        if bias:
+            bias_data = torch.rand((ensemble_size, 1, out_feature)) * 2 * k - k
+            self.bias_weights = nn.Parameter(bias_data, requires_grad=True)
+
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        x = torch.matmul(x, self.weight)
+        if self.bias_weights is not None:
+            x = x + self.bias_weights
+        return x
+
+
 class ActorCritic(nn.Module):
     """Parameter holder so one optimizer covers actor and critic (common.py:457-470)."""
 
