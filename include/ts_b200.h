@@ -693,6 +693,26 @@ int ts_redq_critic_rows(const float* q, const float* target, const float* weight
 int ts_redq_actor_rows(const float* q, const float* logp, int32_t E, int64_t B, float alpha, float* dq, float* rows, float* loss,
                        ts_stream_t stream);
 
+/* ---- BDQN (bdqn.cu) ---- */
+/* The 1-step target of BDQN (modelfree/bdqn.py:126-175) from a branching network's value output v [B][1] and branch scores
+ * s [nb][B][A] (Q = v + (s - mean_a s)) on s': per branch the first arg-max a*_k of the selecting network's Q (v_sel, s_sel: the
+ * online network when double, else the lagged one) read from the evaluating network's Q (v_val, s_val);
+ * y[b] = fp32(rew[i] + fp32(gamma * m) * (1 - end[i])), i = idx[b], m = the fp32 mean over branches summed in numpy's order
+ * (pairwise over blocks of 8, exact for up to 128 branches), rew the buffer's float64 column, end its end flags (done, or an
+ * unfinished episode's last slot).  y_branch [B][nb] (nullable): the per-branch targets fp32(rew + fp32(gamma * Q'_k) (1 - end)).
+ * Any B (grid-stride). */
+int ts_bdqn_target(const float* v_sel, const float* s_sel, const float* v_val, const float* s_val, int64_t B, int32_t nb,
+                   int32_t A, float gamma, const double* rew, const uint8_t* end, const int64_t* idx, float* y, float* y_branch,
+                   ts_stream_t stream);
+/* BDQN's loss (bdqn.py:177-196) on v [B][1], s [nb][B][A], act [B][nb] (each in [0, A)), y [B] and weight [B] (nullable: 1):
+ * td [B][nb] = y - Q at the chosen action of each branch, rows [B] = w mean_k td^2 (scratch), td_sum [B] = sum_k td (signed: the
+ * prioritised buffer's batch.weight), *loss = mean(rows) in a fixed order, and the gradients of the dueling combine:
+ * ds [nb][B][A] = g - mean_a g and dv [B] = sum_k g, g = -2 w td / (nb B) at the chosen action.  y_branch (B = 1 only, nullable):
+ * adds the population variance of the per-branch targets to *loss, as the reference's [nb, nb, A] broadcast does. */
+int ts_bdqn_rows(const float* v, const float* s, const int64_t* act, const float* y, const float* weight, const float* y_branch,
+                 int64_t B, int32_t nb, int32_t A, float* td, float* rows, float* td_sum, float* ds, float* dv, float* loss,
+                 ts_stream_t stream);
+
 /* ---- BCQ (bcq.cu) ---- */
 /* The VAE's reparameterisation (utils/net/continuous.py:464-470): from head = [mean | log_std_raw] [B][2L] and eps [B][L],
  * std = exp(clamp(log_std_raw, -4, 15)) into std_out [B][L] and z = mean + std * eps straight into the decoder input

@@ -57,18 +57,25 @@ def describe_discrete_head(net: Any, role: str) -> tuple[Any, Any, tuple[int, ..
 
 
 def sample_discrete(buffer: ReplayBuffer, sample_size: int | None, obs_source: Callable[..., DeviceObsSource],
-                    device: torch.device, n_actions: int) -> tuple[Batch, Any]:
+                    device: torch.device, n_actions: int, branches: int | None = None) -> tuple[Batch, Any]:
     """Indices from the buffer's host RNG streams (identical to the reference's draws); the observations as
     ``obs_source(buffer, indices, "obs")`` reads them on the device, the actions as int64 device rows, the importance weight
     of a prioritised buffer.  The loss kernels index a row of ``n_actions`` values with each drawn action: an action outside
-    ``[0, n_actions)`` is refused here, before anything is launched."""
+    ``[0, n_actions)`` is refused here, before anything is launched.  ``branches``: multi-discrete actions, one per branch, as
+    ``[B, branches]`` rows; a buffer whose action rows have another shape is refused before the index draw."""
+    if branches is not None:
+        shape = np.shape(buffer.act)[1:]
+        if shape != (branches,):
+            raise ValueError(f"the buffer holds action rows of shape {shape}, the network has {branches} branches: rows of "
+                             f"{branches} actions expected")
     indices = buffer.sample_indices(sample_size)
     act = np.asarray(buffer.act)[indices]
     if act.size and (act.min() < 0 or act.max() >= n_actions):
         raise ValueError(f"the buffer holds actions in [{act.min()}, {act.max()}], the networks have {n_actions} outputs")
     batch = Batch()
     batch.__dict__["obs"] = obs_source(buffer, indices, "obs")
-    batch.__dict__["act"] = to_device(np.ascontiguousarray(act.reshape(-1)).astype(np.int64), device)
+    act = act.reshape(-1) if branches is None else act.reshape(len(act), branches)
+    batch.__dict__["act"] = to_device(np.ascontiguousarray(act).astype(np.int64), device)
     weight = per_weight(buffer, indices, device)
     if weight is not None:
         batch.__dict__["weight"] = weight

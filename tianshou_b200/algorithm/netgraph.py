@@ -5,7 +5,8 @@ A ``FusedStack`` is the kernel-side view of a torch module stack made of ``nn.Li
 utils/net/common.py:76-369, utils/net/continuous.py:96-238, env/atari/atari_network.py:60-122): every layer's
 forward, input gradient and weight gradient is ONE ``ts_net_gemm`` launch (wgmma, fp32-faithful), convolutions
 run as implicit GEMM over im2col rows.  A chain of ``EnsembleLinear`` layers (utils/net/common.py, REDQ's critic ensemble)
-runs every member of a layer in one batched launch (``ts_net_gemm_batched``) on ``[E, rows, features]`` activations.  Parameters live in a ``FlatGroup`` (flat_params.py: one flat fp32 buffer per optimiser,
+runs every member of a layer in one batched launch (``ts_net_gemm_batched``) on ``[E, rows, features]`` activations, and so do
+the identical ``nn.Linear`` MLPs of a ``ModuleList`` read as one ensemble (``compile_branches``: BDQN's action branches).  Parameters live in a ``FlatGroup`` (flat_params.py: one flat fp32 buffer per optimiser,
 ``nn.Parameter``s are views of it) so Adam and the Polyak update are single kernels and ``state_dict()`` keeps
 working.  There is no autograd graph and no eager-PyTorch path: unsupported layers raise ``UnsupportedModelError``.
 """
@@ -48,11 +49,22 @@ class _Layer:
     Wo: int = 0
     # ensemble: members E; weight [E, in, out] (W_e[k * out + n]), bias [E, 1, out]
     E: int = 0
+    # an ensemble of nn.Linear members (compile_branches): member e's (weight [out, in], bias [out]); ``weight`` / ``bias`` are
+    # member 0's, and the flat group holds the members' weights, then their biases, back to back (layer_params)
+    members: list[tuple[nn.Parameter, nn.Parameter]] | None = None
 
 
 def layer_params(layers: list[_Layer]) -> list[nn.Parameter]:
-    """Every weight and bias of ``layers``, in layer order: the flat order of a ``FlatGroup`` over the chain."""
-    return [p for L in layers if L.weight is not None for p in (L.weight, L.bias)]
+    """Every weight and bias of ``layers``, in layer order: the flat order of a ``FlatGroup`` over the chain.  The members of an
+    ``nn.Linear`` ensemble layer come weights first, then biases, so member e sits ``e * in * out`` (``e * out``) floats after
+    member 0: the uniform member stride of the batched GEMM."""
+    out: list[nn.Parameter] = []
+    for L in layers:
+        if L.members is not None:
+            out += [w for w, _ in L.members] + [b for _, b in L.members]
+        elif L.weight is not None:
+            out += [L.weight, L.bias]
+    return out
 
 
 def _activation_code(m: nn.Module) -> int:
@@ -141,6 +153,23 @@ def compile_sequential(mods: list[nn.Module], input_shape: tuple[int, ...], ense
     return layers
 
 
+def compile_branches(branches: nn.ModuleList, in_dim: int) -> list[_Layer]:
+    """``branches`` -- a ``ModuleList`` of identically shaped MLPs of ``nn.Linear`` + ReLU / Tanh, all reading the same
+    ``[rows, in_dim]`` input -- as one ensemble chain of ``len(branches)`` members.  Each member keeps ``nn.Linear``'s ``[out, in]``
+    weight layout; every layer's forward, weight gradient and input gradient is one batched launch."""
+    if len(branches) == 0:
+        raise UnsupportedModelError("an ensemble of branches needs at least one branch")
+    chains = [compile_sequential(module_layers(b), (in_dim,)) for b in branches]
+    sig = [(L.kind, L.in_dim, L.out_dim, L.act) for L in chains[0]]
+    if any(L.kind != "linear" for L in chains[0]):
+        raise UnsupportedModelError("branches must be MLPs of nn.Linear layers")
+    for k, c in enumerate(chains[1:], 1):
+        if [(L.kind, L.in_dim, L.out_dim, L.act) for L in c] != sig:
+            raise UnsupportedModelError(f"branch {k} differs in shape or activations from branch 0: {sig}")
+    return [_Layer("ensemble", L.weight, L.bias, L.act, L.in_dim, L.out_dim, E=len(chains),
+                   members=[(c[i].weight, c[i].bias) for c in chains]) for i, L in enumerate(chains[0])]
+
+
 def _out_shape(layers: list[_Layer], shape: tuple[int, ...]) -> tuple[int, ...]:
     for L in layers:
         if L.kind == "linear":
@@ -163,6 +192,13 @@ class FusedStack:
         self._bufs: dict[tuple, torch.Tensor] = {}
         self._ws_sizes: dict[tuple[int, int, int], int] = {}
         self._lib = load_library()
+        for L in layers:
+            if L.members is not None:
+                w0, b0 = group.offset(L.weight), group.offset(L.bias)
+                if any(group.offset(w) != w0 + e * L.in_dim * L.out_dim or group.offset(b) != b0 + e * L.out_dim
+                       for e, (w, b) in enumerate(L.members)):
+                    raise UnsupportedModelError(f"{name}: the flat group does not hold the members of a layer at a uniform "
+                                                "stride (build it from layer_params)")
 
     # ------------------------------------------------------------------ scratch
     def _buf(self, key: tuple, n: int) -> torch.Tensor:
@@ -219,7 +255,8 @@ class FusedStack:
             elif L.kind == "ensemble":      # [E, rows, out]; the first layer reads the shared [rows, in] input
                 n_out = L.E * rows * L.out_dim
                 y = self._buf((tag, "y", i), n_out)[:n_out].view(L.E, rows, L.out_dim)
-                self._gemm_batched(L.E, ptr(cur), L.in_dim, 0, 0 if i == 0 else rows * L.in_dim, self._w(L, params), L.out_dim, 1,
+                ldw, w_mn = (L.in_dim, 0) if L.members is not None else (L.out_dim, 1)
+                self._gemm_batched(L.E, ptr(cur), L.in_dim, 0, 0 if i == 0 else rows * L.in_dim, self._w(L, params), ldw, w_mn,
                                    L.in_dim * L.out_dim, ptr(y), L.out_dim, rows * L.out_dim, rows, L.out_dim, L.in_dim,
                                    bias=self._b(L, params), s_bias=L.out_dim, act=L.act)
             elif L.kind == "conv":
@@ -312,8 +349,12 @@ class FusedStack:
                 if param_grads:
                     gw = g.grad.data_ptr() + 4 * g.offset(L.weight)
                     gb = g.grad.data_ptr() + 4 * g.offset(L.bias)
-                    self._gemm_batched(L.E, ptr(x_in), L.in_dim, 1, s_x, ptr(dz), L.out_dim, 1, s_z, gw, L.out_dim,
-                                       L.in_dim * L.out_dim, L.in_dim, L.out_dim, rows)
+                    if L.members is not None:       # dW_e [out, in] = dz_e^T x_e
+                        self._gemm_batched(L.E, ptr(dz), L.out_dim, 1, s_z, ptr(x_in), L.in_dim, 1, s_x, gw, L.in_dim,
+                                           L.in_dim * L.out_dim, L.out_dim, L.in_dim, rows)
+                    else:                           # dW_e [in, out] = x_e^T dz_e
+                        self._gemm_batched(L.E, ptr(x_in), L.in_dim, 1, s_x, ptr(dz), L.out_dim, 1, s_z, gw, L.out_dim,
+                                           L.in_dim * L.out_dim, L.in_dim, L.out_dim, rows)
                     call("ts_net_colsum_batched", L.E, ptr(dz), L.out_dim, s_z, rows, L.out_dim, gb, L.out_dim, 0, st)
                 if need_dx:
                     lo, hi = (0, L.in_dim) if (i > 0 or input_cols is None) else input_cols
@@ -321,7 +362,9 @@ class FusedStack:
                     n_dx = L.E * rows * width
                     dx = self._buf((tag, "dx", i), n_dx)[:n_dx].view(L.E, rows, width)
                     mask = ptr(act_src) + 4 * lo if prev_act != ACT_NONE else None
-                    self._gemm_batched(L.E, ptr(dz), L.out_dim, 0, s_z, self._w(L) + 4 * lo * L.out_dim, L.out_dim, 0,
+                    w_lo, ldw, w_mn = ((self._w(L) + 4 * lo, L.in_dim, 1) if L.members is not None
+                                       else (self._w(L) + 4 * lo * L.out_dim, L.out_dim, 0))
+                    self._gemm_batched(L.E, ptr(dz), L.out_dim, 0, s_z, w_lo, ldw, w_mn,
                                        L.in_dim * L.out_dim, ptr(dx), width, rows * width, rows, width, L.out_dim, mask=mask,
                                        ld_mask=L.in_dim, s_mask=s_x, mask_kind=prev_act if prev_act != ACT_NONE else ACT_RELU)
                     if i == 0:      # d loss / d input of the shared input: the members' gradients summed in member order

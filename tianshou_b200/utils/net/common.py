@@ -1,4 +1,4 @@
-"""MLP / Net building blocks (API of tianshou/utils/net/common.py:76-369, :457-470).
+"""MLP / Net building blocks (API of tianshou/utils/net/common.py:76-369, :457-470, :553-674).
 
 These are ordinary ``nn.Module``s: the Collector runs them for action inference and
 ``state_dict()`` round-trips unchanged.  The device updates do not call them -- they read the very
@@ -137,6 +137,38 @@ class EnsembleLinear(nn.Module):
         if self.bias_weights is not None:
             x = x + self.bias_weights
         return x
+
+
+class BranchingNet(nn.Module):
+    """Branching dueling Q-network of BDQN (common.py:553-674, arXiv:1711.08946): a shared trunk ``common`` (an MLP ending in
+    its last hidden layer's activation), a state-value MLP ``value`` with one output, and ``num_branches`` identical action MLPs
+    ``branches`` with ``action_per_branch`` outputs each, all reading the trunk.  ``forward`` gives ``[B, num_branches,
+    action_per_branch]`` Q-values ``value + (scores - scores.mean(2))``.  An empty ``common_hidden_sizes`` fails here, as in the
+    reference."""
+
+    def __init__(self, *, state_shape: int | Sequence[int], num_branches: int = 0, action_per_branch: int = 2,
+                 common_hidden_sizes: list[int] | None = None, value_hidden_sizes: list[int] | None = None,
+                 action_hidden_sizes: list[int] | None = None, norm_layer: ModuleType | None = None, norm_args: Any = None,
+                 activation: ModuleType | None = nn.ReLU, act_args: Any = None) -> None:
+        super().__init__()
+        common_hidden_sizes = common_hidden_sizes or []
+        value_hidden_sizes = value_hidden_sizes or []
+        action_hidden_sizes = action_hidden_sizes or []
+        self.num_branches = num_branches
+        self.action_per_branch = action_per_branch
+        kw = dict(norm_layer=norm_layer, norm_args=norm_args, activation=activation, act_args=act_args)
+        self.common = MLP(input_dim=int(np.prod(state_shape)), output_dim=0, hidden_sizes=common_hidden_sizes, **kw)
+        self.value = MLP(input_dim=common_hidden_sizes[-1], output_dim=1, hidden_sizes=value_hidden_sizes, **kw)
+        self.branches = nn.ModuleList([
+            MLP(input_dim=common_hidden_sizes[-1], output_dim=action_per_branch, hidden_sizes=action_hidden_sizes, **kw)
+            for _ in range(self.num_branches)])
+
+    def forward(self, obs: Any, state: Any = None, info: dict | None = None) -> tuple[torch.Tensor, Any]:
+        common_out = self.common(obs)
+        value_out = torch.unsqueeze(self.value(common_out), 1)
+        action_scores = torch.stack([b(common_out) for b in self.branches], 1)
+        action_scores = action_scores - torch.mean(action_scores, 2, keepdim=True)
+        return value_out + action_scores, state
 
 
 class ActorCritic(nn.Module):
