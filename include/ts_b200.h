@@ -813,6 +813,30 @@ int ts_qrdqn_target(const float* q_online, const float* q_next, int64_t B, int32
 int ts_qrdqn_rows(const float* q, const int64_t* act, const float* returns, const float* tau_hat, const float* weight, int64_t B,
                   int32_t A, int32_t N, float min_q_weight, float* dq, float* prio, float* rows, float* losses, ts_stream_t stream);
 
+/* ---- C51 (c51.cu) ---- */
+/* C51's target distribution (modelfree/c51.py:113-124 with compute_q_value = (p * support).sum(2), :62-63): logits_online,
+ * logits_next [B][A][N] are the network's raw last-layer outputs at s_{t+n} (logits_next the lagged network's, or logits_online
+ * itself); per row b, p_a = softmax over the N atoms of logits_online[b][a], Q_a = sum_k p_ak support[k] in fp32,
+ * a* = argmax_a Q_a with torch.argmax's rule (lowest index among ties, a NaN is the maximum), next_dist [B][N] =
+ * softmax(logits_next[b][a*]); act_out [B] (nullable) = a*.  One warp per row, grid-stride; any A >= 1, N >= 2, B >= 0 (B == 0
+ * launches nothing). */
+int ts_c51_target(const float* logits_online, const float* logits_next, const float* support, int64_t B, int32_t A, int32_t N,
+                  float* next_dist, int64_t* act_out, ts_stream_t stream);
+/* The categorical cross-entropy of C51 (c51.py:125-160) on logits [B][A][N] at s (raw: the softmax is taken here), the n-step
+ * returns [B][N] (r + gamma^n support * mask), support [N], next_dist [B][N] from ts_c51_target and the importance weight [B]
+ * (nullable: 1).  With t_k = clamp(returns[b][k], v_min, v_max), target_j = sum_k clamp(1 - |t_k - support_j| / delta_z, 0, 1)
+ * next_dist[b][k] (the reference's dense projection, k summed in order), p = softmax(logits[b][act[b]]):
+ * CE_b = -sum_j target_j log(p_j + 1e-8), prio [B] = CE_b (unweighted); losses[4] = (loss, loss, mean_b CE_b, 0) with
+ * loss = mean_b(weight_b CE_b).  dlogits [B][A][N] = d loss / d logits, every element written: with
+ * g_j = -(weight_b / B) target_j / (p_j + 1e-8), the taken block gets p_k (g_k - sum_j p_j g_j), every other block 0; the target
+ * carries no gradient.  act must lie in [0, A): the caller checks it.  rows [3][B] is scratch.  One block per row (threads over
+ * the atoms, four arrays of N floats in shared memory), grid-stride, then one block summing the rows in a fixed order, no
+ * atomics: two calls on the same input are bit-identical.  Any B >= 1, A >= 1, 2 <= N <= 3072, delta_z > 0, v_min <= v_max;
+ * anything else is refused. */
+int ts_c51_rows(const float* logits, const int64_t* act, const float* returns, const float* support, float v_min, float v_max,
+                float delta_z, const float* next_dist, const float* weight, int64_t B, int32_t A, int32_t N, float* dlogits,
+                float* prio, float* rows, float* losses, ts_stream_t stream);
+
 /* ---- IQN (iqn.cu) ---- */
 /* The network of IQN (utils/net/discrete.py:163-216) is a trunk on B rows (feat [B][D]), the cosine embedding of S fractions per
  * row and a head on the B * S rows h[b * S + s] = feat[b] * e[b * S + s], sample-major, so the head's output is q [B][S][A].  The

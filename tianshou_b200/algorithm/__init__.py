@@ -5,6 +5,7 @@ from .imitation import (BCQ, CQL, GAIL, TD3BC, BCQPolicy, BCQTrainingStats, CQLT
                         GailTrainingStats)
 from .modelfree.a2c import A2CTrainingStats, ActorCriticOnPolicyAlgorithm
 from .modelfree.bdqn import BDQN, BDQNPolicy
+from .modelfree.c51 import C51, C51Policy
 from .modelfree.discrete_sac import DiscreteSAC
 from .modelfree.fqf import FQF, FQFPolicy, FQFTrainingStats
 from .modelfree.iqn import IQN, IQNPolicy
@@ -24,5 +25,5 @@ __all__ = [
     "ProbabilisticActorPolicy", "DiscreteActorPolicy", "AdamOptimizerFactory", "LRSchedulerFactoryLinear", "OptimizerFactory",
     "RMSpropOptimizerFactory", "DiscreteBCQ", "DiscreteBCQPolicy", "DiscreteBCQTrainingStats", "DiscreteCRR",
     "DiscreteCRRTrainingStats", "QRDQN", "QRDQNPolicy", "DiscreteCQL", "DiscreteCQLTrainingStats", "IQN", "IQNPolicy",
-    "FQF", "FQFPolicy", "FQFTrainingStats", "REDQ", "REDQPolicy", "REDQTrainingStats", "BDQN", "BDQNPolicy",
+    "FQF", "FQFPolicy", "FQFTrainingStats", "REDQ", "REDQPolicy", "REDQTrainingStats", "BDQN", "BDQNPolicy", "C51", "C51Policy",
 ]

@@ -19,7 +19,7 @@ from .._cabi import to_device
 from ..data import Batch, ReplayBuffer
 from .base import Algorithm
 from .flat_params import DeviceScratch, FlatGroup, UnsupportedModelError
-from .netgraph import module_layers
+from .netgraph import ACT_NONE, compile_sequential, module_layers
 from .obs_source import DeviceObsSource, device_obs_source
 from .twin_critic import per_weight
 
@@ -38,6 +38,18 @@ def describe_q_network(model: Any) -> tuple[Any, tuple[int, ...], float]:
     if isinstance(first, nn.Linear):
         return inner, (int(first.in_features),), scale
     raise UnsupportedModelError(f"cannot infer the input shape of {type(inner).__name__}")
+
+
+def atom_chain(inner: Any, in_shape: tuple[int, ...], n_actions: int, n_atoms: int, kind: str, atom_name: str) -> list:
+    """The layer chain of a distributional Q-network (QR-DQN's quantiles, C51's atoms): ``inner`` read as a plain chain ending in
+    ``Linear(., n_actions * n_atoms)`` with no activation, the output viewed as ``[B, n_actions, n_atoms]``; anything else is
+    refused.  ``kind`` names the network, ``atom_name`` the per-action outputs (``num_<atom_name>`` is the keyword)."""
+    layers = compile_sequential(module_layers(inner), in_shape)
+    if layers[-1].kind != "linear" or layers[-1].act != ACT_NONE:
+        raise UnsupportedModelError(f"the {kind} network must end in a linear layer over actions * num_{atom_name}")
+    if layers[-1].out_dim != n_actions * n_atoms:
+        raise UnsupportedModelError(f"the network has {layers[-1].out_dim} outputs, not {n_actions} actions x {n_atoms} {atom_name}")
+    return layers
 
 
 def describe_discrete_head(net: Any, role: str) -> tuple[Any, Any, tuple[int, ...], float]:

@@ -76,12 +76,16 @@ def optimizer_hyperparams(optimizer: torch.optim.Optimizer, *, rmsprop: bool = T
                 weight_decay=float(g["weight_decay"]))
 
 
-def bind_optimizer(optim: Any, group: FlatGroup, *, rmsprop: bool = False) -> None:
+def bind_optimizer(optim: Any, group: FlatGroup, *, rmsprop: bool = False, frozen: tuple[nn.Parameter, ...] = ()) -> None:
     """Let ``group`` hold the state of ``optim`` (an ``Algorithm.Optimizer``): the kernels step the flat buffers with the
     torch optimiser's hyper-parameters, and ``state_dict()`` / ``load_state_dict()`` go through ``group``.  ``rmsprop``:
-    the caller steps through ``FlatGroup.optimizer_step`` or the actor-critic kernels, which also take torch RMSprop."""
+    the caller steps through ``FlatGroup.optimizer_step`` or the actor-critic kernels, which also take torch RMSprop.
+    ``frozen``: parameters with ``requires_grad=False`` that the optimiser lists but never steps (C51's ``support``); they
+    keep their place in its param group, get no state and stay out of ``group``."""
     optimizer_hyperparams(optim._optim, rmsprop=rmsprop)
-    if set(map(id, optim._optim.param_groups[0]["params"])) != set(map(id, group.params)):
+    if any(p.requires_grad for p in frozen):
+        raise UnsupportedModelError("a parameter the optimiser may skip must have requires_grad=False")
+    if set(map(id, optim._optim.param_groups[0]["params"])) != set(map(id, group.params)) | set(map(id, frozen)):
         raise UnsupportedModelError("optimizer parameters differ from the fused network's parameters")
     optim._flat = group
 

@@ -25,9 +25,9 @@ from torch import nn
 from ..._cabi import call, ptr, stream_ptr
 from ...data import Batch, ReplayBuffer
 from ..base import OffPolicyAlgorithm
-from ..discrete_q import DiscreteQCore, describe_q_network, lagged_group
+from ..discrete_q import DiscreteQCore, atom_chain, describe_q_network, lagged_group
 from ..flat_params import FlatGroup, UnsupportedModelError, bind_optimizer
-from ..netgraph import ACT_NONE, FusedStack, compile_sequential, layer_params, module_layers
+from ..netgraph import FusedStack, layer_params
 from ..optim import OptimizerFactory
 from ..twin_critic import _EvalModeModule, cuda_device_of, pop_batch_weight
 from .dqn import DiscreteQLearningPolicy, SimpleLossTrainingStats
@@ -81,13 +81,8 @@ class QRDQN(DiscreteQCore, OffPolicyAlgorithm):
         if getattr(inner, "softmax", False):
             raise UnsupportedModelError("Net(softmax=True): QR-DQN reads the network output as quantiles; build it with "
                                         "softmax=False")
-        layers = compile_sequential(module_layers(inner), in_shape)
-        if layers[-1].kind != "linear" or layers[-1].act != ACT_NONE:
-            raise UnsupportedModelError("the quantile network must end in a linear layer over actions * num_quantiles")
         n_actions = int(policy.action_space.n)
-        if layers[-1].out_dim != n_actions * self.num_quantiles:
-            raise UnsupportedModelError(f"the network has {layers[-1].out_dim} outputs, not {n_actions} actions x "
-                                        f"{self.num_quantiles} quantiles")
+        layers = atom_chain(inner, in_shape, n_actions, self.num_quantiles, "quantile", "quantiles")
         self._init_discrete(dev, in_shape, in_scale, n_actions)
         self._group = FlatGroup(layer_params(layers), dev)
         self._net = FusedStack(layers, self._group, "qr")

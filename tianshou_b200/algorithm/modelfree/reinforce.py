@@ -3,15 +3,23 @@ from __future__ import annotations
 
 import warnings
 from collections.abc import Callable
+from dataclasses import dataclass
 from typing import Any, Literal
 
 import numpy as np
 import torch
 
-from ...data import Batch
-from ..base import Policy
+from ...data import Batch, SequenceSummaryStats
+from ..base import Policy, TrainingStats
 
 TDistFn = Callable[..., torch.distributions.Distribution]
+
+
+@dataclass(kw_only=True)
+class LossSequenceTrainingStats(TrainingStats):
+    """The loss of an update (reinforce.py:58-60); C51 fills it with a float, as the reference does."""
+
+    loss: SequenceSummaryStats
 
 
 class ProbabilisticActorPolicy(Policy):

@@ -83,3 +83,18 @@ class QRDQNet(DQNet):
     def forward(self, obs: Any, state: Any = None, info: dict | None = None) -> tuple[torch.Tensor, Any]:
         obs, state = super().forward(obs)
         return obs.view(-1, self.action_num, self.num_quantiles), state
+
+
+class C51Net(DQNet):
+    """A distributional perspective on reinforcement learning (atari_network.py:125-151): a ``DQNet`` whose last Linear has
+    ``actions * num_atoms`` outputs, a softmax over each action's atoms, returned as ``[B, actions, num_atoms]``."""
+
+    def __init__(self, *, c: int, h: int, w: int, action_shape: Sequence[int] | int, num_atoms: int = 51) -> None:
+        self.action_num = int(np.prod(action_shape))
+        super().__init__(c=c, h=h, w=w, action_shape=[self.action_num * num_atoms])
+        self.num_atoms = num_atoms
+
+    def forward(self, obs: Any, state: Any = None, info: dict | None = None) -> tuple[torch.Tensor, Any]:
+        obs, state = super().forward(obs)
+        obs = obs.view(-1, self.num_atoms).softmax(dim=-1)
+        return obs.view(-1, self.action_num, self.num_atoms), state
