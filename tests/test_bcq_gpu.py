@@ -4,38 +4,23 @@ steps against float64 autograd of the eager restatement, the lagged perturbation
 inside the update, ``state_dict()`` round trips, the refusals, the device policy path against the reference loop and the kernels'
 register report."""
 import copy
-import os
 import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
-from test_oracle_bcq import _cfg, check_params, oracle_batch, oracle_nets
+from offpolicy_testutil import DEV, Box, Discrete, assert_spill_free, golden_cfg, ptxas_report, stream
+from test_oracle_bcq import check_net_params, oracle_batch, oracle_nets
 from ts_testutil import load_golden, record_parity
 
-DEV = "cuda:0"
 gpu = pytest.mark.gpu
 BIG = 300000                 # rows past the grid cap of every grid-stride kernel
 
 
-class _Box:
-    def __init__(self, dim, m=1.0):
-        self.shape = (dim,)
-        self.low = -m * np.ones(dim, np.float32)
-        self.high = m * np.ones(dim, np.float32)
-
-
-def _st():
-    from tianshou_b200._cabi import stream_ptr
-    return stream_ptr(torch.device(DEV))
-
-
 def _call(name, *args):
     from tianshou_b200._cabi import call, ptr
-    call(name, *[ptr(a) if isinstance(a, torch.Tensor) else a for a in args], _st())
+    call(name, *[ptr(a) if isinstance(a, torch.Tensor) else a for a in args], stream())
     torch.cuda.synchronize()
 
 
@@ -186,7 +171,7 @@ def test_select_kernel_first_argmax_with_nan(G, S, A):
 
 
 # ------------------------------------------------------------------------------------------------------------ goldens
-def _build(cfg, **over):
+def build_from_cfg(cfg, **over):
     """tianshou_b200's BCQ with the recipe's seeded initial weights, on the GPU."""
     from oracle.oracle_discrete_sac import seeded_params
 
@@ -206,7 +191,7 @@ def _build(cfg, **over):
     for k, mod in enumerate((pert, c1, c2, vae)):
         if mod is not None:
             seeded_params(mod, int(cfg["init_seed"]) + k)
-    policy = BCQPolicy(actor_perturbation=pert.to(DEV), critic=c1.to(DEV), vae=vae.to(DEV), action_space=_Box(A, m),
+    policy = BCQPolicy(actor_perturbation=pert.to(DEV), critic=c1.to(DEV), vae=vae.to(DEV), action_space=Box(A, m),
                        forward_sampled_times=int(cfg["S"]))
     kw = dict(policy=policy, actor_perturbation_optim=AdamOptimizerFactory(lr=float(cfg["actor_lr"])),
               critic_optim=AdamOptimizerFactory(lr=float(cfg["critic_lr"])), vae_optim=AdamOptimizerFactory(lr=float(cfg["vae_lr"])),
@@ -217,7 +202,7 @@ def _build(cfg, **over):
     return BCQ(**kw)
 
 
-def _buffer(g, mirror):
+def buffer_from_golden(g, mirror):
     from tianshou_b200.data import ReplayBuffer
     buf = ReplayBuffer.from_data(*(g["buf_" + k].copy() for k in ("obs", "act", "rew", "terminated", "truncated", "done", "obs_next")))
     if mirror:
@@ -244,10 +229,10 @@ def test_update_matches_reference(variant, mirror):
     from tianshou_b200.data import Batch
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden(f"bcq_ref_{variant}.npz")
-    cfg = _cfg(g)
-    algo = _build(cfg)
+    cfg = golden_cfg(g)
+    algo = build_from_cfg(cfg)
     assert sorted(algo.state_dict().keys()) == list(g["state_dict_keys"]), "state_dict() keys differ from the reference's"
-    buf = _buffer(g, mirror)
+    buf = buffer_from_golden(g, mirror)
     algo._noise_fn = _cpu_noise
     captured = {}
     orig = algo._preprocess_batch
@@ -266,7 +251,7 @@ def test_update_matches_reference(variant, mirror):
         if bool(cfg["compact"]) and u < U - 1:
             continue
         for prefix, mods in _modules(algo):
-            check_params(tag, mods, g, o + prefix, rtol=1e-3, atol=0.1 * float(cfg["critic_lr"]))
+            check_net_params(tag, mods, g, o + prefix, rtol=1e-3, atol=0.1 * float(cfg["critic_lr"]))
     if "policy_obs" in g.files:
         torch.manual_seed(900)
         with torch.no_grad():
@@ -281,8 +266,8 @@ def test_lagged_perturbation_moves_by_polyak_only():
     updated perturbation network, whatever it held before."""
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden("bcq_ref_net.npz")
-    cfg = _cfg(g)
-    a, b = _build(cfg), _build(cfg)
+    cfg = golden_cfg(g)
+    a, b = build_from_cfg(cfg), build_from_cfg(cfg)
     with torch.no_grad():
         for p in b.actor_perturbation_target.parameters():
             p.add_(5.0)                             # a different lagged perturbation network ...
@@ -292,7 +277,7 @@ def test_lagged_perturbation_moves_by_polyak_only():
         torch.manual_seed(2)
         old = algo._g_at.flat.clone()
         with policy_within_training_step(algo.policy):
-            algo.update(_buffer(g, mirror=True), int(cfg["bs"]))
+            algo.update(buffer_from_golden(g, mirror=True), int(cfg["bs"]))
         tau = float(cfg["tau"])
         want = old * (1 - tau) + algo._g_actor.flat * tau
         torch.testing.assert_close(algo._g_at.flat, want, rtol=1e-6, atol=1e-6)
@@ -353,7 +338,7 @@ def grad_case(O, A, H, VH, L, per_row, B=256, edge=""):
     m, N, phi = 2.0, 10, 0.5
     cfg = dict(obs=O, act=A, hidden=H, vae_hidden=VH, latent=L, max_action=m, phi=phi, per_row=per_row, critic2=True, actor_lr=1e-3,
                critic_lr=1e-3, critic2_lr=3e-4, vae_lr=1e-3, gamma=0.99, tau=0.005, lmbda=0.75, N=N, S=10, init_seed=O + A)
-    algo = _build(cfg)
+    algo = build_from_cfg(cfg)
     buf = _random_buffer(O, A, 900, seed=O, m=m)
     eps_seen = []
     algo._noise_fn = lambda shape: (eps_seen.append(torch.randn(shape, device=DEV)), eps_seen[-1])[1]
@@ -421,9 +406,9 @@ def test_device_update_has_no_torch_host_sync(variant):
     torch.cuda.set_sync_debug_mode("error")."""
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden(f"bcq_ref_{variant}.npz")
-    cfg = _cfg(g)
-    algo = _build(cfg)
-    buf = _buffer(g, mirror=True)
+    cfg = golden_cfg(g)
+    algo = build_from_cfg(cfg)
+    buf = buffer_from_golden(g, mirror=True)
     with policy_within_training_step(algo.policy):
         algo.update(buf, int(cfg["bs"]))                 # first update: scratch buffers exist afterwards
         batch, _ = algo._sample(buf, int(cfg["bs"]))
@@ -443,21 +428,21 @@ def test_state_dict_round_trip_continues_identically(variant):
     """A fresh algorithm loaded from another's ``state_dict()`` after two updates continues bit for bit."""
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden(f"bcq_ref_{variant}.npz")
-    cfg = _cfg(g)
-    a = _build(cfg)
+    cfg = golden_cfg(g)
+    a = build_from_cfg(cfg)
     a._noise_fn = _cpu_noise
     for u in range(2):
         torch.manual_seed(1 + u)
         with policy_within_training_step(a.policy):
-            a.update(_buffer(g, False), int(cfg["bs"]))
-    b = _build(cfg)
+            a.update(buffer_from_golden(g, False), int(cfg["bs"]))
+    b = build_from_cfg(cfg)
     b._noise_fn = _cpu_noise
     with torch.no_grad():
         for p in b.parameters():
             p.add_(0.01)
     b.load_state_dict(copy.deepcopy(a.state_dict()))
     for algo in (a, b):
-        buf = _buffer(g, mirror=False)
+        buf = buffer_from_golden(g, mirror=False)
         np.random.seed(3)
         for u in range(3):
             torch.manual_seed(10 + u)
@@ -477,7 +462,7 @@ def test_device_policy_matches_reference_loop(per_row):
     from tianshou_b200.data import Batch
     cfg = dict(obs=11, act=3, hidden=(64, 64), vae_hidden=(64, 64), latent=6, max_action=1.0, phi=0.5, per_row=per_row, critic2=False,
                actor_lr=1e-3, critic_lr=1e-3, critic2_lr=1e-3, vae_lr=1e-3, gamma=0.99, tau=0.005, lmbda=0.75, N=10, S=100, init_seed=8)
-    algo = _build(cfg)
+    algo = build_from_cfg(cfg)
     obs = np.random.default_rng(4).standard_normal((10, 11)).astype(np.float32)
     torch.manual_seed(77)
     with torch.no_grad():
@@ -511,23 +496,19 @@ def test_refusals():
     from tianshou_b200.utils.net.continuous import VAE, ContinuousCritic, Perturbation
     O, A, L = 4, 2, 3
 
-    class _Discrete:
-        n = 3
-        shape = ()
-
     def make(dev=DEV, space=None, pert=None, critic=None, vae=None, vae_optim=None, **kw):
         pert = pert or Perturbation(preprocess_net=MLP(input_dim=O + A, output_dim=A, hidden_sizes=(8,)), max_action=1.0)
         critic = critic or ContinuousCritic(preprocess_net=Net(state_shape=(O,), action_shape=(A,), hidden_sizes=(8,), concat=True))
         vae = vae or VAE(encoder=MLP(input_dim=O + A, hidden_sizes=(8,)), decoder=MLP(input_dim=O + L, output_dim=A, hidden_sizes=(8,)),
                          hidden_dim=8, latent_dim=L, max_action=1.0)
-        pol = BCQPolicy(actor_perturbation=pert.to(dev), critic=critic.to(dev), vae=vae.to(dev), action_space=space or _Box(A))
+        pol = BCQPolicy(actor_perturbation=pert.to(dev), critic=critic.to(dev), vae=vae.to(dev), action_space=space or Box(A))
         return BCQ(policy=pol, actor_perturbation_optim=AdamOptimizerFactory(lr=1e-3), critic_optim=AdamOptimizerFactory(lr=1e-3),
                    vae_optim=vae_optim or AdamOptimizerFactory(lr=1e-3), **kw)
 
     make()
     make(pert=Perturbation(preprocess_net=Net(state_shape=(O + A,), action_shape=(A,), hidden_sizes=(8,)), max_action=1.0))
     with pytest.raises(UnsupportedModelError, match="Box"):
-        make(space=_Discrete())
+        make(space=Discrete(3))
     with pytest.raises(UnsupportedModelError, match="no CPU path"):
         make(dev="cpu")
     with pytest.raises(UnsupportedModelError, match="no CPU path"):
@@ -567,21 +548,15 @@ def _vae_on_cpu(O, A, L):
               hidden_dim=8, latent_dim=L, max_action=1.0)
     pert = Perturbation(preprocess_net=MLP(input_dim=O + A, output_dim=A, hidden_sizes=(8,)), max_action=1.0).to(DEV)
     critic = ContinuousCritic(preprocess_net=Net(state_shape=(O,), action_shape=(A,), hidden_sizes=(8,), concat=True)).to(DEV)
-    pol = BCQPolicy(actor_perturbation=pert, critic=critic, vae=vae, action_space=_Box(A))
+    pol = BCQPolicy(actor_perturbation=pert, critic=critic, vae=vae, action_space=Box(A))
     return BCQ(policy=pol, actor_perturbation_optim=AdamOptimizerFactory(lr=1e-3), critic_optim=AdamOptimizerFactory(lr=1e-3),
                vae_optim=AdamOptimizerFactory(lr=1e-3))
 
 
 # ------------------------------------------------------------------------------------------------------------ resources
 def test_bcq_kernels_have_no_stack_frame_or_spills(tmp_path):
-    from tianshou_b200.csrc import build as B
-    if shutil.which(B.NVCC) is None and not os.path.exists(B.NVCC):
-        pytest.skip("nvcc not available")
-    r = subprocess.run([B.NVCC, *B.FLAGS, "-c", os.path.join(B.HERE, "bcq.cu"), "-o", str(tmp_path / "b.o")], capture_output=True, text=True)
-    assert r.returncode == 0, r.stdout + r.stderr
-    hits = re.findall(r"Compiling entry function '(\S+)' for 'sm_90a'\n(?:.*\n)*?\s*(\d+) bytes stack frame, (\d+) bytes spill "
-                      r"stores, (\d+) bytes spill loads", r.stdout + r.stderr)
-    names = sorted(re.search(r"\d+bcq_(\w+?)_kernelE", h[0]).group(1) for h in hits)
+    report = ptxas_report("bcq.cu", tmp_path)
+    names = sorted(re.search(r"\d+bcq_(\w+?)_kernelE", e).group(1) for e in report)
     assert names == sorted(["vae_reparam", "vae_loss", "vae_head_bwd", "decode_input", "act_rows", "perturb", "perturb_bwd", "target",
-                            "select"]), hits
-    assert all(tuple(map(int, h[1:])) == (0, 0, 0) for h in hits), hits
+                            "select"]), report
+    assert_spill_free(report)

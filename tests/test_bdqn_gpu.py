@@ -5,32 +5,18 @@ gradient that sums the value head and the branches), ``update()`` against output
 float64 autograd at bipedal_bdq.py's width, a smaller batch after a larger one, bit-identical repeats, the absence of host
 synchronisation inside the update, ``state_dict()`` round trips, the refusals and the register report."""
 import copy
-import os
 import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
+from offpolicy_testutil import DEV, MultiDiscrete, assert_spill_free, golden_cfg, load_params, ptxas_report, stream
 from ts_testutil import load_golden, record_parity
 
-DEV = "cuda:0"
 gpu = pytest.mark.gpu
 KEYS = ("obs", "act", "rew", "terminated", "truncated", "obs_next")
 GRID_CAP_ROWS = 132 * 4 * 256 * 2       # past the grid-stride cap of bdqn.cu's row kernels on any H100 (<= 132 SMs)
-
-
-class _MultiDiscrete:
-    def __init__(self, nvec):
-        self.nvec = np.asarray(nvec)
-        self.shape = self.nvec.shape
-
-
-def _st():
-    from tianshou_b200._cabi import stream_ptr
-    return stream_ptr(torch.device(DEV))
 
 
 def _net(O, nb, A, common, value, action, act=torch.nn.ReLU, **kw):
@@ -41,7 +27,7 @@ def _net(O, nb, A, common, value, action, act=torch.nn.ReLU, **kw):
 
 def _algo(net, lr=1e-3, **kw):
     from tianshou_b200.algorithm import BDQN, AdamOptimizerFactory, BDQNPolicy
-    policy = BDQNPolicy(model=net, action_space=_MultiDiscrete([net.action_per_branch] * net.num_branches))
+    policy = BDQNPolicy(model=net, action_space=MultiDiscrete([net.action_per_branch] * net.num_branches))
     return BDQN(policy=policy, optim=AdamOptimizerFactory(lr=lr), **kw)
 
 
@@ -79,7 +65,7 @@ def test_bdqn_kernels_vs_fp64(B, nb, A):
     y = torch.full((B,), float("nan"), device=DEV)
     yb = torch.full((B, nb), float("nan"), device=DEV)
     call("ts_bdqn_target", ptr(d["v_on"]), ptr(d["s_on"]), ptr(d["v_tg"]), ptr(d["s_tg"]), B, nb, A, gamma, ptr(d["rew"]),
-         ptr(d["end"]), ptr(d["idx"]), ptr(y), ptr(yb), _st())
+         ptr(d["end"]), ptr(d["idx"]), ptr(y), ptr(yb), stream())
     torch.cuda.synchronize()
     q_on, q_tg = _q64(v_on, s_on), _q64(v_tg, s_tg)
     astar = q_on.argmax(-1, keepdim=True)
@@ -103,7 +89,7 @@ def test_bdqn_kernels_vs_fp64(B, nb, A):
             torch.full((1,), float("nan"), device=DEV)
         ybr = yb if B == 1 else None
         call("ts_bdqn_rows", ptr(d["v_on"]), ptr(d["s_on"]), ptr(d["act"]), ptr(yt), ptr(d["w"]) if weighted else None, ptr(ybr), B,
-             nb, A, ptr(td), ptr(rows), ptr(tds), ptr(ds), ptr(dv), ptr(loss), _st())
+             nb, A, ptr(td), ptr(rows), ptr(tds), ptr(ds), ptr(dv), ptr(loss), stream())
         torch.cuda.synchronize()
         vv = v_on.double().requires_grad_(True)
         ss = s_on.double().requires_grad_(True)
@@ -125,7 +111,7 @@ def test_bdqn_kernels_vs_fp64(B, nb, A):
         record_parity(f"{t}/dv", dv.cpu().numpy(), vv.grad.numpy(), rtol=1e-5, atol=1e-6 * float(vv.grad.abs().max()))
         again = torch.empty(1, device=DEV)
         call("ts_bdqn_rows", ptr(d["v_on"]), ptr(d["s_on"]), ptr(d["act"]), ptr(yt), ptr(d["w"]) if weighted else None, ptr(ybr), B,
-             nb, A, ptr(td), ptr(rows), ptr(tds), ptr(ds), ptr(dv), ptr(again), _st())
+             nb, A, ptr(td), ptr(rows), ptr(tds), ptr(ds), ptr(dv), ptr(again), stream())
         torch.cuda.synchronize()
         assert torch.equal(again, loss)
 
@@ -143,7 +129,7 @@ def test_bdqn_target_branch_mean_follows_numpy():
                                                torch.zeros(B, dtype=torch.uint8), torch.arange(B))]
         y = torch.empty(B, device=DEV)
         call("ts_bdqn_target", ptr(dd[0]), ptr(dd[1]), ptr(dd[0]), ptr(dd[1]), B, nb, A, 1.0, ptr(dd[2]), ptr(dd[3]), ptr(dd[4]),
-             ptr(y), None, _st())
+             ptr(y), None, stream())
         torch.cuda.synchronize()
         sn = s.permute(1, 0, 2).numpy()                     # [B, nb, A] float32
         q = sn - ((sn[..., 0] + sn[..., 1]) / np.float32(2))[..., None]
@@ -195,21 +181,11 @@ def test_branch_stack_vs_fp64_autograd(B, nb, act, heads):
 
 
 # ------------------------------------------------------------------------------------------------------------ goldens
-def _cfg(g):
-    return {k[4:]: g[k] for k in g.files if k.startswith("cfg_")}
-
-
-def _load(mod, g, prefix):
-    with torch.no_grad():
-        for i, p in enumerate(mod.parameters()):
-            p.copy_(torch.as_tensor(g[f"{prefix}{i}"]).reshape(p.shape))
-
-
 def _build(cfg, g=None, **over):
     net = _net(int(cfg["obs"]), int(cfg["nb"]), int(cfg["A"]), [int(x) for x in cfg["common"]], [int(x) for x in cfg["value"]],
                [int(x) for x in cfg["action"]], torch.nn.Tanh if str(cfg["act_fn"]) == "tanh" else torch.nn.ReLU).to(DEV)
     if g is not None:
-        _load(net, g, "p0_net_")
+        load_params(net, g, "p0_net_")
     kw = dict(lr=float(cfg["lr"]), gamma=float(cfg["gamma"]), target_update_freq=int(cfg["target_update_freq"]),
               is_double=bool(cfg["is_double"]))
     kw.update(over)
@@ -218,7 +194,7 @@ def _build(cfg, g=None, **over):
 
 def _buffer(g, mirror):
     from tianshou_b200.data import Batch, PrioritizedReplayBuffer, ReplayBuffer, VectorReplayBuffer
-    cfg = _cfg(g)
+    cfg = golden_cfg(g)
     size, E = int(cfg["size"]), int(cfg["envs"])
     if bool(cfg["per"]):
         buf = PrioritizedReplayBuffer(size, alpha=float(cfg["per_alpha"]), beta=float(cfg["per_beta"]), device=DEV)
@@ -248,7 +224,7 @@ def _buffer(g, mirror):
 def test_update_matches_reference(variant, mirror):
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden(f"bdqn_ref_{variant}.npz")
-    cfg = _cfg(g)
+    cfg = golden_cfg(g)
     algo = _build(cfg, g)
     assert sorted(algo.state_dict().keys()) == list(g["state_dict_keys"]), "state_dict() keys differ from the reference's"
     buf = _buffer(g, mirror)
@@ -350,7 +326,7 @@ def _run(algo, buf, sizes, seed0):
 @gpu
 def test_identical_updates_are_bit_identical():
     g = load_golden("bdqn_ref_bipedal.npz")
-    cfg = _cfg(g)
+    cfg = golden_cfg(g)
     res = []
     for _ in range(2):
         algo = _build(cfg, g)
@@ -389,7 +365,7 @@ def test_device_update_has_no_host_sync_but_the_loss(per):
     buffer's td sums are read after it, by the priority update, as in the reference)."""
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden("bdqn_ref_per_trunc.npz" if per else "bdqn_ref_bipedal.npz")
-    cfg = _cfg(g)
+    cfg = golden_cfg(g)
     algo = _build(cfg, g)
     buf = _buffer(g, mirror=True)
     bs = int(cfg["bs"])
@@ -422,7 +398,7 @@ def test_device_update_has_no_host_sync_but_the_loss(per):
 @gpu
 def test_state_dict_round_trip_continues_identically():
     g = load_golden("bdqn_ref_bipedal.npz")
-    cfg = _cfg(g)
+    cfg = golden_cfg(g)
     a = _build(cfg, g)
     _run(a, _buffer(g, mirror=False), [int(cfg["bs"])] * 3, 1)
     b = _build(cfg, g)
@@ -498,7 +474,7 @@ def test_reference_construction_builds():
     from tianshou_b200.utils.net.common import BranchingNet
     net = BranchingNet(state_shape=(3,), num_branches=1, action_per_branch=40, common_hidden_sizes=[64, 64],
                        value_hidden_sizes=[64], action_hidden_sizes=[64]).to(DEV)
-    policy = BDQNPolicy(model=net, action_space=_MultiDiscrete([40]), eps_training=0.76, eps_inference=0.01)
+    policy = BDQNPolicy(model=net, action_space=MultiDiscrete([40]), eps_training=0.76, eps_inference=0.01)
     algorithm = BDQN(policy=policy, optim=AdamOptimizerFactory(lr=1e-3), gamma=0.9, target_update_freq=200)
     from tianshou_b200.data import Batch
     out = policy(Batch(obs=np.zeros((5, 3), np.float32), info={}))
@@ -507,14 +483,7 @@ def test_reference_construction_builds():
 
 # ------------------------------------------------------------------------------------------------------------ resources
 def test_bdqn_kernels_have_no_stack_frame_or_spills(tmp_path):
-    from tianshou_b200.csrc import build as B
-    if shutil.which(B.NVCC) is None and not os.path.exists(B.NVCC):
-        pytest.skip("nvcc not available")
-    r = subprocess.run([B.NVCC, *B.FLAGS, "-c", os.path.join(B.HERE, "bdqn.cu"), "-o", str(tmp_path / "t.o")], capture_output=True,
-                       text=True)
-    assert r.returncode == 0, r.stdout + r.stderr
-    hits = re.findall(r"Compiling entry function '(\S+)' for 'sm_90a'\n(?:.*\n)*?\s*(\d+) bytes stack frame, (\d+) bytes spill "
-                      r"stores, (\d+) bytes spill loads", r.stdout + r.stderr)
-    names = sorted(re.search(r"bdqn_(target|rows|dscore|sum)_kernel", h[0]).group(1) for h in hits)
-    assert names == ["dscore", "rows", "sum", "target"], hits
-    assert all(tuple(map(int, h[1:])) == (0, 0, 0) for h in hits), hits
+    report = ptxas_report("bdqn.cu", tmp_path)
+    names = sorted(re.search(r"bdqn_(target|rows|dscore|sum)_kernel", e).group(1) for e in report)
+    assert names == ["dscore", "rows", "sum", "target"], report
+    assert_spill_free(report)

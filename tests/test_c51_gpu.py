@@ -4,10 +4,6 @@ float64 autograd, the batch sizes the kernels and GEMMs split on, the ``state_di
 refusals and the kernels' register report."""
 import copy
 import math
-import os
-import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -15,24 +11,16 @@ import torch
 
 from oracle import oracle_c51 as oc
 from oracle import oracle_discrete_sac as ods
-from test_qrdqn_gpu import _Discrete, buffer_from_golden, check_final_state, make_buffer
+from offpolicy_testutil import (B_LARGE, B_SMALL, DEV, EPS, GEMM_BK, Discrete, assert_spill_free, capture_batches, capture_grads,
+                                check_final_state, check_second_batch_size, gemm_splits_k, grid_caps, ptxas_report, sm_count,
+                                stream, vector_buffer_from_golden)
+from test_qrdqn_gpu import make_buffer
 from ts_testutil import load_golden, record_parity
 
-DEV = "cuda:0"
 gpu = pytest.mark.gpu
-EPS = float(np.finfo(np.float32).eps)
 A_CASES = (1, 2, 6, 18)
 N_CASES = (2, 51, 201)
 VARIANTS = ["c51_ref_mlp", "c51_ref_cnn", "c51_ref_per"]
-
-
-def _st():
-    from tianshou_b200._cabi import stream_ptr
-    return stream_ptr(torch.device(DEV))
-
-
-def sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
 
 
 # ------------------------------------------------------------------------------------------------------------ target kernel
@@ -47,7 +35,7 @@ def test_target_kernel_matches_oracle(A, N):
     ``target_update_freq == 0`` case."""
     from tianshou_b200._cabi import call, ptr
     g = torch.Generator().manual_seed(A * 1000 + N)
-    B = sms() * 16 * 8 + 37 if (A, N) == (6, 51) else 301
+    B = sm_count() * 16 * 8 + 37 if (A, N) == (6, 51) else 301
     lo = torch.randint(-3, 4, (B, A, N), generator=g).float()
     ln = torch.randn(B, A, N, generator=g) * 2
     if A > 1:
@@ -61,7 +49,7 @@ def test_target_kernel_matches_oracle(A, N):
     top2 = np.sort(q64, 1)[:, -2:] if A > 1 else np.zeros((B, 2))
     clear = (top2[:, 1] - top2[:, 0]) > 1e-4 * 10.0 if A > 1 else np.ones(B, bool)
     for nxt, src in ((lnd, ln), (lod, lo)):
-        call("ts_c51_target", ptr(lod), ptr(nxt), ptr(z), B, A, N, ptr(out), ptr(act), _st())
+        call("ts_c51_target", ptr(lod), ptr(nxt), ptr(z), B, A, N, ptr(out), ptr(act), stream())
         torch.cuda.synchronize()
         got_a = act.cpu().numpy()
         assert np.array_equal(got_a[clear], ref_a[clear])
@@ -71,7 +59,7 @@ def test_target_kernel_matches_oracle(A, N):
         want = oc.softmax(src.numpy()[np.arange(B), got_a])
         bound = (N / 32 + 8 + 2 * 2 * float(src.abs().max())) * EPS * want + 1e-30
         assert np.all(np.abs(out.cpu().numpy() - want) <= bound)
-    call("ts_c51_target", ptr(lod), ptr(lod), ptr(z), 0, A, N, ptr(out), None, _st())      # B == 0: nothing to do
+    call("ts_c51_target", ptr(lod), ptr(lod), ptr(z), 0, A, N, ptr(out), None, stream())      # B == 0: nothing to do
     torch.cuda.synchronize()
 
 
@@ -82,7 +70,7 @@ def _rows(logits, act, ret, z, v_min, v_max, dz, nd, w):
     dl, prio = torch.empty(B, A, N, device=DEV), torch.empty(B, device=DEV)
     rows, losses = torch.empty(3, B, device=DEV), torch.empty(4, device=DEV)
     call("ts_c51_rows", ptr(logits), ptr(act), ptr(ret), ptr(z), v_min, v_max, dz, ptr(nd), ptr(w), B, A, N, ptr(dl), ptr(prio),
-         ptr(rows), ptr(losses), _st())
+         ptr(rows), ptr(losses), stream())
     torch.cuda.synchronize()
     return losses.cpu().numpy(), dl.cpu().numpy(), prio.cpu().numpy()
 
@@ -107,7 +95,7 @@ def test_rows_kernel_vs_fp64(A, N, weighted):
         rounding.
       - the loss averages w_b CE_b in row_sums3_kernel: (B / 1024 + 12) eps times the mean, on top of the rows' errors."""
     rng = np.random.default_rng(A * 7919 + N * 31 + weighted)
-    B = sms() * 8 + 37 if (A, N, weighted) == (6, 51, True) else 41
+    B = sm_count() * 8 + 37 if (A, N, weighted) == (6, 51, True) else 41
     v_min, v_max = (-3.0, 7.0) if N % 2 else (-10.0, 10.0)
     z32 = oc.support(N, v_min, v_max)
     dz = (v_max - v_min) / (N - 1)
@@ -164,14 +152,14 @@ def test_kernels_refuse_bad_arguments():
 
     def rows(N=4, dz=1.0, logits=x, v_min=-1.0, v_max=1.0):
         call("ts_c51_rows", ptr(logits), ptr(a), ptr(x), ptr(x), v_min, v_max, dz, ptr(x), None, 1, 1, N, ptr(x), ptr(x), ptr(x),
-             ptr(x), _st())
+             ptr(x), stream())
 
     for kw in (dict(N=3073), dict(N=1), dict(dz=0.0), dict(dz=-1.0), dict(dz=float("nan")), dict(logits=None), dict(v_min=2.0)):
         with pytest.raises(RuntimeError, match="ts_c51_rows"):
             rows(**kw)
     for N, lo in ((1, x), (4, None)):
         with pytest.raises(RuntimeError, match="ts_c51_target"):
-            call("ts_c51_target", ptr(lo), ptr(x), ptr(x), 1, 1, N, ptr(x), None, _st())
+            call("ts_c51_target", ptr(lo), ptr(x), ptr(x), 1, 1, N, ptr(x), None, stream())
 
 
 # ------------------------------------------------------------------------------------------------------------ vs reference
@@ -192,7 +180,7 @@ def build_from_golden(g):
     A, N = int(g["cfg_A"]), int(g["cfg_N"])
     model = model_from_cfg(kind, A, N, **kw)
     ods.seeded_params(model, int(g["cfg_init_seed"]))
-    policy = C51Policy(model=model, action_space=_Discrete(A), num_atoms=N, v_min=float(g["cfg_v_min"]), v_max=float(g["cfg_v_max"]))
+    policy = C51Policy(model=model, action_space=Discrete(A), num_atoms=N, v_min=float(g["cfg_v_min"]), v_max=float(g["cfg_v_max"]))
     return C51(policy=policy, optim=AdamOptimizerFactory(lr=float(g["cfg_lr"])), gamma=float(g["cfg_gamma"]),
                n_step_return_horizon=int(g["cfg_n_step"]), target_update_freq=int(g["cfg_freq"]))
 
@@ -211,36 +199,24 @@ def test_update_matches_reference(variant, mirror):
     optimiser's param indices (``support`` at 0, without state)."""
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden(f"{variant}.npz")
-    algo, buf = build_from_golden(g), buffer_from_golden(g, mirror)
+    algo, buf = build_from_golden(g), vector_buffer_from_golden(g, mirror)
     keys = [str(k) for k in g["state_dict_keys"]]
     assert list(algo.state_dict().keys()) == keys
-    cap = {}
-    orig_pre, orig_post = algo._preprocess_batch, algo._postprocess_batch
-
-    def pre(batch, buffer, indices):
-        b = orig_pre(batch, buffer, indices)
-        cap["indices"], cap["returns"] = np.asarray(indices).copy(), b.returns.detach().cpu().numpy().copy()
-        return b
-
-    def post(batch, buffer, indices):
-        cap["prio"] = batch.weight.detach().cpu().numpy().copy()
-        return orig_post(batch, buffer, indices)
-
-    algo._preprocess_batch, algo._postprocess_batch = pre, post
-    for u in range(int(g["cfg_updates"])):
-        np.random.seed(500 + u)
-        with policy_within_training_step(algo.policy):
-            stats = algo.update(buffer=buf, sample_size=int(g["cfg_bs"]))
-        tag = f"{variant}_m{int(mirror)}_u{u}"
-        assert np.array_equal(cap["indices"], g[f"u{u}_indices"]), "sampled indices differ from the reference's"
-        ref_ret = g[f"u{u}_returns"]
-        record_parity(f"{tag}/returns", cap["returns"], ref_ret, rtol=1e-5, atol=1e-5 * float(np.abs(ref_ret).max()))
-        assert isinstance(stats.loss, float)
-        record_parity(f"{tag}/losses", np.array([stats.loss]), g[f"u{u}_losses"], rtol=2e-5, atol=2e-6)
-        record_parity(f"{tag}/prio", cap["prio"], g[f"u{u}_prio"], rtol=2e-5, atol=2e-6)
-        if bool(g["cfg_per"]):
-            leaves = np.asarray(buf.weight[np.arange(len(buf))])
-            record_parity(f"{tag}/tree_leaves", leaves, g[f"u{u}_tree_leaves"], rtol=2e-5, atol=1e-7)
+    with capture_batches(algo) as cap:
+        for u in range(int(g["cfg_updates"])):
+            np.random.seed(500 + u)
+            with policy_within_training_step(algo.policy):
+                stats = algo.update(buffer=buf, sample_size=int(g["cfg_bs"]))
+            tag = f"{variant}_m{int(mirror)}_u{u}"
+            assert np.array_equal(cap["indices"], g[f"u{u}_indices"]), "sampled indices differ from the reference's"
+            ref_ret = g[f"u{u}_returns"]
+            record_parity(f"{tag}/returns", cap["returns"].cpu().numpy(), ref_ret, rtol=1e-5, atol=1e-5 * float(np.abs(ref_ret).max()))
+            assert isinstance(stats.loss, float)
+            record_parity(f"{tag}/losses", np.array([stats.loss]), g[f"u{u}_losses"], rtol=2e-5, atol=2e-6)
+            record_parity(f"{tag}/prio", cap["prio"].cpu().numpy(), g[f"u{u}_prio"], rtol=2e-5, atol=2e-6)
+            if bool(g["cfg_per"]):
+                leaves = np.asarray(buf.weight[np.arange(len(buf))])
+                record_parity(f"{tag}/tree_leaves", leaves, g[f"u{u}_tree_leaves"], rtol=2e-5, atol=1e-7)
     check_final_state(f"{variant}_m{int(mirror)}", g, algo)
     assert list(algo.state_dict().keys()) == keys
     ids, state_ids = _optimizer_layout(algo)
@@ -255,36 +231,20 @@ def grad_case(kind, B=64, edge=""):
     fp32-faithful (bf16x3) and a weight gradient sums B products per element: 2e-4 relative plus 1e-4 of the tensor's largest
     value, as in test_qrdqn_gpu."""
     from tianshou_b200.algorithm import AdamOptimizerFactory, C51, C51Policy
-    from tianshou_b200.algorithm.flat_params import FlatGroup
     from tianshou_b200.utils import policy_within_training_step
     torch.manual_seed(3)
     rng = np.random.default_rng(4)
     A, N, v_min, v_max = 5, 33, -4.0, 6.0
     model = model_from_cfg(kind, A, N, hidden=(48, 40))
-    policy = C51Policy(model=model, action_space=_Discrete(A), num_atoms=N, v_min=v_min, v_max=v_max)
+    policy = C51Policy(model=model, action_space=Discrete(A), num_atoms=N, v_min=v_min, v_max=v_max)
     algo = C51(policy=policy, optim=AdamOptimizerFactory(lr=1e-3), gamma=0.9, n_step_return_horizon=2, target_update_freq=3)
     buf = make_buffer(kind, A, rng)
-    cap = {}
     grp = algo._group
-
-    def adam(optimizer, mgn):
-        cap["grad"] = grp.grad[: grp.n].clone()
-        FlatGroup.adam_step(grp, optimizer, mgn)
-
-    grp.adam_step = adam
-    orig_pre = algo._preprocess_batch
-
-    def pre(batch, buffer, indices):
-        b = orig_pre(batch, buffer, indices)
-        cap["indices"], cap["returns"] = np.asarray(indices).copy(), b.returns.detach().cpu().double()
-        return b
-
-    algo._preprocess_batch = pre
     ref = copy.deepcopy(model).to("cpu", torch.float64)         # the weights before the step
     np.random.seed(7)
-    with policy_within_training_step(algo.policy):
+    with capture_batches(algo) as cap, capture_grads(grp) as grads, policy_within_training_step(algo.policy):
         stats = algo.update(buffer=buf, sample_size=B)
-    idx = cap["indices"]
+    idx, returns = cap["indices"], cap["returns"].cpu().double()
     obs = np.asarray(buf.obs)
     obs_next = obs[buf.next(idx)] if kind == "cnn" else np.asarray(buf.obs_next)[idx]
     x_of = lambda raw: torch.as_tensor((raw.astype(np.float64) / 255.0).astype(np.float32) if kind == "cnn" else raw).double()
@@ -295,17 +255,17 @@ def grad_case(kind, B=64, edge=""):
     with torch.no_grad():
         pn = probs(x_of(obs_next))
         nd = pn[torch.arange(B), (pn * z).sum(2).argmax(1)]
-        target = oc.reference_target(nd, cap["returns"], z, v_min, v_max, (v_max - v_min) / (N - 1))
+        target = oc.reference_target(nd, returns, z, v_min, v_max, (v_max - v_min) / (N - 1))
     act = np.asarray(buf.act)[idx].astype(np.int64)
     loss, _ = oc.reference_loss(probs(x_of(obs[idx])), act, target, 1.0)
     loss.backward()
     ref_params = [p for m in chain.modules() if isinstance(m, (torch.nn.Linear, torch.nn.Conv2d)) for p in (m.weight, m.bias)]
     for i, (p, r) in enumerate(zip(grp.params, ref_params, strict=True)):
         want = r.grad.numpy()
-        got = grp.view(cap["grad"], p).view(p.shape).cpu().numpy()
+        got = grp.view(grads[-1], p).view(p.shape).cpu().numpy()
         record_parity(f"c51_grad{edge}/{kind}/grad_{i}", got, want, rtol=2e-4, atol=1e-4 * float(np.abs(want).max()) + 1e-12)
     record_parity(f"c51_grad{edge}/{kind}/loss", np.array([stats.loss]), np.array([loss.item()]), rtol=2e-5, atol=2e-6)
-    assert len(idx) == B and cap["returns"].shape[0] == B, "the update must run on the B sampled rows"
+    assert len(idx) == B and returns.shape[0] == B, "the update must run on the B sampled rows"
 
 
 @gpu
@@ -315,7 +275,6 @@ def test_update_gradient_vs_fp64_autograd(kind):
 
 
 def _edge_batch(cls):
-    from test_offpolicy_batch_edges_gpu import GEMM_BK, grid_caps
     if cls == "B1":
         return 1
     if cls in ("splitK_below", "splitK_above"):
@@ -329,7 +288,6 @@ def _edge_batch(cls):
 def test_update_vs_fp64_autograd_at_batch_edges(cls):
     """The batch sizes of test_offpolicy_batch_edges_gpu applied to C51: B = 1, the largest weight-gradient GEMM at one and at
     two K chunks (unsplit / split K), and the smallest batch past the grid caps of both new kernels."""
-    from test_offpolicy_batch_edges_gpu import gemm_splits_k, grid_caps
     B = _edge_batch(cls)
     if cls.startswith("splitK"):
         assert gemm_splits_k(B) == (cls == "splitK_above")
@@ -344,26 +302,10 @@ def test_update_vs_fp64_autograd_at_batch_edges(cls):
 def test_second_batch_size_is_bit_identical_to_a_fresh_instance(order):
     """As test_offpolicy_batch_edges_gpu part 2: one batch size, every scratch tensor poisoned with NaN, then another; the
     second update must equal a fresh instance's, loaded from the same ``state_dict()``, bit for bit."""
-    from test_offpolicy_batch_edges_gpu import (B_LARGE, B_SMALL, _carry_outside_state_dict, _poison, _rng_state, _set_rng_state,
-                                                _state, _update)
     g = load_golden("c51_ref_mlp.npz")
-    buf = buffer_from_golden(g, False)
     B1, B2 = (B_LARGE, B_SMALL) if order == "large_then_small" else (B_SMALL, B_LARGE)
-    a = build_from_golden(g)
-    _update(a, buf, B1, seed=1)
-    b = build_from_golden(g)
-    b.load_state_dict(copy.deepcopy(a.state_dict()))
-    _carry_outside_state_dict(a, b)
-    rng = _rng_state(buf)
-    assert _poison(a) > 0
-    cap_a, stats_a = _update(a, buf, B2, seed=2)
-    _set_rng_state(buf, rng)
-    cap_b, stats_b = _update(b, buf, B2, seed=2)
-    assert np.array_equal(cap_a["indices"], cap_b["indices"]) and len(cap_a["indices"]) == B2
-    assert stats_a == stats_b and math.isfinite(stats_a["loss"])
-    assert cap_a["prio"].numel() == B2 and torch.equal(cap_a["prio"], cap_b["prio"])
-    for x, y in zip(_state(a), _state(b), strict=True):
-        assert torch.equal(x, y)
+    cap, _ = check_second_batch_size(lambda: build_from_golden(g), vector_buffer_from_golden(g, False), B1, B2)
+    assert cap["prio"] is not None
 
 
 # ------------------------------------------------------------------------------------------------------------ state_dict
@@ -374,7 +316,7 @@ def test_state_dict_round_trip_continues_identically(variant):
     ``_iter`` is a plain attribute, as in the reference: whoever restores a run restores it too."""
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden(f"{variant}.npz")
-    a, buf_a = build_from_golden(g), buffer_from_golden(g)
+    a, buf_a = build_from_golden(g), vector_buffer_from_golden(g)
     for u in range(3):
         np.random.seed(u)
         with policy_within_training_step(a.policy):
@@ -387,7 +329,7 @@ def test_state_dict_round_trip_continues_identically(variant):
     b._iter = a._iter
     assert torch.equal(a.policy.support, b.policy.support)
     for algo in (a, b):
-        buf = buffer_from_golden(g)
+        buf = vector_buffer_from_golden(g)
         for u in range(3):
             np.random.seed(10 + u)
             with policy_within_training_step(algo.policy):
@@ -405,7 +347,7 @@ def test_policy_forward_takes_arg_max_of_expected_values():
     from tianshou_b200.data import Batch
     torch.manual_seed(0)
     model = model_from_cfg("mlp", 5, 17, obs=4, hidden=(32,))
-    policy = C51Policy(model=model, action_space=_Discrete(5), num_atoms=17, v_min=-2.0, v_max=3.0)
+    policy = C51Policy(model=model, action_space=Discrete(5), num_atoms=17, v_min=-2.0, v_max=3.0)
     assert policy.support.device == torch.device(DEV)
     rng = np.random.default_rng(0)
     obs = rng.standard_normal((300, 4)).astype(np.float32)
@@ -433,7 +375,7 @@ def test_refusals():
 
     def make(model=None, opt=AdamOptimizerFactory, n=A, **kw):
         model = model or model_from_cfg("mlp", A, N, hidden=(16,))
-        return C51(policy=C51Policy(model=model, action_space=_Discrete(n), num_atoms=N), optim=opt(lr=1e-3), **kw)
+        return C51(policy=C51Policy(model=model, action_space=Discrete(n), num_atoms=N), optim=opt(lr=1e-3), **kw)
 
     algo = make()
     for model in (Net(state_shape=(4,), action_shape=A, hidden_sizes=(16,), num_atoms=N),
@@ -454,7 +396,7 @@ def test_refusals():
             make(**kw)
     for kw in (dict(num_atoms=1), dict(v_min=1.0, v_max=1.0), dict(v_min=2.0, v_max=1.0)):
         with pytest.raises(AssertionError):
-            C51Policy(model=model_from_cfg("mlp", A, N, hidden=(16,)), action_space=_Discrete(A), **kw)
+            C51Policy(model=model_from_cfg("mlp", A, N, hidden=(16,)), action_space=Discrete(A), **kw)
     # an action the network has no atoms for is refused on the host, before any kernel indexes with it
     buf = VectorReplayBuffer(40, 4, device=DEV)
     rng = np.random.default_rng(0)
@@ -468,14 +410,7 @@ def test_refusals():
 
 # ------------------------------------------------------------------------------------------------------------ resources
 def test_kernels_have_no_stack_frame_or_spills(tmp_path):
-    from tianshou_b200.csrc import build as B
-    if shutil.which(B.NVCC) is None and not os.path.exists(B.NVCC):
-        pytest.skip("nvcc not available")
-    r = subprocess.run([B.NVCC, *B.FLAGS, "-c", os.path.join(B.HERE, "c51.cu"), "-o", str(tmp_path / "c.o")], capture_output=True,
-                       text=True)
-    assert r.returncode == 0, r.stdout + r.stderr
-    hits = re.findall(r"Compiling entry function '(\S+)' for 'sm_90a'\n(?:.*\n)*?\s*(\d+) bytes stack frame, (\d+) bytes spill "
-                      r"stores, (\d+) bytes spill loads", r.stdout + r.stderr)
+    report = ptxas_report("c51.cu", tmp_path)
     kernels = ("c51_rows_kernel", "c51_target_kernel", "row_sums3_kernel")
-    assert len(hits) == 3 and all(any(k in h[0] for k in kernels) for h in hits), hits
-    assert all(tuple(map(int, h[1:])) == (0, 0, 0) for h in hits), hits
+    assert len(report) == 3 and all(any(k in e for k in kernels) for e in report), report
+    assert_spill_free(report)

@@ -3,36 +3,26 @@ outputs of the imported reference (tests/golden/cql_ref_*.npz from oracle/gen_go
 the gradients of the actor, both critics and the Lagrange multiplier against float64 autograd of the eager restatement, the
 absence of host synchronisation inside the update, ``state_dict()`` round trips, the refusals and the kernels' register report."""
 import copy
-import os
 import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
+from offpolicy_testutil import DEV, Box, assert_spill_free, check_params, golden_cfg, load_params, ptxas_report, stream
 from ts_testutil import load_golden, record_parity, set_buffer_state
 
-DEV = "cuda:0"
 gpu = pytest.mark.gpu
-
-
-class _Box:
-    def __init__(self, dim):
-        self.shape = (dim,)
-        self.low = -np.ones(dim, np.float32)
-        self.high = np.ones(dim, np.float32)
 
 
 # ------------------------------------------------------------------------------------------------------------ kernels
 def _kernels(q1, q2, y, B, R, lp_c, lp_x, rand_logp, cal, T, w, log_alpha, amin, amax, thr):
-    from tianshou_b200._cabi import call, ptr, stream_ptr
+    from tianshou_b200._cabi import call, ptr
     N = B * R
     dq1, dq2 = torch.empty(B + 3 * N, device=DEV), torch.empty(B + 3 * N, device=DEV)
     sq, lse = torch.empty(2 * B, device=DEV), torch.empty(2 * N, device=DEV)
     grad, out = torch.full((1,), float("nan"), device=DEV), torch.full((4,), float("nan"), device=DEV)
-    st = stream_ptr(torch.device(DEV))
+    st = stream()
     call("ts_cql_rows", ptr(q1), ptr(q2), ptr(y), B, R, ptr(lp_c), ptr(lp_x), rand_logp, ptr(cal), T, w, ptr(log_alpha), amin, amax,
          ptr(dq1), ptr(dq2), ptr(sq), ptr(lse), st)
     call("ts_cql_losses", ptr(q1), ptr(q2), ptr(sq), ptr(lse), B, N, T, w, ptr(log_alpha), amin, amax, thr,
@@ -129,14 +119,14 @@ def test_rows_and_losses_kernels_vs_fp64(B, R, A, T, calibrated, lagrange, kind)
 @gpu
 @pytest.mark.parametrize("B", [5, 300000])
 def test_target_kernel_vs_fp32_reference_order(B):
-    from tianshou_b200._cabi import call, ptr, stream_ptr
+    from tianshou_b200._cabi import call, ptr
     g = torch.Generator().manual_seed(B)
     q1, q2, lp, rew = (torch.randn(B, generator=g) for _ in range(4))
     done = (torch.rand(B, generator=g) < 0.3).float()
     alpha, gamma = 0.2, 0.99
     out = torch.empty(B, device=DEV)
     d = [t.to(DEV) for t in (q1, q2, lp, rew, done)]          # kept alive until the kernel has run
-    call("ts_cql_target", ptr(d[0]), ptr(d[1]), ptr(d[2]), alpha, ptr(d[3]), ptr(d[4]), gamma, B, ptr(out), stream_ptr(torch.device(DEV)))
+    call("ts_cql_target", ptr(d[0]), ptr(d[1]), ptr(d[2]), alpha, ptr(d[3]), ptr(d[4]), gamma, B, ptr(out), stream())
     torch.cuda.synchronize()
     ref = rew.double() + (1.0 - done.double()) * np.float64(np.float32(gamma)) * (torch.min(q1, q2).double() - np.float32(alpha) * lp.double())
     record_parity(f"cql_target/B{B}", out.cpu().numpy(), ref.numpy(), rtol=1e-6, atol=1e-6)
@@ -144,18 +134,7 @@ def test_target_kernel_vs_fp32_reference_order(B):
 
 
 # ------------------------------------------------------------------------------------------------------------ goldens
-def _load(mod, g, prefix):
-    with torch.no_grad():
-        for i, p in enumerate(mod.parameters()):
-            p.copy_(torch.as_tensor(g[f"{prefix}{i}"]).reshape(p.shape))
-
-
-def _check_params(tag, mod, g, prefix, lr):
-    for i, p in enumerate(mod.parameters()):
-        record_parity(f"{tag}/{prefix}{i}", p.detach().cpu().numpy(), g[f"{prefix}{i}"], rtol=1e-3, atol=0.1 * lr)
-
-
-def _build(cfg, g=None, **over):
+def build_from_cfg(cfg, g=None, **over):
     from tianshou_b200.algorithm import CQL, AdamOptimizerFactory
     from tianshou_b200.algorithm.modelfree.sac import AutoAlpha, SACPolicy
     from tianshou_b200.utils.net.common import Net
@@ -167,9 +146,9 @@ def _build(cfg, g=None, **over):
     c1 = crit()
     c2 = crit() if bool(cfg["critic2"]) else None
     if g is not None:
-        _load(actor, g, "p0_actor_"); _load(c1, g, "p0_c1_")
+        load_params(actor, g, "p0_actor_"); load_params(c1, g, "p0_c1_")
         if c2 is not None:
-            _load(c2, g, "p0_c2_")
+            load_params(c2, g, "p0_c2_")
     alpha = AutoAlpha(-float(A), 0.0, AdamOptimizerFactory(lr=float(cfg["alpha_lr"]))).to(DEV) if bool(cfg["auto"]) else float(cfg["alpha"])
     kw = dict(cql_alpha_lr=float(cfg["cql_alpha_lr"]), cql_weight=float(cfg["cql_weight"]), tau=float(cfg["tau"]), gamma=float(cfg["gamma"]),
               alpha=alpha, temperature=float(cfg["temperature"]), with_lagrange=bool(cfg["with_lagrange"]),
@@ -177,22 +156,18 @@ def _build(cfg, g=None, **over):
               num_repeat_actions=int(cfg["R"]), alpha_min=float(cfg["alpha_min"]), alpha_max=float(cfg["alpha_max"]),
               max_grad_norm=float(cfg["max_grad_norm"]), calibrated=bool(cfg["calibrated"]))
     kw.update(over)
-    return CQL(policy=SACPolicy(actor=actor, action_space=_Box(A)), policy_optim=AdamOptimizerFactory(lr=float(cfg["actor_lr"])),
+    return CQL(policy=SACPolicy(actor=actor, action_space=Box(A)), policy_optim=AdamOptimizerFactory(lr=float(cfg["actor_lr"])),
                critic=c1, critic_optim=AdamOptimizerFactory(lr=float(cfg["critic_lr"])), critic2=c2,
                critic2_optim=AdamOptimizerFactory(lr=float(cfg["critic2_lr"])) if c2 is not None else None, **kw)
 
 
-def _cfg(g):
-    return {k[4:]: g[k] for k in g.files if k.startswith("cfg_")}
-
-
-def _buffer(g, mirror):
+def buffer_from_golden(g, mirror):
     from tianshou_b200.data import Batch, ReplayBuffer
     keys = ("obs", "act", "rew", "terminated", "truncated", "done", "obs_next")
-    if int(_cfg(g)["adds"]) == 0:
+    if int(golden_cfg(g)["adds"]) == 0:
         buf = ReplayBuffer.from_data(*(g["buf_" + k].copy() for k in keys))
     else:
-        buf = ReplayBuffer(int(_cfg(g)["size"]), device=DEV)
+        buf = ReplayBuffer(int(golden_cfg(g)["size"]), device=DEV)
         buf.set_batch(Batch(**{k: g["buf_" + k].copy() for k in keys}))
         ins, size = int(g["buf_insertion_idx"]), int(g["buf_size"])
         set_buffer_state(buf, np.array([(ins - 1) % size]), np.array([size]))
@@ -209,10 +184,10 @@ def _buffer(g, mirror):
 def test_update_matches_reference(variant, mirror):
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden(f"cql_ref_{variant}.npz")
-    cfg = _cfg(g)
-    algo = _build(cfg, g)
+    cfg = golden_cfg(g)
+    algo = build_from_cfg(cfg, g)
     assert sorted(algo.state_dict().keys()) == list(g["state_dict_keys"]), "state_dict() keys differ from the reference's"
-    buf = algo.process_buffer(_buffer(g, mirror))
+    buf = algo.process_buffer(buffer_from_golden(g, mirror))
     if bool(cfg["calibrated"]):
         record_parity(f"cql/{variant}/calibration_returns", np.asarray(buf._meta["calibration_returns"]), g["calibration_returns"],
                       rtol=1e-12, atol=1e-12)
@@ -246,10 +221,10 @@ def test_update_matches_reference(variant, mirror):
         record_parity(f"{tag}/alpha", np.array([stats.alpha]), np.array([g[o + "alpha"]]), rtol=1e-6, atol=0)
         if bool(cfg["auto"]):
             record_parity(f"{tag}/alpha_loss", np.array([stats.alpha_loss]), np.array([g[o + "alpha_loss"]]), rtol=2e-5, atol=1e-7)
-        _check_params(tag, algo.policy.actor, g, o + "actor_", float(cfg["actor_lr"]))
-        _check_params(tag, algo.critic, g, o + "c1_", float(cfg["critic_lr"])); _check_params(tag, algo.critic2, g, o + "c2_", c2_lr)
-        _check_params(tag, algo.critic_old, g, o + "c1old_", float(cfg["critic_lr"]))
-        _check_params(tag, algo.critic2_old, g, o + "c2old_", c2_lr)
+        check_params(tag, algo.policy.actor, g, o + "actor_", float(cfg["actor_lr"]))
+        check_params(tag, algo.critic, g, o + "c1_", float(cfg["critic_lr"])); check_params(tag, algo.critic2, g, o + "c2_", c2_lr)
+        check_params(tag, algo.critic_old, g, o + "c1old_", float(cfg["critic_lr"]))
+        check_params(tag, algo.critic2_old, g, o + "c2old_", c2_lr)
 
 
 # ------------------------------------------------------------------------------------------------------------ gradients
@@ -291,7 +266,7 @@ def grad_case(O, A, H, R, B=128, edge=""):
                tau=0.005, gamma=0.99, temperature=1.0, with_lagrange=True, lagrange_threshold=10.0, min_action=-0.5, max_action=1.0,
                R=R, alpha_min=0.0, alpha_max=1e6, max_grad_norm=1e9, calibrated=True, actor_lr=1e-4, critic_lr=3e-4)
     torch.manual_seed(3)
-    algo = _build(cfg)
+    algo = build_from_cfg(cfg)
     with torch.no_grad():
         algo.cql_log_alpha.fill_(0.4)
     nets = cql_nets(O, A, H)
@@ -360,8 +335,8 @@ def test_device_update_has_no_torch_host_sync():
     """Everything after the sampling runs under torch.cuda.set_sync_debug_mode("error") (fixed alpha, mirrored buffer)."""
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden("cql_ref_d4rl.npz")
-    algo = _build(_cfg(g), g)
-    buf = algo.process_buffer(_buffer(g, mirror=True))
+    algo = build_from_cfg(golden_cfg(g), g)
+    buf = algo.process_buffer(buffer_from_golden(g, mirror=True))
     with policy_within_training_step(algo.policy):
         algo.update(buf, 32)                      # first update: scratch buffers exist afterwards
         batch, indices = algo._sample(buf, 32)
@@ -383,13 +358,13 @@ def test_state_dict_round_trip_continues_identically(variant):
     Adam (not in state_dict(), as in the reference) and AutoAlpha's Adam are carried over by hand."""
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden(f"cql_ref_{variant}.npz")
-    cfg = _cfg(g)
-    a = _build(cfg, g)
-    buf_a = a.process_buffer(_buffer(g, mirror=False))
+    cfg = golden_cfg(g)
+    a = build_from_cfg(cfg, g)
+    buf_a = a.process_buffer(buffer_from_golden(g, mirror=False))
     torch.manual_seed(1)
     with policy_within_training_step(a.policy):
         a.update(buf_a, int(cfg["bs"]))
-    b = _build(cfg, g)
+    b = build_from_cfg(cfg, g)
     with torch.no_grad():
         for p in b.parameters():
             p.add_(0.01)
@@ -400,7 +375,7 @@ def test_state_dict_round_trip_continues_identically(variant):
     if bool(cfg["auto"]):
         b.alpha._optim.load_state_dict(copy.deepcopy(a.alpha._optim.state_dict()))
     for algo in (a, b):
-        buf = algo.process_buffer(_buffer(g, mirror=False))
+        buf = algo.process_buffer(buffer_from_golden(g, mirror=False))
         for u in range(2):
             torch.manual_seed(10 + u)
             with policy_within_training_step(algo.policy):
@@ -426,7 +401,7 @@ def test_refusals():
         actor = ContinuousActorProbabilistic(preprocess_net=Net(state_shape=(O,), hidden_sizes=(8,)), action_shape=(A,), unbounded=True,
                                              conditioned_sigma=c_sigma).to(dev)
         c = ContinuousCritic(preprocess_net=Net(state_shape=(O,), action_shape=(A,), hidden_sizes=(8,), concat=True)).to(dev)
-        return CQL(policy=SACPolicy(actor=actor, action_space=_Box(A)), policy_optim=opt(lr=1e-3), critic=c, critic_optim=opt(lr=1e-3), **kw)
+        return CQL(policy=SACPolicy(actor=actor, action_space=Box(A)), policy_optim=opt(lr=1e-3), critic=c, critic_optim=opt(lr=1e-3), **kw)
 
     make()
     with pytest.raises(UnsupportedModelError, match="no CPU path"):
@@ -447,13 +422,7 @@ def test_refusals():
 
 # ------------------------------------------------------------------------------------------------------------ resources
 def test_cql_kernels_have_no_stack_frame_or_spills(tmp_path):
-    from tianshou_b200.csrc import build as B
-    if shutil.which(B.NVCC) is None and not os.path.exists(B.NVCC):
-        pytest.skip("nvcc not available")
-    r = subprocess.run([B.NVCC, *B.FLAGS, "-c", os.path.join(B.HERE, "cql.cu"), "-o", str(tmp_path / "c.o")], capture_output=True, text=True)
-    assert r.returncode == 0, r.stdout + r.stderr
-    hits = re.findall(r"Compiling entry function '(\S+)' for 'sm_90a'\n(?:.*\n)*?\s*(\d+) bytes stack frame, (\d+) bytes spill "
-                      r"stores, (\d+) bytes spill loads", r.stdout + r.stderr)
-    names = sorted(re.search(r"cql_(rows|losses|target)_kernel", h[0]).group(1) for h in hits)
-    assert names == ["losses", "rows", "target"], hits
-    assert all(tuple(map(int, h[1:])) == (0, 0, 0) for h in hits), hits
+    report = ptxas_report("cql.cu", tmp_path)
+    names = sorted(re.search(r"cql_(rows|losses|target)_kernel", e).group(1) for e in report)
+    assert names == ["losses", "rows", "target"], report
+    assert_spill_free(report)

@@ -3,10 +3,6 @@
 oracle/gen_golden_discrete_bcq.py), ``state_dict()`` keys and round trip, the policy's torch path, the refusals and the kernels'
 register report."""
 import copy
-import os
-import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -14,23 +10,17 @@ import torch
 
 from oracle import oracle_discrete_bcq as odb
 from oracle import oracle_discrete_sac as ods
+from offpolicy_testutil import (DEV, EPS, Discrete, assert_spill_free, capture_batches, capture_grads, check_final_state,
+                                ptxas_report, sm_count, stream, vector_buffer_from_golden)
 from ts_testutil import load_golden, record_parity
 
-DEV = "cuda:0"
 gpu = pytest.mark.gpu
-EPS = float(np.finfo(np.float32).eps)
 A_CASES = (1, 2, 6, 18, 33, 64, 1000)
-
-
-class _Discrete:
-    def __init__(self, n):
-        self.n = n
-        self.shape = ()
 
 
 def past_grid_rows():
     """More rows than the per-row kernels' grid has warps, and not a multiple of anything."""
-    return torch.cuda.get_device_properties(0).multi_processor_count * 16 * 8 + 37
+    return sm_count() * 16 * 8 + 37
 
 
 def row_bound(A, terms):
@@ -49,7 +39,7 @@ def block_bound(B, terms):
 @pytest.mark.parametrize("A", A_CASES)
 def test_target_kernel_matches_torch_expression(A):
     """Exact: the kernel forms the masked values in fp32 as torch does, so the chosen action is torch's, ties included."""
-    from tianshou_b200._cabi import call, ptr, stream_ptr
+    from tianshou_b200._cabi import call, ptr
     g = torch.Generator().manual_seed(A)
     B = past_grid_rows() if A == 6 else 301
     q = torch.randint(-2, 3, (B, A), generator=g).float()          # exact ties, also under the mask
@@ -60,7 +50,7 @@ def test_target_kernel_matches_torch_expression(A):
         ref_a = (q - torch.finfo(torch.float32).max * ((z - z.max(-1, keepdim=True).values) < log_tau).float()).argmax(-1)
         out, act = torch.empty(B, device=DEV), torch.empty(B, dtype=torch.int64, device=DEV)
         qd, zd, od = q.to(DEV), z.to(DEV), q_old.to(DEV)
-        call("ts_discrete_bcq_target", ptr(qd), ptr(zd), ptr(od), log_tau, B, A, ptr(out), ptr(act), stream_ptr(torch.device(DEV)))
+        call("ts_discrete_bcq_target", ptr(qd), ptr(zd), ptr(od), log_tau, B, A, ptr(out), ptr(act), stream())
         torch.cuda.synchronize()
         assert torch.equal(act.cpu(), ref_a), f"A={A} log_tau={log_tau}"
         assert torch.equal(out.cpu(), q_old[torch.arange(B), ref_a])
@@ -70,12 +60,12 @@ def test_target_kernel_matches_torch_expression(A):
 
 
 def _bcq_rows(q, z, act, ret, penalty):
-    from tianshou_b200._cabi import call, ptr, stream_ptr
+    from tianshou_b200._cabi import call, ptr
     B, A = q.shape
     dq, dz = torch.empty(B, A, device=DEV), torch.empty(B, A, device=DEV)
     rows, losses = torch.empty(3, B, device=DEV), torch.empty(4, device=DEV)
     call("ts_discrete_bcq_rows", ptr(q), ptr(z), ptr(act), ptr(ret), B, A, penalty, ptr(dq), ptr(dz), ptr(rows), ptr(losses),
-         stream_ptr(torch.device(DEV)))
+         stream())
     torch.cuda.synchronize()
     return losses.cpu().numpy(), dq.cpu().numpy(), dz.cpu().numpy()
 
@@ -234,43 +224,10 @@ def heads_from_golden(g, critic_b=False):
     return a, b
 
 
-def buffer_from_golden(g, mirror=False):
-    from tianshou_b200.data import Batch, VectorReplayBuffer
-    E, cap = int(g["cfg_E"]), int(g["cfg_cap"])
-    cnn = str(g["cfg_kind"]) == "cnn"
-    kw = dict(stack_num=4, ignore_obs_next=True, save_only_last_obs=True) if cnn else {}
-    buf = VectorReplayBuffer(E * cap, E, device=DEV, device_mirror=mirror, **kw)
-    for i in range(int(g["cfg_steps"])):
-        s = {k: g[f"roll{i}_{k}"] for k in ("obs", "act", "rew", "terminated", "truncated")}
-        if cnn:
-            s["obs"] = np.repeat(s["obs"][:, None], 4, axis=1)        # only the last frame is stored
-            s["obs_next"] = s["obs"]
-        else:
-            s["obs_next"] = g[f"roll{i}_obs_next"]
-        buf.add(Batch(**s), buffer_ids=np.arange(E))
-    return buf
-
-
-def check_final_state(tag, g, algo, lagged):
-    """Final parameters / Adam moments / lagged parameters within the bars DESIGN.md section 4 uses for DQN and discrete SAC: Adam
-    normalises a step to ~lr per element, so the absolute term is stated in units of one step."""
-    view = ods.golden_view if bool(g["cfg_compact"]) else (lambda t: t.detach().cpu().numpy())
-    lr = float(g["cfg_lr"])
-    grp = algo._group
-    for i, p in enumerate(grp.params):
-        record_parity(f"{tag}/pf_{i}", view(p), g[f"pf_{i}"], rtol=1e-3, atol=0.1 * lr)
-        m, v = g[f"m_{i}"], g[f"v_{i}"]
-        record_parity(f"{tag}/m_{i}", view(grp.view(grp.exp_avg, p).view(p.shape)), m, rtol=2e-3, atol=2e-3 * float(np.abs(m).max()) + 1e-12)
-        record_parity(f"{tag}/v_{i}", view(grp.view(grp.exp_avg_sq, p).view(p.shape)), v, rtol=4e-3, atol=4e-3 * float(np.abs(v).max()) + 1e-20)
-    assert grp.sync_step_from_device() == int(g["adam_step"]) and algo._iter == int(g["iter"])
-    for i, p in enumerate(lagged):
-        record_parity(f"{tag}/old_{i}", view(p), g[f"old_{i}"], rtol=1e-3, atol=0.1 * lr)
-
-
 def build_bcq(g):
     from tianshou_b200.algorithm import AdamOptimizerFactory, DiscreteBCQ, DiscreteBCQPolicy
     model, imitator = heads_from_golden(g)
-    policy = DiscreteBCQPolicy(model=model, imitator=imitator, action_space=_Discrete(int(g["cfg_A"])),
+    policy = DiscreteBCQPolicy(model=model, imitator=imitator, action_space=Discrete(int(g["cfg_A"])),
                                target_update_freq=int(g["cfg_freq"]), unlikely_action_threshold=float(g["cfg_tau"]))
     return DiscreteBCQ(policy=policy, optim=AdamOptimizerFactory(lr=float(g["cfg_lr"])), gamma=float(g["cfg_gamma"]),
                        n_step_return_horizon=int(g["cfg_n_step"]), target_update_freq=int(g["cfg_freq"]),
@@ -284,27 +241,20 @@ def test_update_matches_reference(variant, mirror):
     golden is the online model one or two steps back)."""
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden(f"dbcq_ref_{variant}.npz")
-    algo, buf = build_bcq(g), buffer_from_golden(g, mirror)
+    algo, buf = build_bcq(g), vector_buffer_from_golden(g, mirror)
     assert list(algo.state_dict().keys()) == [str(k) for k in g["state_dict_keys"]]
-    cap = {}
-    orig_pre = algo._preprocess_batch
-
-    def pre(batch, buffer, indices):
-        b = orig_pre(batch, buffer, indices)
-        cap["indices"], cap["returns"] = np.asarray(indices).copy(), b.returns.detach().cpu().numpy().copy()
-        return b
-
-    algo._preprocess_batch = pre
-    for u in range(int(g["cfg_updates"])):
-        np.random.seed(500 + u)
-        with policy_within_training_step(algo.policy):
-            stats = algo.update(buffer=buf, sample_size=int(g["cfg_bs"]))
-        tag = f"dbcq_{variant}_m{int(mirror)}_u{u}"
-        assert np.array_equal(cap["indices"], g[f"u{u}_indices"]), "sampled indices differ from the reference's"
-        ref_ret = g[f"u{u}_returns"]
-        record_parity(f"{tag}/returns", cap["returns"].reshape(ref_ret.shape), ref_ret, rtol=1e-5, atol=1e-5 * float(np.abs(ref_ret).max()))
-        got = np.array([stats.loss, stats.q_loss, stats.i_loss, stats.reg_loss])
-        record_parity(f"{tag}/losses", got, g[f"u{u}_losses"], rtol=2e-5, atol=2e-6)
+    with capture_batches(algo) as cap:
+        for u in range(int(g["cfg_updates"])):
+            np.random.seed(500 + u)
+            with policy_within_training_step(algo.policy):
+                stats = algo.update(buffer=buf, sample_size=int(g["cfg_bs"]))
+            tag = f"dbcq_{variant}_m{int(mirror)}_u{u}"
+            assert np.array_equal(cap["indices"], g[f"u{u}_indices"]), "sampled indices differ from the reference's"
+            ref_ret = g[f"u{u}_returns"]
+            record_parity(f"{tag}/returns", cap["returns"].cpu().numpy().reshape(ref_ret.shape), ref_ret, rtol=1e-5,
+                          atol=1e-5 * float(np.abs(ref_ret).max()))
+            got = np.array([stats.loss, stats.q_loss, stats.i_loss, stats.reg_loss])
+            record_parity(f"{tag}/losses", got, g[f"u{u}_losses"], rtol=2e-5, atol=2e-6)
     check_final_state(f"dbcq_{variant}_m{int(mirror)}", g, algo, list(algo.model_old.parameters()))
     assert list(algo.state_dict().keys()) == [str(k) for k in g["state_dict_keys"]]
 
@@ -321,14 +271,13 @@ def grad_case(name, kind, shared, kw, B=64, edge=""):
     (discrete_bcq.py:244-252) on copies of the modules with the same weights, batch and returns.  Adam's first step is
     lr * sign(g), so a gradient off by a constant factor leaves the parameters unchanged; this is the check that sees it."""
     from tianshou_b200.algorithm import AdamOptimizerFactory, DiscreteBCQ, DiscreteBCQPolicy
-    from tianshou_b200.algorithm.flat_params import FlatGroup
     from tianshou_b200.data import Batch, VectorReplayBuffer
     from tianshou_b200.utils import policy_within_training_step
     torch.manual_seed(5 + len(name))
     rng = np.random.default_rng(len(name))
     A, E, T, penalty = 6, 4, 48, 0.2
     model, imitator = make_heads(kind, shared, A, (24,), **kw)
-    algo = DiscreteBCQ(policy=DiscreteBCQPolicy(model=model, imitator=imitator, action_space=_Discrete(A), target_update_freq=3,
+    algo = DiscreteBCQ(policy=DiscreteBCQPolicy(model=model, imitator=imitator, action_space=Discrete(A), target_update_freq=3,
                                                 unlikely_action_threshold=0.4),
                        optim=AdamOptimizerFactory(lr=1e-3), gamma=0.9, target_update_freq=3, imitation_logits_penalty=penalty)
     cnn = kind == "cnn"
@@ -341,38 +290,23 @@ def grad_case(name, kind, shared, kw, B=64, edge=""):
         buf.add(Batch(obs=obs, act=rng.integers(0, A, E), rew=rng.standard_normal(E) * 2, terminated=term,
                       truncated=np.full(E, t % 17 == 16) & ~term, obs_next=nxt), buffer_ids=np.arange(E))
         obs = nxt
-    cap = {}
     grp = algo._group
-
-    def adam(optimizer, mgn):
-        cap["grad"], cap["flat"] = grp.grad[: grp.n].clone(), grp.flat.clone()
-        FlatGroup.adam_step(grp, optimizer, mgn)
-
-    grp.adam_step = adam
-    orig_pre = algo._preprocess_batch
-
-    def pre(batch, buffer, indices):
-        b = orig_pre(batch, buffer, indices)
-        cap["indices"], cap["returns"] = np.asarray(indices).copy(), b.returns.detach().reshape(-1).cpu().double()
-        return b
-
-    algo._preprocess_batch = pre
     ref = copy64(model, imitator)            # the weights before the step
     np.random.seed(7)
-    with policy_within_training_step(algo.policy):
+    with capture_batches(algo) as cap, capture_grads(grp) as grads, policy_within_training_step(algo.policy):
         stats = algo.update(buffer=buf, sample_size=B)
     idx = cap["indices"]
     raw = np.asarray(buf.obs)[idx]
     x = torch.as_tensor((raw.astype(np.float64) / 255.0).astype(np.float32) if cnn else raw).double()
     act = torch.as_tensor(np.asarray(buf.act)[idx].astype(np.int64))
     q, z = chain64(ref[0])(x), chain64(ref[1])(x)
-    ql = torch.nn.functional.smooth_l1_loss(q[torch.arange(B), act], cap["returns"])
+    ql = torch.nn.functional.smooth_l1_loss(q[torch.arange(B), act], cap["returns"].reshape(-1).cpu().double())
     il = torch.nn.functional.nll_loss(torch.log_softmax(z, -1), act)
     reg = z.pow(2).mean()
     loss = ql + il + penalty * reg
     loss.backward()
     from tianshou_b200.algorithm.shared_trunk import two_head_parameters
-    check_flat_grads(f"dbcq_grad{edge}/{name}", grp.params, grp, cap["grad"], two_head_parameters(ref[0], ref[1]))
+    check_flat_grads(f"dbcq_grad{edge}/{name}", grp.params, grp, grads[-1], two_head_parameters(ref[0], ref[1]))
     record_parity(f"dbcq_grad{edge}/{name}/losses", np.array([stats.loss, stats.q_loss, stats.i_loss, stats.reg_loss]),
                   np.array([loss.item(), ql.item(), il.item(), reg.item()]), rtol=2e-5, atol=2e-6)
     assert len(idx) == B, "the update must run on the B sampled rows"
@@ -386,7 +320,7 @@ def test_state_dict_round_trip_continues_identically(variant):
     ``_iter`` is a plain attribute, as in the reference: whoever restores a run restores it too."""
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden(f"dbcq_ref_{variant}.npz")
-    a, buf_a = build_bcq(g), buffer_from_golden(g)
+    a, buf_a = build_bcq(g), vector_buffer_from_golden(g)
     for u in range(3):
         np.random.seed(u)
         with policy_within_training_step(a.policy):
@@ -398,7 +332,7 @@ def test_state_dict_round_trip_continues_identically(variant):
     b.load_state_dict(copy.deepcopy(a.state_dict()))
     b._iter = a._iter
     for algo in (a, b):
-        buf = buffer_from_golden(g)
+        buf = vector_buffer_from_golden(g)
         for u in range(3):
             np.random.seed(10 + u)
             with policy_within_training_step(algo.policy):
@@ -418,7 +352,7 @@ def test_policy_forward_and_exploration_noise():
     model, imitator = make_heads("mlp", True, A, (16,), hidden=(32,))
     with torch.no_grad():          # a logit spread wide enough that the threshold masks some actions
         imitator.last.model[-1].weight.mul_(20.0)
-    policy = DiscreteBCQPolicy(model=model, imitator=imitator, action_space=_Discrete(A), unlikely_action_threshold=0.5,
+    policy = DiscreteBCQPolicy(model=model, imitator=imitator, action_space=Discrete(A), unlikely_action_threshold=0.5,
                                eps_inference=0.3)
     obs = np.random.default_rng(0).standard_normal((500, 11)).astype(np.float32)
     out = policy(Batch(obs=obs, info=Batch()))
@@ -453,7 +387,7 @@ def test_refusals():
     def make(model=None, imitator=None, opt=AdamOptimizerFactory, n=A, **kw):
         m, i = make_heads("mlp", True, A, (8,), hidden=(16,))
         model, imitator = model or m, imitator or i
-        return DiscreteBCQ(policy=DiscreteBCQPolicy(model=model, imitator=imitator, action_space=_Discrete(n)), optim=opt(lr=1e-3), **kw)
+        return DiscreteBCQ(policy=DiscreteBCQPolicy(model=model, imitator=imitator, action_space=Discrete(n)), optim=opt(lr=1e-3), **kw)
 
     algo = make()
     head = lambda trunk, **kw: DiscreteActor(preprocess_net=trunk, action_shape=A, **{"softmax_output": False, **kw}).to(DEV)
@@ -494,12 +428,6 @@ def test_refusals():
 @pytest.mark.parametrize("source,kernels", [("discrete_bcq.cu", ("discrete_bcq_rows_kernel", "discrete_bcq_target_kernel", "row_sums3_kernel")),
                                             ("discrete_crr.cu", ("discrete_crr_rows_kernel", "discrete_crr_sums_kernel", "row_sums3_kernel"))])
 def test_kernels_have_no_stack_frame_or_spills(tmp_path, source, kernels):
-    from tianshou_b200.csrc import build as B
-    if shutil.which(B.NVCC) is None and not os.path.exists(B.NVCC):
-        pytest.skip("nvcc not available")
-    r = subprocess.run([B.NVCC, *B.FLAGS, "-c", os.path.join(B.HERE, source), "-o", str(tmp_path / "d.o")], capture_output=True, text=True)
-    assert r.returncode == 0, r.stdout + r.stderr
-    hits = re.findall(r"Compiling entry function '(\S+)' for 'sm_90a'\n(?:.*\n)*?\s*(\d+) bytes stack frame, (\d+) bytes spill "
-                      r"stores, (\d+) bytes spill loads", r.stdout + r.stderr)
-    assert hits and all(any(k in h[0] for k in kernels) for h in hits), hits
-    assert all(tuple(map(int, h[1:])) == (0, 0, 0) for h in hits), hits
+    report = ptxas_report(source, tmp_path)
+    assert all(any(k in e for k in kernels) for e in report), report
+    assert_spill_free(report)

@@ -10,21 +10,22 @@ import torch
 from torch.distributions import Categorical
 
 from oracle import oracle_discrete_crr as odc
-from test_discrete_bcq_gpu import (A_CASES, DEV, EPS, TRUNK_CASES, _Discrete, buffer_from_golden, chain64, check_final_state,
-                                   check_flat_grads, copy64, heads_from_golden, make_heads, past_grid_rows)
+from offpolicy_testutil import (DEV, EPS, Discrete, capture_batches, capture_grads, check_final_state, stream,
+                                vector_buffer_from_golden)
+from test_discrete_bcq_gpu import A_CASES, TRUNK_CASES, chain64, check_flat_grads, copy64, heads_from_golden, make_heads, past_grid_rows
 from ts_testutil import load_golden, record_parity
 
 gpu = pytest.mark.gpu
 
 
 def _crr_rows(q, z, act, qo, zo, rew, done, gamma, mode, beta, bound, w):
-    from tianshou_b200._cabi import ABI, call, ptr, stream_ptr
+    from tianshou_b200._cabi import ABI, call, ptr
     B, A = q.shape
     dq, dz = torch.empty(B, A, device=DEV), torch.empty(B, A, device=DEV)
     rows, losses = torch.empty(4 * B + 2, device=DEV), torch.empty(4, device=DEV)
     code = ABI.consts[{"exp": "TS_CRR_EXP", "binary": "TS_CRR_BINARY", "all": "TS_CRR_ALL"}[mode]]
     call("ts_discrete_crr_rows", ptr(q), ptr(z), ptr(act), ptr(qo), ptr(zo), ptr(rew), ptr(done), B, A, gamma, code, beta, bound, w,
-         ptr(dq), ptr(dz), ptr(rows), ptr(losses), stream_ptr(torch.device(DEV)))
+         ptr(dq), ptr(dz), ptr(rows), ptr(losses), stream())
     torch.cuda.synchronize()
     return losses.cpu().numpy(), dq.cpu().numpy(), dz.cpu().numpy()
 
@@ -86,7 +87,7 @@ def build_crr(g, **over):
               beta=float(g["cfg_beta"]), min_q_weight=float(g["cfg_min_q_weight"]), target_update_freq=int(g["cfg_freq"]),
               return_standardization=bool(g["cfg_ret_std"]))
     kw.update(over)
-    return DiscreteCRR(policy=DiscreteActorPolicy(actor=actor, action_space=_Discrete(int(g["cfg_A"]))), critic=critic,
+    return DiscreteCRR(policy=DiscreteActorPolicy(actor=actor, action_space=Discrete(int(g["cfg_A"]))), critic=critic,
                        optim=AdamOptimizerFactory(lr=float(g["cfg_lr"])), **kw)
 
 
@@ -97,23 +98,21 @@ def test_update_matches_reference(variant, mirror):
     reference copies on: the golden's lagged parameters are the last copy's."""
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden(f"dcrr_ref_{variant}.npz")
-    algo, buf = build_crr(g), buffer_from_golden(g, mirror)
+    algo, buf = build_crr(g), vector_buffer_from_golden(g, mirror)
     assert list(algo.state_dict().keys()) == [str(k) for k in g["state_dict_keys"]]
-    cap = {}
-    orig_pre = algo._preprocess_batch
-    algo._preprocess_batch = lambda batch, buffer, indices: (cap.update(indices=np.asarray(indices).copy()), orig_pre(batch, buffer, indices))[1]
-    for u in range(int(g["cfg_updates"])):
-        np.random.seed(500 + u)
-        with policy_within_training_step(algo.policy):
-            stats = algo.update(buffer=buf, sample_size=int(g["cfg_bs"]))
-        assert np.array_equal(cap["indices"], g[f"u{u}_indices"]), "sampled indices differ from the reference's"
-        got = np.array([stats.loss, stats.actor_loss, stats.critic_loss, stats.cql_loss])
-        record_parity(f"dcrr_{variant}_m{int(mirror)}_u{u}/losses", got, g[f"u{u}_losses"], rtol=2e-5, atol=2e-6)
+    with capture_batches(algo) as cap:
+        for u in range(int(g["cfg_updates"])):
+            np.random.seed(500 + u)
+            with policy_within_training_step(algo.policy):
+                stats = algo.update(buffer=buf, sample_size=int(g["cfg_bs"]))
+            assert np.array_equal(cap["indices"], g[f"u{u}_indices"]), "sampled indices differ from the reference's"
+            got = np.array([stats.loss, stats.actor_loss, stats.critic_loss, stats.cql_loss])
+            record_parity(f"dcrr_{variant}_m{int(mirror)}_u{u}/losses", got, g[f"u{u}_losses"], rtol=2e-5, atol=2e-6)
     lagged = [*algo.actor_old.parameters(), *algo.critic_old.parameters()] if int(g["cfg_freq"]) > 0 else []
     check_final_state(f"dcrr_{variant}_m{int(mirror)}", g, algo, lagged)
     # return standardisation changes nothing: the loss never reads the returns
     if variant == "sep" and not mirror:
-        other, buf2 = build_crr(g, return_standardization=False), buffer_from_golden(g)
+        other, buf2 = build_crr(g, return_standardization=False), vector_buffer_from_golden(g)
         for u in range(int(g["cfg_updates"])):
             np.random.seed(500 + u)
             with policy_within_training_step(other.policy):
@@ -133,7 +132,6 @@ def grad_case(name, kind, shared, kw, mode, B=64, edge=""):
     against float64 autograd of the reference loss
     (discrete_crr.py:131-158, its [B] x [B, 1] broadcast included) on copies of the modules."""
     from tianshou_b200.algorithm import AdamOptimizerFactory, DiscreteActorPolicy, DiscreteCRR
-    from tianshou_b200.algorithm.flat_params import FlatGroup
     from tianshou_b200.algorithm.shared_trunk import two_head_parameters
     from tianshou_b200.data import Batch, VectorReplayBuffer
     from tianshou_b200.utils import policy_within_training_step
@@ -141,7 +139,7 @@ def grad_case(name, kind, shared, kw, mode, B=64, edge=""):
     rng = np.random.default_rng(len(name) + len(mode))
     A, E, T, gamma, beta, bound, w = 6, 4, 48, 0.9, 0.5, 1.1, 3.0
     actor, critic = make_heads(kind, shared, A, (24,), critic_b=True, **kw)
-    algo = DiscreteCRR(policy=DiscreteActorPolicy(actor=actor, action_space=_Discrete(A)), critic=critic, optim=AdamOptimizerFactory(lr=1e-3),
+    algo = DiscreteCRR(policy=DiscreteActorPolicy(actor=actor, action_space=Discrete(A)), critic=critic, optim=AdamOptimizerFactory(lr=1e-3),
                        gamma=gamma, policy_improvement_mode=mode, ratio_upper_bound=bound, beta=beta, min_q_weight=w, target_update_freq=2)
     with torch.no_grad():         # the lagged networks differ from the online ones
         for p in [*algo.actor_old.parameters(), *algo.critic_old.parameters()]:
@@ -160,19 +158,10 @@ def grad_case(name, kind, shared, kw, mode, B=64, edge=""):
         buf.add(Batch(obs=obs, act=rng.integers(0, A, E), rew=rng.standard_normal(E) * 2, terminated=term,
                       truncated=np.full(E, t % 17 == 16) & ~term, obs_next=nxt), buffer_ids=np.arange(E))
         obs = nxt
-    cap = {}
     grp = algo._group
-
-    def adam(optimizer, mgn):
-        cap["grad"] = grp.grad[: grp.n].clone()
-        FlatGroup.adam_step(grp, optimizer, mgn)
-
-    grp.adam_step = adam
-    orig_pre = algo._preprocess_batch
-    algo._preprocess_batch = lambda batch, buffer, indices: (cap.update(indices=np.asarray(indices).copy()), orig_pre(batch, buffer, indices))[1]
     ref, ref_old = copy64(actor, critic), copy64(algo.actor_old.module, algo.critic_old.module)
     np.random.seed(7)
-    with policy_within_training_step(algo.policy):
+    with capture_batches(algo) as cap, capture_grads(grp) as grads, policy_within_training_step(algo.policy):
         stats = algo.update(buffer=buf, sample_size=B)
     idx = cap["indices"]
     rd = lambda a: torch.as_tensor((a.astype(np.float64) / 255.0).astype(np.float32) if cnn else a).double()
@@ -195,7 +184,7 @@ def grad_case(name, kind, shared, kw, mode, B=64, edge=""):
     cql = (q.logsumexp(1) - qa.squeeze(-1)).mean()
     loss = actor_loss + critic_loss + w * cql
     loss.backward()
-    check_flat_grads(f"dcrr_grad{edge}/{name}_{mode}", grp.params, grp, cap["grad"], two_head_parameters(ref[0], ref[1]))
+    check_flat_grads(f"dcrr_grad{edge}/{name}_{mode}", grp.params, grp, grads[-1], two_head_parameters(ref[0], ref[1]))
     record_parity(f"dcrr_grad{edge}/{name}_{mode}/losses", np.array([stats.loss, stats.actor_loss, stats.critic_loss, stats.cql_loss]),
                   np.array([loss.item(), actor_loss.item(), critic_loss.item(), cql.item()]), rtol=5e-5, atol=5e-6)
     assert len(idx) == B, "the update must run on the B sampled rows"
@@ -205,7 +194,7 @@ def grad_case(name, kind, shared, kw, mode, B=64, edge=""):
 def test_state_dict_round_trip_continues_identically():
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden("dcrr_ref_mlp.npz")
-    a, buf_a = build_crr(g), buffer_from_golden(g)
+    a, buf_a = build_crr(g), vector_buffer_from_golden(g)
     for u in range(3):
         np.random.seed(u)
         with policy_within_training_step(a.policy):
@@ -217,7 +206,7 @@ def test_state_dict_round_trip_continues_identically():
     b.load_state_dict(copy.deepcopy(a.state_dict()))
     b._iter = a._iter             # a plain attribute, as in the reference: whoever restores a run restores it too
     for algo in (a, b):
-        buf = buffer_from_golden(g)
+        buf = vector_buffer_from_golden(g)
         for u in range(3):
             np.random.seed(10 + u)
             with policy_within_training_step(algo.policy):
@@ -237,7 +226,7 @@ def test_refusals():
     def make(actor=None, critic=None, n=A):
         actor = actor or DiscreteActor(preprocess_net=trunk, action_shape=A, softmax_output=False)
         critic = critic or DiscreteCritic(preprocess_net=trunk, last_size=A)
-        return DiscreteCRR(policy=DiscreteActorPolicy(actor=actor.to(DEV), action_space=_Discrete(n)), critic=critic.to(DEV),
+        return DiscreteCRR(policy=DiscreteActorPolicy(actor=actor.to(DEV), action_space=Discrete(n)), critic=critic.to(DEV),
                            optim=AdamOptimizerFactory(lr=1e-3))
 
     make()

@@ -3,43 +3,27 @@ reference (tests/golden/dsac_ref_*.npz from oracle/gen_golden_discrete_sac.py), 
 steps against float64 autograd, the torch generator against the eager restatement, ``state_dict()`` round trips, the
 refusals, the Collector's policy path and the kernel's register report."""
 import copy
-import os
-import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
+from oracle import oracle_discrete_sac as ods
+from offpolicy_testutil import DEV, Box, Discrete, assert_spill_free, check_params, load_params, ptxas_report, sm_count, stream
 from ts_testutil import load_golden, record_parity
 
-DEV = "cuda:0"
 gpu = pytest.mark.gpu
-
-
-class _Discrete:
-    def __init__(self, n):
-        self.n = n
-        self.shape = ()
-
-
-class _Box:
-    def __init__(self, dim):
-        self.shape = (dim,)
-        self.low = -np.ones(dim, np.float32)
-        self.high = np.ones(dim, np.float32)
 
 
 # ------------------------------------------------------------------------------------------------------------ rows kernel
 def _rows(logits, q1, q2, alpha, grad=True):
-    from tianshou_b200._cabi import call, ptr, stream_ptr
+    from tianshou_b200._cabi import call, ptr
     B, A = logits.shape
     v, ent = torch.empty(B, device=DEV), torch.empty(B, device=DEV)
     probs = torch.empty(B, A, device=DEV)
     d = torch.empty(B, A, device=DEV) if grad else None
     call("ts_discrete_sac_rows", ptr(logits), ptr(q1), ptr(q2), alpha, B, A, ptr(v), ptr(ent), ptr(probs), ptr(d), 1.0 / B,
-         stream_ptr(torch.device(DEV)))
+         stream())
     torch.cuda.synchronize()
     return v, ent, probs, d
 
@@ -69,7 +53,7 @@ def test_rows_kernel_vs_fp64(A, kind):
     g = torch.Generator(device="cpu").manual_seed(A * 7 + len(kind))
     B = 300
     if kind == "past_grid_cap":
-        B = torch.cuda.get_device_properties(0).multi_processor_count * 16 * 8 + 37     # more rows than warps in the grid
+        B = sm_count() * 16 * 8 + 37     # more rows than warps in the grid
     z = torch.randn(B, A, generator=g) * 3.0
     if kind == "saturated":      # logit spreads > 100: some probabilities underflow to 0 in fp32
         z[: B // 2] *= 60.0
@@ -123,13 +107,7 @@ def _trunk(kind, O=None, H=None, W=None, hidden=None, feat=None, A=None, denom=2
     return ScaledObsInputActionReprNet(DQNet(4, H, W, A, features_only=True, output_dim_added_layer=feat), denom=denom)
 
 
-def _load(mod, g, prefix):
-    with torch.no_grad():
-        for i, p in enumerate(mod.parameters()):
-            p.copy_(torch.as_tensor(g[f"{prefix}{i}"]).reshape(p.shape))
-
-
-def _build_from_golden(g):
+def build_from_golden(g):
     from tianshou_b200.algorithm import AdamOptimizerFactory, DiscreteSAC
     from tianshou_b200.algorithm.modelfree.discrete_sac import DiscreteSACPolicy
     from tianshou_b200.algorithm.modelfree.sac import AutoAlpha
@@ -147,18 +125,18 @@ def _build_from_golden(g):
             from oracle.oracle_discrete_sac import seeded_params
             seeded_params(m, int(g["cfg_init_seed"]) + k)
         else:
-            _load(m, g, pfx)
+            load_params(m, g, pfx)
     alpha = (AutoAlpha(float(0.98 * np.log(A)), 0.0, AdamOptimizerFactory(lr=float(g["cfg_alpha_lr"]))).to(DEV) if bool(g["cfg_auto"])
              else float(g["cfg_alpha"]))
     clr = float(g["cfg_critic_lr"])
-    return DiscreteSAC(policy=DiscreteSACPolicy(actor=actor, action_space=_Discrete(A)),
+    return DiscreteSAC(policy=DiscreteSACPolicy(actor=actor, action_space=Discrete(A)),
                        policy_optim=AdamOptimizerFactory(lr=float(g["cfg_actor_lr"])), critic=c1,
                        critic_optim=AdamOptimizerFactory(lr=clr), critic2=c2,
                        critic2_optim=AdamOptimizerFactory(lr=clr) if c2 is not None else None, tau=float(g["cfg_tau"]),
                        gamma=float(g["cfg_gamma"]), alpha=alpha, n_step_return_horizon=int(g["cfg_n_step"]))
 
 
-def _buffer_from_golden(g, mirror):
+def buffer_from_golden(g, mirror):
     from tianshou_b200.data import Batch, PrioritizedVectorReplayBuffer, VectorReplayBuffer
     E, cap = int(g["cfg_E"]), int(g["cfg_cap"])
     cnn = str(g["cfg_kind"]) == "cnn"
@@ -181,23 +159,14 @@ def _buffer_from_golden(g, mirror):
     return buf
 
 
-def _check_params(tag, mod, g, prefix, lr):
-    """Every stored parameter; a compact golden stores each tensor as ``golden_view`` (a fixed-stride sample)."""
-    from oracle.oracle_discrete_sac import golden_view
-    view = golden_view if bool(g["cfg_compact"]) else (lambda t: t.detach().cpu().numpy())
-    for i, p in enumerate(mod.parameters()):
-        # Adam normalises the step to ~lr per element: the absolute term is stated in units of one step
-        record_parity(f"{tag}/{prefix}{i}", view(p), g[f"{prefix}{i}"], rtol=1e-3, atol=0.1 * lr)
-
-
 # ------------------------------------------------------------------------------------------------------------ vs reference
 @gpu
 @pytest.mark.parametrize("variant,mirror", [(v, m) for v in ("mlp", "auto", "cnn") for m in (False, True)])
 def test_update_matches_reference(variant, mirror):
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden(f"dsac_ref_{variant}.npz")
-    algo = _build_from_golden(g)
-    buf = _buffer_from_golden(g, mirror)
+    algo = build_from_golden(g)
+    buf = buffer_from_golden(g, mirror)
     per, auto = bool(g["cfg_per"]), bool(g["cfg_auto"])
     alr, clr = float(g["cfg_actor_lr"]), float(g["cfg_critic_lr"])
     cap = {}
@@ -238,9 +207,11 @@ def test_update_matches_reference(variant, mirror):
         else:
             assert stats.alpha_loss is None
         if o + "actor_0" in g:
-            _check_params(tag, algo.policy.actor, g, o + "actor_", alr)
-            _check_params(tag, algo.critic, g, o + "c1_", clr); _check_params(tag, algo.critic2, g, o + "c2_", clr)
-            _check_params(tag, algo.critic_old, g, o + "c1old_", clr); _check_params(tag, algo.critic2_old, g, o + "c2old_", clr)
+            # a compact golden stores each tensor as ``golden_view`` (a fixed-stride sample)
+            view = ods.golden_view if bool(g["cfg_compact"]) else None
+            for mod, prefix, lr in ((algo.policy.actor, "actor_", alr), (algo.critic, "c1_", clr), (algo.critic2, "c2_", clr),
+                                    (algo.critic_old, "c1old_", clr), (algo.critic2_old, "c2old_", clr)):
+                check_params(tag, mod, g, o + prefix, lr, view)
 
 
 # ------------------------------------------------------------------------------------------------------------ gradients
@@ -344,7 +315,7 @@ def grad_case(kind, per, auto, separate_critic2, last_hidden, B=None, edge=""):
     c1 = crit()
     c2 = crit() if separate_critic2 else None
     alpha = AutoAlpha(float(0.98 * np.log(A)), float(np.log(0.3)), AdamOptimizerFactory(lr=3e-2)).to(DEV) if auto else 0.3
-    algo = DiscreteSAC(policy=DiscreteSACPolicy(actor=actor, action_space=_Discrete(A)), policy_optim=AdamOptimizerFactory(lr=1e-3),
+    algo = DiscreteSAC(policy=DiscreteSACPolicy(actor=actor, action_space=Discrete(A)), policy_optim=AdamOptimizerFactory(lr=1e-3),
                        critic=c1, critic_optim=AdamOptimizerFactory(lr=1e-3), critic2=c2,
                        critic2_optim=AdamOptimizerFactory(lr=1e-3) if c2 is not None else None, tau=0.005, gamma=gamma, alpha=alpha)
     groups = [algo._g_c[0], algo._g_c[1], algo._g_actor]
@@ -442,8 +413,8 @@ def test_generator_state_matches_eager_restatement():
     from oracle import oracle_discrete_sac as ods
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden("dsac_ref_mlp.npz")
-    algo = _build_from_golden(g)
-    buf = _buffer_from_golden(g, mirror=False)
+    algo = build_from_golden(g)
+    buf = buffer_from_golden(g, mirror=False)
     cap = {}
     orig_pre = algo._preprocess_batch
 
@@ -455,7 +426,7 @@ def test_generator_state_matches_eager_restatement():
     A, O, Hs = int(g["cfg_A"]), int(g["cfg_obs"]), tuple(int(x) for x in g["cfg_hidden"])
     nets = [ods.mlp_head_net(O, Hs, A) for _ in range(3)]
     for n, pfx in zip(nets, ("p0_actor_", "p0_c1_", "p0_c2_")):
-        _load(n, g, pfx)
+        load_params(n, g, pfx)
     actor, c1, c2 = (n.to(DEV) for n in nets)
     olds = [copy.deepcopy(c1), copy.deepcopy(c2)]
     opts = [torch.optim.Adam(m.parameters(), lr=1e-3) for m in (actor, c1, c2)]
@@ -485,12 +456,12 @@ def test_state_dict_round_trip_continues_identically(variant):
     optimiser state, and AutoAlpha's log_alpha (its torch optimiser's state travels separately, as in the reference)."""
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden(f"dsac_ref_{variant}.npz")
-    a, buf_a = _build_from_golden(g), _buffer_from_golden(g, mirror=False)
+    a, buf_a = build_from_golden(g), buffer_from_golden(g, mirror=False)
     np.random.seed(1)
     with policy_within_training_step(a.policy):
         a.update(buffer=buf_a, sample_size=int(g["cfg_bs"]))
     torch.manual_seed(77)
-    b = _build_from_golden(g)
+    b = build_from_golden(g)
     with torch.no_grad():         # different weights before the load, so the load is what makes them equal
         for p in b.parameters():
             p.add_(0.01)
@@ -498,7 +469,7 @@ def test_state_dict_round_trip_continues_identically(variant):
     if variant == "auto":        # AutoAlpha's own Adam is not one of the algorithm's optimisers (sac.py:168-215, as in the reference)
         b.alpha._optim.load_state_dict(copy.deepcopy(a.alpha._optim.state_dict()))
     for algo in (a, b):          # both continue on fresh, identical buffers with the same draws
-        buf = _buffer_from_golden(g, mirror=False)
+        buf = buffer_from_golden(g, mirror=False)
         for u in range(2):
             np.random.seed(10 + u)
             torch.manual_seed(10 + u)
@@ -525,7 +496,7 @@ def test_refusals():
     def make(actor=None, c1=None, c2=None, opt=AdamOptimizerFactory, dev=DEV):
         actor = actor or DiscreteActor(preprocess_net=net(), action_shape=A, softmax_output=False)
         c1 = c1 or DiscreteCritic(preprocess_net=net(), last_size=A)
-        return DiscreteSAC(policy=DiscreteSACPolicy(actor=actor.to(dev), action_space=_Discrete(A)), policy_optim=opt(lr=1e-3),
+        return DiscreteSAC(policy=DiscreteSACPolicy(actor=actor.to(dev), action_space=Discrete(A)), policy_optim=opt(lr=1e-3),
                            critic=c1.to(dev), critic_optim=opt(lr=1e-3), critic2=None if c2 is None else c2.to(dev))
 
     make()      # the supported baseline builds
@@ -552,7 +523,7 @@ def test_refusals():
     with pytest.raises(UnsupportedModelError, match="softmax preprocess"):
         make(c1=DiscreteCritic(preprocess_net=net(softmax=True), last_size=A))
     with pytest.raises(AssertionError):
-        DiscreteSACPolicy(actor=DiscreteActor(preprocess_net=net(), action_shape=A, softmax_output=False), action_space=_Box(A))
+        DiscreteSACPolicy(actor=DiscreteActor(preprocess_net=net(), action_shape=A, softmax_output=False), action_space=Box(A))
 
 
 # ------------------------------------------------------------------------------------------------------------ policy
@@ -569,7 +540,7 @@ def test_policy_forward_mode_and_sample():
     actor = DiscreteActor(preprocess_net=Net(state_shape=(3,), hidden_sizes=(8,)), action_shape=A, softmax_output=False).to(DEV)
     with torch.no_grad():      # near-uniform probabilities: samples must spread over the actions
         actor.last.model[-1].weight.mul_(0.01)
-    policy = DiscreteSACPolicy(actor=actor, action_space=_Discrete(A))
+    policy = DiscreteSACPolicy(actor=actor, action_space=Discrete(A))
     obs = np.random.default_rng(0).standard_normal((2000, 3)).astype(np.float32)
     out = policy(Batch(obs=obs, info=Batch()))
     assert torch.equal(out.act, out.logits.argmax(-1)) and out.dist.probs.shape == (2000, A)
@@ -583,13 +554,6 @@ def test_policy_forward_mode_and_sample():
 
 # ------------------------------------------------------------------------------------------------------------ resources
 def test_rows_kernel_has_no_stack_frame_or_spills(tmp_path):
-    from tianshou_b200.csrc import build as B
-    if shutil.which(B.NVCC) is None and not os.path.exists(B.NVCC):
-        pytest.skip("nvcc not available")
-    r = subprocess.run([B.NVCC, *B.FLAGS, "-c", os.path.join(B.HERE, "discrete_sac.cu"), "-o", str(tmp_path / "d.o")],
-                       capture_output=True, text=True)
-    assert r.returncode == 0, r.stdout + r.stderr
-    hits = re.findall(r"Compiling entry function '(\S+)' for 'sm_90a'\n(?:.*\n)*?\s*(\d+) bytes stack frame, (\d+) bytes spill "
-                      r"stores, (\d+) bytes spill loads", r.stdout + r.stderr)
-    assert [h[0] for h in hits] and all("discrete_sac_rows_kernel" in h[0] for h in hits), hits
-    assert all(tuple(map(int, h[1:])) == (0, 0, 0) for h in hits), hits
+    report = ptxas_report("discrete_sac.cu", tmp_path)
+    assert all("discrete_sac_rows_kernel" in e for e in report), report
+    assert_spill_free(report)

@@ -3,7 +3,6 @@
 oracle/gen_golden_fqf.py), one update's gradients of both parameter groups against float64 autograd, bit-identical repeats,
 the ``state_dict()`` round trip, the batch edges, the policy's torch path, the refusals and the kernels' register report."""
 import copy
-import math
 
 import numpy as np
 import pytest
@@ -13,13 +12,13 @@ from torch import nn
 from oracle import oracle_discrete_sac as ods
 from oracle import oracle_fqf as of
 from oracle import oracle_iqn as oi
-from test_iqn_gpu import _register_report, fp64_quantiles
-from test_qrdqn_gpu import _Discrete, _st, buffer_from_golden, check_final_state, make_buffer, sms
+from offpolicy_testutil import (DEV, EPS, Discrete, assert_spill_free, capture_batches, capture_grads, check_final_state,
+                                check_second_batch_size, ptxas_report, sm_count, stream, vector_buffer_from_golden)
+from test_iqn_gpu import fp64_quantiles
+from test_qrdqn_gpu import make_buffer
 from ts_testutil import load_golden, record_parity, sum_length_rel
 
-DEV = "cuda:0"
 gpu = pytest.mark.gpu
-EPS = float(np.finfo(np.float32).eps)
 TINY = 2.0 ** -149                      # fp32's smallest subnormal: the spacing of every result below 2^-126
 VARIANTS = ["fqf_ref_mlp", "fqf_ref_relu", "fqf_ref_cnn", "fqf_ref_per"]
 
@@ -36,7 +35,7 @@ def _fractions(z):
     out = {k: torch.empty(*s, device=DEV) for k, s in (("taus", (B, N + 1)), ("tau_hats", (B, N)), ("inner", (B, N - 1)),
                                                        ("p", (B, N)), ("logp", (B, N)), ("H", (B,)))}
     call("ts_fqf_fractions", ptr(zd), B, N, ptr(out["taus"]), ptr(out["tau_hats"]), ptr(out["inner"]), ptr(out["p"]),
-         ptr(out["logp"]), ptr(out["H"]), _st())
+         ptr(out["logp"]), ptr(out["H"]), stream())
     torch.cuda.synchronize()
     return {k: v.cpu().numpy() for k, v in out.items()}
 
@@ -65,7 +64,7 @@ def test_fractions_kernel_vs_fp64(N, extreme):
     one rounding of the float64 value.  tau_hats is exactly (taus[:-1] + taus[1:]) / 2 in fp32, inner exactly taus[:, 1:-1].
     B runs past the block-per-row grid (8 blocks per SM) in one case."""
     rng = np.random.default_rng(N * 10 + extreme)
-    B = sms() * 8 + 37 if (N, extreme) == (13, False) else 41
+    B = sm_count() * 8 + 37 if (N, extreme) == (13, False) else 41
     z = _logits(B, N, rng, extreme)
     got = _fractions(z)
     ref = of.fractions(z)
@@ -106,7 +105,7 @@ def test_target_kernel_exact(A, N):
     actions.  B runs past the one-warp-per-row grid in one case; the same-buffer call is ``target_update_freq == 0``."""
     from tianshou_b200._cabi import call, ptr
     g = torch.Generator().manual_seed(A * 1000 + N)
-    B = sms() * 16 * 8 + 37 if (A, N) == (6, 13) else 301
+    B = sm_count() * 16 * 8 + 37 if (A, N) == (6, 13) else 301
     q = torch.randint(-3, 4, (B, N, A), generator=g).float()
     w = torch.randint(1, 8, (B, N), generator=g).double()
     taus = (torch.cumsum(torch.cat([torch.zeros(B, 1), w.float() / 1024], 1), 1)).float()          # dyadic: every width exact
@@ -116,7 +115,7 @@ def test_target_kernel_exact(A, N):
         q[B - 1, N - 1, A - 1] = float("nan")
     out, act = torch.empty(B, N, device=DEV), torch.empty(B, dtype=torch.int64, device=DEV)
     qd, td, nd = q.to(DEV), taus.to(DEV), q_next.to(DEV)
-    call("ts_fqf_target", ptr(qd), ptr(td), ptr(nd), B, A, N, ptr(out), ptr(act), _st())
+    call("ts_fqf_target", ptr(qd), ptr(td), ptr(nd), B, A, N, ptr(out), ptr(act), stream())
     torch.cuda.synchronize()
     ref_a = torch.as_tensor(of.fqf_select(q.numpy(), taus.numpy()))
     if A > 1:
@@ -128,7 +127,7 @@ def test_target_kernel_exact(A, N):
         assert bool(lead.any()) and bool((act.cpu()[: B // 3][lead] == 0).all())
         assert not torch.equal(ref_a, q.mean(1).argmax(1)), "the widths must matter"
     out_same = torch.empty(B, N, device=DEV)
-    call("ts_fqf_target", ptr(qd), ptr(td), ptr(qd), B, A, N, ptr(out_same), None, _st())
+    call("ts_fqf_target", ptr(qd), ptr(td), ptr(qd), B, A, N, ptr(out_same), None, stream())
     torch.cuda.synchronize()
     torch.testing.assert_close(out_same.cpu(), q[torch.arange(B), :, ref_a], rtol=0, atol=0, equal_nan=True)
 
@@ -139,7 +138,7 @@ def _fraction_rows(q_hat, q_tau, act, fr, ent_coef):
     B, N, A = q_hat.shape
     dz, rows, losses = torch.empty(B, N, device=DEV), torch.empty(3, B, device=DEV), torch.empty(8, device=DEV).fill_(7.0)
     a = (dev(q_hat), dev(q_tau), dev(act, torch.int64), dev(fr["taus"]), dev(fr["p"]), dev(fr["logp"]), dev(fr["H"]))
-    call("ts_fqf_fraction_rows", *(ptr(t) for t in a), B, A, N, float(ent_coef), ptr(dz), ptr(rows), losses.data_ptr() + 16, _st())
+    call("ts_fqf_fraction_rows", *(ptr(t) for t in a), B, A, N, float(ent_coef), ptr(dz), ptr(rows), losses.data_ptr() + 16, stream())
     torch.cuda.synchronize()
     l = losses.cpu().numpy()
     assert np.all(l[:4] == 7.0), "only the four floats past the pointer are written"
@@ -161,7 +160,7 @@ def test_fraction_rows_kernel_vs_fp64(N, extreme, ent_coef):
     product.  fraction_b sums g_i taus_i over the block, (N / 128 + 10) eps of sum |g tau| plus the g errors; the batch means
     come from row_sums3_kernel, (B / 1024 + 12) eps of the mean magnitude.  B runs past the block-per-row grid in one case."""
     rng = np.random.default_rng(N * 100 + extreme * 10 + int(ent_coef))
-    B, A = (sms() * 8 + 37 if (N, extreme, ent_coef) == (32, False, 10.0) else 41), 4
+    B, A = (sm_count() * 8 + 37 if (N, extreme, ent_coef) == (32, False, 10.0) else 41), 4
     fr = {k: v for k, v in _fractions(_logits(B, N, rng, extreme)).items()}
     q_hat = rng.standard_normal((B, N, A)).astype(np.float32)
     q_tau = rng.standard_normal((B, N - 1, A)).astype(np.float32)
@@ -211,13 +210,13 @@ def test_kernels_refuse_what_a_block_cannot_hold():
     a = torch.zeros(1, dtype=torch.int64, device=DEV)
     for N in (12289, 1, 0):
         with pytest.raises(RuntimeError, match="ts_fqf_fractions"):
-            call("ts_fqf_fractions", ptr(x), 1, N, ptr(x), ptr(x), ptr(x), ptr(x), ptr(x), ptr(x), _st())
+            call("ts_fqf_fractions", ptr(x), 1, N, ptr(x), ptr(x), ptr(x), ptr(x), ptr(x), ptr(x), stream())
         with pytest.raises(RuntimeError, match="ts_fqf_fraction_rows"):
             call("ts_fqf_fraction_rows", ptr(x), ptr(x), ptr(a), ptr(x), ptr(x), ptr(x), ptr(x), 1, 1, N, 0.0, ptr(x), ptr(x),
-                 ptr(x), _st())
+                 ptr(x), stream())
     with pytest.raises(RuntimeError, match="ent_coef"):
         call("ts_fqf_fraction_rows", ptr(x), ptr(x), ptr(a), ptr(x), ptr(x), ptr(x), ptr(x), 1, 1, 2, float("inf"), ptr(x),
-             ptr(x), ptr(x), _st())
+             ptr(x), ptr(x), stream())
 
 
 # ------------------------------------------------------------------------------------------------------------ vs reference
@@ -243,7 +242,7 @@ def build_from_golden(g):
     model, fm = model_from_cfg(kind, A, N, int(g["cfg_C"]), last=tuple(int(x) for x in g["cfg_last"]), **kw)
     ods.seeded_params(model, int(g["cfg_init_seed"]))
     of.seed_fraction_net(fm.net, int(g["cfg_init_seed"]) + 100)
-    policy = FQFPolicy(model=model, fraction_model=fm, action_space=_Discrete(A))
+    policy = FQFPolicy(model=model, fraction_model=fm, action_space=Discrete(A))
     frac = (RMSpropOptimizerFactory if str(g["cfg_frac_opt"]) == "rmsprop" else AdamOptimizerFactory)(lr=float(g["cfg_frac_lr"]))
     return FQF(policy=policy, optim=AdamOptimizerFactory(lr=float(g["cfg_lr"])), fraction_optim=frac, gamma=float(g["cfg_gamma"]),
                num_fractions=N, ent_coef=float(g["cfg_ent_coef"]), n_step_return_horizon=int(g["cfg_n_step"]),
@@ -281,37 +280,25 @@ def test_update_matches_reference_run(variant, mirror):
     the fraction loss and the first RMSprop steps amplify it), so that run stops after three updates."""
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden(f"{variant}.npz")
-    algo, buf = build_from_golden(g), buffer_from_golden(g, mirror)
+    algo, buf = build_from_golden(g), vector_buffer_from_golden(g, mirror)
     keys = [str(k) for k in g["state_dict_keys"]]
     assert list(algo.state_dict().keys()) == keys and len(algo._optimizers) == int(g["optimizer_count"]) == 2
     assert algo._optimizers == [algo.optim, algo.fraction_optim]
-    cap = {}
-    orig_pre, orig_post = algo._preprocess_batch, algo._postprocess_batch
-
-    def pre(batch, buffer, indices):
-        b = orig_pre(batch, buffer, indices)
-        cap["indices"], cap["returns"] = np.asarray(indices).copy(), b.returns.detach().cpu().numpy().copy()
-        return b
-
-    def post(batch, buffer, indices):
-        cap["prio"] = batch.weight.detach().cpu().numpy().copy()
-        return orig_post(batch, buffer, indices)
-
-    algo._preprocess_batch, algo._postprocess_batch = pre, post
-    for u in range(int(g["cfg_updates"])):
-        np.random.seed(500 + u)
-        with policy_within_training_step(algo.policy):
-            stats = algo.update(buffer=buf, sample_size=int(g["cfg_bs"]))
-        tag = f"{variant}_m{int(mirror)}_u{u}"
-        assert np.array_equal(cap["indices"], g[f"u{u}_indices"]), "sampled indices differ from the reference's"
-        ref_ret = g[f"u{u}_returns"]
-        record_parity(f"{tag}/returns", cap["returns"], ref_ret, rtol=1e-5, atol=1e-5 * float(np.abs(ref_ret).max()))
-        got = np.array([stats.loss, stats.quantile_loss, stats.fraction_loss, stats.entropy_loss])
-        record_parity(f"{tag}/losses", got, g[f"u{u}_losses"], rtol=2e-5, atol=2e-6 * float(np.abs(g[f"u{u}_losses"]).max()))
-        record_parity(f"{tag}/prio", cap["prio"], g[f"u{u}_prio"], rtol=2e-5, atol=2e-6)
-        if bool(g["cfg_per"]):
-            leaves = np.asarray(buf.weight[np.arange(len(buf))])
-            record_parity(f"{tag}/tree_leaves", leaves, g[f"u{u}_tree_leaves"], rtol=2e-5, atol=1e-7)
+    with capture_batches(algo) as cap:
+        for u in range(int(g["cfg_updates"])):
+            np.random.seed(500 + u)
+            with policy_within_training_step(algo.policy):
+                stats = algo.update(buffer=buf, sample_size=int(g["cfg_bs"]))
+            tag = f"{variant}_m{int(mirror)}_u{u}"
+            assert np.array_equal(cap["indices"], g[f"u{u}_indices"]), "sampled indices differ from the reference's"
+            ref_ret = g[f"u{u}_returns"]
+            record_parity(f"{tag}/returns", cap["returns"].cpu().numpy(), ref_ret, rtol=1e-5, atol=1e-5 * float(np.abs(ref_ret).max()))
+            got = np.array([stats.loss, stats.quantile_loss, stats.fraction_loss, stats.entropy_loss])
+            record_parity(f"{tag}/losses", got, g[f"u{u}_losses"], rtol=2e-5, atol=2e-6 * float(np.abs(g[f"u{u}_losses"]).max()))
+            record_parity(f"{tag}/prio", cap["prio"].cpu().numpy(), g[f"u{u}_prio"], rtol=2e-5, atol=2e-6)
+            if bool(g["cfg_per"]):
+                leaves = np.asarray(buf.weight[np.arange(len(buf))])
+                record_parity(f"{tag}/tree_leaves", leaves, g[f"u{u}_tree_leaves"], rtol=2e-5, atol=1e-7)
     check_final_state(f"{variant}_m{int(mirror)}", g, algo)
     check_fraction_state(f"{variant}_m{int(mirror)}", g, algo)
     assert list(algo.state_dict().keys()) == keys
@@ -326,7 +313,6 @@ def grad_case(kind, B=64, N=13, ent_coef=10.0, edge=""):
     dz^T feat, at the same bars: g_i is a difference of neighbouring quantiles, but the fp32 quantiles' errors stay far below
     them (DESIGN.md section 4)."""
     from tianshou_b200.algorithm import FQF, AdamOptimizerFactory, FQFPolicy, RMSpropOptimizerFactory
-    from tianshou_b200.algorithm.flat_params import FlatGroup
     from tianshou_b200.utils import policy_within_training_step
     torch.manual_seed(3)
     rng = np.random.default_rng(4)
@@ -336,34 +322,16 @@ def grad_case(kind, B=64, N=13, ent_coef=10.0, edge=""):
     else:
         model, fm = model_from_cfg("mlp", A, N, C=33, hidden=(48,), trunk_out=40 if kind == "mlp" else 0, last=(40,))
     of.seed_fraction_net(fm.net, 9)
-    policy = FQFPolicy(model=model, fraction_model=fm, action_space=_Discrete(A))
+    policy = FQFPolicy(model=model, fraction_model=fm, action_space=Discrete(A))
     algo = FQF(policy=policy, optim=AdamOptimizerFactory(lr=1e-3), fraction_optim=RMSpropOptimizerFactory(lr=1e-4), gamma=0.9,
                num_fractions=N, ent_coef=ent_coef, n_step_return_horizon=2, target_update_freq=3)
     buf = make_buffer(kind, A, rng)
-    cap = {}
     grp, fgrp = algo._group, algo._fgroup
-
-    def adam(optimizer, mgn):
-        cap["grad"] = grp.grad[: grp.n].clone()
-        FlatGroup.adam_step(grp, optimizer, mgn)
-
-    def fstep(optimizer, mgn):
-        cap["fgrad"] = fgrp.grad[: fgrp.n].clone()
-        FlatGroup.optimizer_step(fgrp, optimizer, mgn)
-
-    grp.adam_step, fgrp.optimizer_step = adam, fstep
-    orig_pre = algo._preprocess_batch
-
-    def pre(batch, buffer, indices):
-        b = orig_pre(batch, buffer, indices)
-        cap["indices"], cap["returns"] = np.asarray(indices).copy(), b.returns.detach().cpu().double()
-        return b
-
-    algo._preprocess_batch = pre
     ref = copy.deepcopy(model).to("cpu", torch.float64)
     rfm = copy.deepcopy(fm).to("cpu", torch.float64)
     np.random.seed(7)
-    with policy_within_training_step(algo.policy):
+    with (capture_batches(algo) as cap, capture_grads(grp) as grads, capture_grads(fgrp, "optimizer_step") as fgrads,
+          policy_within_training_step(algo.policy)):
         stats = algo.update(buffer=buf, sample_size=B)
     idx = cap["indices"]
     assert len(idx) == B
@@ -385,17 +353,17 @@ def grad_case(kind, B=64, N=13, ent_coef=10.0, edge=""):
         q_tau = fp64_quantiles(ref, x, taus[:, 1:-1])
     act = torch.as_tensor(np.asarray(buf.act)[idx].astype(np.int64))
     rows = torch.arange(B)
-    loss, _ = oi.reference_loss(q, act, cap["returns"], tau_hats, 1.0)
+    loss, _ = oi.reference_loss(q, act, cap["returns"].cpu().double(), tau_hats, 1.0)
     floss, fl, el = of.reference_fraction_loss(z, q[rows, act, :].detach(), q_tau[rows, act, :], ent_coef)
     (loss + floss).backward()
     rel = max(1e-4, sum_length_rel(B * N))
     for i, (p, r) in enumerate(zip(grp.params, ref.parameters(), strict=True)):
         want = r.grad.numpy()
-        got = grp.view(cap["grad"], p).view(p.shape).cpu().numpy()
+        got = grp.view(grads[-1], p).view(p.shape).cpu().numpy()
         record_parity(f"fqf_grad{edge}/{kind}/grad_{i}", got, want, rtol=2e-4, atol=rel * float(np.abs(want).max()) + 1e-12)
     for i, (p, r) in enumerate(zip(fgrp.params, rfm.parameters(), strict=True)):
         want = r.grad.numpy()
-        got = fgrp.view(cap["fgrad"], p).view(p.shape).cpu().numpy()
+        got = fgrp.view(fgrads[-1], p).view(p.shape).cpu().numpy()
         record_parity(f"fqf_grad{edge}/{kind}/fgrad_{i}", got, want, rtol=2e-4, atol=1e-4 * float(np.abs(want).max()) + 1e-12)
     want = [loss.item() + floss.item(), loss.item(), fl.item(), el.item()]
     got = [stats.loss, stats.quantile_loss, stats.fraction_loss, stats.entropy_loss]
@@ -413,7 +381,7 @@ def test_update_gradients_of_both_groups_vs_fp64_autograd(kind):
 @pytest.mark.parametrize("batch", ["one", "odd", "past_grid"])
 def test_update_gradients_at_batch_edges(batch):
     """B = 1, an odd B and the smallest B that takes the block-per-row kernels (8 blocks per SM) past their grid."""
-    B = {"one": 1, "odd": 17, "past_grid": sms() * 8 + 1}[batch]
+    B = {"one": 1, "odd": 17, "past_grid": sm_count() * 8 + 1}[batch]
     grad_case("mlp", B=B, N=32, edge=f"_{batch}")
 
 
@@ -422,26 +390,12 @@ def test_update_gradients_at_batch_edges(batch):
 def test_second_batch_size_is_bit_identical_to_a_fresh_instance(order):
     """One batch size, every scratch tensor filled with NaN, then another: both groups, the lagged copy, the statistics and the
     priorities equal, bit for bit, the second update of a fresh instance loaded from the same ``state_dict()``."""
-    from test_offpolicy_batch_edges_gpu import _poison, _rng_state, _set_rng_state, _state, _update
     g = load_golden("fqf_ref_relu.npz")         # a uniform buffer: a prioritised one would carry the first update's priorities
-    buf = buffer_from_golden(g)
-    large, small = sms() * 8 + 1, 3
+    large, small = sm_count() * 8 + 1, 3
     B1, B2 = (large, small) if order == "large_then_small" else (small, large)
-    a = build_from_golden(g)
-    _update(a, buf, B1, seed=1)
-    b = build_from_golden(g)
-    b.load_state_dict(copy.deepcopy(a.state_dict()))
-    b._iter = a._iter
-    rng = _rng_state(buf)
-    assert _poison(a) > 0
-    cap_a, stats_a = _update(a, buf, B2, seed=2)
-    _set_rng_state(buf, rng)
-    cap_b, stats_b = _update(b, buf, B2, seed=2)
-    assert np.array_equal(cap_a["indices"], cap_b["indices"]) and len(cap_a["indices"]) == B2
-    assert stats_a == stats_b and all(math.isfinite(v) for v in stats_a.values())
-    assert torch.equal(cap_a["prio"], cap_b["prio"])
-    sa, sb = _state(a), _state(b)
-    assert len(sa) == 12 and all(torch.equal(x, y) for x, y in zip(sa, sb, strict=True))
+    carry_iter = lambda a, b: setattr(b, "_iter", a._iter)
+    cap, state = check_second_batch_size(lambda: build_from_golden(g), vector_buffer_from_golden(g), B1, B2, carry=carry_iter)
+    assert cap["prio"] is not None and len(state) == 12
 
 
 # ------------------------------------------------------------------------------------------------------------ repeats, state_dict
@@ -455,7 +409,7 @@ def test_two_updates_from_one_state_agree_bit_for_bit():
     g = load_golden("fqf_ref_mlp.npz")
     algos = [build_from_golden(g), build_from_golden(g)]
     for a in algos:
-        buf = buffer_from_golden(g)
+        buf = vector_buffer_from_golden(g)
         for u in range(2):
             np.random.seed(20 + u)
             with policy_within_training_step(a.policy):
@@ -471,7 +425,7 @@ def test_state_dict_round_trip_continues_identically(variant):
     optimisers' state (RMSprop's square_avg, or Adam's moments).  ``_iter`` is a plain attribute, as in the reference."""
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden(f"{variant}.npz")
-    a, buf_a = build_from_golden(g), buffer_from_golden(g)
+    a, buf_a = build_from_golden(g), vector_buffer_from_golden(g)
     for u in range(3):
         np.random.seed(u)
         with policy_within_training_step(a.policy):
@@ -487,7 +441,7 @@ def test_state_dict_round_trip_continues_identically(variant):
     b.load_state_dict(sd)
     b._iter = a._iter
     for algo in (a, b):
-        buf = buffer_from_golden(g)
+        buf = vector_buffer_from_golden(g)
         for u in range(3):
             np.random.seed(10 + u)
             with policy_within_training_step(algo.policy):
@@ -505,7 +459,7 @@ def test_policy_action_and_fractions():
     torch.manual_seed(0)
     model, fm = model_from_cfg("mlp", 5, 11, C=17, hidden=(32,), trunk_out=0, last=(24,))
     of.seed_fraction_net(fm.net, 3)
-    policy = FQFPolicy(model=model, fraction_model=fm, action_space=_Discrete(5))
+    policy = FQFPolicy(model=model, fraction_model=fm, action_space=Discrete(5))
     obs = np.random.default_rng(0).standard_normal((300, 4)).astype(np.float32)
     batch = Batch(obs=obs, info=Batch())
     for training in (True, False):
@@ -532,7 +486,7 @@ def test_refusals():
 
     def make(model=None, fm=None, opt=AdamOptimizerFactory, fopt=RMSpropOptimizerFactory, **kw):
         m, f = model_from_cfg("mlp", A, N, C=8, hidden=(16,), trunk_out=16, last=(16,))
-        return FQF(policy=FQFPolicy(model=model or m, fraction_model=fm or f, action_space=_Discrete(A)), optim=opt(lr=1e-3),
+        return FQF(policy=FQFPolicy(model=model or m, fraction_model=fm or f, action_space=Discrete(A)), optim=opt(lr=1e-3),
                    fraction_optim=fopt(lr=1e-4), **kw)
 
     algo = make()
@@ -582,7 +536,7 @@ def test_refusals():
 
 # ------------------------------------------------------------------------------------------------------------ resources
 def test_kernels_have_no_stack_frame_or_spills(tmp_path):
-    hits = _register_report("fqf.cu", tmp_path)
+    report = ptxas_report("fqf.cu", tmp_path)
     kernels = ("fqf_fractions_kernel", "fqf_target_kernel", "fqf_fraction_rows_kernel", "row_sums3_kernel")
-    assert len(hits) == len(kernels) and all(any(k in h[0] for h in hits) for k in kernels), hits
-    assert all(tuple(map(int, h[1:])) == (0, 0, 0) for h in hits), hits
+    assert len(report) == len(kernels) and all(any(k in e for e in report) for k in kernels), report
+    assert_spill_free(report)

@@ -11,18 +11,14 @@ Yardsticks:
     the per-step losses at the per-row bars, accuracies exactly, parameters at 1e-3 + 0.1 lr, generator states identical.
 """
 import copy
-import os
-import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
+from offpolicy_testutil import DEV, ptxas_report, sm_count, stream
 from ts_testutil import Box, load_golden, record_parity, restore_vector_buffer
 
-DEV = "cuda:0"
 VARIANTS = ["gail_ref_tc", "gail_ref_merge", "gail_ref_steps", "gail_ref_layered"]
 gpu = pytest.mark.gpu
 
@@ -90,9 +86,9 @@ def _golden_algo(g, expert=None):
 @pytest.mark.parametrize("n", [1, 17, 1000, None])
 def test_reward_rows_vs_fp64(n):
     """-logsigmoid(-x) per row; None: 2 grid caps + 7 rows, every row must be written."""
-    from tianshou_b200._cabi import call, ptr, stream_ptr
+    from tianshou_b200._cabi import call, ptr
     if n is None:
-        n = torch.cuda.get_device_properties(0).multi_processor_count * 16 * 256 * 2 + 7
+        n = sm_count() * 16 * 256 * 2 + 7
     special = np.array([0.0, 1e-30, -1e-30, 20.0, -20.0, 88.0, -88.0, 100.0, -100.0, 1e4, -1e4], dtype=np.float32)
     x = (np.random.default_rng(n).standard_normal(n) * 5.0).astype(np.float32)
     x[: min(n, special.size)] = special[: min(n, special.size)]
@@ -100,7 +96,7 @@ def test_reward_rows_vs_fp64(n):
     ref = (-torch.nn.functional.logsigmoid(-xt.double())).numpy()
     torch_err = np.abs((-torch.nn.functional.logsigmoid(-xt)).double().numpy() - ref)
     rew = torch.full((n,), float("nan"), dtype=torch.float64, device=DEV)
-    call("ts_gail_reward_rows", ptr(xt.to(DEV)), n, ptr(rew), stream_ptr(torch.device(DEV)))
+    call("ts_gail_reward_rows", ptr(xt.to(DEV)), n, ptr(rew), stream())
     got = rew.cpu().numpy()
     assert np.isfinite(got).all()
     record_parity(f"gail_reward_rows/n{n}", got, ref, rtol=0.0, atol=8 * float(torch_err.max()) + 1e-7 * float(np.abs(ref).max()))
@@ -111,14 +107,14 @@ def test_reward_rows_vs_fp64(n):
 def test_disc_rows_vs_fp64_autograd(n_pi, n_exp):
     """Loss, accuracies and d loss / d logit of one discriminator step; exact zeros are counted on neither side, saturated
     rows (|x| = 100, 1e4) have gradients 0 or +-1 / n."""
-    from tianshou_b200._cabi import call, ptr, stream_ptr
+    from tianshou_b200._cabi import call, ptr
     rng = np.random.default_rng(n_pi)
     x = (rng.standard_normal(n_pi + n_exp) * 3.0).astype(np.float32)
     x[::7] = 0.0
     x[3::11] = 100.0
     x[5::13] = -1e4
     xt = torch.as_tensor(x)
-    st = stream_ptr(torch.device(DEV))
+    st = stream()
     outs = []
     for _ in range(2):
         dl = torch.empty(n_pi + n_exp, device=DEV)
@@ -399,16 +395,7 @@ def test_discriminator_loop_has_no_torch_host_sync():
 # ---------------------------------------------------------------------------------------------------------- resources
 def test_gail_kernels_are_spill_free(tmp_path):
     """ptxas's report for gail.cu (sm_90a): no stack frame and no spills in either kernel."""
-    from tianshou_b200.csrc import build as B
-    if shutil.which(B.NVCC) is None and not os.path.exists(B.NVCC):
-        pytest.skip("nvcc not available")
-    r = subprocess.run([B.NVCC, *B.FLAGS, "-c", os.path.join(B.HERE, "gail.cu"), "-o", str(tmp_path / "gail.o")],
-                       capture_output=True, text=True)
-    assert r.returncode == 0, r.stdout + r.stderr
-    found = {}
-    for m in re.finditer(r"Compiling entry function '(\S+)' for 'sm_90a'\n(?:.*\n)*?\s*(\d+) bytes stack frame, (\d+) bytes spill "
-                         r"stores, (\d+) bytes spill loads", r.stdout + r.stderr):
-        found[m.group(1)] = tuple(int(m.group(i)) for i in (2, 3, 4))
+    found = ptxas_report("gail.cu", tmp_path)
     for name in ("gail_reward_kernel", "gail_disc_kernel"):
         hits = [v for k, v in found.items() if name in k]
         assert hits == [(0, 0, 0)], (name, found)

@@ -3,10 +3,6 @@
 (tests/golden/iqn_ref_*.npz from oracle/gen_golden_iqn.py), one update's gradient against float64 autograd, bit-identical
 repeats, the ``state_dict()`` round trip, the policy's torch path, the refusals and the kernels' register report."""
 import copy
-import os
-import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -14,12 +10,12 @@ import torch
 
 from oracle import oracle_discrete_sac as ods
 from oracle import oracle_iqn as oi
-from test_qrdqn_gpu import _Discrete, _st, buffer_from_golden, check_final_state, make_buffer, sms
+from offpolicy_testutil import (DEV, EPS, Discrete, assert_spill_free, capture_batches, capture_grads, check_final_state,
+                                ptxas_report, sm_count, stream, vector_buffer_from_golden)
+from test_qrdqn_gpu import make_buffer
 from ts_testutil import load_golden, record_parity, sum_length_rel
 
-DEV = "cuda:0"
 gpu = pytest.mark.gpu
-EPS = float(np.finfo(np.float32).eps)
 VARIANTS = ["iqn_ref_mlp", "iqn_ref_sizes", "iqn_ref_cnn", "iqn_ref_per"]
 ACTS = {"none": 0, "relu": 1, "tanh": 2}
 
@@ -33,7 +29,7 @@ def _cos(taus, C):
     from tianshou_b200._cabi import call, ptr
     t = dev(taus.reshape(-1))
     out = torch.empty(t.numel(), C, device=DEV)
-    call("ts_iqn_cos", ptr(t), t.numel(), C, ptr(out), _st())
+    call("ts_iqn_cos", ptr(t), t.numel(), C, ptr(out), stream())
     torch.cuda.synchronize()
     return out.cpu().numpy()
 
@@ -47,7 +43,7 @@ def test_cos_kernel_argument_and_accuracy(C):
     fused product) falls outside the bound.  The case with C = 64 checks that it does.  tau = 0 gives 1 exactly; tau just
     below 1 is the largest fraction torch.rand returns.  R runs past the one-warp-per-row grid."""
     rng = np.random.default_rng(C)
-    R = sms() * 16 * 8 + 37 if C == 17 else 300
+    R = sm_count() * 16 * 8 + 37 if C == 17 else 300
     taus = rng.random(R).astype(np.float32)
     taus[0], taus[1] = 0.0, np.nextafter(np.float32(1.0), np.float32(0.0))
     got = _cos(taus, C)
@@ -82,7 +78,7 @@ def test_mix_and_mix_backward_vs_fp64(D, S, act):
     nothing.  B runs past the element-wise grid (8 blocks per SM) in the largest case."""
     from tianshou_b200._cabi import call, ptr
     rng = np.random.default_rng(D * 100 + S * 3 + ACTS[act])
-    B = sms() * 8 * 256 // D + 5 if (D, S) == (3136, 8) else 33
+    B = sm_count() * 8 * 256 // D + 5 if (D, S) == (3136, 8) else 33
     feat, e, dh = _mix_case(B, S, D, rng)
     if act == "relu":
         feat = np.maximum(feat, 0.0)
@@ -90,14 +86,14 @@ def test_mix_and_mix_backward_vs_fp64(D, S, act):
         feat = np.tanh(feat).astype(np.float32)
     f_d, e_d, dh_d = dev(feat), dev(e), dev(dh)
     h = torch.empty(B * S, D, device=DEV)
-    call("ts_iqn_mix", ptr(f_d), ptr(e_d), B, S, D, ptr(h), _st())
+    call("ts_iqn_mix", ptr(f_d), ptr(e_d), B, S, D, ptr(h), stream())
     want_h = (np.repeat(feat, S, axis=0) * e).astype(np.float32)
     assert np.array_equal(h.cpu().numpy(), want_h)
 
     def backward():
         dfeat, de = torch.empty(B, D, device=DEV), torch.empty(B * S, D, device=DEV)
         call("ts_iqn_mix_backward", ptr(dh_d), ptr(f_d), ptr(e_d), B, S, D, ACTS[act], ptr(f_d) if act != "none" else None,
-             ptr(dfeat), ptr(de), _st())
+             ptr(dfeat), ptr(de), stream())
         torch.cuda.synchronize()
         return dfeat.cpu().numpy(), de.cpu().numpy()
 
@@ -125,7 +121,7 @@ def test_target_kernel_exact(A, S_on, S_next):
     runs past the one-warp-per-row grid in one case; the same-buffer call is ``target_update_freq == 0``."""
     from tianshou_b200._cabi import call, ptr
     g = torch.Generator().manual_seed(A * 1000 + S_on * 10 + S_next)
-    B = sms() * 16 * 8 + 37 if (A, S_on) == (6, 8) and S_next == 5 else 301
+    B = sm_count() * 16 * 8 + 37 if (A, S_on) == (6, 8) and S_next == 5 else 301
     q = torch.randint(-3, 4, (B, S_on, A), generator=g).float()
     q_next = torch.randn(B, S_next, A, generator=g)
     if A > 1:
@@ -133,7 +129,7 @@ def test_target_kernel_exact(A, S_on, S_next):
         q[B - 1, S_on - 1, A - 1] = float("nan")                       # a NaN mean wins
     out, act = torch.empty(B, S_next, device=DEV), torch.empty(B, dtype=torch.int64, device=DEV)
     qd, nd = q.to(DEV), q_next.to(DEV)
-    call("ts_iqn_target", ptr(qd), ptr(nd), B, A, S_on, S_next, ptr(out), ptr(act), _st())
+    call("ts_iqn_target", ptr(qd), ptr(nd), B, A, S_on, S_next, ptr(out), ptr(act), stream())
     torch.cuda.synchronize()
     ref_a = q.mean(1).argmax(1)
     assert torch.equal(act.cpu(), ref_a)
@@ -143,7 +139,7 @@ def test_target_kernel_exact(A, S_on, S_next):
         assert bool(lead.any()) and bool((act.cpu()[: B // 3][lead] == 0).all())
         assert int(act[B - 1]) == A - 1
     out_same = torch.empty(B, S_on, device=DEV)
-    call("ts_iqn_target", ptr(qd), ptr(qd), B, A, S_on, S_on, ptr(out_same), None, _st())
+    call("ts_iqn_target", ptr(qd), ptr(qd), B, A, S_on, S_on, ptr(out_same), None, stream())
     torch.cuda.synchronize()
     torch.testing.assert_close(out_same.cpu(), q[torch.arange(B), :, ref_a], rtol=0, atol=0, equal_nan=True)
 
@@ -156,7 +152,7 @@ def _rows(q, act, ret, taus, w):
     dq, prio = torch.empty(B, S_on, A, device=DEV), torch.empty(B, device=DEV)
     rows, losses = torch.empty(3, B, device=DEV), torch.empty(4, device=DEV)
     call("ts_iqn_rows", ptr(q), ptr(act), ptr(ret), ptr(taus), ptr(w), B, A, S_on, S_t, ptr(dq), ptr(prio), ptr(rows), ptr(losses),
-         _st())
+         stream())
     torch.cuda.synchronize()
     return losses.cpu().numpy(), dq.cpu().numpy(), prio.cpu().numpy()
 
@@ -174,7 +170,7 @@ def test_rows_kernel_vs_fp64(A, S_on, S_t, weighted):
     then adds the per-thread partials, five butterfly levels and eight warp partials, (S_t + 20) eps in all for qr_b and prio_b
     (every term is >= 0).  The batch mean comes from row_sums3_kernel: (B / 1024 + 12) eps times the mean magnitude."""
     rng = np.random.default_rng(A * 7919 + S_on * 31 + S_t + weighted * 3)
-    B = sms() * 8 + 37 if (A, S_on, weighted) == (6, 8, True) else 41
+    B = sm_count() * 8 + 37 if (A, S_on, weighted) == (6, 8, True) else 41
     q = (rng.standard_normal((B, S_on, A)) * 2).astype(np.float32)
     act = rng.integers(0, A, B)
     ret = (q[np.arange(B), 0, act][:, None] + rng.standard_normal((B, S_t)) * 1.5).astype(np.float32)
@@ -216,7 +212,7 @@ def test_rows_kernel_refuses_what_shared_memory_cannot_hold():
     a = torch.zeros(1, dtype=torch.int64, device=DEV)
     for S_on, S_t in ((8, 12289), (2, 100000), (0, 8)):
         with pytest.raises(RuntimeError, match="ts_iqn_rows"):
-            call("ts_iqn_rows", ptr(x), ptr(a), ptr(x), ptr(x), None, 1, 1, S_on, S_t, ptr(x), ptr(x), ptr(x), ptr(x), _st())
+            call("ts_iqn_rows", ptr(x), ptr(a), ptr(x), ptr(x), None, 1, 1, S_on, S_t, ptr(x), ptr(x), ptr(x), ptr(x), stream())
 
 
 # ------------------------------------------------------------------------------------------------------------ vs reference
@@ -240,7 +236,7 @@ def build_from_golden(g, mirror_taus=None):
     A = int(g["cfg_A"])
     model = model_from_cfg(kind, A, int(g["cfg_C"]), last=tuple(int(x) for x in g["cfg_last"]), **kw)
     ods.seeded_params(model, int(g["cfg_init_seed"]))
-    policy = IQNPolicy(model=model, action_space=_Discrete(A), sample_size=int(g["cfg_S"]), online_sample_size=int(g["cfg_S_on"]),
+    policy = IQNPolicy(model=model, action_space=Discrete(A), sample_size=int(g["cfg_S"]), online_sample_size=int(g["cfg_S_on"]),
                        target_sample_size=int(g["cfg_S_t"]))
     return IQN(policy=policy, optim=AdamOptimizerFactory(lr=float(g["cfg_lr"])), gamma=float(g["cfg_gamma"]),
                n_step_return_horizon=int(g["cfg_n_step"]), target_update_freq=int(g["cfg_freq"]))
@@ -273,36 +269,24 @@ def test_update_matches_reference_run(variant, mirror):
     leaves), then the final state at the QR-DQN bars (DESIGN.md section 4) and the reference's ``state_dict()`` keys."""
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden(f"{variant}.npz")
-    algo, buf = build_from_golden(g), buffer_from_golden(g, mirror)
+    algo, buf = build_from_golden(g), vector_buffer_from_golden(g, mirror)
     keys = [str(k) for k in g["state_dict_keys"]]
     assert list(algo.state_dict().keys()) == keys
     rest = replay_taus(algo, _golden_taus(g))
-    cap = {}
-    orig_pre, orig_post = algo._preprocess_batch, algo._postprocess_batch
-
-    def pre(batch, buffer, indices):
-        b = orig_pre(batch, buffer, indices)
-        cap["indices"], cap["returns"] = np.asarray(indices).copy(), b.returns.detach().cpu().numpy().copy()
-        return b
-
-    def post(batch, buffer, indices):
-        cap["prio"] = batch.weight.detach().cpu().numpy().copy()
-        return orig_post(batch, buffer, indices)
-
-    algo._preprocess_batch, algo._postprocess_batch = pre, post
-    for u in range(int(g["cfg_updates"])):
-        np.random.seed(500 + u)
-        with policy_within_training_step(algo.policy):
-            stats = algo.update(buffer=buf, sample_size=int(g["cfg_bs"]))
-        tag = f"{variant}_m{int(mirror)}_u{u}"
-        assert np.array_equal(cap["indices"], g[f"u{u}_indices"]), "sampled indices differ from the reference's"
-        ref_ret = g[f"u{u}_returns"]
-        record_parity(f"{tag}/returns", cap["returns"], ref_ret, rtol=1e-5, atol=1e-5 * float(np.abs(ref_ret).max()))
-        record_parity(f"{tag}/losses", np.array([stats.loss]), g[f"u{u}_losses"], rtol=2e-5, atol=2e-6)
-        record_parity(f"{tag}/prio", cap["prio"], g[f"u{u}_prio"], rtol=2e-5, atol=2e-6)
-        if bool(g["cfg_per"]):
-            leaves = np.asarray(buf.weight[np.arange(len(buf))])
-            record_parity(f"{tag}/tree_leaves", leaves, g[f"u{u}_tree_leaves"], rtol=2e-5, atol=1e-7)
+    with capture_batches(algo) as cap:
+        for u in range(int(g["cfg_updates"])):
+            np.random.seed(500 + u)
+            with policy_within_training_step(algo.policy):
+                stats = algo.update(buffer=buf, sample_size=int(g["cfg_bs"]))
+            tag = f"{variant}_m{int(mirror)}_u{u}"
+            assert np.array_equal(cap["indices"], g[f"u{u}_indices"]), "sampled indices differ from the reference's"
+            ref_ret = g[f"u{u}_returns"]
+            record_parity(f"{tag}/returns", cap["returns"].cpu().numpy(), ref_ret, rtol=1e-5, atol=1e-5 * float(np.abs(ref_ret).max()))
+            record_parity(f"{tag}/losses", np.array([stats.loss]), g[f"u{u}_losses"], rtol=2e-5, atol=2e-6)
+            record_parity(f"{tag}/prio", cap["prio"].cpu().numpy(), g[f"u{u}_prio"], rtol=2e-5, atol=2e-6)
+            if bool(g["cfg_per"]):
+                leaves = np.asarray(buf.weight[np.arange(len(buf))])
+                record_parity(f"{tag}/tree_leaves", leaves, g[f"u{u}_tree_leaves"], rtol=2e-5, atol=1e-7)
     assert next(rest, None) is None, "every fraction the reference drew is used, in order"
     check_final_state(f"{variant}_m{int(mirror)}", g, algo)
     assert list(algo.state_dict().keys()) == keys
@@ -333,7 +317,6 @@ def grad_case(kind, B=64, S_on=6, S_t=7, edge=""):
     device and float64 here (a relative 6e-8 per element): 2e-4 relative plus 1e-4 of the tensor's largest value, as in
     test_qrdqn_gpu."""
     from tianshou_b200.algorithm import IQN, AdamOptimizerFactory, IQNPolicy
-    from tianshou_b200.algorithm.flat_params import FlatGroup
     from tianshou_b200.utils import policy_within_training_step
     torch.manual_seed(3)
     rng = np.random.default_rng(4)
@@ -342,18 +325,11 @@ def grad_case(kind, B=64, S_on=6, S_t=7, edge=""):
         model = model_from_cfg("cnn", A, C=33, last=(48,))
     else:
         model = model_from_cfg("mlp", A, C=33, hidden=(48,), trunk_out=40 if kind == "mlp" else 0, last=(40,))
-    policy = IQNPolicy(model=model, action_space=_Discrete(A), online_sample_size=S_on, target_sample_size=S_t)
+    policy = IQNPolicy(model=model, action_space=Discrete(A), online_sample_size=S_on, target_sample_size=S_t)
     algo = IQN(policy=policy, optim=AdamOptimizerFactory(lr=1e-3), gamma=0.9, n_step_return_horizon=2, target_update_freq=3)
     assert algo._trunk_act == (1 if kind == "relu_trunk" else 0)
     buf = make_buffer(kind, A, rng)
-    cap = {}
     grp = algo._group
-
-    def adam(optimizer, mgn):
-        cap["grad"] = grp.grad[: grp.n].clone()
-        FlatGroup.adam_step(grp, optimizer, mgn)
-
-    grp.adam_step = adam
     draws = []
     orig_draw = algo._draw_taus
 
@@ -362,17 +338,9 @@ def grad_case(kind, B=64, S_on=6, S_t=7, edge=""):
         return draws[-1]
 
     algo._draw_taus = draw
-    orig_pre = algo._preprocess_batch
-
-    def pre(batch, buffer, indices):
-        b = orig_pre(batch, buffer, indices)
-        cap["indices"], cap["returns"] = np.asarray(indices).copy(), b.returns.detach().cpu().double()
-        return b
-
-    algo._preprocess_batch = pre
     ref = copy.deepcopy(model).to("cpu", torch.float64)         # the weights before the step
     np.random.seed(7)
-    with policy_within_training_step(algo.policy):
+    with capture_batches(algo) as cap, capture_grads(grp) as grads, policy_within_training_step(algo.policy):
         stats = algo.update(buffer=buf, sample_size=B)
     assert len(draws) == 3 and draws[0].shape == (B, S_on) and draws[1].shape == (B, S_t) and draws[2].shape == (B, S_on)
     assert len(cap["indices"]) == B, "the update must run on the B sampled rows"
@@ -385,11 +353,11 @@ def grad_case(kind, B=64, S_on=6, S_t=7, edge=""):
         x = torch.as_tensor(raw).double()
     q = fp64_quantiles(ref, x, draws[2].cpu().double())
     act = np.asarray(buf.act)[idx].astype(np.int64)
-    loss, _ = oi.reference_loss(q, act, cap["returns"], draws[2].cpu().double(), 1.0)
+    loss, _ = oi.reference_loss(q, act, cap["returns"].cpu().double(), draws[2].cpu().double(), 1.0)
     loss.backward()
     for i, (p, r) in enumerate(zip(grp.params, ref.parameters(), strict=True)):
         want = r.grad.numpy()
-        got = grp.view(cap["grad"], p).view(p.shape).cpu().numpy()
+        got = grp.view(grads[-1], p).view(p.shape).cpu().numpy()
         # the embedding and head gradients sum B x S_on rows: the documented sum-length term where it passes 1e-4
         rel = max(1e-4, sum_length_rel(B * S_on))
         record_parity(f"iqn_grad{edge}/{kind}/grad_{i}", got, want, rtol=2e-4, atol=rel * float(np.abs(want).max()) + 1e-12)
@@ -409,7 +377,7 @@ def test_two_updates_from_one_state_agree_bit_for_bit():
     algos = [build_from_golden(g), build_from_golden(g)]
     for a in algos:
         a._draw_taus = _seeded_draws(5)
-        buf = buffer_from_golden(g)
+        buf = vector_buffer_from_golden(g)
         for u in range(2):
             np.random.seed(20 + u)
             with policy_within_training_step(a.policy):
@@ -426,7 +394,7 @@ def test_state_dict_round_trip_continues_identically(variant):
     optimiser state.  ``_iter`` is a plain attribute, as in the reference: whoever restores a run restores it too."""
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden(f"{variant}.npz")
-    a, buf_a = build_from_golden(g), buffer_from_golden(g)
+    a, buf_a = build_from_golden(g), vector_buffer_from_golden(g)
     a._draw_taus = _seeded_draws(1)
     for u in range(3):
         np.random.seed(u)
@@ -440,7 +408,7 @@ def test_state_dict_round_trip_continues_identically(variant):
     b._iter = a._iter
     for algo in (a, b):
         algo._draw_taus = _seeded_draws(2)
-        buf = buffer_from_golden(g)
+        buf = vector_buffer_from_golden(g)
         for u in range(3):
             np.random.seed(10 + u)
             with policy_within_training_step(algo.policy):
@@ -460,7 +428,7 @@ def test_policy_sample_sizes_and_arg_max():
     torch.manual_seed(0)
     model = model_from_cfg("mlp", 5, C=17, hidden=(32,), trunk_out=0, last=(24,))
     assert isinstance(model, ImplicitQuantileNetwork)
-    policy = IQNPolicy(model=model, action_space=_Discrete(5), sample_size=11, online_sample_size=6, target_sample_size=4)
+    policy = IQNPolicy(model=model, action_space=Discrete(5), sample_size=11, online_sample_size=6, target_sample_size=4)
     obs = np.random.default_rng(0).standard_normal((300, 4)).astype(np.float32)
     batch = Batch(obs=obs, info=Batch())
     policy.train()
@@ -480,7 +448,7 @@ def test_policy_sample_sizes_and_arg_max():
     assert torch.equal(again.logits, logits) and torch.equal(again.taus, taus)
     for kw in (dict(sample_size=1), dict(online_sample_size=1), dict(target_sample_size=1)):
         with pytest.raises(AssertionError, match="should be greater than 1"):
-            IQNPolicy(model=model, action_space=_Discrete(5), **kw)
+            IQNPolicy(model=model, action_space=Discrete(5), **kw)
 
 
 # ------------------------------------------------------------------------------------------------------------ refusals
@@ -497,7 +465,7 @@ def test_refusals():
 
     def make(model=None, opt=AdamOptimizerFactory, n=A, **kw):
         model = model or model_from_cfg("mlp", A, C=8, hidden=(16,), trunk_out=16, last=(16,))
-        return IQN(policy=IQNPolicy(model=model, action_space=_Discrete(n)), optim=opt(lr=1e-3), **kw)
+        return IQN(policy=IQNPolicy(model=model, action_space=Discrete(n)), optim=opt(lr=1e-3), **kw)
 
     algo = make()
     assert isinstance(algo, QRDQN)
@@ -542,22 +510,12 @@ def test_refusals():
 
 
 # ------------------------------------------------------------------------------------------------------------ resources
-def _register_report(src, tmp_path):
-    from tianshou_b200.csrc import build as B
-    if shutil.which(B.NVCC) is None and not os.path.exists(B.NVCC):
-        pytest.skip("nvcc not available")
-    r = subprocess.run([B.NVCC, *B.FLAGS, "-c", os.path.join(B.HERE, src), "-o", str(tmp_path / "k.o")], capture_output=True,
-                       text=True)
-    assert r.returncode == 0, r.stdout + r.stderr
-    return re.findall(r"Compiling entry function '(\S+)' for 'sm_90a'\n(?:.*\n)*?\s*(\d+) bytes stack frame, (\d+) bytes spill "
-                      r"stores, (\d+) bytes spill loads", r.stdout + r.stderr)
-
-
 def test_kernels_have_no_stack_frame_or_spills(tmp_path):
-    hits = _register_report("iqn.cu", tmp_path)
+    report = ptxas_report("iqn.cu", tmp_path)
     kernels = ("iqn_cos_kernel", "iqn_mix_kernel", "iqn_mix_backward_kernel", "iqn_target_kernel", "iqn_rows_kernel",
                "row_sums3_kernel")
-    assert len(hits) == len(kernels) and all(any(k in h[0] for h in hits) for k in kernels), hits
-    assert all(tuple(map(int, h[1:])) == (0, 0, 0) for h in hits), hits
-    hits = _register_report("qrdqn.cu", tmp_path)
-    assert len(hits) == 3 and all(tuple(map(int, h[1:])) == (0, 0, 0) for h in hits), hits
+    assert len(report) == len(kernels) and all(any(k in e for e in report) for k in kernels), report
+    assert_spill_free(report)
+    report = ptxas_report("qrdqn.cu", tmp_path)
+    assert len(report) == 3, report
+    assert_spill_free(report)

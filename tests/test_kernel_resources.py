@@ -5,11 +5,10 @@ spills or a stack frame, at both padded obs widths; the training kernels keep th
 (2.3 KB per thread before the kernels were templated on the padded obs width).  No wgmma may be serialised by the compiler."""
 import os
 import re
-import shutil
-import subprocess
 
 import pytest
 
+from offpolicy_testutil import parse_ptxas, ptxas_log
 from tianshou_b200.csrc import build as B
 
 MLP_TC = os.path.join(B.HERE, "mlp_tc.cu")
@@ -18,17 +17,8 @@ SPILL_BOUND = 512   # bytes of spill stores / loads of ppo_tc_kernel<EPOCH, KXP>
 
 @pytest.fixture(scope="module")
 def report(tmp_path_factory):
-    if shutil.which(B.NVCC) is None and not os.path.exists(B.NVCC):
-        pytest.skip("nvcc not available")
-    out = tmp_path_factory.mktemp("ptxas") / "mlp_tc.o"
-    r = subprocess.run([B.NVCC, *B.FLAGS, "-c", MLP_TC, "-o", str(out)], capture_output=True, text=True)
-    assert r.returncode == 0, r.stdout + r.stderr
-    log = r.stdout + r.stderr
-    kernels = {}
-    for m in re.finditer(r"Compiling entry function '(\S+)' for 'sm_90a'\n(?:.*\n)*?\s*(\d+) bytes stack frame, (\d+) bytes spill "
-                         r"stores, (\d+) bytes spill loads", log):
-        kernels[m.group(1)] = (int(m.group(2)), int(m.group(3)), int(m.group(4)))
-    return log, kernels
+    log = ptxas_log(MLP_TC, tmp_path_factory.mktemp("ptxas"))
+    return log, parse_ptxas(log)
 
 
 def _entry(kernels, pattern):

@@ -6,36 +6,10 @@ import numpy as np
 import pytest
 import torch
 
+from offpolicy_testutil import DEV, Box, Discrete, check_params, load_params
 from ts_testutil import load_golden, record_parity, set_buffer_state
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-
-
-class _Box:
-    def __init__(self, dim):
-        self.shape = (dim,)
-        self.low = -np.ones(dim, np.float32)
-        self.high = np.ones(dim, np.float32)
-
-
-class _Discrete:
-    def __init__(self, n):
-        self.n = n
-        self.shape = ()
-
-
-def _load(mod, g, prefix):
-    with torch.no_grad():
-        for i, p in enumerate(mod.parameters()):
-            p.copy_(torch.as_tensor(g[f"{prefix}{i}"]).reshape(p.shape))
-
-
-def _check_params(tag, mod, g, prefix, lr):
-    for i, p in enumerate(mod.parameters()):
-        ref = g[f"{prefix}{i}"]
-        # Adam normalises the step to ~lr per element: the absolute term is stated in units of one step
-        record_parity(f"{tag}/{prefix}{i}", p.detach().cpu().numpy(), ref, rtol=1e-3, atol=0.1 * lr)
 
 
 # ------------------------------------------------------------------------------------------------------------ SAC
@@ -50,8 +24,8 @@ def _build_sac(g, **kw):
                                          conditioned_sigma=True).to(DEV)
     c1 = ContinuousCritic(preprocess_net=Net(state_shape=(O,), action_shape=(A,), hidden_sizes=H, concat=True)).to(DEV)
     c2 = ContinuousCritic(preprocess_net=Net(state_shape=(O,), action_shape=(A,), hidden_sizes=H, concat=True)).to(DEV)
-    _load(actor, g, "p0_actor_"); _load(c1, g, "p0_c1_"); _load(c2, g, "p0_c2_")
-    policy = SACPolicy(actor=actor, action_space=_Box(A))
+    load_params(actor, g, "p0_actor_"); load_params(c1, g, "p0_c1_"); load_params(c2, g, "p0_c2_")
+    policy = SACPolicy(actor=actor, action_space=Box(A))
     algo = SAC(policy=policy, policy_optim=AdamOptimizerFactory(lr=lr), critic=c1, critic_optim=AdamOptimizerFactory(lr=lr),
                critic2=c2, critic2_optim=AdamOptimizerFactory(lr=lr), tau=float(g["cfg_tau"]), gamma=float(g["cfg_gamma"]),
                alpha=float(g["cfg_alpha"]), n_step_return_horizon=int(g["cfg_n_step"]), **kw)
@@ -92,8 +66,8 @@ def test_sac_update_matches_reference(mirror):
         record_parity(f"{tag}/returns", captured["returns"].reshape(ref_ret.shape), ref_ret, rtol=1e-5, atol=1e-5 * float(np.abs(ref_ret).max()))
         got = np.array([stats.actor_loss, stats.critic1_loss, stats.critic2_loss])
         record_parity(f"{tag}/losses", got, g[o + "losses"], rtol=2e-5, atol=2e-6)
-        _check_params(tag, actor, g, o + "actor_", lr); _check_params(tag, c1, g, o + "c1_", lr); _check_params(tag, c2, g, o + "c2_", lr)
-        _check_params(tag, algo.critic_old, g, o + "c1old_", lr); _check_params(tag, algo.critic2_old, g, o + "c2old_", lr)
+        check_params(tag, actor, g, o + "actor_", lr); check_params(tag, c1, g, o + "c1_", lr); check_params(tag, c2, g, o + "c2_", lr)
+        check_params(tag, algo.critic_old, g, o + "c1old_", lr); check_params(tag, algo.critic2_old, g, o + "c2old_", lr)
         assert stats.alpha == pytest.approx(float(g["cfg_alpha"])) and stats.alpha_loss is None and stats.train_time > 0
 
 
@@ -120,8 +94,8 @@ def test_sac_cuda_graph_matches_reference():
         assert np.array_equal(algo._graph["h_idx"].numpy(), g[o + "indices"]), "sampled indices differ from the reference's"
         got = np.array([stats.actor_loss, stats.critic1_loss, stats.critic2_loss])
         record_parity(f"{tag}/losses", got, g[o + "losses"], rtol=2e-5, atol=2e-6)
-        _check_params(tag, actor, g, o + "actor_", lr); _check_params(tag, c1, g, o + "c1_", lr); _check_params(tag, c2, g, o + "c2_", lr)
-        _check_params(tag, algo.critic_old, g, o + "c1old_", lr); _check_params(tag, algo.critic2_old, g, o + "c2old_", lr)
+        check_params(tag, actor, g, o + "actor_", lr); check_params(tag, c1, g, o + "c1_", lr); check_params(tag, c2, g, o + "c2_", lr)
+        check_params(tag, algo.critic_old, g, o + "c1old_", lr); check_params(tag, algo.critic2_old, g, o + "c2old_", lr)
     assert algo._graph["graph"] is not None and algo._graph["calls"] == n_up
     for grp in algo._g_c:
         grp.sync_step_from_device()
@@ -150,7 +124,7 @@ def test_sac_refuses_networks_off_one_cuda_device():
                                          conditioned_sigma=True).to(DEV)
     critic = ContinuousCritic(preprocess_net=Net(state_shape=(O,), action_shape=(A,), hidden_sizes=(8,), concat=True))
     with pytest.raises(UnsupportedModelError, match="no CPU path"):
-        SAC(policy=SACPolicy(actor=actor, action_space=_Box(A)), policy_optim=AdamOptimizerFactory(lr=1e-3), critic=critic,
+        SAC(policy=SACPolicy(actor=actor, action_space=Box(A)), policy_optim=AdamOptimizerFactory(lr=1e-3), critic=critic,
             critic_optim=AdamOptimizerFactory(lr=1e-3))
     assert next(critic.parameters()).device.type == "cpu"
 
@@ -163,8 +137,8 @@ def _build_dqn(g):
     H, W, A = int(g["cfg_H"]), int(g["cfg_W"]), int(g["cfg_A"])
     lr = float(g["cfg_lr"])
     net = ScaledObsInputActionReprNet(DQNet(4, H, W, A)).to(DEV)
-    _load(net, g, "p0_q_")
-    policy = DiscreteQLearningPolicy(model=net, action_space=_Discrete(A))
+    load_params(net, g, "p0_q_")
+    policy = DiscreteQLearningPolicy(model=net, action_space=Discrete(A))
     huber = float(g["cfg_huber"])
     algo = DQN(policy=policy, optim=AdamOptimizerFactory(lr=lr), gamma=float(g["cfg_gamma"]), n_step_return_horizon=int(g["cfg_n_step"]),
                target_update_freq=int(g["cfg_target_freq"]), is_double=bool(g["cfg_is_double"]),
@@ -219,9 +193,9 @@ def test_dqn_update_matches_reference(variant, mirror):
         record_parity(f"{tag}/loss", np.array([stats.loss]), np.array([float(g[o + "loss"])]), rtol=2e-5, atol=1e-6)
         record_parity(f"{tag}/tree_leaves", np.asarray(buf.weight[np.arange(len(buf))]), g[o + "tree_leaves"], rtol=1e-4, atol=1e-7)
     o = f"u{n_up - 1}_"
-    _check_params(f"dqn{variant}_m{int(mirror)}", net, g, o + "q_", lr)
+    check_params(f"dqn{variant}_m{int(mirror)}", net, g, o + "q_", lr)
     if algo.model_old is not None:
-        _check_params(f"dqn{variant}_m{int(mirror)}", algo.model_old, g, o + "qold_", lr)
+        check_params(f"dqn{variant}_m{int(mirror)}", algo.model_old, g, o + "qold_", lr)
 
 
 def test_dqn_policy_forward_and_eps_greedy():
@@ -277,7 +251,7 @@ def _check_grads(tag, mod, group, grad, ref_mod, rows=0):
         record_parity(f"{tag}/grad_{name}", got, ref, rtol=2e-4, atol=rel * float(np.abs(ref).max()) + 1e-12)
 
 
-def _sac_grad_case(O, A, H, separate_critic2, per, auto_alpha, seed, B=256, edge=""):
+def sac_grad_case(O, A, H, separate_critic2, per, auto_alpha, seed, B=256, edge=""):
     """One SAC update at batch ``B`` checked against float64 autograd; returns the captured batch and the update's stats."""
     from tianshou_b200.algorithm import AdamOptimizerFactory
     from tianshou_b200.algorithm.modelfree.sac import SAC, AutoAlpha, SACPolicy
@@ -304,7 +278,7 @@ def _sac_grad_case(O, A, H, separate_critic2, per, auto_alpha, seed, B=256, edge
     alpha = AutoAlpha(target_entropy=-float(A), log_alpha=float(np.log(0.2)), optim=AdamOptimizerFactory(lr=3e-2)).to(DEV) \
         if auto_alpha else 0.2
     lr = 1e-3
-    algo = SAC(policy=SACPolicy(actor=actor, action_space=_Box(A)), policy_optim=AdamOptimizerFactory(lr=lr), critic=c1,
+    algo = SAC(policy=SACPolicy(actor=actor, action_space=Box(A)), policy_optim=AdamOptimizerFactory(lr=lr), critic=c1,
                critic_optim=AdamOptimizerFactory(lr=lr), critic2=c2, critic2_optim=AdamOptimizerFactory(lr=lr) if c2 else None,
                tau=0.005, gamma=0.99, alpha=alpha)
     E, T = 8, 64
@@ -427,10 +401,10 @@ def test_sac_update_gradients_vs_fp64_autograd(O, A, H, separate_critic2, per, a
     rsample noise.  Adam's first step is lr * sign(g), so a gradient off by a constant factor leaves the parameters
     unchanged; this is the check that sees it.  critic2=None (the default) deep-copies the critic, so both critics stay
     identical and every row of the actor step is a tie of min(Q1, Q2)."""
-    _sac_grad_case(O, A, H, separate_critic2, per, auto_alpha, seed=O + A)
+    sac_grad_case(O, A, H, separate_critic2, per, auto_alpha, seed=O + A)
 
 
-def _dqn_grad_setup(kind, A, seed, per, alpha_beta=(0.6, 0.4)):
+def dqn_grad_setup(kind, A, seed, per, alpha_beta=(0.6, 0.4)):
     """A Q-network and a filled buffer.  kind: 'mlp' (Net on flat fp32 observations), 'mlp_scaled' (the same behind
     ScaledObsInputActionReprNet(denom=4): the flat gather divides by the denominator), 'cnn_stacked' (NatureCNN on
     stored uint8 [4, H, W] stacks: stack_num 1, obs_next = obs[next(i)])."""
@@ -489,10 +463,10 @@ DQN_GRAD_CASES = [
 @pytest.mark.parametrize("kind,loss,per,is_double,tuf", DQN_GRAD_CASES,
                          ids=[f"{c[0]}-{c[1]}-per{int(c[2])}-double{int(c[3])}-tuf{c[4]}" for c in DQN_GRAD_CASES])
 def test_dqn_update_gradients_vs_fp64_autograd(kind, loss, per, is_double, tuf):
-    _dqn_grad_case(kind, loss, per, is_double, tuf)
+    dqn_grad_case(kind, loss, per, is_double, tuf)
 
 
-def _dqn_grad_case(kind, loss, per, is_double, tuf, B=None, edge=""):
+def dqn_grad_case(kind, loss, per, is_double, tuf, B=None, edge=""):
     """Two DQN updates: the flat gradient snapshotted at FlatGroup.adam_step against float64 autograd of the reference loss
     (dqn.py:384-401: MSE weighted by the PER importance weights, or the unweighted Huber loss with delta 0.5, which puts
     rows on both sides) on a copy of the same module with the same parameters and batch; the TD errors handed to the
@@ -505,9 +479,9 @@ def _dqn_grad_case(kind, loss, per, is_double, tuf, B=None, edge=""):
     from tianshou_b200.algorithm.modelfree.dqn import DQN, DiscreteQLearningPolicy
     from tianshou_b200.utils import policy_within_training_step
     A, gamma, delta = 6, 0.9, 0.5
-    net, buf = _dqn_grad_setup(kind, A, seed=len(kind) * 10 + int(per), per=per)
+    net, buf = dqn_grad_setup(kind, A, seed=len(kind) * 10 + int(per), per=per)
     init64 = copy.deepcopy(net).to("cpu", torch.float64)
-    algo = DQN(policy=DiscreteQLearningPolicy(model=net, action_space=_Discrete(A)), optim=AdamOptimizerFactory(lr=1e-3),
+    algo = DQN(policy=DiscreteQLearningPolicy(model=net, action_space=Discrete(A)), optim=AdamOptimizerFactory(lr=1e-3),
                gamma=gamma, n_step_return_horizon=1, target_update_freq=tuf, is_double=is_double,
                huber_loss_delta=delta if loss == "huber" else None)
     assert (algo.model_old is None) == (tuf == 0)
@@ -610,7 +584,7 @@ def test_dqn_stored_stacks_bit_identical_to_single_frame_storage():
     net0 = ScaledObsInputActionReprNet(DQNet(4, H, W, A)).to(DEV)
     out = []
     for buf in (single, stored):
-        algo = DQN(policy=DiscreteQLearningPolicy(model=copy.deepcopy(net0), action_space=_Discrete(A)),
+        algo = DQN(policy=DiscreteQLearningPolicy(model=copy.deepcopy(net0), action_space=Discrete(A)),
                    optim=AdamOptimizerFactory(lr=1e-3), gamma=0.9, n_step_return_horizon=1, is_double=True)
         rec = {"q": [], "grad": [], "idx": [], "returns": []}
         real_q, real_step, orig_pre = algo._q_values, algo._group.adam_step, algo._preprocess_batch
@@ -653,7 +627,7 @@ def test_dqn_state_dict_keys():
     from tianshou_b200.algorithm import AdamOptimizerFactory
     from tianshou_b200.algorithm.modelfree.dqn import DQN, DiscreteQLearningPolicy
     from tianshou_b200.utils.net.common import Net
-    policy = DiscreteQLearningPolicy(model=Net(state_shape=(4,), action_shape=3, hidden_sizes=(16,)).to(DEV), action_space=_Discrete(3))
+    policy = DiscreteQLearningPolicy(model=Net(state_shape=(4,), action_shape=3, hidden_sizes=(16,)).to(DEV), action_space=Discrete(3))
     algo = DQN(policy=policy, optim=AdamOptimizerFactory(lr=1e-3), target_update_freq=10)
     assert list(algo.state_dict().keys()) == DQN_MLP_STATE_DICT_KEYS
 
@@ -671,8 +645,8 @@ def test_dqn_state_dict_round_trip_continues_identically():
     A = 6
 
     def build(seed):
-        net, buf = _dqn_grad_setup("mlp", A, seed=seed, per=False)
-        return DQN(policy=DiscreteQLearningPolicy(model=net, action_space=_Discrete(A)), optim=AdamOptimizerFactory(lr=1e-3),
+        net, buf = dqn_grad_setup("mlp", A, seed=seed, per=False)
+        return DQN(policy=DiscreteQLearningPolicy(model=net, action_space=Discrete(A)), optim=AdamOptimizerFactory(lr=1e-3),
                    gamma=0.9, n_step_return_horizon=2, target_update_freq=10), buf
 
     a, buf_a = build(5)
@@ -684,7 +658,7 @@ def test_dqn_state_dict_round_trip_continues_identically():
     b.load_state_dict(copy.deepcopy(a.state_dict()))
     b._iter = a._iter
     for algo in (a, b):
-        buf = _dqn_grad_setup("mlp", A, seed=5, per=False)[1]
+        buf = dqn_grad_setup("mlp", A, seed=5, per=False)[1]
         for u in range(3):
             np.random.seed(10 + u)
             with policy_within_training_step(algo.policy):
@@ -709,11 +683,11 @@ def test_drawn_actions_outside_the_network_outputs_are_refused(algo_name, bad):
     A = 3
     net = lambda **kw: Net(state_shape=(4,), hidden_sizes=(16,), **kw).to(DEV)
     if algo_name == "dqn":
-        algo = DQN(policy=DiscreteQLearningPolicy(model=net(action_shape=A), action_space=_Discrete(A)),
+        algo = DQN(policy=DiscreteQLearningPolicy(model=net(action_shape=A), action_space=Discrete(A)),
                    optim=AdamOptimizerFactory(lr=1e-3), target_update_freq=2)
     else:
         actor = DiscreteActor(preprocess_net=net(), action_shape=A, softmax_output=False).to(DEV)
-        algo = DiscreteSAC(policy=DiscreteSACPolicy(actor=actor, action_space=_Discrete(A)), policy_optim=AdamOptimizerFactory(lr=1e-3),
+        algo = DiscreteSAC(policy=DiscreteSACPolicy(actor=actor, action_space=Discrete(A)), policy_optim=AdamOptimizerFactory(lr=1e-3),
                            critic=DiscreteCritic(preprocess_net=net(), last_size=A).to(DEV), critic_optim=AdamOptimizerFactory(lr=1e-3))
     buf = VectorReplayBuffer(40, 4, device=DEV)
     rng = np.random.default_rng(0)

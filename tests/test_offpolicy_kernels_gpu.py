@@ -8,10 +8,10 @@ import numpy as np
 import pytest
 import torch
 
+from offpolicy_testutil import DEV, sm_count, stream
 from ts_testutil import record_parity
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
 F32_EPS = float(np.finfo(np.float32).eps)
 SIG_MIN, SIG_MAX = -20.0, 2.0
 
@@ -20,8 +20,8 @@ _LIVE: list = []      # the tensors whose raw pointers the pending call uses: ke
 
 
 def _call(name, *args):
-    from tianshou_b200._cabi import call, stream_ptr
-    call(name, *args, stream_ptr(torch.device(DEV)))
+    from tianshou_b200._cabi import call
+    call(name, *args, stream())
     torch.cuda.synchronize()
     _LIVE.clear()
 
@@ -390,7 +390,7 @@ ROW_KERNELS = ["stack_prev", "squashed_gaussian", "squashed_gaussian_bwd", "crit
 def test_per_row_kernels_write_rows_past_the_grid_cap(kernel):
     """TS_LAUNCH_1D caps the grid at num_sms * 16 blocks of 256 threads.  Each per-row kernel gets 1000 rows (elements, for
     the head backward) more than that, with NaN-prefilled outputs: every row must be written and correct."""
-    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    sms = sm_count()
     n = sms * 16 * 256 + 1000
     rng = np.random.default_rng(7)
     if kernel == "stack_prev":

@@ -7,13 +7,10 @@ import numpy as np
 import pytest
 import torch
 
+from offpolicy_testutil import golden_cfg
 from ts_testutil import load_golden, record_parity
 
 VARIANTS = ["d4rl", "net", "small"]
-
-
-def _cfg(g):
-    return {k[4:]: g[k] for k in g.files if k.startswith("cfg_")}
 
 
 def oracle_nets(cfg):
@@ -43,9 +40,9 @@ def oracle_batch(g, idx, dtype=torch.float32):
                 done=torch.as_tensor(g["buf_done"][idx]))
 
 
-def check_params(tag, mods, g, prefix, rtol, atol):
+def check_net_params(tag, mods, g, prefix, rtol, atol):
     from oracle.oracle_discrete_sac import golden_view
-    compact = bool(_cfg(g)["compact"])
+    compact = bool(golden_cfg(g)["compact"])
     params = [p for m in mods for p in m.parameters()]
     for i, p in enumerate(params):
         got = golden_view(p) if compact else p.detach().cpu().numpy()
@@ -56,7 +53,7 @@ def check_params(tag, mods, g, prefix, rtol, atol):
 def test_oracle_matches_reference(variant):
     from oracle.oracle_bcq import bcq_policy, bcq_update
     g = load_golden(f"bcq_ref_{variant}.npz")
-    cfg = _cfg(g)
+    cfg = golden_cfg(g)
     nets = oracle_nets(cfg)
     opts = [torch.optim.Adam(nets.p.parameters(), lr=float(cfg["actor_lr"])), torch.optim.Adam(nets.c[0].parameters(), lr=float(cfg["critic_lr"])),
             torch.optim.Adam(nets.c[1].parameters(), lr=float(cfg["critic2_lr"] if bool(cfg["critic2"]) else cfg["critic_lr"])),
@@ -74,7 +71,7 @@ def test_oracle_matches_reference(variant):
             continue
         for prefix, mods in (("pert_", [nets.p]), ("c1_", [nets.c[0]]), ("c2_", [nets.c[1]]), ("vae_", nets.vae_modules()),
                              ("pold_", [nets.p_old]), ("c1old_", [nets.c_old[0]]), ("c2old_", [nets.c_old[1]])):
-            check_params(tag, mods, g, o + prefix, rtol=1e-4, atol=1e-6)
+            check_net_params(tag, mods, g, o + prefix, rtol=1e-4, atol=1e-6)
     if "policy_obs" in g.files:
         torch.manual_seed(900)
         act = bcq_policy(nets, torch.as_tensor(g["policy_obs"]), int(cfg["S"]))
@@ -85,7 +82,7 @@ def test_oracle_matches_reference(variant):
 def test_net_golden_binds_the_clamp_and_has_done_rows():
     """The ``net`` case exercises what it is there for: perturbed actions at +-max_action, many done rows, N = 1."""
     g = load_golden("bcq_ref_net.npz")
-    cfg = _cfg(g)
+    cfg = golden_cfg(g)
     nets = oracle_nets(cfg)
     b = oracle_batch(g, g["u0_indices"])
     torch.manual_seed(7)

@@ -7,20 +7,11 @@ import numpy as np
 import pytest
 import torch
 
+from offpolicy_testutil import MultiDiscrete, golden_cfg, load_params
 from ts_testutil import load_golden, record_parity
 
 VARIANTS = ["pendulum", "bipedal", "per_trunc", "b1"]
 PRIO_EPS = float(np.finfo(np.float32).eps)
-
-
-def _cfg(g):
-    return {k[4:]: g[k] for k in g.files if k.startswith("cfg_")}
-
-
-def _load(mod, g, prefix):
-    with torch.no_grad():
-        for i, p in enumerate(mod.parameters()):
-            p.copy_(torch.as_tensor(g[f"{prefix}{i}"]).reshape(p.shape))
 
 
 def _check(tag, mod, g, prefix, lr):
@@ -47,9 +38,9 @@ def end_flags(g):
 def test_oracle_matches_reference(variant):
     from oracle.oracle_bdqn import bdqn_update
     g = load_golden(f"bdqn_ref_{variant}.npz")
-    cfg = _cfg(g)
+    cfg = golden_cfg(g)
     net = branching_net(cfg)
-    _load(net, g, "p0_net_")
+    load_params(net, g, "p0_net_")
     freq = int(cfg["target_update_freq"])
     old = copy.deepcopy(net) if freq > 0 else None
     lr = float(cfg["lr"])
@@ -75,15 +66,15 @@ def test_goldens_cover_what_they_claim():
     """pendulum refreshes its lagged network inside the recorded updates; bipedal's buffer has unfinished episodes that end flags
     turn on; per_trunc ends episodes by truncation (which BDQN does not bootstrap) and ran past its capacity."""
     g = load_golden("bdqn_ref_pendulum.npz")
-    assert int(_cfg(g)["updates"]) > int(_cfg(g)["target_update_freq"]) > 0
+    assert int(golden_cfg(g)["updates"]) > int(golden_cfg(g)["target_update_freq"]) > 0
     assert not np.array_equal(g["u2_old_0"], g["u3_old_0"])
     g = load_golden("bdqn_ref_bipedal.npz")
     assert len(g["buf_unfinished"]) > 0 and not g["buf_done"][g["buf_unfinished"]].any()
-    sampled = np.concatenate([g[f"u{u}_indices"] for u in range(int(_cfg(g)["updates"]))])
+    sampled = np.concatenate([g[f"u{u}_indices"] for u in range(int(golden_cfg(g)["updates"]))])
     assert np.isin(sampled, g["buf_unfinished"]).any()
     g = load_golden("bdqn_ref_per_trunc.npz")
-    assert (g["buf_truncated"] & ~g["buf_terminated"]).any() and int(_cfg(g)["adds"]) > int(_cfg(g)["size"])
-    assert int(_cfg(g)["nb"]) > 8
+    assert (g["buf_truncated"] & ~g["buf_terminated"]).any() and int(golden_cfg(g)["adds"]) > int(golden_cfg(g)["size"])
+    assert int(golden_cfg(g)["nb"]) > 8
 
 
 def test_b1_loss_is_the_usual_loss_plus_the_target_variance():
@@ -91,9 +82,9 @@ def test_b1_loss_is_the_usual_loss_plus_the_target_variance():
     per-branch targets, the gradient does not change."""
     from oracle.oracle_bdqn import TARGET_GAMMA, bdqn_loss, bdqn_targets, q_values
     g = load_golden("bdqn_ref_b1.npz")
-    cfg = _cfg(g)
+    cfg = golden_cfg(g)
     net = branching_net(cfg)
-    _load(net, g, "p0_net_")
+    load_params(net, g, "p0_net_")
     idx = g["u0_indices"]
     end = end_flags(g)
     obs, obs_next = torch.as_tensor(g["buf_obs"][idx]), torch.as_tensor(g["buf_obs_next"][idx])
@@ -229,19 +220,13 @@ def test_bdqn_exploration_noise_matches_reference():
     assert np.random.rand() == np.random.RandomState(2).rand()
 
 
-class _MultiDiscrete:
-    def __init__(self, nvec):
-        self.nvec = np.asarray(nvec)
-        self.shape = self.nvec.shape
-
-
 def test_bdqn_constructor_errors():
     from tianshou_b200.algorithm import BDQN, UnsupportedModelError
     from tianshou_b200.algorithm.modelfree.bdqn import BDQNPolicy
     from tianshou_b200.algorithm.optim import AdamOptimizerFactory
     from tianshou_b200.utils.net.common import BranchingNet
     net = BranchingNet(state_shape=3, num_branches=2, action_per_branch=4, common_hidden_sizes=[8])
-    policy = BDQNPolicy(model=net, action_space=_MultiDiscrete([4, 4]))
+    policy = BDQNPolicy(model=net, action_space=MultiDiscrete([4, 4]))
     with pytest.raises(UnsupportedModelError, match="no CPU path"):
         BDQN(policy=policy, optim=AdamOptimizerFactory(lr=1e-3))
     with pytest.raises(TypeError):

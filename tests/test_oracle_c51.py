@@ -8,7 +8,7 @@ import torch
 
 from oracle import oracle_c51 as oc
 from oracle import oracle_discrete_sac as ods
-from test_oracle_discrete_bcq import check_final
+from oracle_testutil import check_final
 from ts_testutil import load_golden
 
 VARIANTS = ["c51_ref_mlp", "c51_ref_cnn", "c51_ref_per"]

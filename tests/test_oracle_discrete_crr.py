@@ -8,7 +8,8 @@ import torch
 from torch.distributions import Categorical
 
 from oracle import oracle_discrete_crr as odc
-from test_oracle_discrete_bcq import check_final, oracle_setup
+from offpolicy_testutil import Discrete
+from oracle_testutil import check_final, oracle_setup
 from ts_testutil import load_golden
 
 VARIANTS = ["mlp", "cnn", "sep"]
@@ -85,11 +86,8 @@ def test_mode_and_gamma_are_checked_on_the_host():
     from tianshou_b200.utils.net.common import Net
     from tianshou_b200.utils.net.discrete import DiscreteActor, DiscreteCritic
 
-    class _Discrete:
-        n, shape = 3, ()
-
     trunk = Net(state_shape=(4,), hidden_sizes=(16,))
-    policy = DiscreteActorPolicy(actor=DiscreteActor(preprocess_net=trunk, action_shape=3, softmax_output=False), action_space=_Discrete())
+    policy = DiscreteActorPolicy(actor=DiscreteActor(preprocess_net=trunk, action_shape=3, softmax_output=False), action_space=Discrete(3))
     critic = DiscreteCritic(preprocess_net=trunk, last_size=3)
     with pytest.raises(ValueError, match="policy_improvement_mode"):
         DiscreteCRR(policy=policy, critic=critic, optim=AdamOptimizerFactory(lr=1e-3), policy_improvement_mode="softmax")

@@ -8,15 +8,10 @@ import pytest
 import torch
 
 from oracle import oracle_discrete_sac as ods
+from offpolicy_testutil import load_params
 from ts_testutil import load_golden
 
 VARIANTS = ["mlp", "auto", "cnn"]
-
-
-def _load(mod, g, prefix):
-    with torch.no_grad():
-        for i, p in enumerate(mod.parameters()):
-            p.copy_(torch.as_tensor(g[f"{prefix}{i}"]).reshape(p.shape))
 
 
 def _init(mods, g):
@@ -25,7 +20,7 @@ def _init(mods, g):
         if bool(g["cfg_compact"]):
             ods.seeded_params(m, int(g["cfg_init_seed"]) + k)
         else:
-            _load(m, g, pfx)
+            load_params(m, g, pfx)
 
 
 def _close(mod, g, prefix, lr, what):

@@ -10,7 +10,7 @@ from torch import nn
 from oracle import oracle_discrete_sac as ods
 from oracle import oracle_fqf as of
 from oracle import oracle_iqn as oi
-from test_oracle_discrete_bcq import check_final
+from oracle_testutil import check_final
 from test_oracle_iqn import oracle_setup
 from ts_testutil import load_golden
 

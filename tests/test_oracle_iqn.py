@@ -8,7 +8,7 @@ import torch
 
 from oracle import oracle_discrete_sac as ods
 from oracle import oracle_iqn as oi
-from test_oracle_discrete_bcq import check_final
+from oracle_testutil import check_final
 from ts_testutil import load_golden
 
 VARIANTS = ["iqn_ref_mlp", "iqn_ref_sizes", "iqn_ref_cnn", "iqn_ref_per"]

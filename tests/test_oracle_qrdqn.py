@@ -8,7 +8,7 @@ import torch
 
 from oracle import oracle_discrete_sac as ods
 from oracle import oracle_qrdqn as oq
-from test_oracle_discrete_bcq import check_final
+from oracle_testutil import check_final
 from ts_testutil import load_golden
 
 VARIANTS = ["qrdqn_ref_mlp", "qrdqn_ref_cnn", "qrdqn_ref_per", "dcql_ref_mlp", "dcql_ref_cnn"]

@@ -5,34 +5,15 @@ import numpy as np
 import pytest
 import torch
 
+from offpolicy_testutil import golden_cfg, load_params, oracle_buffer
 from ts_testutil import load_golden, record_parity
 
 VARIANTS = ["mujoco", "per_mean", "full"]
 
 
-def _cfg(g):
-    return {k[4:]: g[k] for k in g.files if k.startswith("cfg_")}
-
-
-def _load(mod, g, prefix):
-    with torch.no_grad():
-        for i, p in enumerate(mod.parameters()):
-            p.copy_(torch.as_tensor(g[f"{prefix}{i}"]).reshape(p.shape))
-
-
 def _check(tag, mod, g, prefix, lr):
     for i, p in enumerate(mod.parameters()):
         record_parity(f"{tag}/{prefix}{i}", p.detach().numpy(), g[f"{prefix}{i}"], rtol=1e-4, atol=1e-3 * lr)
-
-
-def oracle_buffer(g):
-    """The arrays ``oracle_td3.nstep_targets`` reads, for the single buffer of a golden."""
-    d = {k: g["buf_" + k] for k in ("obs", "act", "rew", "done", "terminated", "obs_next")}
-    size, n = len(g["buf_obs"]), int(g["buf_len"])
-    last = (int(g["buf_insertion_idx"]) - 1) % n
-    d.update(offset=np.array([0, size]), last_index=g["buf_last_index"], lengths=np.array([n]),
-             unfinished=[last] if not d["done"][last] else [])
-    return d
 
 
 def cpu_noise(shape):
@@ -42,10 +23,10 @@ def cpu_noise(shape):
 
 def build_oracle(g):
     from oracle.oracle_redq import AutoAlpha, FixedAlpha, RedqNets
-    cfg = _cfg(g)
+    cfg = golden_cfg(g)
     O, A, H, E = int(cfg["obs"]), int(cfg["act"]), tuple(int(x) for x in cfg["hidden"]), int(cfg["E"])
     nets = RedqNets(O, A, H, E)
-    _load(nets.actor, g, "p0_actor_"); _load(nets.critic, g, "p0_critic_")
+    load_params(nets.actor, g, "p0_actor_"); load_params(nets.critic, g, "p0_critic_")
     nets.critic_old.load_state_dict(nets.critic.state_dict())
     opts = [torch.optim.Adam(nets.actor.parameters(), lr=float(cfg["actor_lr"])),
             torch.optim.Adam(nets.critic.parameters(), lr=float(cfg["critic_lr"]))]

@@ -5,19 +5,10 @@ import numpy as np
 import pytest
 import torch
 
+from offpolicy_testutil import golden_cfg, load_params, oracle_buffer
 from ts_testutil import load_golden, record_parity
 
 VARIANTS = ["mujoco", "per_nstep", "bc", "bc_freq1"]
-
-
-def _cfg(g):
-    return {k[4:]: g[k] for k in g.files if k.startswith("cfg_")}
-
-
-def _load(mod, g, prefix):
-    with torch.no_grad():
-        for i, p in enumerate(mod.parameters()):
-            p.copy_(torch.as_tensor(g[f"{prefix}{i}"]).reshape(p.shape))
 
 
 def _check(tag, mod, g, prefix, lr):
@@ -25,24 +16,14 @@ def _check(tag, mod, g, prefix, lr):
         record_parity(f"{tag}/{prefix}{i}", p.detach().numpy(), g[f"{prefix}{i}"], rtol=1e-4, atol=1e-3 * lr)
 
 
-def oracle_buffer(g):
-    """The arrays ``oracle_td3.nstep_targets`` reads, for the single buffer of a golden."""
-    d = {k: g["buf_" + k] for k in ("obs", "act", "rew", "done", "terminated", "obs_next")}
-    size, n = len(g["buf_obs"]), int(g["buf_len"])
-    last = (int(g["buf_insertion_idx"]) - 1) % n
-    d.update(offset=np.array([0, size]), last_index=g["buf_last_index"], lengths=np.array([n]),
-             unfinished=[last] if not d["done"][last] else [])
-    return d
-
-
 @pytest.mark.parametrize("variant", VARIANTS)
 def test_oracle_matches_reference(variant):
     from oracle.oracle_td3 import Td3Nets, td3_update
     g = load_golden(f"td3_ref_{variant}.npz")
-    cfg = _cfg(g)
+    cfg = golden_cfg(g)
     O, A, H = int(cfg["obs"]), int(cfg["act"]), tuple(int(x) for x in cfg["hidden"])
     nets = Td3Nets(O, A, H, float(cfg["max_action"]))
-    _load(nets.a, g, "p0_actor_"); _load(nets.c[0], g, "p0_c1_"); _load(nets.c[1], g, "p0_c2_")
+    load_params(nets.a, g, "p0_actor_"); load_params(nets.c[0], g, "p0_c1_"); load_params(nets.c[1], g, "p0_c2_")
     nets.a_old.load_state_dict(nets.a.state_dict())
     for k in range(2):
         nets.c_old[k].load_state_dict(nets.c[k].state_dict())
@@ -79,9 +60,9 @@ def test_per_nstep_target_actions_leave_the_action_bounds():
     """With noise_clip=0 and max_action=2 the smoothed target actions are not clamped: some leave [-2, 2], as in the reference."""
     from oracle.oracle_td3 import Td3Nets
     g = load_golden("td3_ref_per_nstep.npz")
-    cfg = _cfg(g)
+    cfg = golden_cfg(g)
     nets = Td3Nets(int(cfg["obs"]), int(cfg["act"]), tuple(int(x) for x in cfg["hidden"]), float(cfg["max_action"]))
-    _load(nets.a, g, "p0_actor_")
+    load_params(nets.a, g, "p0_actor_")
     torch.manual_seed(100)
     with torch.no_grad():
         a = nets.pi(torch.as_tensor(g["buf_obs_next"])) + torch.randn(len(g["buf_obs_next"]), int(cfg["act"])) * float(cfg["policy_noise"])

@@ -3,10 +3,6 @@
 from oracle/gen_golden_qrdqn.py), one update's gradient against float64 autograd, the ``state_dict()`` round trip, the
 policy's torch path, the refusals and the kernels' register report."""
 import copy
-import os
-import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -14,29 +10,14 @@ import torch
 
 from oracle import oracle_discrete_sac as ods
 from oracle import oracle_qrdqn as oq
+from offpolicy_testutil import (DEV, EPS, Discrete, assert_spill_free, capture_batches, capture_grads, check_final_state,
+                                ptxas_report, sm_count, stream, vector_buffer_from_golden)
 from ts_testutil import load_golden, record_parity
 
-DEV = "cuda:0"
 gpu = pytest.mark.gpu
-EPS = float(np.finfo(np.float32).eps)
 A_CASES = (1, 2, 6, 18)
 N_CASES = (2, 200, 201)
 VARIANTS = ["qrdqn_ref_mlp", "qrdqn_ref_cnn", "qrdqn_ref_per", "dcql_ref_mlp", "dcql_ref_cnn"]
-
-
-class _Discrete:
-    def __init__(self, n):
-        self.n = n
-        self.shape = ()
-
-
-def _st():
-    from tianshou_b200._cabi import stream_ptr
-    return stream_ptr(torch.device(DEV))
-
-
-def sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
 
 
 # ------------------------------------------------------------------------------------------------------------ target kernel
@@ -49,14 +30,14 @@ def test_target_kernel_matches_oracle(A, N):
     grid (16 blocks of 8 warps per SM) in one case."""
     from tianshou_b200._cabi import call, ptr
     g = torch.Generator().manual_seed(A * 1000 + N)
-    B = sms() * 16 * 8 + 37 if (A, N) == (6, 200) else 301
+    B = sm_count() * 16 * 8 + 37 if (A, N) == (6, 200) else 301
     q = torch.randint(-3, 4, (B, A, N), generator=g).float()
     q_next = torch.randn(B, A, N, generator=g)
     if A > 1:
         q[: B // 3, A - 1] = q[: B // 3, 0]                          # two equal blocks: the first wins where they lead
     out, act = torch.empty(B, N, device=DEV), torch.empty(B, dtype=torch.int64, device=DEV)
     qd, nd = q.to(DEV), q_next.to(DEV)
-    call("ts_qrdqn_target", ptr(qd), ptr(nd), B, A, N, ptr(out), ptr(act), _st())
+    call("ts_qrdqn_target", ptr(qd), ptr(nd), B, A, N, ptr(out), ptr(act), stream())
     torch.cuda.synchronize()
     ref_a = oq.qr_select(q.numpy())
     assert np.array_equal(act.cpu().numpy(), ref_a) and np.array_equal(ref_a, q.mean(2).argmax(1).numpy())
@@ -64,7 +45,7 @@ def test_target_kernel_matches_oracle(A, N):
     if A > 1:
         lead = q[: B // 3].sum(2).argmax(1) == 0
         assert bool(lead.any()) and bool((act.cpu()[: B // 3][lead] == 0).all())
-    call("ts_qrdqn_target", ptr(qd), ptr(qd), B, A, N, ptr(out), None, _st())      # target_update_freq = 0: q_next is q_online
+    call("ts_qrdqn_target", ptr(qd), ptr(qd), B, A, N, ptr(out), None, stream())      # target_update_freq = 0: q_next is q_online
     torch.cuda.synchronize()
     assert torch.equal(out.cpu(), q[torch.arange(B), torch.as_tensor(ref_a)])
 
@@ -76,7 +57,7 @@ def _rows(q, act, ret, tau, w, mqw):
     dq, prio = torch.empty(B, A, N, device=DEV), torch.empty(B, device=DEV)
     rows, losses = torch.empty(3, B, device=DEV), torch.empty(4, device=DEV)
     call("ts_qrdqn_rows", ptr(q), ptr(act), ptr(ret), ptr(tau), ptr(w), B, A, N, float(mqw), ptr(dq), ptr(prio), ptr(rows), ptr(losses),
-         _st())
+         stream())
     torch.cuda.synchronize()
     return losses.cpu().numpy(), dq.cpu().numpy(), prio.cpu().numpy()
 
@@ -124,7 +105,7 @@ def test_rows_kernel_vs_fp64(A, N, weighted, mqw):
     ceil(N / 32) values, then five levels); softmax and logsumexp over A add (A / 32 + 10) eps.  The batch means come from
     row_sums3_kernel: (B / 1024 + 12) eps times the mean magnitude."""
     rng = np.random.default_rng(A * 7919 + N * 31 + weighted * 3 + int(mqw))
-    B = sms() * 8 + 37 if (A, N, weighted) == (6, 200, True) else 41
+    B = sm_count() * 8 + 37 if (A, N, weighted) == (6, 200, True) else 41
     q = (rng.standard_normal((B, A, N)) * 2).astype(np.float32)
     act = rng.integers(0, A, B)
     ret = (q[np.arange(B), act, :] + rng.standard_normal((B, N)) * 1.5).astype(np.float32)
@@ -178,7 +159,7 @@ def test_rows_kernel_refuses_what_shared_memory_cannot_hold():
     a = torch.zeros(1, dtype=torch.int64, device=DEV)
     for A, N, mqw in ((1, 6145, 0.0), (100, 6100, 1.0), (1, 1, 0.0)):
         with pytest.raises(RuntimeError, match="ts_qrdqn_rows"):
-            call("ts_qrdqn_rows", ptr(x), ptr(a), ptr(x), ptr(x), None, 1, A, N, mqw, ptr(x), ptr(x), ptr(x), ptr(x), _st())
+            call("ts_qrdqn_rows", ptr(x), ptr(a), ptr(x), ptr(x), None, 1, A, N, mqw, ptr(x), ptr(x), ptr(x), ptr(x), stream())
 
 
 # ------------------------------------------------------------------------------------------------------------ vs reference
@@ -199,51 +180,12 @@ def build_from_golden(g):
     A, N = int(g["cfg_A"]), int(g["cfg_N"])
     model = model_from_cfg(kind, A, N, **kw)
     ods.seeded_params(model, int(g["cfg_init_seed"]))
-    policy = QRDQNPolicy(model=model, action_space=_Discrete(A))
+    policy = QRDQNPolicy(model=model, action_space=Discrete(A))
     akw = dict(policy=policy, optim=AdamOptimizerFactory(lr=float(g["cfg_lr"])), gamma=float(g["cfg_gamma"]), num_quantiles=N,
                n_step_return_horizon=int(g["cfg_n_step"]), target_update_freq=int(g["cfg_freq"]))
     if str(g["cfg_algo"]) == "dcql":
         return DiscreteCQL(min_q_weight=float(g["cfg_min_q_weight"]), **akw)
     return QRDQN(**akw)
-
-
-def buffer_from_golden(g, mirror=False):
-    from tianshou_b200.data import Batch, PrioritizedVectorReplayBuffer, VectorReplayBuffer
-    E, cap = int(g["cfg_E"]), int(g["cfg_cap"])
-    cnn = str(g["cfg_kind"]) == "cnn"
-    kw = dict(stack_num=4, ignore_obs_next=True, save_only_last_obs=True) if cnn else {}
-    if bool(g["cfg_per"]):
-        buf = PrioritizedVectorReplayBuffer(E * cap, E, alpha=float(g["cfg_alpha"]), beta=float(g["cfg_beta"]), device=DEV,
-                                            device_mirror=mirror, **kw)
-    else:
-        buf = VectorReplayBuffer(E * cap, E, device=DEV, device_mirror=mirror, **kw)
-    for i in range(int(g["cfg_steps"])):
-        s = {k: g[f"roll{i}_{k}"] for k in ("obs", "act", "rew", "terminated", "truncated")}
-        if cnn:
-            s["obs"] = np.repeat(s["obs"][:, None], 4, axis=1)        # only the last frame is stored
-            s["obs_next"] = s["obs"]
-        else:
-            s["obs_next"] = g[f"roll{i}_obs_next"]
-        buf.add(Batch(**s), buffer_ids=np.arange(E))
-    return buf
-
-
-def check_final_state(tag, g, algo):
-    """Final parameters / Adam moments / lagged parameters within the bars DESIGN.md section 4 uses for DQN and the discrete
-    offline algorithms: Adam normalises a step to ~lr per element, so the absolute term is stated in units of one step."""
-    view = ods.golden_view
-    lr = float(g["cfg_lr"])
-    grp = algo._group
-    for i, p in enumerate(grp.params):
-        record_parity(f"{tag}/pf_{i}", view(p), g[f"pf_{i}"], rtol=1e-3, atol=0.1 * lr)
-        m, v = g[f"m_{i}"], g[f"v_{i}"]
-        record_parity(f"{tag}/m_{i}", view(grp.view(grp.exp_avg, p).view(p.shape)), m, rtol=2e-3, atol=2e-3 * float(np.abs(m).max()) + 1e-12)
-        record_parity(f"{tag}/v_{i}", view(grp.view(grp.exp_avg_sq, p).view(p.shape)), v, rtol=4e-3, atol=4e-3 * float(np.abs(v).max()) + 1e-20)
-    assert grp.sync_step_from_device() == int(g["adam_step"]) and algo._iter == int(g["iter"])
-    lagged = list(algo.model_old.parameters()) if algo.model_old is not None else []
-    assert len(lagged) == (len(grp.params) if int(g["cfg_freq"]) > 0 else 0)
-    for i, p in enumerate(lagged):
-        record_parity(f"{tag}/old_{i}", view(p), g[f"old_{i}"], rtol=1e-3, atol=0.1 * lr)
 
 
 @gpu
@@ -254,37 +196,25 @@ def test_update_matches_reference(variant, mirror):
     priorities written back (PER: and the sum-tree leaves), then the final state."""
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden(f"{variant}.npz")
-    algo, buf = build_from_golden(g), buffer_from_golden(g, mirror)
+    algo, buf = build_from_golden(g), vector_buffer_from_golden(g, mirror)
     keys = [str(k) for k in g["state_dict_keys"]]
     assert list(algo.state_dict().keys()) == keys
-    cap = {}
-    orig_pre, orig_post = algo._preprocess_batch, algo._postprocess_batch
-
-    def pre(batch, buffer, indices):
-        b = orig_pre(batch, buffer, indices)
-        cap["indices"], cap["returns"] = np.asarray(indices).copy(), b.returns.detach().cpu().numpy().copy()
-        return b
-
-    def post(batch, buffer, indices):
-        cap["prio"] = batch.weight.detach().cpu().numpy().copy()
-        return orig_post(batch, buffer, indices)
-
-    algo._preprocess_batch, algo._postprocess_batch = pre, post
     dcql = str(g["cfg_algo"]) == "dcql"
-    for u in range(int(g["cfg_updates"])):
-        np.random.seed(500 + u)
-        with policy_within_training_step(algo.policy):
-            stats = algo.update(buffer=buf, sample_size=int(g["cfg_bs"]))
-        tag = f"{variant}_m{int(mirror)}_u{u}"
-        assert np.array_equal(cap["indices"], g[f"u{u}_indices"]), "sampled indices differ from the reference's"
-        ref_ret = g[f"u{u}_returns"]
-        record_parity(f"{tag}/returns", cap["returns"], ref_ret, rtol=1e-5, atol=1e-5 * float(np.abs(ref_ret).max()))
-        got = np.array([stats.loss, stats.qr_loss, stats.cql_loss] if dcql else [stats.loss])
-        record_parity(f"{tag}/losses", got, g[f"u{u}_losses"], rtol=2e-5, atol=2e-6)
-        record_parity(f"{tag}/prio", cap["prio"], g[f"u{u}_prio"], rtol=2e-5, atol=2e-6)
-        if bool(g["cfg_per"]):
-            leaves = np.asarray(buf.weight[np.arange(len(buf))])
-            record_parity(f"{tag}/tree_leaves", leaves, g[f"u{u}_tree_leaves"], rtol=2e-5, atol=1e-7)
+    with capture_batches(algo) as cap:
+        for u in range(int(g["cfg_updates"])):
+            np.random.seed(500 + u)
+            with policy_within_training_step(algo.policy):
+                stats = algo.update(buffer=buf, sample_size=int(g["cfg_bs"]))
+            tag = f"{variant}_m{int(mirror)}_u{u}"
+            assert np.array_equal(cap["indices"], g[f"u{u}_indices"]), "sampled indices differ from the reference's"
+            ref_ret = g[f"u{u}_returns"]
+            record_parity(f"{tag}/returns", cap["returns"].cpu().numpy(), ref_ret, rtol=1e-5, atol=1e-5 * float(np.abs(ref_ret).max()))
+            got = np.array([stats.loss, stats.qr_loss, stats.cql_loss] if dcql else [stats.loss])
+            record_parity(f"{tag}/losses", got, g[f"u{u}_losses"], rtol=2e-5, atol=2e-6)
+            record_parity(f"{tag}/prio", cap["prio"].cpu().numpy(), g[f"u{u}_prio"], rtol=2e-5, atol=2e-6)
+            if bool(g["cfg_per"]):
+                leaves = np.asarray(buf.weight[np.arange(len(buf))])
+                record_parity(f"{tag}/tree_leaves", leaves, g[f"u{u}_tree_leaves"], rtol=2e-5, atol=1e-7)
     check_final_state(f"{variant}_m{int(mirror)}", g, algo)
     assert list(algo.state_dict().keys()) == keys
 
@@ -318,55 +248,39 @@ def grad_case(kind, mqw, B=64, edge=""):
     The GEMMs are fp32-faithful (bf16x3) and a weight gradient sums B products per element: 2e-4 relative plus 1e-4 of the
     tensor's largest value, as in test_discrete_bcq_gpu."""
     from tianshou_b200.algorithm import AdamOptimizerFactory, DiscreteCQL, QRDQN, QRDQNPolicy
-    from tianshou_b200.algorithm.flat_params import FlatGroup
     from tianshou_b200.utils import policy_within_training_step
     torch.manual_seed(3)
     rng = np.random.default_rng(4)
     A, N = 5, 33
     model = model_from_cfg(kind, A, N, hidden=(48, 40))
-    policy = QRDQNPolicy(model=model, action_space=_Discrete(A))
+    policy = QRDQNPolicy(model=model, action_space=Discrete(A))
     kw = dict(policy=policy, optim=AdamOptimizerFactory(lr=1e-3), gamma=0.9, num_quantiles=N, n_step_return_horizon=2,
               target_update_freq=3)
     algo = DiscreteCQL(min_q_weight=mqw, **kw) if mqw else QRDQN(**kw)
     buf = make_buffer(kind, A, rng)
-    cap = {}
     grp = algo._group
-
-    def adam(optimizer, mgn):
-        cap["grad"] = grp.grad[: grp.n].clone()
-        FlatGroup.adam_step(grp, optimizer, mgn)
-
-    grp.adam_step = adam
-    orig_pre = algo._preprocess_batch
-
-    def pre(batch, buffer, indices):
-        b = orig_pre(batch, buffer, indices)
-        cap["indices"], cap["returns"] = np.asarray(indices).copy(), b.returns.detach().cpu().double()
-        return b
-
-    algo._preprocess_batch = pre
     ref = copy.deepcopy(model).to("cpu", torch.float64)         # the weights before the step
     np.random.seed(7)
-    with policy_within_training_step(algo.policy):
+    with capture_batches(algo) as cap, capture_grads(grp) as grads, policy_within_training_step(algo.policy):
         stats = algo.update(buffer=buf, sample_size=B)
-    idx = cap["indices"]
+    idx, returns = cap["indices"], cap["returns"].cpu().double()
     raw = np.asarray(buf.obs)[idx]
     x = torch.as_tensor((raw.astype(np.float64) / 255.0).astype(np.float32) if kind == "cnn" else raw).double()
     inner = ref.module if kind == "cnn" else ref
     chain = inner.net if kind == "cnn" else inner.model.model
     q = chain(x).view(B, A, N)
     act = np.asarray(buf.act)[idx].astype(np.int64)
-    loss, qr, cql, _ = oq.reference_loss(q, act, cap["returns"], torch.as_tensor(oq.tau_hat(N), dtype=torch.float64), 1.0, mqw)
+    loss, qr, cql, _ = oq.reference_loss(q, act, returns, torch.as_tensor(oq.tau_hat(N), dtype=torch.float64), 1.0, mqw)
     loss.backward()
     ref_params = [p for m in chain.modules() if isinstance(m, (torch.nn.Linear, torch.nn.Conv2d)) for p in (m.weight, m.bias)]
     for i, (p, r) in enumerate(zip(grp.params, ref_params, strict=True)):
         want = r.grad.numpy()
-        got = grp.view(cap["grad"], p).view(p.shape).cpu().numpy()
+        got = grp.view(grads[-1], p).view(p.shape).cpu().numpy()
         record_parity(f"qrdqn_grad{edge}/{kind}_m{int(mqw)}/grad_{i}", got, want, rtol=2e-4, atol=1e-4 * float(np.abs(want).max()) + 1e-12)
     got = [stats.loss, stats.qr_loss, stats.cql_loss] if mqw else [stats.loss]
     want = [loss.item(), qr.item(), cql.item()] if mqw else [loss.item()]
     record_parity(f"qrdqn_grad{edge}/{kind}_m{int(mqw)}/losses", np.array(got), np.array(want), rtol=2e-5, atol=2e-6)
-    assert len(idx) == B and cap["returns"].shape[0] == B, "the update must run on the B sampled rows"
+    assert len(idx) == B and returns.shape[0] == B, "the update must run on the B sampled rows"
 
 
 # ------------------------------------------------------------------------------------------------------------ state_dict
@@ -377,7 +291,7 @@ def test_state_dict_round_trip_continues_identically(variant):
     ``_iter`` is a plain attribute, as in the reference: whoever restores a run restores it too."""
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden(f"{variant}.npz")
-    a, buf_a = build_from_golden(g), buffer_from_golden(g)
+    a, buf_a = build_from_golden(g), vector_buffer_from_golden(g)
     for u in range(3):
         np.random.seed(u)
         with policy_within_training_step(a.policy):
@@ -390,7 +304,7 @@ def test_state_dict_round_trip_continues_identically(variant):
     b._iter = a._iter
     assert torch.equal(a.tau_hat, b.tau_hat)
     for algo in (a, b):
-        buf = buffer_from_golden(g)
+        buf = vector_buffer_from_golden(g)
         for u in range(3):
             np.random.seed(10 + u)
             with policy_within_training_step(algo.policy):
@@ -408,7 +322,7 @@ def test_policy_forward_takes_arg_max_of_quantile_means():
     from tianshou_b200.data import Batch
     torch.manual_seed(0)
     model = model_from_cfg("mlp", 5, 17, obs=4, hidden=(32,))
-    policy = QRDQNPolicy(model=model, action_space=_Discrete(5))
+    policy = QRDQNPolicy(model=model, action_space=Discrete(5))
     obs = np.random.default_rng(0).standard_normal((300, 4)).astype(np.float32)
     out = policy(Batch(obs=obs, info=Batch()))
     logits, _ = model(obs)
@@ -428,7 +342,7 @@ def test_refusals():
 
     def make(model=None, opt=AdamOptimizerFactory, n=A, cls=QRDQN, **kw):
         model = model or model_from_cfg("mlp", A, N, hidden=(16,))
-        return cls(policy=QRDQNPolicy(model=model, action_space=_Discrete(n)), optim=opt(lr=1e-3), num_quantiles=N, **kw)
+        return cls(policy=QRDQNPolicy(model=model, action_space=Discrete(n)), optim=opt(lr=1e-3), num_quantiles=N, **kw)
 
     algo = make()
     with pytest.raises(UnsupportedModelError, match="softmax"):
@@ -445,7 +359,7 @@ def test_refusals():
         with pytest.raises(AssertionError):
             make(**kw)
     with pytest.raises(AssertionError, match="num_quantiles"):
-        QRDQN(policy=QRDQNPolicy(model=model_from_cfg("mlp", A, 1, hidden=(16,)), action_space=_Discrete(A)),
+        QRDQN(policy=QRDQNPolicy(model=model_from_cfg("mlp", A, 1, hidden=(16,)), action_space=Discrete(A)),
               optim=AdamOptimizerFactory(lr=1e-3), num_quantiles=1)
     with pytest.raises(ValueError, match="min_q_weight"):
         make(cls=DiscreteCQL, min_q_weight=-1.0)
@@ -462,14 +376,7 @@ def test_refusals():
 
 # ------------------------------------------------------------------------------------------------------------ resources
 def test_kernels_have_no_stack_frame_or_spills(tmp_path):
-    from tianshou_b200.csrc import build as B
-    if shutil.which(B.NVCC) is None and not os.path.exists(B.NVCC):
-        pytest.skip("nvcc not available")
-    r = subprocess.run([B.NVCC, *B.FLAGS, "-c", os.path.join(B.HERE, "qrdqn.cu"), "-o", str(tmp_path / "q.o")], capture_output=True,
-                       text=True)
-    assert r.returncode == 0, r.stdout + r.stderr
-    hits = re.findall(r"Compiling entry function '(\S+)' for 'sm_90a'\n(?:.*\n)*?\s*(\d+) bytes stack frame, (\d+) bytes spill "
-                      r"stores, (\d+) bytes spill loads", r.stdout + r.stderr)
+    report = ptxas_report("qrdqn.cu", tmp_path)
     kernels = ("qrdqn_rows_kernel", "qrdqn_target_kernel", "row_sums3_kernel")
-    assert len(hits) == 3 and all(any(k in h[0] for k in kernels) for h in hits), hits
-    assert all(tuple(map(int, h[1:])) == (0, 0, 0) for h in hits), hits
+    assert len(report) == 3 and all(any(k in e for k in kernels) for e in report), report
+    assert_spill_free(report)

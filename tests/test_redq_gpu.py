@@ -5,32 +5,17 @@ gradient of every optimiser step against float64 autograd of the eager restateme
 repeats, the absence of host synchronisation inside the update, ``state_dict()`` round trips, the refusals and the register
 report."""
 import copy
-import os
 import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
+from offpolicy_testutil import DEV, Box, assert_spill_free, check_params, golden_cfg, load_params, ptxas_report, stream
 from ts_testutil import load_golden, record_parity
 
-DEV = "cuda:0"
 gpu = pytest.mark.gpu
 KEYS = ("obs", "act", "rew", "terminated", "truncated", "obs_next")
-
-
-class _Box:
-    def __init__(self, dim, m=1.0):
-        self.shape = (dim,)
-        self.low = -m * np.ones(dim, np.float32)
-        self.high = m * np.ones(dim, np.float32)
-
-
-def _st():
-    from tianshou_b200._cabi import stream_ptr
-    return stream_ptr(torch.device(DEV))
 
 
 # ------------------------------------------------------------------------------------------------------------ batched GEMM
@@ -59,7 +44,7 @@ def _batched(E, M, N, K, a_mn, b_mn, *, share_a, bias, act, mask_kind, accumulat
     y_d = y.to(DEV) if y is not None else None
     call("ts_net_gemm_batched", E, ptr(a_st), M if a_mn else K, a_mn, 0 if share_a else M * K, ptr(b_st), N if b_mn else K, b_mn,
          N * K, ptr(c), N, M * N, M, N, K, ptr(bv_d), N, act, ptr(y_d), N, M * N, mask_kind or 1, int(accumulate),
-         ptr(w) if ws_n else None, ws_n, _st())
+         ptr(w) if ws_n else None, ws_n, stream())
     torch.cuda.synchronize()
     ref = torch.matmul(A.double(), B.double().transpose(1, 2)).expand(E, M, N)
     bound = torch.matmul(A.double().abs(), B.double().abs().transpose(1, 2)).expand(E, M, N).clone()
@@ -129,9 +114,9 @@ def test_one_member_batched_gemm_equals_net_gemm_bitwise(shape):
         lda, ldb = (M if a_mn else K), (N if b_mn else K)
         c1, c2 = c0.clone(), c0.clone()
         call("ts_net_gemm", ptr(a), lda, a_mn, ptr(b), ldb, b_mn, ptr(c1), N, M, N, K, ptr(bias), 2, ptr(y), N, 1, 1,
-             ptr(ws) if ws_n else None, ws_n, _st())
+             ptr(ws) if ws_n else None, ws_n, stream())
         call("ts_net_gemm_batched", 1, ptr(a), lda, a_mn, 0, ptr(b), ldb, b_mn, 0, ptr(c2), N, 0, M, N, K, ptr(bias), 0, 2, ptr(y),
-             N, 0, 1, 1, ptr(ws) if ws_n else None, ws_n, _st())
+             N, 0, 1, 1, ptr(ws) if ws_n else None, ws_n, stream())
         torch.cuda.synchronize()
         assert torch.equal(c1, c2), (a_mn, b_mn)
 
@@ -144,9 +129,9 @@ def test_batched_colsum_and_member_sum():
     x = torch.randn(E, M, N, generator=g)
     out = torch.full((E, 1, N), float("nan"), device=DEV)
     xd = x.to(DEV)
-    call("ts_net_colsum_batched", E, ptr(xd), N, M * N, M, N, ptr(out), N, 0, _st())
+    call("ts_net_colsum_batched", E, ptr(xd), N, M * N, M, N, ptr(out), N, 0, stream())
     s = torch.zeros(M, N, device=DEV)
-    call("ts_net_member_sum", ptr(xd), E, M * N, M * N, ptr(s), 0, _st())
+    call("ts_net_member_sum", ptr(xd), E, M * N, M * N, ptr(s), 0, stream())
     torch.cuda.synchronize()
     record_parity("redq_colsum", out.cpu().reshape(E, N).numpy(), x.double().sum(1).numpy(), rtol=1e-5, atol=1e-4)
     ref = x[0].clone()
@@ -242,12 +227,12 @@ def test_redq_kernels_vs_fp64(B, mode):
     d = (lambda f: lambda t: f(id(t)))(d)
     out = torch.full((B,), float("nan"), device=DEV)
     code = ABI.consts["TS_REDQ_MIN" if mode == "min" else "TS_REDQ_MEAN"]
-    call("ts_redq_target", ptr(d(q)), E, B, mask, code, alpha, ptr(d(logp)), ptr(out), _st())
+    call("ts_redq_target", ptr(d(q)), E, B, mask, code, alpha, ptr(d(logp)), ptr(out), stream())
     td, dq = torch.full((E, B), float("nan"), device=DEV), torch.full((E, B), float("nan"), device=DEV)
     rmean, rows, loss = torch.empty(B, device=DEV), torch.empty(B, device=DEV), torch.full((1,), float("nan"), device=DEV)
-    call("ts_redq_critic_rows", ptr(d(q)), ptr(d(target)), ptr(d(w)), E, B, ptr(td), ptr(dq), ptr(rmean), ptr(rows), ptr(loss), _st())
+    call("ts_redq_critic_rows", ptr(d(q)), ptr(d(target)), ptr(d(w)), E, B, ptr(td), ptr(dq), ptr(rmean), ptr(rows), ptr(loss), stream())
     adq, arows, aloss = torch.full((E, B), float("nan"), device=DEV), torch.empty(B, device=DEV), torch.full((1,), float("nan"), device=DEV)
-    call("ts_redq_actor_rows", ptr(d(q)), ptr(d(logp)), E, B, alpha, ptr(adq), ptr(arows), ptr(aloss), _st())
+    call("ts_redq_actor_rows", ptr(d(q)), ptr(d(logp)), E, B, alpha, ptr(adq), ptr(arows), ptr(aloss), stream())
     torch.cuda.synchronize()
     qd = q.double()
     sub = qd[subset]
@@ -268,7 +253,7 @@ def test_redq_kernels_vs_fp64(B, mode):
     record_parity(f"{tag}/actor_loss", aloss.cpu().numpy(), np.array([aref.item()]), rtol=1e-5, atol=1e-6)
     record_parity(f"{tag}/actor_dq", adq.cpu().numpy(), qa.grad.numpy(), rtol=1e-6, atol=0)
     again = torch.empty(1, device=DEV)
-    call("ts_redq_critic_rows", ptr(d(q)), ptr(d(target)), ptr(d(w)), E, B, ptr(td), ptr(dq), ptr(rmean), ptr(rows), ptr(again), _st())
+    call("ts_redq_critic_rows", ptr(d(q)), ptr(d(target)), ptr(d(w)), E, B, ptr(td), ptr(dq), ptr(rmean), ptr(rows), ptr(again), stream())
     torch.cuda.synchronize()
     assert torch.equal(again, loss)
 
@@ -279,25 +264,10 @@ def test_redq_target_refuses_bad_masks():
     q, logp, out = torch.zeros(3, 4, device=DEV), torch.zeros(4, device=DEV), torch.zeros(4, device=DEV)
     for E, mask in ((65, 1), (3, 0), (3, 8)):
         with pytest.raises(RuntimeError):
-            call("ts_redq_target", ptr(q), E, 4, mask, 0, 0.1, ptr(logp), ptr(out), _st())
+            call("ts_redq_target", ptr(q), E, 4, mask, 0, 0.1, ptr(logp), ptr(out), stream())
 
 
 # ------------------------------------------------------------------------------------------------------------ goldens
-def _cfg(g):
-    return {k[4:]: g[k] for k in g.files if k.startswith("cfg_")}
-
-
-def _load(mod, g, prefix):
-    with torch.no_grad():
-        for i, p in enumerate(mod.parameters()):
-            p.copy_(torch.as_tensor(g[f"{prefix}{i}"]).reshape(p.shape))
-
-
-def _check_params(tag, mod, g, prefix, lr):
-    for i, p in enumerate(mod.parameters()):
-        record_parity(f"{tag}/{prefix}{i}", p.detach().cpu().numpy(), g[f"{prefix}{i}"], rtol=1e-3, atol=0.1 * lr)
-
-
 def _build(cfg, g=None, **over):
     from tianshou_b200.algorithm import REDQ, AdamOptimizerFactory, REDQPolicy
     from tianshou_b200.algorithm.modelfree.sac import AutoAlpha
@@ -308,10 +278,10 @@ def _build(cfg, g=None, **over):
                                          conditioned_sigma=True).to(DEV)
     critic = _ensemble_critic(O, A, H, E)
     if g is not None:
-        _load(actor, g, "p0_actor_"); _load(critic, g, "p0_critic_")
+        load_params(actor, g, "p0_actor_"); load_params(critic, g, "p0_critic_")
     alpha = (AutoAlpha(-A, 0.0, AdamOptimizerFactory(lr=float(cfg["alpha_lr"]))).to(DEV) if bool(cfg["auto_alpha"])
              else float(cfg["alpha"]))
-    policy = REDQPolicy(actor=actor, action_space=_Box(A))
+    policy = REDQPolicy(actor=actor, action_space=Box(A))
     kw = dict(policy=policy, policy_optim=AdamOptimizerFactory(lr=float(cfg["actor_lr"])), critic=critic,
               critic_optim=AdamOptimizerFactory(lr=float(cfg["critic_lr"])), ensemble_size=E, subset_size=int(cfg["M"]),
               tau=float(cfg["tau"]), gamma=float(cfg["gamma"]), alpha=alpha, n_step_return_horizon=int(cfg["n_step"]),
@@ -322,7 +292,7 @@ def _build(cfg, g=None, **over):
 
 def _buffer(g, mirror):
     from tianshou_b200.data import Batch, PrioritizedReplayBuffer, ReplayBuffer
-    cfg = _cfg(g)
+    cfg = golden_cfg(g)
     size = int(cfg["size"])
     buf = (PrioritizedReplayBuffer(size, alpha=float(cfg["per_alpha"]), beta=float(cfg["per_beta"]), device=DEV) if bool(cfg["per"])
            else ReplayBuffer(size, device=DEV))
@@ -364,7 +334,7 @@ class _SubsetSpy:
 def test_update_matches_reference(variant, mirror, monkeypatch):
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden(f"redq_ref_{variant}.npz")
-    cfg = _cfg(g)
+    cfg = golden_cfg(g)
     algo = _build(cfg, g)
     assert sorted(algo.state_dict().keys()) == list(g["state_dict_keys"]), "state_dict() keys differ from the reference's"
     buf = _buffer(g, mirror)
@@ -398,9 +368,9 @@ def test_update_matches_reference(variant, mirror, monkeypatch):
         if bool(cfg["per"]):
             record_parity(f"{tag}/is_weight", captured["is_weight"], g[o + "is_weight"], rtol=1e-6, atol=1e-7)
             record_parity(f"{tag}/priorities", np.asarray(buf.weight[np.arange(len(buf))]), g[o + "priorities"], rtol=1e-3, atol=1e-6)
-        _check_params(tag, algo.policy.actor, g, o + "actor_", a_lr)
-        _check_params(tag, algo.critic, g, o + "critic_", lr)
-        _check_params(tag, algo.critic_old, g, o + "cold_", lr)
+        check_params(tag, algo.policy.actor, g, o + "actor_", a_lr)
+        check_params(tag, algo.critic, g, o + "critic_", lr)
+        check_params(tag, algo.critic_old, g, o + "cold_", lr)
     assert algo.critic_gradient_step == int(cfg["updates"])
 
 
@@ -507,7 +477,7 @@ def test_update_gradients_vs_fp64_autograd(mode, monkeypatch):
 def test_identical_updates_are_bit_identical():
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden("redq_ref_mujoco.npz")
-    cfg = _cfg(g)
+    cfg = golden_cfg(g)
     flats = []
     for _ in range(2):
         algo = _build(cfg, g)
@@ -528,7 +498,7 @@ def test_device_update_has_no_torch_host_sync():
     losses are read at the end."""
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden("redq_ref_mujoco.npz")
-    algo = _build(_cfg(g), g)
+    algo = _build(golden_cfg(g), g)
     buf = _buffer(g, mirror=True)
     seen = []
     orig_cpu = torch.Tensor.cpu
@@ -560,7 +530,7 @@ def test_device_update_has_no_torch_host_sync():
 def test_state_dict_round_trip_continues_identically():
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden("redq_ref_mujoco.npz")        # actor_delay 3: the continuation takes an actor step
-    cfg = _cfg(g)
+    cfg = golden_cfg(g)
     a = _build(cfg, g)
     a._noise_fn = _cpu_noise
     buf_a = _buffer(g, mirror=False)
@@ -599,7 +569,7 @@ def test_refusals():
         actor = ContinuousActorProbabilistic(preprocess_net=Net(state_shape=(O,), hidden_sizes=(8,)), action_shape=(A,),
                                              unbounded=unbounded, conditioned_sigma=c_sigma).to(dev)
         critic = critic if critic is not None else _ensemble_critic(O, A, (8,), E).to(dev)
-        return REDQ(policy=REDQPolicy(actor=actor, action_space=_Box(A)), policy_optim=AdamOptimizerFactory(lr=1e-3), critic=critic,
+        return REDQ(policy=REDQPolicy(actor=actor, action_space=Box(A)), policy_optim=AdamOptimizerFactory(lr=1e-3), critic=critic,
                     critic_optim=AdamOptimizerFactory(lr=1e-3), ensemble_size=kw.pop("ensemble_size", E), subset_size=2, **kw)
 
     make()
@@ -628,25 +598,15 @@ def test_refusals():
 
 
 # ------------------------------------------------------------------------------------------------------------ resources
-def _ptxas(src, tmp_path):
-    from tianshou_b200.csrc import build as B
-    if shutil.which(B.NVCC) is None and not os.path.exists(B.NVCC):
-        pytest.skip("nvcc not available")
-    r = subprocess.run([B.NVCC, *B.FLAGS, "-c", os.path.join(B.HERE, src), "-o", str(tmp_path / "t.o")], capture_output=True, text=True)
-    assert r.returncode == 0, r.stdout + r.stderr
-    return re.findall(r"Compiling entry function '(\S+)' for 'sm_90a'\n(?:.*\n)*?\s*(\d+) bytes stack frame, (\d+) bytes spill "
-                      r"stores, (\d+) bytes spill loads", r.stdout + r.stderr)
-
-
 def test_redq_kernels_have_no_stack_frame_or_spills(tmp_path):
-    hits = _ptxas("redq.cu", tmp_path)
-    names = sorted(re.search(r"redq_(target|critic_rows|actor_rows|sum)_kernel", h[0]).group(1) for h in hits)
-    assert names == ["actor_rows", "critic_rows", "sum", "target"], hits
-    assert all(tuple(map(int, h[1:])) == (0, 0, 0) for h in hits), hits
+    report = ptxas_report("redq.cu", tmp_path)
+    names = sorted(re.search(r"redq_(target|critic_rows|actor_rows|sum)_kernel", e).group(1) for e in report)
+    assert names == ["actor_rows", "critic_rows", "sum", "target"], report
+    assert_spill_free(report)
 
 
 def test_net_gemm_kernels_have_no_stack_frame_or_spills(tmp_path):
-    hits = _ptxas("net_gemm.cu", tmp_path)
-    gemm = [h for h in hits if "net_gemm_kernel" in h[0]]
-    assert len(gemm) == 4 and len(hits) == 7, hits
-    assert all(tuple(map(int, h[1:])) == (0, 0, 0) for h in hits), hits
+    report = ptxas_report("net_gemm.cu", tmp_path)
+    gemm = [e for e in report if "net_gemm_kernel" in e]
+    assert len(gemm) == 4 and len(report) == 7, report
+    assert_spill_free(report)

@@ -3,32 +3,17 @@
 step against float64 autograd of the eager restatement, the delayed actor and lagged networks, the absence of host
 synchronisation inside the update, ``state_dict()`` round trips, the refusals and the kernels' register report."""
 import copy
-import os
 import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
+from offpolicy_testutil import DEV, Box, Discrete, assert_spill_free, check_params, golden_cfg, load_params, ptxas_report, stream
 from ts_testutil import load_golden, record_parity
 
-DEV = "cuda:0"
 gpu = pytest.mark.gpu
 KEYS = ("obs", "act", "rew", "terminated", "truncated", "obs_next")
-
-
-class _Box:
-    def __init__(self, dim, m=1.0):
-        self.shape = (dim,)
-        self.low = -m * np.ones(dim, np.float32)
-        self.high = m * np.ones(dim, np.float32)
-
-
-def _st():
-    from tianshou_b200._cabi import stream_ptr
-    return stream_ptr(torch.device(DEV))
 
 
 # ------------------------------------------------------------------------------------------------------------ kernels
@@ -46,7 +31,7 @@ def test_act_rows_kernel_vs_fp64(B, O, A, m, clip, noisy):
     pn = 0.7
     d = [t.to(DEV).contiguous() for t in (z, obs, noise)]
     x = torch.full((B, O + A), float("nan"), device=DEV)
-    call("ts_td3_act_rows", ptr(d[0]), ptr(d[2]) if noisy else None, B, A, m, pn, clip, ptr(d[1]), O, ptr(x), _st())
+    call("ts_td3_act_rows", ptr(d[0]), ptr(d[2]) if noisy else None, B, A, m, pn, clip, ptr(d[1]), O, ptr(x), stream())
     torch.cuda.synchronize()
     a = m * torch.tanh(z.double())
     if noisy:
@@ -69,7 +54,7 @@ def test_target_min_kernel(B):
     q1[0] = float("nan")
     d = [t.to(DEV) for t in (q1, q2)]
     out = torch.empty(B, device=DEV)
-    call("ts_td3_target_min", ptr(d[0]), ptr(d[1]), B, ptr(out), _st())
+    call("ts_td3_target_min", ptr(d[0]), ptr(d[1]), B, ptr(out), stream())
     torch.cuda.synchronize()
     assert torch.equal(out.cpu().nan_to_num(-7.0), torch.min(q1, q2).nan_to_num(-7.0))
 
@@ -77,8 +62,8 @@ def test_target_min_kernel(B):
 def _actor_kernels(q, z, act, dact, B, A, m, alpha):
     from tianshou_b200._cabi import call, ptr
     dq, loss, dz = torch.full((B,), float("nan"), device=DEV), torch.full((1,), float("nan"), device=DEV), torch.empty(B, A, device=DEV)
-    call("ts_td3_actor_rows", ptr(q), ptr(z), ptr(act), B, A, m, alpha, ptr(dq), ptr(loss), _st())
-    call("ts_td3_actor_head_bwd", ptr(z), ptr(dact), ptr(act), B, A, m, ptr(dz), _st())
+    call("ts_td3_actor_rows", ptr(q), ptr(z), ptr(act), B, A, m, alpha, ptr(dq), ptr(loss), stream())
+    call("ts_td3_actor_head_bwd", ptr(z), ptr(dact), ptr(act), B, A, m, ptr(dz), stream())
     torch.cuda.synchronize()
     return dq, loss, dz
 
@@ -117,21 +102,6 @@ def test_actor_rows_and_head_backward_vs_fp64_autograd(B, A, m, bc):
 
 
 # ------------------------------------------------------------------------------------------------------------ goldens
-def _cfg(g):
-    return {k[4:]: g[k] for k in g.files if k.startswith("cfg_")}
-
-
-def _load(mod, g, prefix):
-    with torch.no_grad():
-        for i, p in enumerate(mod.parameters()):
-            p.copy_(torch.as_tensor(g[f"{prefix}{i}"]).reshape(p.shape))
-
-
-def _check_params(tag, mod, g, prefix, lr):
-    for i, p in enumerate(mod.parameters()):
-        record_parity(f"{tag}/{prefix}{i}", p.detach().cpu().numpy(), g[f"{prefix}{i}"], rtol=1e-3, atol=0.1 * lr)
-
-
 def _nets(O, A, H, m=1.0, last_hidden=()):
     from tianshou_b200.utils.net.common import Net
     from tianshou_b200.utils.net.continuous import ContinuousActorDeterministic, ContinuousCritic
@@ -141,7 +111,7 @@ def _nets(O, A, H, m=1.0, last_hidden=()):
     return actor, crit
 
 
-def _build(cfg, g=None, **over):
+def build_from_cfg(cfg, g=None, **over):
     from tianshou_b200.algorithm import TD3, TD3BC, AdamOptimizerFactory
     from tianshou_b200.algorithm.modelfree.ddpg import ContinuousDeterministicPolicy
     O, A, H, m = int(cfg["obs"]), int(cfg["act"]), tuple(int(x) for x in cfg["hidden"]), float(cfg["max_action"])
@@ -149,10 +119,10 @@ def _build(cfg, g=None, **over):
     c1 = crit()
     c2 = crit() if bool(cfg["critic2"]) else None
     if g is not None:
-        _load(actor, g, "p0_actor_"); _load(c1, g, "p0_c1_")
+        load_params(actor, g, "p0_actor_"); load_params(c1, g, "p0_c1_")
         if c2 is not None:
-            _load(c2, g, "p0_c2_")
-    policy = ContinuousDeterministicPolicy(actor=actor, action_space=_Box(A, m), action_scaling=bool(cfg["action_scaling"]))
+            load_params(c2, g, "p0_c2_")
+    policy = ContinuousDeterministicPolicy(actor=actor, action_space=Box(A, m), action_scaling=bool(cfg["action_scaling"]))
     kw = dict(policy=policy, policy_optim=AdamOptimizerFactory(lr=float(cfg["actor_lr"])), critic=c1,
               critic_optim=AdamOptimizerFactory(lr=float(cfg["critic_lr"])), critic2=c2,
               critic2_optim=AdamOptimizerFactory(lr=float(cfg["critic2_lr"])) if c2 is not None else None, tau=float(cfg["tau"]),
@@ -164,9 +134,9 @@ def _build(cfg, g=None, **over):
     return TD3(**kw)
 
 
-def _buffer(g, mirror):
+def buffer_from_golden(g, mirror):
     from tianshou_b200.data import Batch, PrioritizedReplayBuffer, ReplayBuffer
-    cfg = _cfg(g)
+    cfg = golden_cfg(g)
     if int(cfg["adds"]) == 0:
         buf = ReplayBuffer.from_data(*(g["buf_" + k].copy() for k in ("obs", "act", "rew", "terminated", "truncated", "done", "obs_next")))
     else:
@@ -195,10 +165,10 @@ def _cpu_noise(shape):
 def test_update_matches_reference(variant, mirror):
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden(f"td3_ref_{variant}.npz")
-    cfg = _cfg(g)
-    algo = _build(cfg, g)
+    cfg = golden_cfg(g)
+    algo = build_from_cfg(cfg, g)
     assert sorted(algo.state_dict().keys()) == list(g["state_dict_keys"]), "state_dict() keys differ from the reference's"
-    buf = _buffer(g, mirror)
+    buf = buffer_from_golden(g, mirror)
     algo._noise_fn = _cpu_noise
     captured = {}
     orig = algo._preprocess_batch
@@ -225,10 +195,10 @@ def test_update_matches_reference(variant, mirror):
         if bool(cfg["per"]):
             record_parity(f"{tag}/is_weight", captured["is_weight"], g[o + "is_weight"], rtol=1e-6, atol=1e-7)
             record_parity(f"{tag}/priorities", np.asarray(buf.weight[np.arange(len(buf))]), g[o + "priorities"], rtol=1e-3, atol=1e-6)
-        _check_params(tag, algo.policy.actor, g, o + "actor_", a_lr)
-        _check_params(tag, algo.critic, g, o + "c1_", lr); _check_params(tag, algo.critic2, g, o + "c2_", c2_lr)
-        _check_params(tag, algo.critic_old, g, o + "c1old_", lr); _check_params(tag, algo.critic2_old, g, o + "c2old_", c2_lr)
-        _check_params(tag, algo.actor_old, g, o + "aold_", a_lr)
+        check_params(tag, algo.policy.actor, g, o + "actor_", a_lr)
+        check_params(tag, algo.critic, g, o + "c1_", lr); check_params(tag, algo.critic2, g, o + "c2_", c2_lr)
+        check_params(tag, algo.critic_old, g, o + "c1old_", lr); check_params(tag, algo.critic2_old, g, o + "c2old_", c2_lr)
+        check_params(tag, algo.actor_old, g, o + "aold_", a_lr)
 
 
 @gpu
@@ -237,8 +207,8 @@ def test_delayed_actor_and_lagged_networks():
     are bit-unchanged, the actor too, and actor_loss repeats the last actor step's loss."""
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden("td3_ref_mujoco.npz")
-    algo = _build(_cfg(g), g)
-    buf = _buffer(g, mirror=True)
+    algo = build_from_cfg(golden_cfg(g), g)
+    buf = buffer_from_golden(g, mirror=True)
     assert algo._cnt == 0 and algo._last == 0
     groups = lambda: [t.flat.clone() for t in (algo._g_actor, *algo._g_ct, algo._g_at)]
     last = None
@@ -300,7 +270,7 @@ def grad_case(O, A, H, algo_kind, B=256, edge=""):
     cfg = dict(obs=O, act=A, hidden=H, max_action=m, critic2=True, critic2_lr=1e-3, action_scaling=False, actor_lr=1e-4,
                critic_lr=3e-4, tau=0.005, gamma=0.99, policy_noise=0.2, freq=2, noise_clip=0.5, n_step=3, algo=algo_kind, alpha=2.5)
     torch.manual_seed(3)
-    algo = _build(cfg)
+    algo = build_from_cfg(cfg)
     buf = _random_buffer(O, A, 700, seed=O + A, m=m)
     noises = []
 
@@ -373,8 +343,8 @@ def test_device_update_has_no_torch_host_sync(variant):
     """The critic steps, the actor step (TD3+BC's lmbda included) and Polyak run under torch.cuda.set_sync_debug_mode("error")."""
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden(f"td3_ref_{variant}.npz")
-    algo = _build(_cfg(g), g)
-    buf = _buffer(g, mirror=True)
+    algo = build_from_cfg(golden_cfg(g), g)
+    buf = buffer_from_golden(g, mirror=True)
     with policy_within_training_step(algo.policy):
         algo.update(buf, 32)                      # first update: scratch buffers exist afterwards
         for cnt in (0, 1):                        # an actor step, then a critic-only step
@@ -398,22 +368,22 @@ def test_state_dict_round_trip_continues_identically(variant):
     point of the actor schedule) continues bit for bit."""
     from tianshou_b200.utils import policy_within_training_step
     g = load_golden(f"td3_ref_{variant}.npz")
-    cfg = _cfg(g)
-    a = _build(cfg, g)
+    cfg = golden_cfg(g)
+    a = build_from_cfg(cfg, g)
     a._noise_fn = _cpu_noise
-    buf_a = _buffer(g, mirror=False)
+    buf_a = buffer_from_golden(g, mirror=False)
     for u in range(2):
         torch.manual_seed(1 + u)
         with policy_within_training_step(a.policy):
             a.update(buf_a, int(cfg["bs"]))
-    b = _build(cfg, g)
+    b = build_from_cfg(cfg, g)
     b._noise_fn = _cpu_noise
     with torch.no_grad():
         for p in b.parameters():
             p.add_(0.01)
     b.load_state_dict(copy.deepcopy(a.state_dict()))
     for algo in (a, b):
-        buf = _buffer(g, mirror=False)
+        buf = buffer_from_golden(g, mirror=False)
         for u in range(3):
             torch.manual_seed(10 + u)
             with policy_within_training_step(algo.policy):
@@ -436,22 +406,18 @@ def test_refusals_and_accepted_actors():
     from tianshou_b200.utils.net.continuous import ContinuousActorDeterministic, ContinuousCritic
     O, A = 4, 2
 
-    class _Discrete:
-        n = 3
-        shape = ()
-
     def make(cls=TD3, dev=DEV, space=None, actor=None, critic=None, m=1.0, last_hidden=(), **kw):
         actor = actor or ContinuousActorDeterministic(preprocess_net=Net(state_shape=(O,), hidden_sizes=(8,)), action_shape=(A,),
                                                       hidden_sizes=last_hidden, max_action=m)
         critic = critic or ContinuousCritic(preprocess_net=Net(state_shape=(O,), action_shape=(A,), hidden_sizes=(8,), concat=True))
-        pol = ContinuousDeterministicPolicy(actor=actor.to(dev), action_space=space or _Box(A, m), action_scaling=space is None and m == 1.0,
+        pol = ContinuousDeterministicPolicy(actor=actor.to(dev), action_space=space or Box(A, m), action_scaling=space is None and m == 1.0,
                                             action_bound_method=None if space is not None else "clip")
         return cls(policy=pol, policy_optim=AdamOptimizerFactory(lr=1e-3), critic=critic.to(dev), critic_optim=AdamOptimizerFactory(lr=1e-3),
                    **kw)
 
     make()
     with pytest.raises(ValueError, match="Box"):
-        make(space=_Discrete())
+        make(space=Discrete(3))
     with pytest.raises(UnsupportedModelError, match="no CPU path"):
         make(dev="cpu")
     with pytest.raises(UnsupportedModelError, match="no CPU path"):
@@ -476,13 +442,7 @@ def test_refusals_and_accepted_actors():
 
 # ------------------------------------------------------------------------------------------------------------ resources
 def test_td3_kernels_have_no_stack_frame_or_spills(tmp_path):
-    from tianshou_b200.csrc import build as B
-    if shutil.which(B.NVCC) is None and not os.path.exists(B.NVCC):
-        pytest.skip("nvcc not available")
-    r = subprocess.run([B.NVCC, *B.FLAGS, "-c", os.path.join(B.HERE, "td3.cu"), "-o", str(tmp_path / "t.o")], capture_output=True, text=True)
-    assert r.returncode == 0, r.stdout + r.stderr
-    hits = re.findall(r"Compiling entry function '(\S+)' for 'sm_90a'\n(?:.*\n)*?\s*(\d+) bytes stack frame, (\d+) bytes spill "
-                      r"stores, (\d+) bytes spill loads", r.stdout + r.stderr)
-    names = sorted(re.search(r"td3_(act_rows|target_min|actor_rows|actor_head_bwd)_kernel", h[0]).group(1) for h in hits)
-    assert names == ["act_rows", "actor_head_bwd", "actor_rows", "target_min"], hits
-    assert all(tuple(map(int, h[1:])) == (0, 0, 0) for h in hits), hits
+    report = ptxas_report("td3.cu", tmp_path)
+    names = sorted(re.search(r"td3_(act_rows|target_min|actor_rows|actor_head_bwd)_kernel", e).group(1) for e in report)
+    assert names == ["act_rows", "actor_head_bwd", "actor_rows", "target_min"], report
+    assert_spill_free(report)

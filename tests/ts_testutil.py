@@ -21,10 +21,10 @@ PARAM_ORDER = ["a_w1", "a_b1", "a_w2", "a_b2", "a_w3", "a_b3", "a_logstd",
 class Box:
     """Minimal stand-in for gymnasium.spaces.Box (gymnasium is not a dependency)."""
 
-    def __init__(self, dim: int):
+    def __init__(self, dim: int, m: float = 1.0):
         self.shape = (dim,)
-        self.low = -np.ones(dim, np.float32)
-        self.high = np.ones(dim, np.float32)
+        self.low = -m * np.ones(dim, np.float32)
+        self.high = m * np.ones(dim, np.float32)
 
 
 def build_actor_critic(obs_dim: int, act_dim: int, device, seed: int = 0):
