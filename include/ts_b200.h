@@ -837,6 +837,25 @@ int ts_c51_rows(const float* logits, const int64_t* act, const float* returns, c
                 float delta_z, const float* next_dist, const float* weight, int64_t B, int32_t A, int32_t N, float* dlogits,
                 float* prio, float* rows, float* losses, ts_stream_t stream);
 
+/* ---- Rainbow (rainbow.cu) ---- */
+/* The train-mode weight of a noisy layer (utils/net/discrete.py NoisyLinear): mu_w, sigma_w [out][in], mu_b, sigma_b [out], the
+ * factorised noise eps_p [in], eps_q [out]; w_eff [out][in] = mu_w + sigma_w * (eps_q[o] * eps_p[i]), b_eff [out] = mu_b +
+ * sigma_b * eps_q[o], each product and sum rounded on its own: bit for bit torch's ger, then *, then +.  Any out, in >= 1. */
+int ts_noisy_weight(const float* mu_w, const float* sigma_w, const float* mu_b, const float* sigma_b, const float* eps_p,
+                    const float* eps_q, int32_t out, int32_t in, float* w_eff, float* b_eff, ts_stream_t stream);
+/* The gradient of a noisy layer's four trainable tensors from dw [out][in] and db [out], the gradients at its effective weight and
+ * bias: g_mu_w = dw, g_sigma_w = dw * (eps_q[o] * eps_p[i]), g_mu_b = db, g_sigma_b = db * eps_q[o], each product rounded on its
+ * own.  Any out, in >= 1. */
+int ts_noisy_grad(const float* dw, const float* db, const float* eps_p, const float* eps_q, int32_t out, int32_t in, float* g_mu_w,
+                  float* g_sigma_w, float* g_mu_b, float* g_sigma_b, ts_stream_t stream);
+/* The dueling combine of the categorical heads (common.py:355-364, atari_network.py:196-206): q [B][A][N] (the Q head's A * N
+ * outputs), v [B][N]; logits [B][A][N] = (q - m) + v with m [B][N] = (sum_a q in index order) / A.  Any B >= 0 (B == 0 launches
+ * nothing), A, N >= 1. */
+int ts_dueling_atoms(const float* q, const float* v, int64_t B, int32_t A, int32_t N, float* logits, ts_stream_t stream);
+/* Its backward from dlogits [B][A][N]: dv [B][N] = s = sum_a dlogits (index order), dq [B][A][N] = dlogits - s / A.  No atomics:
+ * two calls on the same input are bit-identical.  Any B >= 0, A, N >= 1. */
+int ts_dueling_atoms_bwd(const float* dlogits, int64_t B, int32_t A, int32_t N, float* dq, float* dv, ts_stream_t stream);
+
 /* ---- IQN (iqn.cu) ---- */
 /* The network of IQN (utils/net/discrete.py:163-216) is a trunk on B rows (feat [B][D]), the cosine embedding of S fractions per
  * row and a head on the B * S rows h[b * S + s] = feat[b] * e[b * S + s], sample-major, so the head's output is q [B][S][A].  The

@@ -12,6 +12,7 @@ from .modelfree.iqn import IQN, IQNPolicy
 from .modelfree.npg import NPG, NPGTrainingStats
 from .modelfree.ppo import A2C, PPO
 from .modelfree.qrdqn import QRDQN, QRDQNPolicy
+from .modelfree.rainbow import RainbowDQN, RainbowTrainingStats
 from .modelfree.redq import REDQ, REDQPolicy, REDQTrainingStats
 from .modelfree.reinforce import DiscreteActorPolicy, ProbabilisticActorPolicy
 from .modelfree.td3 import TD3, TD3TrainingStats
@@ -26,4 +27,5 @@ __all__ = [
     "RMSpropOptimizerFactory", "DiscreteBCQ", "DiscreteBCQPolicy", "DiscreteBCQTrainingStats", "DiscreteCRR",
     "DiscreteCRRTrainingStats", "QRDQN", "QRDQNPolicy", "DiscreteCQL", "DiscreteCQLTrainingStats", "IQN", "IQNPolicy",
     "FQF", "FQFPolicy", "FQFTrainingStats", "REDQ", "REDQPolicy", "REDQTrainingStats", "BDQN", "BDQNPolicy", "C51", "C51Policy",
+    "RainbowDQN", "RainbowTrainingStats",
 ]

@@ -17,9 +17,10 @@ from torch import nn
 
 from .._cabi import to_device
 from ..data import Batch, ReplayBuffer
+from ..utils.net.discrete import NoisyLinear
 from .base import Algorithm
 from .flat_params import DeviceScratch, FlatGroup, UnsupportedModelError
-from .netgraph import ACT_NONE, compile_sequential, module_layers
+from .netgraph import ACT_NONE, _Layer, _out_shape, compile_sequential, module_layers, network_heads
 from .obs_source import DeviceObsSource, device_obs_source
 from .twin_critic import per_weight
 
@@ -35,21 +36,56 @@ def describe_q_network(model: Any) -> tuple[Any, tuple[int, ...], float]:
     if hasattr(inner, "input_shape"):
         return inner, tuple(inner.input_shape), scale
     first = module_layers(inner)[0]
-    if isinstance(first, nn.Linear):
+    if isinstance(first, (nn.Linear, NoisyLinear)):
         return inner, (int(first.in_features),), scale
     raise UnsupportedModelError(f"cannot infer the input shape of {type(inner).__name__}")
 
 
-def atom_chain(inner: Any, in_shape: tuple[int, ...], n_actions: int, n_atoms: int, kind: str, atom_name: str) -> list:
+def atom_chain(inner: Any, in_shape: tuple[int, ...], n_actions: int, n_atoms: int, kind: str, atom_name: str,
+               noisy: bool = False) -> list:
     """The layer chain of a distributional Q-network (QR-DQN's quantiles, C51's atoms): ``inner`` read as a plain chain ending in
     ``Linear(., n_actions * n_atoms)`` with no activation, the output viewed as ``[B, n_actions, n_atoms]``; anything else is
-    refused.  ``kind`` names the network, ``atom_name`` the per-action outputs (``num_<atom_name>`` is the keyword)."""
-    layers = compile_sequential(module_layers(inner), in_shape)
-    if layers[-1].kind != "linear" or layers[-1].act != ACT_NONE:
-        raise UnsupportedModelError(f"the {kind} network must end in a linear layer over actions * num_{atom_name}")
-    if layers[-1].out_dim != n_actions * n_atoms:
-        raise UnsupportedModelError(f"the network has {layers[-1].out_dim} outputs, not {n_actions} actions x {n_atoms} {atom_name}")
+    refused.  ``kind`` names the network, ``atom_name`` the per-action outputs (``num_<atom_name>`` is the keyword).
+    ``noisy``: ``NoisyLinear`` layers join the chain (Rainbow)."""
+    return _check_head(compile_sequential(module_layers(inner), in_shape, noisy=noisy), n_actions * n_atoms,
+                       f"{n_actions} actions x {n_atoms} {atom_name}", f"the {kind} network", f"actions * num_{atom_name}")
+
+
+def _check_head(layers: list[_Layer], width: int, what: str, name: str, over: str) -> list[_Layer]:
+    if not layers or layers[-1].kind != "linear" or layers[-1].act != ACT_NONE:
+        raise UnsupportedModelError(f"{name} must end in a linear layer over {over}")
+    if layers[-1].out_dim != width:
+        raise UnsupportedModelError(f"the network has {layers[-1].out_dim} outputs, not {what}")
     return layers
+
+
+def dueling_atom_chains(model: Any, n_actions: int, n_atoms: int) -> tuple[Any, tuple[int, ...], float, list[list[_Layer]]]:
+    """(inner module, input shape, input denominator, chains) of a categorical network whose Linear layers may be
+    ``NoisyLinear`` (Rainbow), optionally behind ``ScaledObsInputActionReprNet``.  A network with a V head (``Net(dueling_param=
+    ...)``, ``RainbowNet(is_dueling=True)``) gives three chains: the trunk, the Q head over ``n_actions * n_atoms`` outputs and the
+    V head over ``n_atoms``, both reading the trunk's output.  ``RainbowNet(is_dueling=False)`` gives its trunk and Q head as one
+    chain, any other network its plain chain (``atom_chain``)."""
+    heads = network_heads(model.module if hasattr(model, "denom") and hasattr(model, "module") else model)
+    if heads is None:
+        inner, in_shape, scale = describe_q_network(model)
+        return inner, in_shape, scale, [atom_chain(inner, in_shape, n_actions, n_atoms, "categorical", "atoms", noisy=True)]
+    scale, inner = (float(model.denom), model.module) if hasattr(model, "denom") and hasattr(model, "module") else (1.0, model)
+    trunk_m, q_m, v_m = heads
+    if hasattr(inner, "input_shape"):
+        in_shape = tuple(inner.input_shape)
+    elif trunk_m and hasattr(trunk_m[0], "in_features"):
+        in_shape = (int(trunk_m[0].in_features),)
+    else:
+        raise UnsupportedModelError(f"{type(inner).__name__}: the heads need a trunk that starts with a linear layer (hidden_sizes)")
+    what, over = f"{n_actions} actions x {n_atoms} atoms", "actions * num_atoms"
+    if v_m is None:
+        return inner, in_shape, scale, [_check_head(compile_sequential(trunk_m + q_m, in_shape, noisy=True), n_actions * n_atoms, what,
+                                                    "the Q head", over)]
+    trunk = compile_sequential(trunk_m, in_shape, noisy=True)
+    feat = _out_shape(trunk, in_shape)
+    q = _check_head(compile_sequential(q_m, feat, noisy=True), n_actions * n_atoms, what, "the Q head", over)
+    v = _check_head(compile_sequential(v_m, feat, noisy=True), n_atoms, f"{n_atoms} atoms", "the V head", "num_atoms")
+    return inner, in_shape, scale, [trunk, q, v]
 
 
 def describe_discrete_head(net: Any, role: str) -> tuple[Any, Any, tuple[int, ...], float]:

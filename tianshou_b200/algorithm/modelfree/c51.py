@@ -84,12 +84,11 @@ class C51(DiscreteQCore, OffPolicyAlgorithm):
         dev = cuda_device_of(policy.model)
         self._build_network(policy, dev)
         self.optim = self._create_optimizer(policy, optim)
-        bind_optimizer(self.optim, self._group, frozen=(policy.support,))
-        self.model_old: _EvalModeModule | None = None
+        bind_optimizer(self.optim, self._group, frozen=(policy.support, *self._frozen_params()))
+        self.model_old: nn.Module | None = None
         self._g_old: FlatGroup | None = None
         if self.use_target_network:
-            self.model_old = _EvalModeModule(deepcopy(policy.model))
-            self._g_old = lagged_group(self._group, list(self.model_old.parameters()))
+            self._build_lagged(policy)
 
     def _build_network(self, policy: C51Policy, dev: torch.device) -> None:
         """Read ``policy.model`` as a layer chain over ``actions * num_atoms`` logits whose module applies a softmax over each
@@ -107,6 +106,28 @@ class C51(DiscreteQCore, OffPolicyAlgorithm):
         self._init_discrete(dev, in_shape, in_scale, n_actions)
         self._group = FlatGroup(layer_params(layers), dev)
         self._net = FusedStack(layers, self._group, "c51")
+
+    def _frozen_params(self) -> tuple[nn.Parameter, ...]:
+        """Parameters of ``policy.model`` that the optimiser lists but never steps."""
+        return ()
+
+    def _build_lagged(self, policy: C51Policy) -> None:
+        self.model_old = _EvalModeModule(deepcopy(policy.model))
+        self._g_old = lagged_group(self._group, list(self.model_old.parameters()))
+
+    def _logits(self, src: Any, tag: str, lagged: bool = False) -> tuple[torch.Tensor, Any]:
+        """The raw ``[B, A * N]`` logits of the online (``lagged``: the lagged) network at the observation source ``src``, and
+        what ``_backward`` needs of that pass."""
+        params = None
+        if lagged:
+            self._g_old.ensure_adopted()
+            params = self._g_old.flat
+        acts = self._net.forward(src.x, src.rows, tag, frames=src.frames, params=params)
+        return acts[-1], acts
+
+    def _backward(self, acts: Any, dlogits: torch.Tensor, rows: int) -> None:
+        """Store d loss / d parameters in the group's gradient from d loss / d logits of the ``"up"`` pass."""
+        self._net.backward(acts, dlogits, rows, "up")
 
     @property
     def use_target_network(self) -> bool:
@@ -126,11 +147,10 @@ class C51(DiscreteQCore, OffPolicyAlgorithm):
         """The distribution of Q_old(s', argmax_a sum_k p_ak z_k) over the atoms, ``[B, N]``   (c51.py:113-124)."""
         src = batch.obs_next
         B = src.rows
-        logits_on = self._net.forward(src.x, B, "tq_on", frames=src.frames)[-1]
+        logits_on = self._logits(src, "tq_on")[0]
         logits_next = logits_on
         if self.use_target_network:
-            self._g_old.ensure_adopted()
-            logits_next = self._net.forward(src.x, B, "tq_old", frames=src.frames, params=self._g_old.flat)[-1]
+            logits_next = self._logits(src, "tq_old", lagged=True)[0]
         out = self._buf("next_dist", (B, self.policy.num_atoms))
         call("ts_c51_target", ptr(logits_on), ptr(logits_next), ptr(self.policy.support), B, self.n_actions, self.policy.num_atoms,
              ptr(out), None, stream_ptr(self._dev))
@@ -144,14 +164,14 @@ class C51(DiscreteQCore, OffPolicyAlgorithm):
         src = batch.obs
         B, A, N = src.rows, self.n_actions, pol.num_atoms
         weight = pop_batch_weight(batch, self._dev)
-        acts = self._net.forward(src.x, B, "up", frames=src.frames)
+        logits, acts = self._logits(src, "up")
         returns = batch.returns.reshape(B, N).to(self._dev, torch.float32).contiguous()
         dlogits, prio = self._buf("dlogits", (B, A * N)), self._buf("prio", B)
         rows, losses = self._buf("loss_rows", (3, B)), self._buf("losses", 4)
-        call("ts_c51_rows", ptr(acts[-1]), ptr(batch.act), ptr(returns), ptr(pol.support), float(pol.v_min), float(pol.v_max),
+        call("ts_c51_rows", ptr(logits), ptr(batch.act), ptr(returns), ptr(pol.support), float(pol.v_min), float(pol.v_max),
              float(self.delta_z), ptr(next_dist), ptr(weight), B, A, N, ptr(dlogits), ptr(prio), ptr(rows), ptr(losses),
              stream_ptr(self._dev))
         batch.weight = prio                     # prio-buffer
-        self._net.backward(acts, dlogits, B, "up")
+        self._backward(acts, dlogits, B)
         self._group.adam_step(self.optim._optim, self.optim._max_grad_norm)
         return LossSequenceTrainingStats(loss=float(losses[0].item()))      # the only host read of the loss

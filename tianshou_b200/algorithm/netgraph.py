@@ -6,7 +6,9 @@ utils/net/common.py:76-369, utils/net/continuous.py:96-238, env/atari/atari_netw
 forward, input gradient and weight gradient is ONE ``ts_net_gemm`` launch (wgmma, fp32-faithful), convolutions
 run as implicit GEMM over im2col rows.  A chain of ``EnsembleLinear`` layers (utils/net/common.py, REDQ's critic ensemble)
 runs every member of a layer in one batched launch (``ts_net_gemm_batched``) on ``[E, rows, features]`` activations, and so do
-the identical ``nn.Linear`` MLPs of a ``ModuleList`` read as one ensemble (``compile_branches``: BDQN's action branches).  Parameters live in a ``FlatGroup`` (flat_params.py: one flat fp32 buffer per optimiser,
+the identical ``nn.Linear`` MLPs of a ``ModuleList`` read as one ensemble (``compile_branches``: BDQN's action branches).  A
+``NoisyLinear`` layer (Rainbow) is a Linear layer whose train-mode weight and bias ``ts_noisy_weight`` forms into scratch before
+its GEMM, from the flat parameters and a second flat buffer holding the noise.  Parameters live in a ``FlatGroup`` (flat_params.py: one flat fp32 buffer per optimiser,
 ``nn.Parameter``s are views of it) so Adam and the Polyak update are single kernels and ``state_dict()`` keeps
 working.  There is no autograd graph and no eager-PyTorch path: unsupported layers raise ``UnsupportedModelError``.
 """
@@ -52,19 +54,30 @@ class _Layer:
     # an ensemble of nn.Linear members (compile_branches): member e's (weight [out, in], bias [out]); ``weight`` / ``bias`` are
     # member 0's, and the flat group holds the members' weights, then their biases, back to back (layer_params)
     members: list[tuple[nn.Parameter, nn.Parameter]] | None = None
+    # a NoisyLinear layer (kind "linear"): ``weight`` / ``bias`` are mu_W / mu_bias, ``noise`` = (sigma_W, sigma_bias, eps_p, eps_q)
+    noise: tuple[nn.Parameter, nn.Parameter, nn.Parameter, nn.Parameter] | None = None
 
 
 def layer_params(layers: list[_Layer]) -> list[nn.Parameter]:
     """Every weight and bias of ``layers``, in layer order: the flat order of a ``FlatGroup`` over the chain.  The members of an
     ``nn.Linear`` ensemble layer come weights first, then biases, so member e sits ``e * in * out`` (``e * out``) floats after
-    member 0: the uniform member stride of the batched GEMM."""
+    member 0: the uniform member stride of the batched GEMM.  A noisy layer's are mu_W, sigma_W, mu_bias, sigma_bias (the
+    module's order); its noise ``eps_p`` / ``eps_q`` is not trained and lives apart (``noise_params``)."""
     out: list[nn.Parameter] = []
     for L in layers:
         if L.members is not None:
             out += [w for w, _ in L.members] + [b for _, b in L.members]
+        elif L.noise is not None:
+            out += [L.weight, L.noise[0], L.bias, L.noise[1]]
         elif L.weight is not None:
             out += [L.weight, L.bias]
     return out
+
+
+def noise_params(layers: list[_Layer]) -> list[nn.Parameter]:
+    """``eps_p``, ``eps_q`` of every noisy layer of ``layers``, in layer order: the flat order of the noise buffer a
+    ``FusedStack`` reads them from."""
+    return [e for L in layers if L.noise is not None for e in L.noise[2:]]
 
 
 def _activation_code(m: nn.Module) -> int:
@@ -82,16 +95,26 @@ def _flat_chain(mods: list[nn.Module]) -> list[nn.Module]:
     return out
 
 
-def compile_sequential(mods: list[nn.Module], input_shape: tuple[int, ...], ensemble: bool = False) -> list[_Layer]:
+def compile_sequential(mods: list[nn.Module], input_shape: tuple[int, ...], ensemble: bool = False,
+                       noisy: bool = False) -> list[_Layer]:
     """Linear / Conv2d / ReLU / Flatten chain -> layer list.  ``input_shape`` = (features,) or (C, H, W).  Nested
     ``nn.Sequential`` containers are read as the flat chain they run.  With ``ensemble`` a chain of ``EnsembleLinear`` layers
     (with ReLU / Tanh between them) is an ensemble chain: every layer has the same member count and a bias, and no other layer
-    kind joins it."""
+    kind joins it.  With ``noisy`` a ``NoisyLinear`` is a Linear layer with noise (Rainbow); without it one is refused."""
     from ..utils.net.common import EnsembleLinear
+    from ..utils.net.discrete import NoisyLinear
     layers: list[_Layer] = []
     shape = tuple(int(x) for x in input_shape)
     for m in _flat_chain(mods):
-        if ensemble and isinstance(m, EnsembleLinear):
+        if isinstance(m, NoisyLinear):
+            if not noisy:
+                raise UnsupportedModelError("NoisyLinear layers are run on the device by RainbowDQN only")
+            if len(shape) != 1 or shape[0] != m.in_features:
+                raise UnsupportedModelError(f"NoisyLinear({m.in_features}) after shape {shape}")
+            layers.append(_Layer("linear", m.mu_W, m.mu_bias, ACT_NONE, m.in_features, m.out_features,
+                                 noise=(m.sigma_W, m.sigma_bias, m.eps_p, m.eps_q)))
+            shape = (m.out_features,)
+        elif ensemble and isinstance(m, EnsembleLinear):
             E, d_in, d_out = (int(x) for x in m.weight.shape)
             if len(shape) != 1 or shape[0] != d_in:
                 raise UnsupportedModelError(f"EnsembleLinear({d_in}) after shape {shape}")
@@ -184,10 +207,14 @@ def _out_shape(layers: list[_Layer], shape: tuple[int, ...]) -> tuple[int, ...]:
 class FusedStack:
     """Forward / backward of a layer list on ``[rows, features]`` fp32 matrices (NHWC between conv layers)."""
 
-    def __init__(self, layers: list[_Layer], group: FlatGroup, name: str = "net") -> None:
+    def __init__(self, layers: list[_Layer], group: FlatGroup, name: str = "net", noise: FlatGroup | None = None) -> None:
+        """``noise``: the flat buffer of ``noise_params(layers)``, required when a layer is noisy."""
         self.layers = layers
         self.group = group
+        self.noise = noise
         self.name = name
+        if noise is None and any(L.noise is not None for L in layers):
+            raise UnsupportedModelError(f"{name}: a chain with noisy layers needs the flat buffer of their noise")
         self.device = group.device
         self._bufs: dict[tuple, torch.Tensor] = {}
         self._ws_sizes: dict[tuple[int, int, int], int] = {}
@@ -236,22 +263,39 @@ class FusedStack:
         base = (flat if flat is not None else g.flat).data_ptr()
         return base + 4 * g.offset(L.bias)
 
+    def _noisy_wb(self, i: int, L: _Layer, tag: str, params: torch.Tensor | None, noise: torch.Tensor | None) -> tuple[int, int]:
+        """The train-mode weight and bias of noisy layer i, formed into the scratch of ``tag`` from ``params`` and ``noise`` (the
+        online buffers when None); the backward of the same tag reads the weight back."""
+        g, ng = self.group, self.noise
+        base = (params if params is not None else g.flat).data_ptr()
+        nbase = (noise if noise is not None else ng.flat).data_ptr()
+        w = self._buf((tag, "weff", i), L.out_dim * L.in_dim)
+        b = self._buf((tag, "beff", i), L.out_dim)
+        sw, sb, ep, eq = L.noise
+        call("ts_noisy_weight", base + 4 * g.offset(L.weight), base + 4 * g.offset(sw), base + 4 * g.offset(L.bias),
+             base + 4 * g.offset(sb), nbase + 4 * ng.offset(ep), nbase + 4 * ng.offset(eq), L.out_dim, L.in_dim, ptr(w), ptr(b),
+             stream_ptr(self.device))
+        return ptr(w), ptr(b)
+
     # ------------------------------------------------------------------ forward
     def forward(self, x: torch.Tensor | None, rows: int, tag: str = "a", *, frames: tuple | None = None,
-                params: torch.Tensor | None = None) -> list[torch.Tensor]:
+                params: torch.Tensor | None = None, noise: torch.Tensor | None = None) -> list[torch.Tensor]:
         """Returns the activation list ``[x0, y1, ..., yL]`` (``y_i`` = post-activation output of layer i; for conv layers
         rows * Ho * Wo NHWC rows).  ``frames`` = (uint8 frames, stack_idx int64 [rows, C], denom) feeds the first conv layer
         straight from single-frame storage (frame-stack gather + im2col in one kernel).  ``params``: evaluate with another
-        flat parameter buffer of the same layout (the lagged / target copy)."""
+        flat parameter buffer of the same layout (the lagged / target copy); ``noise``: the noise buffer that goes with it."""
         self.group.ensure_adopted()
+        if self.noise is not None:
+            self.noise.ensure_adopted()
         st = stream_ptr(self.device)
         acts: list[torch.Tensor] = [x]
         cur = x
         for i, L in enumerate(self.layers):
             if L.kind == "linear":
                 y = self._buf((tag, "y", i), rows * L.out_dim)[: rows * L.out_dim].view(rows, L.out_dim)
-                self._gemm(ptr(cur), L.in_dim, 0, self._w(L, params), L.in_dim, 0, ptr(y), L.out_dim, rows, L.out_dim, L.in_dim,
-                           bias=self._b(L, params), act=L.act)
+                w, b = (self._noisy_wb(i, L, tag, params, noise) if L.noise is not None
+                        else (self._w(L, params), self._b(L, params)))
+                self._gemm(ptr(cur), L.in_dim, 0, w, L.in_dim, 0, ptr(y), L.out_dim, rows, L.out_dim, L.in_dim, bias=b, act=L.act)
             elif L.kind == "ensemble":      # [E, rows, out]; the first layer reads the shared [rows, in] input
                 n_out = L.E * rows * L.out_dim
                 y = self._buf((tag, "y", i), n_out)[:n_out].view(L.E, rows, L.out_dim)
@@ -287,8 +331,9 @@ class FusedStack:
         out: list[torch.Tensor] = []
         cur = x_dot
         for i, L in enumerate(self.layers):
-            if L.kind != "linear":
-                raise UnsupportedModelError(f"tangent passes support Linear layers only, not {L.kind} layers")
+            if L.kind != "linear" or L.noise is not None:
+                raise UnsupportedModelError(f"tangent passes support Linear layers only, not {L.kind if L.noise is None else 'noisy'} "
+                                            "layers")
             yd = self._buf((tag, "t", i), rows * L.out_dim)[: rows * L.out_dim].view(rows, L.out_dim)
             mask = ptr(acts[i + 1]) if L.act != ACT_NONE else None
             kind = L.act if L.act != ACT_NONE else ACT_RELU
@@ -329,8 +374,17 @@ class FusedStack:
                 if param_grads:
                     gw = g.grad.data_ptr() + 4 * g.offset(L.weight)
                     gb = g.grad.data_ptr() + 4 * g.offset(L.bias)
+                    if L.noise is not None:     # the gradient at the effective weight and bias, then split over the four tensors
+                        gw = ptr(self._buf((tag, "dweff", i), L.out_dim * L.in_dim))
+                        gb = ptr(self._buf((tag, "dbeff", i), L.out_dim))
                     self._gemm(ptr(dz), L.out_dim, 1, ptr(x_in), L.in_dim, 1, gw, L.in_dim, L.out_dim, L.in_dim, M_rows)
                     call("ts_net_colsum", ptr(dz), L.out_dim, M_rows, L.out_dim, gb, 0, st)
+                    if L.noise is not None:
+                        sw, sb, ep, eq = L.noise
+                        ng, gg = self.noise, g.grad.data_ptr()
+                        call("ts_noisy_grad", gw, gb, ptr(ng.flat) + 4 * ng.offset(ep), ptr(ng.flat) + 4 * ng.offset(eq), L.out_dim,
+                             L.in_dim, gg + 4 * g.offset(L.weight), gg + 4 * g.offset(sw), gg + 4 * g.offset(L.bias),
+                             gg + 4 * g.offset(sb), st)
                 if need_dx:
                     lo, hi = (0, L.in_dim) if (i > 0 or input_cols is None) else input_cols
                     width = hi - lo
@@ -339,7 +393,8 @@ class FusedStack:
                     else:
                         dx = self._buf((tag, "dx", i), M_rows * width)[: M_rows * width].view(M_rows, width)
                     mask = ptr(act_src) + 4 * lo if prev_act != ACT_NONE else None
-                    self._gemm(ptr(dz), L.out_dim, 0, self._w(L) + 4 * lo, L.in_dim, 1, ptr(dx), width, M_rows, width, L.out_dim,
+                    w = ptr(self._bufs[(tag, "weff", i)]) if L.noise is not None else self._w(L)
+                    self._gemm(ptr(dz), L.out_dim, 0, w + 4 * lo, L.in_dim, 1, ptr(dx), width, M_rows, width, L.out_dim,
                                mask=mask, ld_mask=L.in_dim, mask_kind=prev_act if prev_act != ACT_NONE else ACT_RELU,
                                accumulate=(i == 0 and dx_accumulate))
                     dz = dx
@@ -407,8 +462,25 @@ class FusedStack:
         return self.layers[j].act if j >= 0 else ACT_NONE
 
 
+def network_heads(mod: Any) -> tuple[list[nn.Module], list[nn.Module], list[nn.Module] | None] | None:
+    """(trunk, Q head, V head or None) module lists of a network with separate heads -- ``Net(dueling_param=...)`` (trunk
+    ``.model``, heads ``.Q`` / ``.V``) or ``RainbowNet`` (trunk ``.net``, ``.Q``, and ``.V`` when dueling) -- in module
+    registration order; None for any other network."""
+    if getattr(mod, "use_dueling", False):
+        return module_layers(mod.model), module_layers(mod.Q), module_layers(mod.V)
+    q = getattr(mod, "Q", None)
+    if isinstance(q, nn.Sequential) and isinstance(getattr(mod, "net", None), nn.Sequential):
+        v = getattr(mod, "V", None) if getattr(mod, "_is_dueling", False) else None
+        return list(mod.net), list(q), (list(v) if v is not None else None)
+    return None
+
+
 def module_layers(mod: Any) -> list[nn.Module]:
-    """Flat module list of the reference-shaped containers: MLP / Net (``.model`` chains) or a plain Sequential."""
+    """Flat module list of the reference-shaped containers: MLP / Net (``.model`` chains) or a plain Sequential.  A network with
+    separate Q / V heads (``network_heads``) is refused: a chain read from its trunk would drop the heads."""
+    if network_heads(mod) is not None:
+        raise UnsupportedModelError(f"{type(mod).__name__} has separate Q / V heads (a dueling Net or a RainbowNet): RainbowDQN "
+                                    "is the only algorithm that runs such a network on the device")
     if isinstance(mod, nn.Sequential):
         return list(mod)
     inner = getattr(mod, "model", None)

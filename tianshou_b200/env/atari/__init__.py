@@ -1,3 +1,3 @@
-from .atari_network import C51Net, DQNet, QRDQNet, ScaledObsInputActionReprNet, scale_obs
+from .atari_network import C51Net, DQNet, QRDQNet, RainbowNet, ScaledObsInputActionReprNet, scale_obs
 
-__all__ = ["C51Net", "DQNet", "QRDQNet", "ScaledObsInputActionReprNet", "scale_obs"]
+__all__ = ["C51Net", "DQNet", "QRDQNet", "RainbowNet", "ScaledObsInputActionReprNet", "scale_obs"]

@@ -1,4 +1,4 @@
-"""NatureCNN Q-networks (API of tianshou/env/atari/atari_network.py:26-122, :211-235).
+"""NatureCNN Q-networks (API of tianshou/env/atari/atari_network.py:26-235).
 
 Ordinary ``nn.Module``s: the Collector runs them for action selection; ``DQN.update`` reads the same parameter
 storage through a flat view and runs the conv stack as implicit GEMM on the tensor cores (algorithm/netgraph.py).
@@ -13,6 +13,7 @@ import torch
 from torch import nn
 
 from ...utils.net.common import ModuleWithVectorOutput
+from ...utils.net.discrete import NoisyLinear
 from ...utils.torch_utils import torch_device
 
 
@@ -98,3 +99,38 @@ class C51Net(DQNet):
         obs, state = super().forward(obs)
         obs = obs.view(-1, self.num_atoms).softmax(dim=-1)
         return obs.view(-1, self.action_num, self.num_atoms), state
+
+
+class RainbowNet(DQNet):
+    """Rainbow: Combining Improvements in Deep Reinforcement Learning (atari_network.py:154-208): the ``DQNet`` convolutions
+    (``features_only``), then a Q head ``Linear(features, 512), ReLU, Linear(512, actions * num_atoms)`` and, when
+    ``is_dueling``, a V head ``Linear(features, 512), ReLU, Linear(512, num_atoms)``; the Linear layers are ``NoisyLinear(.,
+    ., noisy_std)`` when ``is_noisy``.  ``forward`` returns ``softmax(q - q.mean(1) + v)`` (or ``softmax(q)``) over each action's
+    atoms, ``[B, actions, num_atoms]``."""
+
+    def __init__(self, *, c: int, h: int, w: int, action_shape: Sequence[int] | int, num_atoms: int = 51,
+                 noisy_std: float = 0.5, is_dueling: bool = True, is_noisy: bool = True) -> None:
+        super().__init__(c=c, h=h, w=w, action_shape=action_shape, features_only=True)
+        self.action_num = int(np.prod(action_shape))
+        self.num_atoms = num_atoms
+
+        def linear(x: int, y: int) -> NoisyLinear | nn.Linear:
+            if is_noisy:
+                return NoisyLinear(x, y, noisy_std)
+            return nn.Linear(x, y)
+
+        self.Q = nn.Sequential(linear(self.output_dim, 512), nn.ReLU(inplace=True), linear(512, self.action_num * self.num_atoms))
+        self._is_dueling = is_dueling
+        if self._is_dueling:
+            self.V = nn.Sequential(linear(self.output_dim, 512), nn.ReLU(inplace=True), linear(512, self.num_atoms))
+        self.output_dim = self.action_num * self.num_atoms
+
+    def forward(self, obs: Any, state: Any = None, info: dict | None = None) -> tuple[torch.Tensor, Any]:
+        obs, state = super().forward(obs)
+        q = self.Q(obs).view(-1, self.action_num, self.num_atoms)
+        if self._is_dueling:
+            v = self.V(obs).view(-1, 1, self.num_atoms)
+            logits = q - q.mean(dim=1, keepdim=True) + v
+        else:
+            logits = q
+        return logits.softmax(dim=2), state

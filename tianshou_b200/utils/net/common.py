@@ -90,27 +90,54 @@ class MLP(ModuleWithVectorOutput):
 class Net(ModuleWithVectorOutput):
     """obs -> MLP features (``(logits, state)`` tuple like the reference, common.py:223-369).
     ``num_atoms > 1`` widens the last layer to ``prod(action_shape) * num_atoms`` outputs and returns them as
-    ``[B, actions, num_atoms]`` (the distributional heads of QR-DQN, common.py:298-369); the dueling head is not provided."""
+    ``[B, actions, num_atoms]`` (the distributional heads of QR-DQN, common.py:298-369).  ``dueling_param = (q_kwargs, v_kwargs)``
+    ends the MLP trunk at its last hidden layer and puts two MLPs on it, built from those keyword dicts: ``Q`` with
+    ``prod(action_shape) * num_atoms`` outputs and ``V`` with ``num_atoms``; the output is ``q - q.mean(1) + v`` over
+    ``[B, actions, num_atoms]`` (``[B, actions]`` when ``num_atoms == 1``).  Only RainbowDQN runs a network with these heads on
+    the device."""
 
     def __init__(self, *, state_shape: int | Sequence[int], action_shape: Any = 0,
                  hidden_sizes: Sequence[int] = (), norm_layer: Any = None, norm_args: Any = None,
                  activation: Any = nn.ReLU, act_args: Any = None, softmax: bool = False,
-                 concat: bool = False, num_atoms: int = 1, linear_layer: TLinearLayer = nn.Linear) -> None:
+                 concat: bool = False, num_atoms: int = 1,
+                 dueling_param: tuple[dict[str, Any], dict[str, Any]] | None = None,
+                 linear_layer: TLinearLayer = nn.Linear) -> None:
         input_dim = int(np.prod(state_shape))
         action_dim = int(np.prod(action_shape)) * num_atoms
         if concat:
             input_dim += action_dim
-        model = MLP(input_dim=input_dim, output_dim=action_dim if not concat else 0,
+        use_dueling = dueling_param is not None
+        model = MLP(input_dim=input_dim, output_dim=action_dim if not use_dueling and not concat else 0,
                     hidden_sizes=hidden_sizes, norm_layer=norm_layer, norm_args=norm_args,
                     activation=activation, act_args=act_args, linear_layer=linear_layer)
-        super().__init__(model.output_dim)
+        Q: MLP | None = None
+        V: MLP | None = None
+        if use_dueling:
+            q_kwargs = {**dueling_param[0], "input_dim": model.output_dim}
+            v_kwargs = {**dueling_param[1], "input_dim": model.output_dim}
+            q_kwargs["output_dim"] = 0 if concat else action_dim
+            v_kwargs["output_dim"] = 0 if concat else num_atoms
+            Q, V = MLP(**q_kwargs), MLP(**v_kwargs)
+            output_dim = Q.output_dim
+        else:
+            output_dim = model.output_dim
+        super().__init__(output_dim)
+        self.use_dueling = use_dueling
         self.softmax = softmax
         self.num_atoms = num_atoms
         self.model = model
+        self.Q = Q
+        self.V = V
 
     def forward(self, obs: Any, state: Any = None, info: dict | None = None) -> tuple[torch.Tensor, Any]:
         logits = self.model(obs)
-        if self.num_atoms > 1:
+        if self.use_dueling:
+            q, v = self.Q(logits), self.V(logits)
+            if self.num_atoms > 1:
+                q = q.view(logits.shape[0], -1, self.num_atoms)
+                v = v.view(logits.shape[0], -1, self.num_atoms)
+            logits = q - q.mean(dim=1, keepdim=True) + v
+        elif self.num_atoms > 1:
             logits = logits.view(logits.shape[0], -1, self.num_atoms)
         if self.softmax:
             logits = torch.softmax(logits, dim=-1)

@@ -1,5 +1,5 @@
-"""Discrete-action actor / critic heads, IQN's quantile network and FQF's fraction proposal and full quantile function (API of
-tianshou/utils/net/discrete.py:22-314)."""
+"""Discrete-action actor / critic heads, IQN's quantile network, FQF's fraction proposal and full quantile function and Rainbow's
+noisy layer (API of tianshou/utils/net/discrete.py:22-364)."""
 from __future__ import annotations
 
 from collections.abc import Sequence
@@ -147,3 +147,51 @@ class FullQuantileFunction(ImplicitQuantileNetwork):
             with torch.no_grad():
                 quantiles_tau = self._compute_quantiles(feat, taus[:, 1:-1])
         return (quantiles, fractions, quantiles_tau), hidden
+
+
+class NoisyLinear(nn.Module):
+    """Noisy network layer with factorised Gaussian noise (arXiv:1706.10295, discrete.py:317-364).  In training mode ``forward``
+    uses ``mu_W + sigma_W * ger(eps_q, eps_p)`` and ``mu_bias + sigma_bias * eps_q``, in eval mode ``mu_W`` and ``mu_bias``.
+    ``eps_p [in]`` and ``eps_q [out]`` are parameters with ``requires_grad=False``, so they are in ``state_dict()`` and in an
+    optimiser built from ``parameters()``; ``sample()`` redraws them in place as sign(x) sqrt|x| of ``torch.randn``, ``in``
+    values then ``out``, on the module's device.  Initialised as the reference: mu uniform in +-1/sqrt(in), sigma
+    ``noisy_std / sqrt(in)``, then one ``sample()``."""
+
+    def __init__(self, in_features: int, out_features: int, noisy_std: float = 0.5) -> None:
+        super().__init__()
+        self.mu_W = nn.Parameter(torch.FloatTensor(out_features, in_features))
+        self.sigma_W = nn.Parameter(torch.FloatTensor(out_features, in_features))
+        self.mu_bias = nn.Parameter(torch.FloatTensor(out_features))
+        self.sigma_bias = nn.Parameter(torch.FloatTensor(out_features))
+        self.eps_p = nn.Parameter(torch.FloatTensor(in_features), requires_grad=False)
+        self.eps_q = nn.Parameter(torch.FloatTensor(out_features), requires_grad=False)
+        self.in_features = in_features
+        self.out_features = out_features
+        self.sigma = noisy_std
+        self.reset()
+        self.sample()
+
+    def reset(self) -> None:
+        bound = 1 / np.sqrt(self.in_features)
+        self.mu_W.data.uniform_(-bound, bound)
+        self.mu_bias.data.uniform_(-bound, bound)
+        self.sigma_W.data.fill_(self.sigma / np.sqrt(self.in_features))
+        self.sigma_bias.data.fill_(self.sigma / np.sqrt(self.in_features))
+
+    def f(self, x: torch.Tensor) -> torch.Tensor:
+        x = torch.randn(x.size(0), device=x.device)
+        return x.sign().mul_(x.abs().sqrt_())
+
+    def sample(self) -> None:
+        """Redraw ``eps_p`` then ``eps_q`` in place (the device updates read these very tensors)."""
+        self.eps_p.copy_(self.f(self.eps_p))
+        self.eps_q.copy_(self.f(self.eps_q))
+
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        if self.training:
+            weight = self.mu_W + self.sigma_W * (self.eps_q.ger(self.eps_p))
+            bias = self.mu_bias + self.sigma_bias * self.eps_q.clone()
+        else:
+            weight = self.mu_W
+            bias = self.mu_bias
+        return F.linear(x, weight, bias)
