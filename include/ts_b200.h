@@ -856,6 +856,20 @@ int ts_dueling_atoms(const float* q, const float* v, int64_t B, int32_t A, int32
  * two calls on the same input are bit-identical.  Any B >= 0, A, N >= 1. */
 int ts_dueling_atoms_bwd(const float* dlogits, int64_t B, int32_t A, int32_t N, float* dq, float* dv, ts_stream_t stream);
 
+/* ---- DRQN (lstm.cu) ---- */
+/* One time step of the LSTM of utils/net/common.py Recurrent (torch.nn.LSTM, gate chunks i, f, g, o).  pre [B][4H] holds
+ * x W_ih^T + b_ih + h_{t-1} W_hh^T (ts_net_gemm launches); the kernel adds b_hh [4H].  c_prev [B][H] is nullable (zero: t = 0).
+ * gates [B][4H] = sigmoid / sigmoid / tanh / sigmoid of the pre-activations (saved for the backward), c [B][H] = f c_prev + i g,
+ * h [B][H] = o tanh(c), with full-accuracy expf / tanhf and no atomics.  Any B, H >= 1; rows past B are not touched. */
+int ts_lstm_cell(const float* pre, const float* b_hh, const float* c_prev, int64_t B, int32_t H, float* gates, float* c, float* h,
+                 ts_stream_t stream);
+/* Its backward from the saved gates, c [B][H] (= c_t), c_prev (nullable: zero), the incoming dh [B][H] and the carried dc [B][H]
+ * (nullable: zero, the last step): dgates [B][4H], the gradient at the four pre-activations, and dc_prev [B][H] = dc_t f
+ * (nullable: not written).  dc and dc_prev may be the same array.  No atomics: two calls on the same input are bit-identical.
+ * Any B, H >= 1. */
+int ts_lstm_cell_bwd(const float* gates, const float* c, const float* c_prev, const float* dh, const float* dc, int64_t B, int32_t H,
+                     float* dgates, float* dc_prev, ts_stream_t stream);
+
 /* ---- IQN (iqn.cu) ---- */
 /* The network of IQN (utils/net/discrete.py:163-216) is a trunk on B rows (feat [B][D]), the cosine embedding of S fractions per
  * row and a head on the B * S rows h[b * S + s] = feat[b] * e[b * S + s], sample-major, so the head's output is q [B][S][A].  The

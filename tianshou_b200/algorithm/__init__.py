@@ -7,6 +7,7 @@ from .modelfree.a2c import A2CTrainingStats, ActorCriticOnPolicyAlgorithm
 from .modelfree.bdqn import BDQN, BDQNPolicy
 from .modelfree.c51 import C51, C51Policy
 from .modelfree.discrete_sac import DiscreteSAC
+from .modelfree.dqn import DQN
 from .modelfree.fqf import FQF, FQFPolicy, FQFTrainingStats
 from .modelfree.iqn import IQN, IQNPolicy
 from .modelfree.npg import NPG, NPGTrainingStats
@@ -27,5 +28,5 @@ __all__ = [
     "RMSpropOptimizerFactory", "DiscreteBCQ", "DiscreteBCQPolicy", "DiscreteBCQTrainingStats", "DiscreteCRR",
     "DiscreteCRRTrainingStats", "QRDQN", "QRDQNPolicy", "DiscreteCQL", "DiscreteCQLTrainingStats", "IQN", "IQNPolicy",
     "FQF", "FQFPolicy", "FQFTrainingStats", "REDQ", "REDQPolicy", "REDQTrainingStats", "BDQN", "BDQNPolicy", "C51", "C51Policy",
-    "RainbowDQN", "RainbowTrainingStats",
+    "RainbowDQN", "RainbowTrainingStats", "DQN",
 ]

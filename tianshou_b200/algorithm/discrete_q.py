@@ -155,15 +155,16 @@ class DiscreteQCore(Algorithm):
     observations, draws the batch (refusing actions outside ``[0, n_actions)``), computes the n-step return and refreshes
     the lagged copy on its tick."""
 
-    def _init_discrete(self, dev: torch.device, in_shape: tuple[int, ...], in_scale: float, n_actions: int) -> None:
-        self._dev, self._in_shape, self._in_scale, self.n_actions = dev, in_shape, in_scale, n_actions
+    def _init_discrete(self, dev: torch.device, in_shape: tuple[int, ...], in_scale: float, n_actions: int, seq: bool = False) -> None:
+        """``seq``: the network reads each sample's stacked observations as a sequence (a ``Recurrent`` network)."""
+        self._dev, self._in_shape, self._in_scale, self.n_actions, self._seq = dev, in_shape, in_scale, n_actions, seq
         self._iter = 0
         self._scratch = DeviceScratch(dev)
         self._buf = self._scratch.tensor
 
     def _obs_source(self, buffer: ReplayBuffer, indices: np.ndarray | torch.Tensor, key: str = "obs") -> DeviceObsSource:
         """How the network reads ``buffer[indices].<key>`` without materialising it on the host (obs_source.py)."""
-        return device_obs_source(buffer, indices, key, self._in_shape, self._in_scale, self._dev, self._buf)
+        return device_obs_source(buffer, indices, key, self._in_shape, self._in_scale, self._dev, self._buf, seq=self._seq)
 
     def _sample(self, buffer: ReplayBuffer, sample_size: int | None) -> tuple[Batch, Any]:
         return sample_discrete(buffer, sample_size, self._obs_source, self._dev, self.n_actions)

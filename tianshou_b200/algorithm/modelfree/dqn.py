@@ -1,5 +1,6 @@
 """Deep Q-Network (double DQN, n-step, prioritised replay) with ``update()`` on the device
-(SURVEY 8(f) ranks 2-3, BASELINE configs[2]).
+(SURVEY 8(f) ranks 2-3, BASELINE configs[2]).  With a ``Recurrent`` model it is DRQN (test/discrete/test_drqn.py): the sampled
+observations are the buffer's ``stack_num`` steps as a sequence, run through ``RecurrentStack`` (algorithm/recurrent.py).
 
 Reference: tianshou/algorithm/modelfree/dqn.py (DiscreteQLearningPolicy :36-164, QLearningOffPolicyAlgorithm
 :170-283, DQN :286-404), env/atari/atari_network.py:60-122 (DQNet), data/buffer/buffer_base.py:557-603 (frame
@@ -25,12 +26,14 @@ from torch import nn
 
 from ..._cabi import call, ptr, stream_ptr
 from ...data import Batch, ReplayBuffer, to_numpy
+from ...utils.net.common import Recurrent
 from ..base import OffPolicyAlgorithm, Policy, TrainingStats
 from ..discrete_q import DiscreteQCore, describe_q_network, lagged_group
 from ..flat_params import FlatGroup, UnsupportedModelError, bind_optimizer
 from ..netgraph import ACT_NONE, FusedStack, compile_sequential, layer_params, module_layers
 from ..obs_source import DeviceObsSource
 from ..optim import OptimizerFactory
+from ..recurrent import RecurrentStack
 from ..twin_critic import _EvalModeModule, cuda_device_of, pop_batch_weight
 
 
@@ -104,13 +107,18 @@ class DQN(DiscreteQCore, OffPolicyAlgorithm):
         self.is_double = is_double
         self.huber_loss_delta = huber_loss_delta
         dev = cuda_device_of(policy.model)
-        inner, in_shape, in_scale = describe_q_network(policy.model)
-        layers = compile_sequential(module_layers(inner), in_shape)
-        if layers[-1].kind != "linear" or layers[-1].act != ACT_NONE:
-            raise UnsupportedModelError("Q-network must end in a linear layer over the actions")
-        self._init_discrete(dev, in_shape, in_scale, layers[-1].out_dim)
-        self._group = FlatGroup(layer_params(layers), dev)
-        self._net = FusedStack(layers, self._group, "q")
+        if isinstance(policy.model, Recurrent):        # DRQN: sequences from the buffer's stack, zero initial state
+            self._net = RecurrentStack(policy.model, dev)
+            self._group = self._net.group
+            self._init_discrete(dev, (self._net.D,), 1.0, self._net.A, seq=True)
+        else:
+            inner, in_shape, in_scale = describe_q_network(policy.model)
+            layers = compile_sequential(module_layers(inner), in_shape)
+            if layers[-1].kind != "linear" or layers[-1].act != ACT_NONE:
+                raise UnsupportedModelError("Q-network must end in a linear layer over the actions")
+            self._init_discrete(dev, in_shape, in_scale, layers[-1].out_dim)
+            self._group = FlatGroup(layer_params(layers), dev)
+            self._net = FusedStack(layers, self._group, "q")
         self.optim = self._create_optimizer(policy, optim)
         bind_optimizer(self.optim, self._group)
         self.model_old: _EvalModeModule | None = None

@@ -477,7 +477,11 @@ def network_heads(mod: Any) -> tuple[list[nn.Module], list[nn.Module], list[nn.M
 
 def module_layers(mod: Any) -> list[nn.Module]:
     """Flat module list of the reference-shaped containers: MLP / Net (``.model`` chains) or a plain Sequential.  A network with
-    separate Q / V heads (``network_heads``) is refused: a chain read from its trunk would drop the heads."""
+    separate Q / V heads (``network_heads``) is refused: a chain read from its trunk would drop the heads, and so is a
+    ``Recurrent`` network, which is no chain (its LSTM runs on the device in ``RecurrentStack``, for DQN only)."""
+    from ..utils.net.common import Recurrent
+    if isinstance(mod, Recurrent):
+        raise UnsupportedModelError("a Recurrent (LSTM) network is run on the device by DQN only")
     if network_heads(mod) is not None:
         raise UnsupportedModelError(f"{type(mod).__name__} has separate Q / V heads (a dueling Net or a RainbowNet): RainbowDQN "
                                     "is the only algorithm that runs such a network on the device")

@@ -144,6 +144,38 @@ class Net(ModuleWithVectorOutput):
         return logits, state
 
 
+class Recurrent(ModuleWithVectorOutput):
+    """LSTM Q-network of DRQN (common.py:372-453): ``fc1`` (no activation) -> ``nn.LSTM(layer_num, batch_first)`` -> ``fc2`` on the
+    last step.  ``obs`` is ``[B, len, D]`` (a stacked sample) or ``[B, D]`` (one step, read as a length-1 sequence); ``state`` is
+    None or ``{hidden, cell}`` as ``[B, layer_num, H]``.  Returns ``(logits, {hidden, cell})``.  ``DQN.update`` runs this network on
+    the device (algorithm/recurrent.py); this torch forward is the Collector's path."""
+
+    def __init__(self, *, layer_num: int, state_shape: int | Sequence[int], action_shape: Any,
+                 hidden_layer_size: int = 128) -> None:
+        output_dim = int(np.prod(action_shape))
+        super().__init__(output_dim)
+        self.nn = nn.LSTM(input_size=hidden_layer_size, hidden_size=hidden_layer_size, num_layers=layer_num, batch_first=True)
+        self.fc1 = nn.Linear(int(np.prod(state_shape)), hidden_layer_size)
+        self.fc2 = nn.Linear(hidden_layer_size, output_dim)
+
+    def forward(self, obs: Any, state: Any = None, info: dict | None = None) -> tuple[torch.Tensor, Any]:
+        from ...data import Batch
+        if state is not None and not {"hidden", "cell"}.issubset(state.keys()):
+            raise ValueError(f"Expected to find keys 'hidden' and 'cell' but instead found {state.keys()}")
+        obs = torch.as_tensor(obs, device=torch_device(self), dtype=torch.float32)
+        if len(obs.shape) == 2:
+            obs = obs.unsqueeze(-2)
+        obs = self.fc1(obs)
+        self.nn.flatten_parameters()
+        if state is None:
+            obs, (hidden, cell) = self.nn(obs)
+        else:
+            obs, (hidden, cell) = self.nn(obs, (state["hidden"].transpose(0, 1).contiguous(),
+                                                state["cell"].transpose(0, 1).contiguous()))
+        obs = self.fc2(obs[:, -1])
+        return obs, Batch({"hidden": hidden.transpose(0, 1).detach(), "cell": cell.transpose(0, 1).detach()})
+
+
 class EnsembleLinear(nn.Module):
     """``ensemble_size`` Linear layers applied side by side (common.py:518-550): ``x @ weight + bias_weights`` with
     ``weight [E, in, out]`` and ``bias_weights [E, 1, out]``, so a ``[B, in]`` input gives ``[E, B, out]`` and an
