@@ -931,6 +931,24 @@ int ts_fqf_fraction_rows(const float* q_hat, const float* q_tau, const int64_t* 
                          const float* logp, const float* H, int64_t B, int32_t A, int32_t N, float ent_coef, float* dz, float* rows,
                          float* losses, ts_stream_t stream);
 
+/* ---- imitation learning (imitation.cu) ---- */
+/* The regression loss of imitation_base.py:115-118 on a ContinuousActorDeterministic (utils/net/continuous.py: max_action *
+ * tanh(last(...))): with z [B][A] the last Linear's output and act [B][A] the buffer's actions (any values, also outside
+ * +-max_action), loss[0] = F.mse_loss(max_action * tanh(z), act), the mean over B * A elements, and dz [B][A] = 2 (pi - act) / (B A)
+ * * max_action * (1 - tanh(z)^2) in torch's operation order.  dz grid-stride, then one block summing in a fixed order, no
+ * atomics: two calls on the same input are bit-identical.  Any B, A >= 1. */
+int ts_imitation_mse_rows(const float* z, const float* act, int64_t B, int32_t A, float max_action, float* dz, float* loss,
+                          ts_stream_t stream);
+/* The classification loss of imitation_base.py:119-122, F.nll_loss(F.log_softmax(y), act), the mean over B.  out [B][A] is the
+ * last Linear's output z.  softmax_output = 0: y = z, dz = (softmax(z) - onehot(act)) / B.  softmax_output = 1 (DiscreteActor's
+ * default, utils/net/discrete.py:87): y = softmax(z), log_softmax is taken of those probabilities as the reference codes it, and
+ * dz = p (g - sum_k p_k g_k) with p = softmax(z), g = (softmax(p) - onehot(act)) / B.  rows [B] receives each row's loss.  One
+ * warp per row (lanes stride A, any A), max-shifted log-sum-exps with full-accuracy expf / logf, then one block summing the rows
+ * in a fixed order, no atomics: two calls on the same input are bit-identical.  act must lie in [0, A): the caller checks it.
+ * Any B, A >= 1. */
+int ts_imitation_nll_rows(const float* out, const int64_t* act, int64_t B, int32_t A, int32_t softmax_output, float* dz, float* rows,
+                          float* loss, ts_stream_t stream);
+
 #ifdef TS_B200_DIAGNOSTICS
 /* Diagnostics build only (libts_b200_diag.so, `python -m tianshou_b200.csrc.build --diag`): not part of the product library. */
 /* Hardware self-test of the wgmma building blocks (csrc/wgmma.cuh), one CTA:

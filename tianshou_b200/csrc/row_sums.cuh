@@ -42,6 +42,22 @@ static __global__ void __launch_bounds__(kRowSumThreads) row_sums3_kernel(const 
     }
 }
 
+// The same fixed order for one series computed on the fly, inside a one-block kernel of kRowSumThreads threads: thread t sums
+// term(i) for i = t, t + 1024, ... < n in order, then a shared-memory tree.  Every thread returns the total.
+template <class Term>
+__device__ __forceinline__ float block_sum_fixed(int64_t n, Term term) {
+    __shared__ float s[kRowSumThreads];
+    float a = 0.0f;
+    for (int64_t i = threadIdx.x; i < n; i += kRowSumThreads) a += term(i);
+    s[threadIdx.x] = a;
+    __syncthreads();
+    for (int off = kRowSumThreads / 2; off > 0; off >>= 1) {
+        if ((int)threadIdx.x < off) s[threadIdx.x] += s[threadIdx.x + off];
+        __syncthreads();
+    }
+    return s[0];
+}
+
 // one warp per row, warps stride over the rows: the grid of the per-row kernels
 constexpr int kRowThreads = 256;
 constexpr int kRowsPerBlock = kRowThreads / 32;
