@@ -949,6 +949,32 @@ int ts_imitation_mse_rows(const float* z, const float* act, int64_t B, int32_t A
 int ts_imitation_nll_rows(const float* out, const int64_t* act, int64_t B, int32_t A, int32_t softmax_output, float* dz, float* rows,
                           float* loss, ts_stream_t stream);
 
+/* ---- intrinsic curiosity module (icm.cu) ---- */
+/* The inputs of IntrinsicCuriosityModule's two models (utils/net/discrete.py:418-427) from the feature rows phi [2B][F] =
+ * [phi1 ; phi2] (one feature-net pass over [obs ; obs_next]): fwd_in [B][F + A] = [phi1 | one_hot(act, A)], inv_in [B][2F] =
+ * [phi1 | phi2].  act [B] is int64 (act_f32 = 0) or float32 holding integers (act_f32 = 1); it must lie in [0, A): the caller
+ * checks it.  One grid-stride launch; any B, F, A >= 1. */
+int ts_icm_inputs(const float* phi, const void* act, int32_t act_f32, int64_t B, int32_t F, int32_t A, float* fwd_in, float* inv_in,
+                  ts_stream_t stream);
+/* The ICM losses (modelbased/icm.py:77-109) from phi [2B][F], the forward model's output phi2_hat [B][F] and the inverse model's
+ * act_hat [B][A], with w = forward_loss_weight:
+ *   rows [2][B]    mse[b] = 0.5 sum_j (phi2_hat - phi2)^2, then ce[b] = logsumexp(act_hat[b]) - act_hat[b][act[b]] (max-shifted);
+ *   losses [3]     (((1 - w) mean(ce) + w mean(mse)) lr_scale, mean(mse), mean(ce)): a fixed-order one-block sum;
+ *   dphi2_hat      lr_scale w / B (phi2_hat - phi2);   dact_hat  lr_scale (1 - w) / B (softmax(act_hat) - onehot(act));
+ *   dphi [B:2B][F] -dphi2_hat, the direct term of phi2 (its rows [0:B] are not touched);
+ *   rew_out [B]    (nullable) rew_in[b] + (double)(fp32 mse[b] * reward_scale), the intrinsic reward added to the float64 reward;
+ *                  an array of its own (the reward column it reads may be a replay buffer's).
+ * One warp per row (any F, A), then the one-block sum; no atomics, so two calls on the same input are bit-identical. */
+int ts_icm_rows(const float* phi, const float* phi2_hat, const float* act_hat, const void* act, int32_t act_f32, int64_t B, int32_t F,
+                int32_t A, float lr_scale, float forward_loss_weight, const double* rew_in, float reward_scale, double* rew_out,
+                float* dphi, float* dphi2_hat, float* dact_hat, float* rows, float* losses, ts_stream_t stream);
+/* The gradient at the feature net's output, in place in dphi [2B][F] (rows [B:2B] hold ts_icm_rows' direct term): rows b < B
+ * become dinv[b][0:F] + dfwd[b], rows B + b add dinv[b][F:2F]; dinv [B][2F] is the inverse model's input gradient, dfwd [B][F]
+ * the forward model's over its phi1 columns.  Then times the derivative of the feature net's last activation act (TS_ACT_*) at
+ * its output phi [2B][F] (nullable for TS_ACT_NONE).  Grid-stride; any B, F >= 1. */
+int ts_icm_feature_grad(float* dphi, const float* dinv, const float* dfwd, const float* phi, int32_t act, int64_t B, int32_t F,
+                        ts_stream_t stream);
+
 #ifdef TS_B200_DIAGNOSTICS
 /* Diagnostics build only (libts_b200_diag.so, `python -m tianshou_b200.csrc.build --diag`): not part of the product library. */
 /* Hardware self-test of the wgmma building blocks (csrc/wgmma.cuh), one CTA:

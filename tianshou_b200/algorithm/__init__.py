@@ -3,6 +3,7 @@ from .flat_params import UnsupportedModelError
 from .imitation import (BCQ, CQL, GAIL, TD3BC, BCQPolicy, BCQTrainingStats, CQLTrainingStats, DiscreteBCQ, DiscreteBCQPolicy,
                         DiscreteBCQTrainingStats, DiscreteCQL, DiscreteCQLTrainingStats, DiscreteCRR, DiscreteCRRTrainingStats,
                         GailTrainingStats, OffPolicyImitationLearning)
+from .modelbased import ICMOffPolicyWrapper, ICMOnPolicyWrapper
 from .modelfree.a2c import A2CTrainingStats, ActorCriticOnPolicyAlgorithm
 from .modelfree.bdqn import BDQN, BDQNPolicy
 from .modelfree.c51 import C51, C51Policy
@@ -28,5 +29,6 @@ __all__ = [
     "RMSpropOptimizerFactory", "DiscreteBCQ", "DiscreteBCQPolicy", "DiscreteBCQTrainingStats", "DiscreteCRR",
     "DiscreteCRRTrainingStats", "QRDQN", "QRDQNPolicy", "DiscreteCQL", "DiscreteCQLTrainingStats", "IQN", "IQNPolicy",
     "FQF", "FQFPolicy", "FQFTrainingStats", "REDQ", "REDQPolicy", "REDQTrainingStats", "BDQN", "BDQNPolicy", "C51", "C51Policy",
-    "RainbowDQN", "RainbowTrainingStats", "DQN", "OffPolicyImitationLearning",
+    "RainbowDQN", "RainbowTrainingStats", "DQN", "OffPolicyImitationLearning", "ICMOffPolicyWrapper",
+    "ICMOnPolicyWrapper",
 ]

@@ -364,3 +364,115 @@ class OfflineAlgorithm(Algorithm, ABC):
     def update(self, buffer: ReplayBuffer, sample_size: int | None) -> TrainingStats:
         return self._update(sample_size=sample_size, buffer=buffer,
                             update_with_batch_fn=lambda batch: self._update_with_batch(batch))
+
+
+class TrainingStatsWrapper(TrainingStats):
+    """The stats of a wrapped algorithm's update with the wrapper's own fields on top (algorithm_base.py:99-140): unknown
+    attributes read through to the wrapped stats, and the base fields (``train_time``, ``smoothed_loss``) are kept equal in both.
+    A subclass sets its own fields first and calls ``super().__init__`` last."""
+
+    _setattr_frozen = False
+    _training_stats_public_fields = TrainingStats.__dataclass_fields__.keys()
+
+    def __init__(self, wrapped_stats: TrainingStats) -> None:
+        self._wrapped_stats = wrapped_stats
+        for k in self._training_stats_public_fields:
+            super().__setattr__(k, getattr(self._wrapped_stats, k))
+        self._setattr_frozen = True
+
+    def _get_self_dict(self) -> dict[str, Any]:
+        return {**self._wrapped_stats._get_self_dict(), **self.__dict__}
+
+    @property
+    def wrapped_stats(self) -> TrainingStats:
+        return self._wrapped_stats
+
+    def __getattr__(self, name: str) -> Any:
+        if name == "_wrapped_stats":        # not set yet (inside __init__): no read-through
+            raise AttributeError(name)
+        return getattr(self._wrapped_stats, name)
+
+    def __setattr__(self, name: str, value: Any) -> None:
+        if name in self._training_stats_public_fields:
+            setattr(self._wrapped_stats, name, value)
+            super().__setattr__(name, value)
+            return
+        if not self._setattr_frozen:
+            super().__setattr__(name, value)
+            return
+        if not hasattr(self, name):
+            raise AttributeError(f"Setting new attributes on StatsWrappers outside of init is not allowed. Tried to set {name=}, "
+                                 f"{value=} on {self.__class__.__name__}.")
+        if name in self.__dict__:
+            super().__setattr__(name, value)
+        else:
+            setattr(self._wrapped_stats, name, value)
+
+
+class _WrapperAlgorithmMixin:
+    """What the on- and off-policy wrapper bases share (algorithm_base.py:954-1060): the wrapped algorithm's batch draw, pre- and
+    post-processing.  ``_sample`` delegates too, so the batch is the wrapped algorithm's device batch."""
+
+    wrapped_algorithm: Algorithm
+
+    def _sample(self, buffer: ReplayBuffer, sample_size: int | None) -> tuple[Batch, Any]:
+        return self.wrapped_algorithm._sample(buffer, sample_size)
+
+    def _preprocess_batch(self, batch: Batch, buffer: ReplayBuffer, indices: Any) -> Batch:
+        return self.wrapped_algorithm._preprocess_batch(batch, buffer, indices)
+
+    def _postprocess_batch(self, batch: Batch, buffer: ReplayBuffer, indices: Any) -> None:
+        self.wrapped_algorithm._postprocess_batch(batch, buffer, indices)
+
+    def load_state_dict(self, state_dict: Mapping[str, Any], strict: bool = True, assign: bool = False):  # type: ignore[override]
+        """``state_dict()`` holds the wrapped algorithm's optimiser states under ``wrapped_algorithm._optimizers`` (its own
+        ``state_dict`` adds them); they go back to its optimisers."""
+        state_dict = dict(state_dict)
+        key = "wrapped_algorithm." + Algorithm._STATE_DICT_KEY_OPTIMIZERS
+        inner = state_dict.pop(key, None)
+        result = super().load_state_dict(state_dict, strict=strict, assign=assign)  # type: ignore[misc]
+        if inner is not None:
+            for optim, st in zip(self.wrapped_algorithm._optimizers, inner, strict=True):
+                optim.load_state_dict(st)
+        return result
+
+
+class OnPolicyWrapperAlgorithm(_WrapperAlgorithmMixin, OnPolicyAlgorithm, ABC):
+    """An on-policy algorithm wrapping another (algorithm_base.py:954-1006): the wrapped algorithm's update, then the wrapper's.
+    ``update`` runs inside the wrapped algorithm's ``_minibatch_order_job`` when it has one, so its minibatch orders are drawn
+    while the batch is prepared, as its own ``update`` arranges."""
+
+    def __init__(self, wrapped_algorithm: OnPolicyAlgorithm) -> None:
+        super().__init__(policy=wrapped_algorithm.policy)
+        self.wrapped_algorithm = wrapped_algorithm
+
+    def update(self, buffer: ReplayBuffer, batch_size: int | None, repeat: int) -> TrainingStats:
+        job = getattr(self.wrapped_algorithm, "_minibatch_order_job", None)
+        if job is None:
+            return super().update(buffer=buffer, batch_size=batch_size, repeat=repeat)
+        with job(buffer, repeat):
+            return super().update(buffer=buffer, batch_size=batch_size, repeat=repeat)
+
+    def _update_with_batch(self, batch: Batch, batch_size: int | None, repeat: int) -> TrainingStats:
+        original_stats = self.wrapped_algorithm._update_with_batch(batch, batch_size=batch_size, repeat=repeat)
+        return self._wrapper_update_with_batch(batch, batch_size, repeat, original_stats)
+
+    @abstractmethod
+    def _wrapper_update_with_batch(self, batch: Batch, batch_size: int | None, repeat: int,
+                                   original_stats: TrainingStats) -> TrainingStats: ...
+
+
+class OffPolicyWrapperAlgorithm(_WrapperAlgorithmMixin, OffPolicyAlgorithm, ABC):
+    """An off-policy algorithm wrapping another (algorithm_base.py:1009-1060): the wrapped algorithm's update, then the
+    wrapper's."""
+
+    def __init__(self, wrapped_algorithm: OffPolicyAlgorithm) -> None:
+        super().__init__(policy=wrapped_algorithm.policy)
+        self.wrapped_algorithm = wrapped_algorithm
+
+    def _update_with_batch(self, batch: Batch) -> TrainingStats:
+        original_stats = self.wrapped_algorithm._update_with_batch(batch)
+        return self._wrapper_update_with_batch(batch, original_stats)
+
+    @abstractmethod
+    def _wrapper_update_with_batch(self, batch: Batch, original_stats: TrainingStats) -> TrainingStats: ...

@@ -1,5 +1,5 @@
 """Discrete-action actor / critic heads, IQN's quantile network, FQF's fraction proposal and full quantile function and Rainbow's
-noisy layer (API of tianshou/utils/net/discrete.py:22-364)."""
+noisy layer and the intrinsic curiosity module (API of tianshou/utils/net/discrete.py:22-428)."""
 from __future__ import annotations
 
 from collections.abc import Sequence
@@ -195,3 +195,30 @@ class NoisyLinear(nn.Module):
             weight = self.mu_W
             bias = self.mu_bias
         return F.linear(x, weight, bias)
+
+
+class IntrinsicCuriosityModule(nn.Module):
+    """Intrinsic curiosity module (arXiv:1705.05363, discrete.py:377-428): a feature net, a forward model predicting the next
+    state's features from ``[phi1 | one_hot(act)]`` and an inverse model predicting the action from ``[phi1 | phi2]``.  ``forward``
+    is the reference's torch path; the wrappers of algorithm/modelbased/icm.py run the same computation on the device."""
+
+    def __init__(self, *, feature_net: nn.Module, feature_dim: int, action_dim: int, hidden_sizes: Sequence[int] = ()) -> None:
+        super().__init__()
+        self.feature_net = feature_net
+        self.forward_model = MLP(input_dim=feature_dim + action_dim, output_dim=feature_dim, hidden_sizes=hidden_sizes)
+        self.inverse_model = MLP(input_dim=feature_dim * 2, output_dim=action_dim, hidden_sizes=hidden_sizes)
+        self.feature_dim = feature_dim
+        self.action_dim = action_dim
+
+    def forward(self, s1: np.ndarray | torch.Tensor, act: np.ndarray | torch.Tensor, s2: np.ndarray | torch.Tensor,
+                **kwargs: Any) -> tuple[torch.Tensor, torch.Tensor]:
+        """s1, act, s2 -> (mse_loss, act_hat)."""
+        device = next(self.parameters()).device
+        s1 = torch.as_tensor(s1, dtype=torch.float32, device=device)
+        s2 = torch.as_tensor(s2, dtype=torch.float32, device=device)
+        phi1, phi2 = self.feature_net(s1), self.feature_net(s2)
+        act = torch.as_tensor(act, dtype=torch.long, device=device)
+        phi2_hat = self.forward_model(torch.cat([phi1, F.one_hot(act, num_classes=self.action_dim)], dim=1))
+        mse_loss = 0.5 * F.mse_loss(phi2_hat, phi2, reduction="none").sum(1)
+        act_hat = self.inverse_model(torch.cat([phi1, phi2], dim=1))
+        return mse_loss, act_hat
