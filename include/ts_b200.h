@@ -975,6 +975,50 @@ int ts_icm_rows(const float* phi, const float* phi2_hat, const float* act_hat, c
 int ts_icm_feature_grad(float* dphi, const float* dinv, const float* dfwd, const float* phi, int32_t act, int64_t B, int32_t F,
                         ts_stream_t stream);
 
+/* ---- PSRL (algorithm/modelbased/psrl.py) -------------------------------------------------------------------------------------
+ * Bytes of the workspace of ts_psrl_update for n rows of an n_state x n_action model.  Its first part (counts of the model's
+ * size) must be zero when first used and is left zero by every update; that part's layout does not depend on n, so a workspace
+ * sized for one n serves any smaller n. */
+int64_t ts_psrl_update_workspace_bytes(int64_t n, int32_t n_state, int32_t n_action);
+/* PSRL._update_with_batch + PSRLModel.observe (psrl.py:65-98, :245-276) over n rows, taken in the order perm [n] (int64, a
+ * permutation of [0, n): np.random.permutation's order of batch.split(size=1)).  obs / act / obs_next [n] are int64 indices
+ * (idx_f32 = 0) or float32 holding them (idx_f32 = 1); rew [n] is float32 or float64 (rew_dtype TS_F32 / TS_F64), squared in
+ * float32 when sq_f32 (the buffer's rewards are float32) and in float64 otherwise; done [n] (uint8, nullable unless
+ * add_done_loop) adds the self-loops of obs_next: trans_count[s', :, s'] += 1, rew_count[s', :] += 1.
+ * The batch sums of each (s, a) run in float64 in the permuted order; the counts are exact.  Then, per element, with
+ * explicitly rounded operations: trans_count += counts; sum_count = rew_count + counts; rew_mean = (rew_mean rew_count +
+ * rew_sum) / sum_count; rew_square_sum += square sums; rew_std = sqrt(1 / (sum_count / (rew_square_sum / sum_count - rew_mean^2
+ * + eps32) + 1 / rew_std_prior^2)); rew_count = sum_count.  The five state arrays are float64 [n_state][n_action](, [n_state]).
+ * An index outside its range (negative, not an integer, or >= n_state / n_action) sets result[0] = 1 and changes nothing.
+ * result [3] (float64): the error flag, mean(rew_mean), mean(rew_std) (fixed-order sums): one device-to-host copy.
+ * The caller checks that every column holds n entries: the kernels read each of them at every row. */
+int ts_psrl_update(const void* obs, const void* act, const void* obs_next, int32_t idx_f32, const void* rew, int32_t rew_dtype,
+                   int32_t sq_f32, const uint8_t* done, int32_t add_done_loop, const int64_t* perm, int64_t n, int32_t n_state,
+                   int32_t n_action, double* trans_count, double* rew_mean, double* rew_std, double* rew_square_sum,
+                   double* rew_count, const double* rew_std_prior, void* workspace, int64_t workspace_bytes, double* result,
+                   ts_stream_t stream);
+/* PSRLModel.observe (psrl.py:65-98) with the batch's dense float64 arrays: trans_count_batch [n_state][n_action][n_state],
+ * rew_sum, rew_square_sum_batch, rew_count_batch [n_state][n_action]; the same per-element update as ts_psrl_update.  flag: one
+ * int of device scratch.  result [3]: 0, mean(rew_mean), mean(rew_std). */
+int ts_psrl_observe(const double* trans_count_batch, const double* rew_sum, const double* rew_square_sum_batch,
+                    const double* rew_count_batch, int32_t n_state, int32_t n_action, double* trans_count, double* rew_mean,
+                    double* rew_std, double* rew_square_sum, double* rew_count, const double* rew_std_prior, int* flag,
+                    double* result, ts_stream_t stream);
+/* The most states ts_psrl_value_iteration takes on this device: V [n_state] float64 must fit in one CTA's shared memory. */
+int32_t ts_psrl_max_states(void);
+/* Bytes of the scratch of ts_psrl_value_iteration (contents ignored). */
+int64_t ts_psrl_value_iteration_scratch_bytes(int32_t n_state, int32_t n_action);
+/* PSRLModel.value_iteration (psrl.py:116-150) in one cooperative launch of at most one CTA per SM.  trans_prob [n_state]
+ * [n_action][n_state], rew and noise [n_state][n_action], value [n_state]: all float64.  Sweeps Q = rew + gamma (P . V),
+ * V' = max_a Q, from V = value, while any state has |V' - V| > 1e-8 + eps |V| (np.allclose; NaN is never close), at most
+ * max_iterations sweeps.  Converged: value = V' and out[s] = the first argmax_a (Q + eps noise).  Not converged: value and
+ * out[0:n_state] are left as they were.  out [n_state + 3] (int64): the policy, the sweep count, 1 if converged, and the bits of
+ * max |V' - V| over the last sweep when it was the max_iterations-th.  Each sweep's dot products use one fixed order: reruns are
+ * bit-identical.  The caller checks the shapes: the kernel reads and writes every element those shapes name. */
+int ts_psrl_value_iteration(const double* trans_prob, const double* rew, const double* noise, int32_t n_state, int32_t n_action,
+                            double gamma, double eps, int64_t max_iterations, double* value, void* scratch, int64_t* out,
+                            ts_stream_t stream);
+
 #ifdef TS_B200_DIAGNOSTICS
 /* Diagnostics build only (libts_b200_diag.so, `python -m tianshou_b200.csrc.build --diag`): not part of the product library. */
 /* Hardware self-test of the wgmma building blocks (csrc/wgmma.cuh), one CTA:

@@ -3,7 +3,7 @@ from .flat_params import UnsupportedModelError
 from .imitation import (BCQ, CQL, GAIL, TD3BC, BCQPolicy, BCQTrainingStats, CQLTrainingStats, DiscreteBCQ, DiscreteBCQPolicy,
                         DiscreteBCQTrainingStats, DiscreteCQL, DiscreteCQLTrainingStats, DiscreteCRR, DiscreteCRRTrainingStats,
                         GailTrainingStats, OffPolicyImitationLearning)
-from .modelbased import ICMOffPolicyWrapper, ICMOnPolicyWrapper
+from .modelbased import PSRL, ICMOffPolicyWrapper, ICMOnPolicyWrapper
 from .modelfree.a2c import A2CTrainingStats, ActorCriticOnPolicyAlgorithm
 from .modelfree.bdqn import BDQN, BDQNPolicy
 from .modelfree.c51 import C51, C51Policy
@@ -30,5 +30,5 @@ __all__ = [
     "DiscreteCRRTrainingStats", "QRDQN", "QRDQNPolicy", "DiscreteCQL", "DiscreteCQLTrainingStats", "IQN", "IQNPolicy",
     "FQF", "FQFPolicy", "FQFTrainingStats", "REDQ", "REDQPolicy", "REDQTrainingStats", "BDQN", "BDQNPolicy", "C51", "C51Policy",
     "RainbowDQN", "RainbowTrainingStats", "DQN", "OffPolicyImitationLearning", "ICMOffPolicyWrapper",
-    "ICMOnPolicyWrapper",
+    "ICMOnPolicyWrapper", "PSRL",
 ]

@@ -9,7 +9,7 @@ from concurrent.futures import ThreadPoolExecutor
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SOURCES = ["capi.cu", "gae.cu", "nstep.cu", "index.cu", "segtree.cu", "mlp.cu", "mlp_tc.cu", "peer.cu", "hostperm.cu", "net_gemm.cu", "net_ops.cu", "ppo_rows.cu", "npg.cu", "gail.cu",
-           "discrete_sac.cu", "cql.cu", "td3.cu", "bcq.cu", "discrete_bcq.cu", "discrete_crr.cu", "qrdqn.cu", "iqn.cu", "fqf.cu", "redq.cu", "bdqn.cu", "c51.cu", "rainbow.cu", "lstm.cu", "imitation.cu", "icm.cu", "hostperm_simd.cpp"]      # .cpp = host-only, compiled by g++
+           "discrete_sac.cu", "cql.cu", "td3.cu", "bcq.cu", "discrete_bcq.cu", "discrete_crr.cu", "qrdqn.cu", "iqn.cu", "fqf.cu", "redq.cu", "bdqn.cu", "c51.cu", "rainbow.cu", "lstm.cu", "imitation.cu", "icm.cu", "psrl.cu", "hostperm_simd.cpp"]      # .cpp = host-only, compiled by g++
 DIAG_SOURCES = ["umma_selftest.cu"]       # diagnostics library only (-DTS_B200_DIAGNOSTICS: phase timeline + wgmma self-test)
 LIB = os.path.join(os.path.dirname(HERE), "libts_b200.so")
 DIAG_LIB = os.path.join(os.path.dirname(HERE), "libts_b200_diag.so")

@@ -341,4 +341,55 @@ def narrow_i64_i32(src: torch.Tensor) -> torch.Tensor:
     return out
 
 
+# ------------------------------------------------------------------------------------------------ PSRL
+def psrl_update(obs: torch.Tensor, act: torch.Tensor, obs_next: torch.Tensor, rew: torch.Tensor, done: torch.Tensor | None,
+                perm: torch.Tensor, *, sq_f32: bool, add_done_loop: bool, state: tuple[torch.Tensor, ...],
+                rew_std_prior: torch.Tensor, workspace: torch.Tensor | None, result: torch.Tensor) -> torch.Tensor:
+    """``ts_psrl_update``: the posterior update over the rows in ``perm``'s order.  ``obs`` / ``act`` / ``obs_next`` are all int64
+    or all float32; ``state`` is (trans_count, rew_mean, rew_std, rew_square_sum, rew_count) on one device, updated in place.
+    Returns the workspace (grown when too small: a new one starts zeroed, as the kernels require)."""
+    n = perm.numel()
+    trans_count, rew_mean = state[0], state[1]
+    n_s, n_a = rew_mean.shape
+    dev = rew_mean.device
+    idx_f32 = obs.dtype == torch.float32
+    assert act.dtype == obs.dtype and obs_next.dtype == obs.dtype and (idx_f32 or obs.dtype == torch.int64)
+    need = int(_cabi.load_library().ts_psrl_update_workspace_bytes(n, n_s, n_a))
+    if workspace is None or workspace.numel() < need:
+        workspace = torch.zeros(need, dtype=torch.uint8, device=dev)
+    call("ts_psrl_update", ptr(obs), ptr(act), ptr(obs_next), int(idx_f32), ptr(rew), _dt(rew.dtype), int(sq_f32), ptr(done),
+         int(add_done_loop), ptr(perm), n, n_s, n_a, ptr(trans_count), ptr(rew_mean), *(ptr(t) for t in state[2:]),
+         ptr(rew_std_prior), ptr(workspace), workspace.numel(), ptr(result), stream_ptr(dev))
+    return workspace
+
+
+def psrl_observe(batch: tuple[torch.Tensor, ...], state: tuple[torch.Tensor, ...], rew_std_prior: torch.Tensor,
+                 flag: torch.Tensor, result: torch.Tensor) -> None:
+    """``ts_psrl_observe``: ``batch`` = dense (trans_count, rew_sum, rew_square_sum, rew_count) float64 device arrays."""
+    n_s, n_a = state[1].shape
+    call("ts_psrl_observe", *(ptr(t) for t in batch), n_s, n_a, *(ptr(t) for t in state), ptr(rew_std_prior), ptr(flag),
+         ptr(result), stream_ptr(state[1].device))
+
+
+def psrl_max_states() -> int:
+    return int(_cabi.load_library().ts_psrl_max_states())
+
+
+def psrl_value_iteration(trans_prob: torch.Tensor, rew: torch.Tensor, noise: torch.Tensor, gamma: float, eps: float,
+                         max_iterations: int, value: torch.Tensor, scratch: torch.Tensor | None = None,
+                         out: torch.Tensor | None = None) -> tuple[torch.Tensor, torch.Tensor]:
+    """``ts_psrl_value_iteration``: ``value`` is updated in place when the sweeps converge.  Returns (scratch, out) with ``out``
+    int64 [n_state + 3] = (policy, sweeps, converged, bits of the last max |V' - V|), still on the device."""
+    n_s, n_a = rew.shape
+    dev = rew.device
+    need = int(_cabi.load_library().ts_psrl_value_iteration_scratch_bytes(n_s, n_a))
+    if scratch is None or scratch.numel() < need:
+        scratch = torch.empty(need, dtype=torch.uint8, device=dev)
+    if out is None:
+        out = torch.empty(n_s + 3, dtype=torch.int64, device=dev)
+    call("ts_psrl_value_iteration", ptr(trans_prob), ptr(rew), ptr(noise), n_s, n_a, float(gamma), float(eps), int(max_iterations),
+         ptr(value), ptr(scratch), ptr(out), stream_ptr(dev))
+    return scratch, out
+
+
 __all__ = [n for n in dir() if not n.startswith("_")]
